@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench_train.py -- BASELINE configs[2]/[3]: SmaAt-UNet training step (fwd + bwd + Adam) on B200.
+"""bench_train.py -- BASELINE configs[2]/[3]: SmaAt-UNet training step (fwd + bwd + Adam) on H100.
 
   python bench_train.py [--batch 32] [--steps 10] [--warmup 3] [--mode tf32x3]
   torchrun --nproc-per-node N bench_train.py --global-batch 256      # configs[3]: DDP, one flat gradient all-reduce
 
 Loss = mse_loss(pred.squeeze(1), y, reduction="sum") / B and Adam(lr=1e-3) as in the reference
 (models/regression_lightning.py:47-65).  BatchNorm statistics stay per rank (no SyncBatchNorm in the reference).
-Not part of the driver's bench contract; prints one JSON line for profiles/.
+Separate from bench.py; prints one JSON line.
 """
 import argparse
 import json

@@ -1,5 +1,5 @@
 /*
- * smaat_b200.h -- C ABI of libsmaat_b200.so: the B200 (sm_100a) kernels behind the
+ * smaat_b200.h -- C ABI of libsmaat_b200.so: the H100 (sm_90a) kernels behind the
  * SmaAt-UNet hot path (depthwise-separable conv blocks + CBAM + their glue): forward for
  * inference, train-mode forward + backward, and the training step's loss/metric pass.
  *
@@ -13,8 +13,7 @@
  *   - all tensors are fp32, NCHW, dense in (H, W); device pointers owned by the caller
  *     (PyTorch caching allocator).  The library allocates nothing persistent.
  *   - every call only ENQUEUES work on `stream` (a cudaStream_t passed as void*):
- *     no device synchronisation, no allocation -> CUDA-graph capturable
- *     (the one exception is the debug hook smaat_debug_dsconv_timing).
+ *     no device synchronisation, no allocation -> CUDA-graph capturable.
  *   - return value: 0 on success, negative SMAAT_E_* otherwise; smaat_last_error()
  *     returns a thread-local description.  Nothing throws or exits across the ABI.
  *   - "bstride" arguments are batch strides in ELEMENTS (>= C*H*W) so a kernel can
@@ -30,7 +29,7 @@
 extern "C" {
 #endif
 
-#define SMAAT_ABI_VERSION 1
+#define SMAAT_ABI_VERSION 2   /* 2: the tensor-memory kernel's debug hooks and smaat_debug_dsconv_timing are gone */
 
 #define SMAAT_OK 0
 #define SMAAT_E_BADARG (-1)   /* shape / pointer / alignment rejected by host-side validation */
@@ -39,8 +38,8 @@ extern "C" {
 
 /* pointwise arithmetic modes (smaat_pw1x1_fwd) */
 #define SMAAT_PW_FP32_SIMT 0  /* CUDA-core FFMA, exact fp32 products                      */
-#define SMAAT_PW_TF32 1       /* tcgen05 kind::tf32, fp32 accumulate in TMEM (1 pass)     */
-#define SMAAT_PW_TF32X3 2     /* tcgen05 3xTF32 split (a_hi*b_hi + a_lo*b_hi + a_hi*b_lo) */
+#define SMAAT_PW_TF32 1       /* wgmma tf32, fp32 accumulate (1 pass)                     */
+#define SMAAT_PW_TF32X3 2     /* wgmma 3xTF32 split (a_hi*b_hi + a_lo*b_hi + a_hi*b_lo)   */
 
 int smaat_abi_version(void);
 const char* smaat_last_error(void);
@@ -82,16 +81,17 @@ int smaat_pw1x1_fwd(const float* x, const float* w, const float* w_lo,
 /* ---- fused DepthwiseSeparableConv: depthwise 3x3 -> pointwise 1x1 -> affine (+ReLU) in ONE kernel ----
  * replaces DepthwiseSeparableConv.forward (models/layers.py:47-50) + eval BatchNorm2d + ReLU
  * (parts_ds.py:25-26,34-35); the k*Cin-channel depthwise result stays on chip (CUDA-core stencil writes
- * the tcgen05 A operand directly).  Arguments as smaat_dw3x3_fwd (input = virtual concat [x0, x1],
+ * the wgmma A operand tiles directly).  Arguments as smaat_dw3x3_fwd (input = virtual concat [x0, x1],
  * dw_w: (k*Cin,3,3), dw_b: (k*Cin) or NULL) and smaat_pw1x1_fwd (pw_w: (Cout, k*Cin) -- the tf32 hi
  * parts in TF32X3 mode, pw_w_lo the lo parts; scale/shift/stats/relu as there).
  * mode: SMAAT_PW_TF32 or SMAAT_PW_TF32X3.  Returns SMAAT_E_UNSUPPORTED for shapes the fused kernel
- * does not take (k not in {1,2}, Cout > 128, W % 4, patch waste > 35 %): callers then run
+ * does not take (k not in {1,2}; Cout < 8, or Cout > 128 unless a multiple of 128 up to 512 without batch
+ * statistics or OutConv; W % 4; patch waste > 35 %): callers then run
  * smaat_dw3x3_fwd + smaat_pw1x1_fwd.  smaat_dsconv_eligible returns 1/0 for the same test. */
 int smaat_dsconv_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                           const float* pw_w, int H, int W, int k, int Cout);
 /* Same test with the batch-statistics request made explicit: `with_stats` != 0 asks for the kernel that accumulates the
- * per-channel sum / sum of squares of its output (train-mode BatchNorm, parts_ds.py:25,34) -- the shared-memory-operand kernel. */
+ * per-channel sum / sum of squares of its output (train-mode BatchNorm, parts_ds.py:25,34): Cout <= 128 only. */
 int smaat_dsconv_eligible2(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                            const float* pw_w, int H, int W, int k, int Cout, int with_stats);
 int smaat_dsconv_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
@@ -100,30 +100,20 @@ int smaat_dsconv_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x
                      int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
 /* The network's last two modules in one kernel: the fused DS conv above followed by OutConv(Cout -> 1 class)
  * (models/SmaAt_UNet.py:55-56, unet_parts.py:67-73).  oc_w: (Cout), oc_b: (1) or NULL, logits: (B, 1, H, W); the
- * Cout-channel activation is reduced in the epilogue registers (TMEM lane = pixel) and never written.  Same eligibility
- * as smaat_dsconv_fwd. */
+ * Cout-channel activation is reduced in the epilogue registers and never written.  Same eligibility
+ * as smaat_dsconv_fwd, with Cout <= 128. */
 int smaat_dsconv_outconv_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                              const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
                              const float* scale, const float* shift, const float* oc_w, const float* oc_b, float* logits,
                              int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
 
-/* Which kernel smaat_dsconv_fwd / smaat_dsconv_outconv_fwd run (same reference lines, models/layers.py:47-50): 0 = auto
- * (default: the TMEM-operand kernel, csrc/dsconv_tmem.cu, where it applies -- k = 2, Cout <= 128, no batch statistics --
- * else the shared-memory-operand kernel, csrc/dsconv_fused.cu), 1 = shared-memory-operand kernel only, 2 = TMEM-operand
- * kernel only.  Process-wide; the environment variable SMAAT_DS_IMPL presets it.  For A/B measurements and tests. */
+/* How the fused DS conv (smaat_dsconv_fwd / smaat_dsconv_outconv_fwd, same reference lines, models/layers.py:47-50) hands the
+ * depthwise result to the tensor core: 0 = auto (default; 2, the faster of the two on an H100), 1 = K-major tiles in shared memory that wgmma reads
+ * through a descriptor, 2 = tiles the consumers load into registers for wgmma's register-A form.  Same results up to
+ * summation order.  Process-wide; the environment variable SMAAT_DS_IMPL presets it.  For A/B measurements and tests. */
 int smaat_set_dsconv_impl(int impl);
 
-/* Debug hook: stage timers of the fused kernel's CTA 0 (16 clock64 counters accumulated over launches; layout in
- * csrc/dsconv_fused.cu).  Copies them to the HOST array `out` and clears them; synchronises the device. */
-int smaat_debug_dsconv_timing(unsigned long long* out);
-/* Same for the TMEM-operand kernel (24 counters; layout in csrc/dsconv_tmem.cu). */
-int smaat_debug_dsconv_tmem_timing(unsigned long long* out);
-/* Per-CTA (start ns, end ns, SM id) of the last timed launch of the TMEM-operand kernel: 3 * n_ctas entries, n_ctas <= 256. */
-int smaat_debug_dsconv_tmem_cta_timing(unsigned long long* out, int n_ctas);
-/* Event trace of CTA 0 (launch made with SMAAT_DSCONV_TIMING=2): 16 clock64 stamps per unit, n_units <= 256 (layout in the .cu). */
-int smaat_debug_dsconv_tmem_trace(long long* out, int n_units);
-
-/* 1 if this (x, w, K, Cout, P) can take the tcgen05 path (P % 4 == 0, K % 4 == 0, 16-byte aligned
+/* 1 if this (x, w, K, Cout, P) can take the tensor-core (wgmma) path (P % 4 == 0, K % 4 == 0, 16-byte aligned
  * pointers, Cout >= 8), else 0: the caller then uses SMAAT_PW_FP32_SIMT. */
 int smaat_pw1x1_tc_eligible(const float* x, const float* w, int K, int Cout, int P);
 
@@ -224,7 +214,7 @@ int smaat_dw3x3_bwd_weight(const float* dd, const float* x0, int C0, int64_t x0_
  * db[o] += sum dz.  (The input gradient is
  * smaat_pw1x1_fwd(dz, W^T): use smaat_transpose for W^T.) */
 int smaat_pw1x1_bwd_weight(const float* dz, const float* d, float* dW, float* db, int B, int K, int Cout, int P, void* stream);
-/* tensor-core (tcgen05, split over pixels + fp32 atomics) variant; mode SMAAT_PW_TF32 / SMAAT_PW_TF32X3;
+/* tensor-core (wgmma, split over pixels + fp32 atomics) variant; mode SMAAT_PW_TF32 / SMAAT_PW_TF32X3;
  * SMAAT_E_UNSUPPORTED when P % 4 != 0 (use the CUDA-core smaat_pw1x1_bwd_weight). */
 int smaat_pw1x1_bwd_weight_tc(const float* dz, const float* d, float* dW, float* db, int B, int K, int Cout, int P,
                               int mode, void* stream);

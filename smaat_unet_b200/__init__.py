@@ -1,4 +1,4 @@
-"""smaat_unet_b200 -- B200 (sm_100a) implementation of the SmaAt-UNet forward hot path.
+"""smaat_unet_b200 -- H100 (sm_90a) implementation of the SmaAt-UNet forward hot path.
 
 Drop-in ``nn.Module`` replacements for the reference's DS-conv blocks and CBAM
 (``modules``), the same model assembly (``model.SmaAt_UNet``), a helper that rebinds the

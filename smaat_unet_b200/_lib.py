@@ -24,12 +24,8 @@ SIGNATURES = {
     "smaat_pw1x1_tc_eligible": [_p, _p, _i, _i, _i],
     "smaat_dsconv_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i],
     "smaat_dsconv_eligible2": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i],
-    "smaat_dsconv_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _i, _p],
-    "smaat_debug_dsconv_timing": [_p],
     "smaat_set_dsconv_impl": [_i],
-    "smaat_debug_dsconv_tmem_timing": [_p],
-    "smaat_debug_dsconv_tmem_cta_timing": [_p, _i],
-    "smaat_debug_dsconv_tmem_trace": [_p, _i],
+    "smaat_dsconv_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_outconv_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_split_tf32": [_p, _p, _p, _l, _p],
     "smaat_bn_fold": [_p, _p, _p, _p, _p, _f, _p, _p, _i, _p],
@@ -100,7 +96,7 @@ def load():
         fn = getattr(lib, name)
         fn.argtypes = argtypes
         fn.restype = restype
-    if lib.smaat_abi_version() != 1:
+    if lib.smaat_abi_version() != 2:
         raise RuntimeError("smaat_unet_b200: ABI version mismatch between _lib.py and libsmaat_b200.so")
     _lib = lib
     return lib

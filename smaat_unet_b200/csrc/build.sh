@@ -1,23 +1,21 @@
 #!/usr/bin/env bash
-# Builds libsmaat_b200.so in-tree for sm_100a (B200).  nvcc cross-compiles without a GPU.
+# Builds libsmaat_b200.so in-tree for sm_90a (H100).  nvcc cross-compiles without a GPU.
 set -euo pipefail
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 OUT=../libsmaat_b200.so
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O2,-Wall
+FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O2,-Wall
        -Xptxas -v -cudart static)
-# SMAAT_DT_INSTRUMENT=1: stage timers / event trace / knock-out flags of the TMEM-operand DS-conv kernel (diagnostic builds only)
-INSTR=${SMAAT_DT_INSTRUMENT:-0}
-FLAGS+=(-DSMAAT_DT_INSTRUMENT=$INSTR)
-SRCS=(runtime.cu dw3x3.cu dw3x3_small.cu pw1x1.cu pw1x1_simt.cu pw1x1_tc.cu pw1x1_wgrad_tc.cu dsconv_fused.cu dsconv_tmem.cu glue.cu upsample.cu cbam.cu bn.cu backward.cu bn_bwd.cu loss_metrics.cu dw3x3_bwd.cu cbam_bwd.cu optim.cu convt.cu)
+SRCS=(runtime.cu dw3x3.cu dw3x3_small.cu pw1x1.cu pw1x1_simt.cu pw1x1_tc.cu pw1x1_wgrad_tc.cu dsconv_fused.cu glue.cu upsample.cu cbam.cu bn.cu backward.cu bn_bwd.cu loss_metrics.cu dw3x3_bwd.cu cbam_bwd.cu optim.cu convt.cu)
 mkdir -p ../../build
-if [[ "$(cat ../../build/.instrument 2>/dev/null || echo 0)" != "$INSTR" ]]; then rm -f ../../build/dsconv_tmem.o; echo "$INSTR" > ../../build/.instrument; fi
+# objects built with other flags (another architecture, say) are rebuilt
+if [[ "$(cat ../../build/.flags 2>/dev/null || true)" != "${FLAGS[*]}" ]]; then rm -f ../../build/*.o; echo "${FLAGS[*]}" > ../../build/.flags; fi
 OBJS=()
 pids=()
 for s in "${SRCS[@]}"; do
   o=../../build/${s%.cu}.o
   OBJS+=("$o")
-  if [[ ! -f "$o" || "$s" -nt "$o" || common.cuh -nt "$o" || tc_common.cuh -nt "$o" || ../../include/smaat_b200.h -nt "$o" ]]; then
+  if [[ ! -f "$o" || "$s" -nt "$o" || common.cuh -nt "$o" || tc_common.cuh -nt "$o" || wgmma.cuh -nt "$o" || ../../include/smaat_b200.h -nt "$o" ]]; then
     ( "$NVCC" "${FLAGS[@]}" -c "$s" -o "$o" > "../../build/${s%.cu}.log" 2>&1 || { cat "../../build/${s%.cu}.log"; exit 1; } ) &
     pids+=($!)
   fi

@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for libsmaat_b200 (sm_100a only).
+// common.cuh -- shared host/device helpers for libsmaat_b200 (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>

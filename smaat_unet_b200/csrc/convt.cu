@@ -3,7 +3,7 @@
 //
 // With kernel = stride = 2 the transposed convolution has no overlapping taps: output pixel (2i + dy, 2j + dx) of channel o is
 //   bias[o] + sum_c x[c, i, j] * W[c, o, dy, dx]
-// i.e. ONE pointwise GEMM from Cin to 4 * Cout "packed" channels (dy, dx, o) -- run by the tcgen05 pointwise kernel
+// i.e. ONE pointwise GEMM from Cin to 4 * Cout "packed" channels (dy, dx, o) -- run by the wgmma pointwise kernel
 // (pw1x1_tc.cu) on a repacked weight -- followed by a 2x2 pixel shuffle.  This file holds the three data-movement kernels
 // around that GEMM: weight repack, pixel shuffle (+ bias + pad), and their transposes for the backward pass.
 #include "common.cuh"

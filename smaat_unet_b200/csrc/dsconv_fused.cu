@@ -1,40 +1,39 @@
 // dsconv_fused.cu -- DepthwiseSeparableConv forward as ONE kernel: depthwise 3x3 on the CUDA
-// cores feeding the pointwise 1x1 on the tensor cores, with the BN-affine/ReLU epilogue.
+// cores feeding the pointwise 1x1 on the Hopper tensor cores (wgmma), with the BN-affine/ReLU epilogue.
 //
 // Replaces DepthwiseSeparableConv.forward (reference models/layers.py:47-50: depthwise then
-// pointwise, nothing in between) + eval BatchNorm2d + ReLU (parts_ds.py:25-26,34-35).  The
-// k x -expanded depthwise result never reaches HBM: per B=32 forward the DS blocks move
-// 4*B*S^2*(Cin + Cout) bytes instead of 4*B*S^2*(Cin + 2*k*Cin + Cout) (SURVEY 8d: 32.7 -> 10.4 GB).
+// pointwise, nothing in between) + eval BatchNorm2d + ReLU (parts_ds.py:25-26,34-35) [+ OutConv,
+// unet_parts.py:67-73, for the network's last conv].  The k x -expanded depthwise result never reaches
+// HBM: per B=32 forward the DS blocks move 4*B*S^2*(Cin + Cout) bytes instead of
+// 4*B*S^2*(Cin + 2*k*Cin + Cout).
 //
-// One persistent CTA per SM; a tile is a PH x PW = 128-pixel patch of one image (M = 128 TMEM
-// lanes) and ALL Cout <= 128 output channels (N_TILE TMEM columns), so the depthwise work is done
-// exactly once.  K = k*Cin is walked in chunks of 32 depthwise channels (CC = 32/k input channels):
+// One persistent CTA per SM; a tile is a PH x PW = 128-pixel patch of one image and one pass of N_TILE <= 128 output
+// channels (Cout <= 128: one pass, so the depthwise work is done exactly once; Cout in {256, 384, 512}: passes of 128).
+// K = k*Cin is walked in chunks of 32 depthwise channels (CC = 32/k input channels):
 //   warp 0      TMA: (PH+2) x (PW+8) x CC input halo box per chunk (OOB zero fill = padding=1; box
 //               starts at x0-4: the inner TMA coordinate must be 16-byte aligned) into an IS-deep ring;
-//               input may be the virtual concat [x0, x1] of UpDS (parts_ds.py:85)
-//   warps 6-17  three depthwise producer groups (128 threads each; group g takes every third chunk): 3x3 stencil
+//               input may be the virtual concat [x0, x1] of UpDS (parts_ds.py:85).  An L2 prefetch of the next tile's boxes
+//               (cp.async.bulk.prefetch.tensor) made bench.py's B = 32 forward slower: 2 220 vs 2 346-2 369 frames/s (H100
+//               80GB HBM3 SXM, 700 W; two runs with, six without), so there is none
+//   warp 1      prefetches the weight chunks (K-major SW128, [hi rows | lo rows]) into their own ring
+//   warps 4-11  two consumer warpgroups (64 pixels each): wgmma (TF32X3: A_hi B_hi + A_lo B_hi + A_hi B_lo per k-step) into
+//               register accumulators, with the A operand either read by the tensor core from the A ring (A_SMEM) or
+//               loaded into registers from it first, then the epilogue:
+//               scale/shift/ReLU -> NCHW stores (or the fused 1-class OutConv dot product; or BatchNorm batch statistics)
+//   warps 12..  NG depthwise producer groups (128 threads each; group g takes every NG-th chunk): 3x3 stencil
 //               from the staged tile with a sliding register window (one LDS.128 per row, edge columns from the
-//               neighbouring quads by shuffle), then write the result straight into the UMMA A-operand layout
-//               (MN-major tf32, 128B span / 32B-atom swizzle) -- as hi and lo tf32 parts in TF32X3 mode (the split
-//               is free here: values are in registers) -- into a 3/4-stage A ring
-//   warp 18     prefetches the weight chunks (K-major SW128, [hi rows | lo rows]) into their own ring
-//   warp 1      MMA issuer: warp-uniform loop, one elected lane issues tcgen05.mma kind::tf32 into TMEM (TF32X3: a wide
-//               A_hi x [B_hi | B_lo] MMA + A_lo x B_hi per k-step) and commits
-//   warps 2-5   epilogue: tcgen05.ld (lane = pixel, 16 columns per step) -> scale/shift/ReLU -> coalesced NCHW stores
-//               (or the fused 1-class OutConv dot product; or BatchNorm batch statistics from fragment-shaped
-//               reads); two TMEM accumulator stages overlap it with the next tile's MMAs
-// Debug: SMAAT_DSCONV_TIMING=1 makes CTA 0 record per-stage cycle counters (smaat_debug_dsconv_timing).
+//               neighbouring quads by shuffle), then write the result into an AS-stage A ring -- as hi and lo tf32 parts
+//               in TF32X3 mode (the split is free here: values are in registers) -- in one of two layouts:
+//                 A_SMEM   [pixel][k] 128B-swizzled K-major tiles, the layout wgmma reads through a descriptor (one scalar
+//                          store per value: a thread's 4 pixels are 4 rows);
+//                 !A_SMEM  [k][pixel] 128B-swizzled tiles (one 16-byte store per 4 pixels), which the consumers load into
+//                          registers conflict-free (tc_common.cuh) and feed to wgmma's register-A form
+// Which one runs is smaat_set_dsconv_impl's choice (csrc/dsconv_fused.cu, below).
 #include <stdlib.h>
 
 #include "tc_common.cuh"
 
 namespace smaat {
-
-// Stage timing of CTA 0 (clock64 cycles, accumulated over launches until read): see smaat_debug_dsconv_timing.
-//  [0] producer group 0: wait input box   [1] wait free A stage   [2] stencil + A-operand writes   [3] chunks
-//  [4] MMA lane: wait A   [5] wait B   [6] wait free accumulator   [7] issue   [8] chunks
-//  [9] epilogue warp 2: wait accumulator  [10] drain + store   [11] tiles      [12] kernel cycles
-__device__ unsigned long long g_ds_timing[16];
 
 struct DsParams {
   const float* dw_w;
@@ -48,8 +47,7 @@ struct DsParams {
   const float* oc_b;
   float* oc_y;
   int C0, C1, H, W, Cout, relu, K;
-  int tiles_x, tiles_y, total_tiles, nchunks;
-  int timing;          // SMAAT_DSCONV_TIMING=1: CTA 0 records stage timers (debug)
+  int tiles_x, tiles_y, npass, total_tiles, nchunks;
 };
 
 template <int N_TILE, int KPL, int PW, bool X3>
@@ -64,36 +62,31 @@ struct DsCfg {
   static constexpr int BST_BYTES = (X3 ? 2 : 1) * B_BYTES;     // B ring stage: hi [+ lo]
   static constexpr int OFF_ALO = A_BYTES;
   static constexpr int OFF_BLO = B_BYTES;
-  // A ring: 3 stages in TF32X3 (32 KB each; the input ring must stay deep enough to cover HBM latency), 4 in TF32
-  static constexpr int AS = X3 ? ((KPL == 1 && N_TILE > 64) ? 2 : 3) : 4;
-  // depthwise producer groups (128 threads each).  NG <= AS always: the per-stage a_empty barriers are tested by phase parity,
-  // which is only unambiguous while a group can never be two hand-backs of a stage behind (see csrc/dsconv_tmem.cu)
-  static constexpr int NG = AS < 3 ? 2 : 3;
+  static constexpr int AS = X3 ? (N_TILE > 64 ? 2 : 3) : 4;     // A ring (the input ring must stay deep enough to cover HBM latency)
+  // depthwise producer groups (128 threads each), sized by the register file: the consumers hold N_TILE / 2 accumulators
+  // per thread.  NG <= AS always: the per-stage a_empty barriers are tested by phase parity, which is only unambiguous while
+  // a group can never be two hand-backs of a stage behind
+  static constexpr int NG = N_TILE > 64 ? 1 : 2;
   static constexpr int BS = X3 ? 2 : 4;                         // weight ring, prefetched by its own warp
-  static constexpr int IS_FIT = (218 * 1024 - AS * AST_BYTES - BS * BST_BYTES) / IN_BYTES;
+  static constexpr int AFF_N = 512;                            // scale | shift | OutConv weights of up to 512 channels
+  static constexpr int BAR_BYTES = 512;
+  static constexpr int IS_FIT = (224 * 1024 - 1024 - BAR_BYTES - 3 * AFF_N * 4 - AS * AST_BYTES - BS * BST_BYTES) / IN_BYTES;
   static constexpr int IS = IS_FIT > 8 ? 8 : IS_FIT;           // input ring: as deep as shared memory allows
   static constexpr int OFF_A = ((IS * IN_BYTES + 1023) / 1024) * 1024;
   static constexpr int OFF_BR = OFF_A + AS * AST_BYTES;
   static constexpr int OFF_BAR = OFF_BR + BS * BST_BYTES;
-  static constexpr int BAR_BYTES = 512;
-  static_assert((IS * NG + IS + 2 * AS + 2 * BS + 4) * 8 + 8 <= BAR_BYTES, "barrier block");
-  static constexpr int AFF_N = 128;
-  static constexpr int TOTAL = OFF_BAR + BAR_BYTES + 3 * AFF_N * 4 + 1024;   // scale | shift | OutConv weights
+  static_assert((IS * NG + IS + 2 * AS + 2 * BS) * 8 <= BAR_BYTES, "barrier block");
+  static constexpr int TOTAL = OFF_BAR + BAR_BYTES + 3 * AFF_N * 4 + 1024;
   static constexpr uint32_t B_TX = BST_BYTES;
-  static constexpr int LOADER_WARP = 6 + 4 * NG;               // weight-ring loader
-  static constexpr int THREADS = 64 + 128 + 128 * NG + 32;     // TMA, MMA | 4 epilogue warps | producers | loader
+  static constexpr int PROD_WARP = 12;                         // first producer warp
+  static constexpr int THREADS = 384 + 128 * NG;               // TMA, loader, 2 idle | 2 consumer warpgroups | producers
   static_assert(IS >= 2, "input ring");
-  // TF32X3: the weight stage holds [hi rows | lo rows] contiguously, so ONE N = 2*N_TILE MMA computes A_hi*[B_hi | B_lo]
-  // into 2*N_TILE accumulator columns and a second N = N_TILE MMA adds A_lo*B_hi to the first half: 2 instead of 3 MMAs
-  // per k-step (each MMA re-reads its 4 KB A slice from shared memory whatever N is); the epilogue adds the two halves.
-  static constexpr int ACC_COLS = X3 ? 2 * N_TILE : N_TILE;
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;               // two accumulator stages
+  static_assert(NG <= AS, "phase-parity barriers");
   static_assert(IN_BYTES % 128 == 0, "TMA destination alignment");
   static_assert(TOTAL <= 227 * 1024, "shared memory budget");
-  static_assert(N_TILE <= AFF_N, "epilogue affine staging");
 };
 
-template <int N_TILE, int KPL, int PW, bool X3>
+template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
 __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
     dsconv_fused_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
                         const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
@@ -107,22 +100,28 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
   // [IS][NG] TMA input box landed, one barrier per (stage, group that reads the fill): a group meets a stage only at every
   // NG-th of its fills (unless NG divides IS), and TMA loads may complete out of order -- a parity test on a per-stage
-  // barrier could then be satisfied by the wrong fill (csrc/dsconv_tmem.cu has the failure this caused there)
+  // barrier could then be satisfied by the wrong fill
   uint64_t* in_full = bars;
   uint64_t* in_empty = in_full + IS * L::NG;      // [IS] producer group finished reading the box (128 arrivals)
   uint64_t* a_full = in_empty + IS;               // [AS] A operand written (128 arrivals)
-  uint64_t* a_empty = a_full + AS;                // [AS] MMAs reading the A stage retired (commit)
+  uint64_t* a_empty = a_full + AS;                // [AS] the 8 consumer warps' MMAs reading the A stage retired
   uint64_t* b_full = a_empty + AS;                // [BS] weight chunk landed (TMA tx)
-  uint64_t* b_empty = b_full + BS;                // [BS] MMAs reading the B stage retired (commit)
-  uint64_t* tmem_full = b_empty + BS;             // [2]
-  uint64_t* tmem_empty = tmem_full + 2;           // [2]  (128 arrivals)
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint64_t* b_empty = b_full + BS;                // [BS] the 8 consumer warps' MMAs reading the B stage retired
   float* aff = reinterpret_cast<float*>(smem + L::OFF_BAR + L::BAR_BYTES);
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler too
   const int lane = threadIdx.x & 31;
   const int nch = p.nchunks;
-  const int tiles_per_img = p.tiles_x * p.tiles_y;
+  const int tiles_per_img = p.tiles_x * p.tiles_y * p.npass;
+  // tile -> (image b, patch row ty, patch column tx, channel pass np); the passes of a patch are consecutive tiles
+  auto decode = [&](int tile, int& b, int& ty, int& tx, int& np) {
+    b = tile / tiles_per_img;
+    int t2 = tile - b * tiles_per_img;
+    np = t2 % p.npass;
+    t2 /= p.npass;
+    ty = t2 / p.tiles_x;
+    tx = t2 - ty * p.tiles_x;
+  };
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&map_in0);
@@ -135,38 +134,28 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
     }
     for (int s = 0; s < AS; ++s) {
       mbar_init(&a_full[s], 128);
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_empty[s], 8);
     }
     for (int s = 0; s < BS; ++s) {
       mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], 128);
+      mbar_init(&b_empty[s], 8);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, L::TMEM_COLS);
   for (int c = threadIdx.x; c < L::AFF_N; c += blockDim.x) {
     aff[c] = (c < p.Cout && p.scale) ? __ldg(p.scale + c) : 1.f;
     aff[L::AFF_N + c] = (c < p.Cout && p.shift) ? __ldg(p.shift + c) : 0.f;
     aff[2 * L::AFF_N + c] = (c < p.Cout && p.oc_w) ? __ldg(p.oc_w + c) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const long long t_kernel0 = ((p.timing & 1) && blockIdx.x == 0 && threadIdx.x == 0) ? clock64() : 0;
 
   if (warp == 0) {
     // ===== TMA: input halo boxes, running ahead through the IS-deep ring =====
     if (lane == 0) {
       uint32_t gc = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int b = tile / tiles_per_img;
-        const int t2 = tile - b * tiles_per_img;
-        const int ty = t2 / p.tiles_x, tx = t2 - ty * p.tiles_x;
+        int b, ty, tx, np;
+        decode(tile, b, ty, tx, np);
         const int x0 = tx * PW, y0 = ty * PH;
         for (int i = 0; i < nch; ++i, ++gc) {
           const int s = gc % IS;
@@ -181,221 +170,175 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
                   "r"(smem_u32(smem + s * L::IN_BYTES)),
               "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(full)), "r"(x0 - 4), "r"(y0 - 1), "r"(cc), "r"(b)
               : "memory");
-          // pull the same chunk of this CTA's NEXT tile into L2 now: by the time it is TMA-loaded the HBM
-          // latency is already paid, so a few 15 KB boxes in flight per SM are enough to stream at HBM speed
-          const int ntile = tile + gridDim.x;
-          if (ntile < p.total_tiles) {
-            const int nb = ntile / tiles_per_img;
-            const int nt2 = ntile - nb * tiles_per_img;
-            const int nty = nt2 / p.tiles_x, ntx = nt2 - nty * p.tiles_x;
-            asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(
-                             reinterpret_cast<uint64_t>(m)),
-                         "r"(ntx * PW - 4), "r"(nty * PH - 1), "r"(cc), "r"(nb)
-                         : "memory");
-          }
         }
       }
     }
-  } else if (warp == L::LOADER_WARP) {
-    // ===== weight-ring loader: K-major SW128 chunks (hi [+lo]), decoupled from the input ring =====
+    return;
+  }
+  if (warp == 1) {
+    // ===== weight-ring loader: K-major SW128 chunks (hi [+lo]) of this tile's channel pass, decoupled from the input ring =====
     if (lane == 0) {
       uint32_t gc = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        int b, ty, tx, np;
+        decode(tile, b, ty, tx, np);
         for (int i = 0; i < nch; ++i, ++gc) {
           const int sb = gc % BS;
-          // rings of equal depth advance in lockstep: one commit (a_empty) releases both the A and the weight stage
-          mbar_wait((AS == BS) ? &a_empty[sb] : &b_empty[sb], ((gc / BS) & 1u) ^ 1u);
+          mbar_wait(&b_empty[sb], ((gc / BS) & 1u) ^ 1u);
           mbar_arrive_expect_tx(&b_full[sb], L::B_TX);
-          tma_load_2d(b_base + sb * L::BST_BYTES, &map_w, &b_full[sb], i * TC_BK, 0);
-          if (X3) tma_load_2d(b_base + sb * L::BST_BYTES + L::OFF_BLO, &map_wlo, &b_full[sb], i * TC_BK, 0);
+          tma_load_2d(b_base + sb * L::BST_BYTES, &map_w, &b_full[sb], i * TC_BK, np * N_TILE);
+          if (X3) tma_load_2d(b_base + sb * L::BST_BYTES + L::OFF_BLO, &map_wlo, &b_full[sb], i * TC_BK, np * N_TILE);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer: the whole warp walks the loop (warp-uniform control flow and descriptors, which the compiler keeps
-    // in uniform registers), one elected lane issues.  Descriptors are built once per chunk and advanced by constant adds:
-    // the issuing thread's own instruction stream was the limit (~30 SASS instructions, ~115 cycles per MMA before). =====
-    constexpr uint32_t idesc = make_idesc_tf32(N_TILE);
-    constexpr uint32_t idesc_wide = make_idesc_tf32(X3 ? 2 * N_TILE : N_TILE);
-    const bool rec = (p.timing & 1) && (blockIdx.x == 0) && (lane == 0);
-    uint32_t gc = 0, tcount = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++tcount) {
-      const uint32_t acc = tcount & 1u;
-      const long long te0 = rec ? clock64() : 0;
-      mbar_wait(&tmem_empty[acc], ((tcount >> 1) & 1u) ^ 1u);
-      if (rec) atomicAdd(&g_ds_timing[6], (unsigned long long)(clock64() - te0));
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * L::ACC_COLS;
+    return;
+  }
+  if (warp < 4) return;
+
+  if (warp < L::PROD_WARP) {
+    // ===== consumer warpgroups: MMAs into register accumulators, then the epilogue =====
+    const int wg = (warp >> 2) - 1, wq = warp & 3;
+    const int g = lane >> 2, t = lane & 3;
+    // patch pixels of accumulator rows g, g + 8: A_SMEM tiles hold pixel m in row m
+    const int m0 = A_SMEM ? 64 * wg + 16 * wq + g : tc_row_pixel(wg, wq, 0, g);
+    const int m1 = A_SMEM ? m0 + 8 : tc_row_pixel(wg, wq, 1, g);
+    const float act_lo = p.relu ? 0.f : -INFINITY;
+    const int64_t P = (int64_t)p.H * p.W;
+    uint32_t gc = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      int b, ty, tx, np;
+      decode(tile, b, ty, tx, np);
+      float acc[N_TILE / 2];
+#pragma unroll
+      for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.f;
       for (int i = 0; i < nch; ++i, ++gc) {
         const int sa = gc % AS, sb = gc % BS;
-        long long tk0 = 0, tk1 = 0, tk2 = 0;
-        if (rec) tk0 = clock64();
         mbar_wait(&a_full[sa], (gc / AS) & 1u);
-        if (rec) tk1 = clock64();
         mbar_wait(&b_full[sb], (gc / BS) & 1u);
-        if (rec) tk2 = clock64();
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_addr = smem_u32(a_base + sa * L::AST_BYTES);
-          const uint32_t b_addr = smem_u32(b_base + sb * L::BST_BYTES);
-          // k-step kk: A advances 8 k-rows = 1 KB, the K-major weights 8 tf32 = 32 B (descriptor address field = bytes >> 4)
-          const uint64_t ad0 = make_a_desc(a_addr, TC_BK * 128);
-          const uint64_t al0 = make_a_desc(a_addr + L::OFF_ALO, TC_BK * 128);
-          const uint64_t bd0 = make_b_desc(b_addr);
-          const int kc = min(TC_BK, p.K - i * TC_BK);
-          if (kc == TC_BK) {
+        const unsigned char* ast = a_base + sa * L::AST_BYTES;
+        const uint64_t bd0 = make_kmajor_desc(smem_u32(b_base + sb * L::BST_BYTES));
+        const uint64_t bl0 = make_kmajor_desc(smem_u32(b_base + sb * L::BST_BYTES + L::OFF_BLO));
+        if (A_SMEM) {
+          const uint32_t a_addr = smem_u32(ast) + (uint32_t)(wg * 64 * 128);   // this warpgroup's 64 rows: 8 swizzle atoms
+          const uint64_t ad0 = make_kmajor_desc(a_addr), al0 = make_kmajor_desc(a_addr + L::OFF_ALO);
+          wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < TC_BK / 8; ++kk) {
-              const uint32_t first = (kk > 0) ? 1u : (i > 0 ? 1u : 0u);
-              if (X3) {
-                // D[:, 0:N) += A_hi*B_hi and D[:, N:2N) += A_hi*B_lo in one wide MMA over the contiguous hi|lo weight rows,
-                // then D[:, 0:N) += A_lo*B_hi
-                umma_tf32(d_tmem, ad0 + (uint64_t)(kk * 64), bd0 + (uint64_t)(kk * 2), idesc_wide, first);
-                umma_tf32(d_tmem, al0 + (uint64_t)(kk * 64), bd0 + (uint64_t)(kk * 2), idesc, 1u);
-              } else {
-                umma_tf32(d_tmem, ad0 + (uint64_t)(kk * 64), bd0 + (uint64_t)(kk * 2), idesc, first);
-              }
-            }
-          } else {
-            const int nmma = (kc + 7) >> 3;
-            for (int kk = 0; kk < nmma; ++kk) {
-              const uint32_t first = (i > 0 || kk > 0) ? 1u : 0u;
-              if (X3) {
-                umma_tf32(d_tmem, ad0 + (uint64_t)(kk * 64), bd0 + (uint64_t)(kk * 2), idesc_wide, first);
-                umma_tf32(d_tmem, al0 + (uint64_t)(kk * 64), bd0 + (uint64_t)(kk * 2), idesc, 1u);
-              } else {
-                umma_tf32(d_tmem, ad0 + (uint64_t)(kk * 64), bd0 + (uint64_t)(kk * 2), idesc, first);
-              }
-            }
-          }
-          umma_commit(&a_empty[sa]);  // each commit tracks completion of all MMAs issued so far
-          if (AS != BS) umma_commit(&b_empty[sb]);
-          if (i == nch - 1) umma_commit(&tmem_full[acc]);
-        }
-        __syncwarp();
-        if (rec) {
-          const long long tk3 = clock64();
-          atomicAdd(&g_ds_timing[4], (unsigned long long)(tk1 - tk0));
-          atomicAdd(&g_ds_timing[5], (unsigned long long)(tk2 - tk1));
-          atomicAdd(&g_ds_timing[7], (unsigned long long)(tk3 - tk2));
-          atomicAdd(&g_ds_timing[8], 1ull);
-        }
-      }
-    }
-  } else if (warp < 6) {
-    // ===== epilogue warps 2..5 =====
-    const int q = warp & 3;
-    const float act_lo = p.relu ? 0.f : -INFINITY;
-    const int m = q * 32 + lane;  // pixel of the patch = TMEM lane
-    const int pr = m / PW, pc = m % PW;
-    const int64_t P = (int64_t)p.H * p.W;
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++tcount) {
-      const int b = tile / tiles_per_img;
-      const int t2 = tile - b * tiles_per_img;
-      const int ty = t2 / p.tiles_x, tx = t2 - ty * p.tiles_x;
-      const int gy = ty * PH + pr, gx = tx * PW + pc;
-      const bool pvalid = (gy < p.H) && (gx < p.W);
-      const uint32_t acc = tcount & 1u;
-      const bool rec = (p.timing & 1) && (blockIdx.x == 0) && (warp == 2) && (lane == 0);
-      long long tq0 = 0, tq1 = 0;
-      if (rec) tq0 = clock64();
-      mbar_wait(&tmem_full[acc], (tcount >> 1) & 1u);
-      if (rec) tq1 = clock64();
-      tc_fence_after();
-      float* ypix = p.y + (int64_t)b * p.y_bstride + (int64_t)gy * p.W + gx;
-      float oc_dot = 0.f;   // fused OutConv: this pixel's dot product over all Cout activations (lane = pixel)
-      const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16) + acc * L::ACC_COLS;
-      if (p.stats) {
-        // BatchNorm batch statistics from the RAW accumulators, re-read in fragment layout (tc_common.cuh); patch pixels
-        // outside the image are masked (their stencil still sees the image edge), channels past Cout are exact zeros (TMA
-        // zero fill of the weight rows); the affine is applied to the sums analytically
-        const uint32_t vmask = __ballot_sync(0xffffffffu, pvalid);
-        const double npix = (double)__popc(vmask);
-#pragma unroll 1
-        for (int c0 = 0; c0 < N_TILE; c0 += 32) {
-          if (c0 >= p.Cout) break;
-          float s1, s2;
-          tmem_colsum32<X3 ? N_TILE : 0>(tacc + (uint32_t)c0, lane, s1, s2, vmask);
-          const int c = c0 + tmem_colsum32_col(lane);
-          if (c < p.Cout) {
-            const double sc = (double)aff[c], sh = (double)aff[L::AFF_N + c];
-            atomicAdd(p.stats + c, sc * (double)s1 + npix * sh);
-            atomicAdd(p.stats + p.Cout + c, sc * sc * (double)s2 + 2.0 * sc * sh * (double)s1 + npix * sh * sh);
-          }
-        }
-      }
-      // 16 accumulator columns per step keep the epilogue within the 104-register budget of the 608-thread CTA
-#pragma unroll 1
-      for (int c0 = 0; c0 < N_TILE; c0 += 16) {
-        if (c0 >= p.Cout) break;
-        uint32_t r[16];
-        tmem_ld16(tacc + (uint32_t)c0, r);
-        if (X3) {   // second half of the accumulator: the A_hi*B_lo term
-          uint32_t r2[16];
-          tmem_ld16(tacc + (uint32_t)(N_TILE + c0), r2);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(r2[j]));
-        }
-        float scv[16], shv[16];
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4) {
-          const float4 a = *reinterpret_cast<const float4*>(aff + c0 + 4 * j4);
-          const float4 t = *reinterpret_cast<const float4*>(aff + L::AFF_N + c0 + 4 * j4);
-          scv[4 * j4] = a.x; scv[4 * j4 + 1] = a.y; scv[4 * j4 + 2] = a.z; scv[4 * j4 + 3] = a.w;
-          shv[4 * j4] = t.x; shv[4 * j4 + 1] = t.y; shv[4 * j4 + 2] = t.z; shv[4 * j4 + 3] = t.w;
-        }
-        tmem_ld_wait();
-        const int nchn = min(16, p.Cout - c0);
-        float* yp = ypix + (int64_t)c0 * P;
-        if (p.oc_y) {
-          // channels past Cout have zero accumulators, identity affine and zero OutConv weight: no mask needed
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            const float4 w4 = *reinterpret_cast<const float4*>(aff + 2 * L::AFF_N + c0 + 4 * j4);
-            const float wv[4] = {w4.x, w4.y, w4.z, w4.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int j = 4 * j4 + e;
-              oc_dot = fmaf(fmaxf(fmaf(__uint_as_float(r[j]), scv[j], shv[j]), act_lo), wv[e], oc_dot);
-            }
-          }
-        } else if (nchn == 16) {
-          if (pvalid) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              *yp = fmaxf(fmaf(__uint_as_float(r[j]), scv[j], shv[j]), act_lo);
-              yp += P;
+          for (int kk = 0; kk < TC_BK / 8; ++kk) {
+            Wgmma<N_TILE>::ss(acc, ad0 + (uint64_t)(2 * kk), bd0 + (uint64_t)(2 * kk), 1u);
+            if (X3) {
+              Wgmma<N_TILE>::ss(acc, al0 + (uint64_t)(2 * kk), bd0 + (uint64_t)(2 * kk), 1u);
+              Wgmma<N_TILE>::ss(acc, ad0 + (uint64_t)(2 * kk), bl0 + (uint64_t)(2 * kk), 1u);
             }
           }
         } else {
 #pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (pvalid && j < nchn) yp[(int64_t)j * P] = fmaxf(fmaf(__uint_as_float(r[j]), scv[j], shv[j]), act_lo);
+        for (int kk = 0; kk < TC_BK / 8; ++kk) {
+          float vh[4], vl[4];
+          load_a_frag(ast, kk, t, m0, m1, vh);
+          if (X3) load_a_frag(ast + L::OFF_ALO, kk, t, m0, m1, vl);
+          uint32_t ahi[4], alo[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            ahi[e] = __float_as_uint(vh[e]);
+            alo[e] = X3 ? __float_as_uint(vl[e]) : 0u;
+          }
+          wgmma_fence();
+          Wgmma<N_TILE>::rs(acc, ahi, bd0 + (uint64_t)(2 * kk), 1u);
+          if (X3) {
+            Wgmma<N_TILE>::rs(acc, alo, bd0 + (uint64_t)(2 * kk), 1u);
+            Wgmma<N_TILE>::rs(acc, ahi, bl0 + (uint64_t)(2 * kk), 1u);
+          }
+        }
+        }
+        wgmma_commit();
+        wgmma_wait0();
+        wgmma_keep(acc);
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&a_empty[sa]);
+          mbar_arrive(&b_empty[sb]);
         }
       }
-      if (p.oc_y && pvalid) p.oc_y[(int64_t)b * P + (int64_t)gy * p.W + gx] = oc_dot + (p.oc_b ? __ldg(p.oc_b) : 0.f);
-      tc_fence_before();
-      mbar_arrive(&tmem_empty[acc]);
-      if (rec) {
-        atomicAdd(&g_ds_timing[9], (unsigned long long)(tq1 - tq0));
-        atomicAdd(&g_ds_timing[10], (unsigned long long)(clock64() - tq1));
-        atomicAdd(&g_ds_timing[11], 1ull);
+
+      // ----- epilogue: rows g / g + 8 are patch pixels m0 / m1, columns n0 + 8j + 2t + {0, 1}
+      const int n0 = np * N_TILE;
+      const int gy0 = ty * PH + m0 / PW, gx0 = tx * PW + m0 % PW;
+      const int gy1 = ty * PH + m1 / PW, gx1 = tx * PW + m1 % PW;
+      const bool v0 = gy0 < p.H && gx0 < p.W, v1 = gy1 < p.H && gx1 < p.W;
+      const int64_t o0 = (int64_t)gy0 * p.W + gx0, o1 = (int64_t)gy1 * p.W + gx1;
+      if (p.stats) {
+        // BatchNorm batch statistics from the RAW accumulators (one pass: Cout <= 128); patch pixels outside the image are
+        // masked (their stencil still sees the image edge), channels past Cout are exact zeros (TMA zero fill of the weight
+        // rows); the affine is applied to the sums analytically
+        const double npix = (double)((__popc(__ballot_sync(0xffffffffu, v0)) + __popc(__ballot_sync(0xffffffffu, v1))) / 4);
+#pragma unroll
+        for (int j = 0; j < N_TILE / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float a = v0 ? acc[4 * j + e] : 0.f, bb = v1 ? acc[4 * j + 2 + e] : 0.f;
+            const float s1 = frag_colsum(a + bb), s2 = frag_colsum(fmaf(a, a, bb * bb));
+            const int c = 8 * j + 2 * t + e;
+            if (lane < 4 && c < p.Cout) {
+              const double sc = (double)aff[c], sh = (double)aff[L::AFF_N + c];
+              atomicAdd(p.stats + c, sc * (double)s1 + npix * sh);
+              atomicAdd(p.stats + p.Cout + c, sc * sc * (double)s2 + 2.0 * sc * sh * (double)s1 + npix * sh * sh);
+            }
+          }
+        }
+      }
+      if (p.oc_y) {
+        // fused OutConv: each pixel's dot product over all Cout <= N_TILE activations.  Channels past Cout have zero
+        // accumulators, identity affine and zero OutConv weight: no mask needed
+        float d0 = 0.f, d1 = 0.f;
+#pragma unroll
+        for (int j = 0; j < N_TILE / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = 8 * j + 2 * t + e;
+            const float sc = aff[c], sh = aff[L::AFF_N + c], w = aff[2 * L::AFF_N + c];
+            d0 = fmaf(fmaxf(fmaf(acc[4 * j + e], sc, sh), act_lo), w, d0);
+            d1 = fmaf(fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo), w, d1);
+          }
+        }
+        d0 += __shfl_xor_sync(0xffffffffu, d0, 1);
+        d0 += __shfl_xor_sync(0xffffffffu, d0, 2);
+        d1 += __shfl_xor_sync(0xffffffffu, d1, 1);
+        d1 += __shfl_xor_sync(0xffffffffu, d1, 2);
+        const float ob = p.oc_b ? __ldg(p.oc_b) : 0.f;
+        if (t == 0) {
+          if (v0) p.oc_y[(int64_t)b * P + o0] = d0 + ob;
+          if (v1) p.oc_y[(int64_t)b * P + o1] = d1 + ob;
+        }
+      } else {
+        float* yb = p.y + (int64_t)b * p.y_bstride;
+#pragma unroll
+        for (int j = 0; j < N_TILE / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = n0 + 8 * j + 2 * t + e;
+            if (c < p.Cout) {
+              const float sc = aff[c], sh = aff[L::AFF_N + c];
+              float* yc = yb + (int64_t)c * P;
+              if (v0) yc[o0] = fmaxf(fmaf(acc[4 * j + e], sc, sh), act_lo);
+              if (v1) yc[o1] = fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo);
+            }
+          }
+        }
       }
     }
-  } else {
-    // ===== depthwise producer groups: NG groups of 4 warps (warps 6 ..), group g takes every NG-th chunk =====
-    const int g = (warp - 6) >> 2;
-    const int t = threadIdx.x - 192 - 128 * g;  // 0..127
+    return;
+  }
+
+  {
+    // ===== depthwise producer groups: NG groups of 4 warps (warps 12 ..), group g takes every NG-th chunk =====
+    const int g = (warp - L::PROD_WARP) >> 2;
+    const int t = threadIdx.x - 32 * L::PROD_WARP - 128 * g;  // 0..127
     const int Cin = p.C0 + p.C1;
     uint32_t gc = 0, iph = 0;       // iph: phase bit per input stage of this group's fill barriers
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       for (int i = 0; i < nch; ++i, ++gc) {
         if ((int)(gc % (uint32_t)L::NG) != g) continue;
         const int s = gc % IS;
-        const bool rec = (p.timing & 1) && (blockIdx.x == 0) && (t == 0) && (g == 0);
-        long long tk0 = 0, tk1 = 0, tk2 = 0;
         // depthwise weights of this thread's (first) task: issued before the ring waits so that their latency hides there
         float wr[KPL][9], br[KPL];
         auto task_channel = [&](int task) { return (PW == 32) ? (task >> 3) : (((task >> 4) << 1) | ((task >> 2) & 1)); };
@@ -411,20 +354,17 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
           }
         };
         load_weights(t);
-        if (rec) tk0 = clock64();
         mbar_wait(&in_full[s * L::NG + g], (iph >> s) & 1u);
         iph ^= 1u << s;
-        if (rec) tk1 = clock64();
         const int sa = gc % AS;
-        mbar_wait(&a_empty[sa], ((gc / AS) & 1u) ^ 1u);  // MMAs that read this A stage 3 chunks ago retired
-        if (rec) tk2 = clock64();
+        mbar_wait(&a_empty[sa], ((gc / AS) & 1u) ^ 1u);  // the MMAs that read this A stage AS chunks ago retired
         unsigned char* my_op = a_base + sa * L::AST_BYTES;
         const float* in_stage = reinterpret_cast<const float*>(smem + s * L::IN_BYTES);
 #pragma unroll 1
         for (int task = t; task < CC * 8; task += 128) {
           // task -> (input channel ci, column quad qc, row group rg).  A quarter-warp (8 lanes: one 128-bit shared-memory
           // wavefront) must touch 8 different 16-byte bank groups: PW = 32 -> the 8 quads of one channel row; PW = 16 ->
-          // the 4 quads of TWO channels (16 words apart in the input tile, and 2 k-rows apart = a different 32-byte-atom
+          // the 4 quads of TWO channels (16 words apart in the input tile, and 2 k-rows apart = a different
           // swizzle phase in the A operand).  Pairing the two row groups of one channel instead (rows 4 apart: 96 words in
           // the input tile, 4 KB in the A operand) put both halves on the same banks: every LDS.128 / STS.128 2-way.
           int ci, qc, rg;
@@ -473,6 +413,17 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
                 a = fmaf(wr[kk][6], w2[j], a); a = fmaf(wr[kk][7], w2[j + 1], a); a = fmaf(wr[kk][8], w2[j + 2], a);
                 o4[j] = a;
               }
+              if (A_SMEM) {
+                const int kr = ci * KPL + kk;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                  const uint32_t off = kmajor_offset(m + j, kr);
+                  const float h = X3 ? tf32_hi(o4[j]) : o4[j];
+                  *reinterpret_cast<float*>(my_op + off) = h;
+                  if (X3) *reinterpret_cast<float*>(my_op + L::OFF_ALO + off) = o4[j] - h;
+                }
+                continue;
+              }
               const uint32_t off = a_tile_offset(ci * KPL + kk, m);
               if (X3) {
                 const float4 h = make_float4(tf32_hi(o4[0]), tf32_hi(o4[1]), tf32_hi(o4[2]), tf32_hi(o4[3]));
@@ -484,33 +435,19 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
             }
           }
         }
-        fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor-core (async) proxy
+        if (A_SMEM) fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
         mbar_arrive(&a_full[sa]);
         mbar_arrive(&in_empty[s]);
-        if (rec) {
-          const long long tk3 = clock64();
-          atomicAdd(&g_ds_timing[0], (unsigned long long)(tk1 - tk0));
-          atomicAdd(&g_ds_timing[1], (unsigned long long)(tk2 - tk1));
-          atomicAdd(&g_ds_timing[2], (unsigned long long)(tk3 - tk2));
-          atomicAdd(&g_ds_timing[3], 1ull);
-        }
       }
     }
   }
-  __syncthreads();
-  if ((p.timing & 1) && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&g_ds_timing[12], (unsigned long long)(clock64() - t_kernel0));
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, L::TMEM_COLS);
-  }
 }
 
-template <int N_TILE, int KPL, int PW, bool X3>
+template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
 static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl, DsParams p,
                      int B, cudaStream_t st) {
   using L = DsCfg<N_TILE, KPL, PW, X3>;
-  auto kern = dsconv_fused_kernel<N_TILE, KPL, PW, X3>;
+  auto kern = dsconv_fused_kernel<N_TILE, KPL, PW, X3, A_SMEM>;
   static std::atomic<uint64_t> attr_mask{0};   // cudaFuncSetAttribute is per device
   if (first_use_on_device(attr_mask)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
@@ -518,7 +455,8 @@ static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtenso
   }
   p.tiles_x = ceil_div(p.W, PW);
   p.tiles_y = ceil_div(p.H, L::PH);
-  const int64_t total = (int64_t)B * p.tiles_x * p.tiles_y;
+  p.npass = ceil_div(p.Cout, N_TILE);
+  const int64_t total = (int64_t)B * p.tiles_x * p.tiles_y * p.npass;
   SMAAT_REQUIRE(total < (1ll << 31), "dsconv: too many tiles");
   p.total_tiles = (int)total;
   p.nchunks = ceil_div(p.C0 + p.C1, L::CC);
@@ -528,7 +466,7 @@ static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtenso
   return SMAAT_OK;
 }
 
-// patch width: 32 (PH = 4) or 16 (PH = 8), whichever wastes fewer MMA lanes; 0 = not worth fusing
+// patch width: 32 (PH = 4) or 16 (PH = 8), whichever wastes fewer MMA rows; 0 = not worth fusing
 static int pick_pw(int H, int W) {
   double best = 1e9;
   int pw = 0;
@@ -545,9 +483,10 @@ static int pick_pw(int H, int W) {
 }
 
 static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* pw_w,
-                        const float* pw_w_lo, int H, int W, int k, int Cout) {
+                        const float* pw_w_lo, int H, int W, int k, int Cout, bool stats, bool outconv) {
   if (k != 1 && k != 2) return false;
-  if (Cout > 128 || Cout < 8) return false;
+  // Cout > 128: whole passes of 128 channels; batch statistics and the fused OutConv need all channels in one pass
+  if (Cout < 8 || Cout > 512 || (Cout > 128 && (Cout % 128 != 0 || stats || outconv))) return false;
   if (W % 4 != 0 || !aligned16(x0) || bs0 % 4 != 0) return false;
   if (C1 > 0 && (!aligned16(x1) || bs1 % 4 != 0 || C0 % (TC_BK / k) != 0)) return false;
   const int K = k * (C0 + C1);
@@ -555,16 +494,11 @@ static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, i
   return pick_pw(H, W) != 0;
 }
 
-// second-generation kernel (dsconv_tmem.cu): A operand in tensor memory; k = 2, Cout <= 128, no batch statistics
-bool dsconv_tmem_eligible(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* pw_w,
-                          const float* pw_w_lo, int H, int W, int k, int Cout);
-int dsconv_tmem_run(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride, const float* dw_w,
-                    const float* dw_b, const float* pw_w, const float* pw_w_lo, const float* scale, const float* shift, float* y,
-                    int64_t y_bstride, const float* oc_w, const float* oc_b, float* oc_y, int B, int H, int W, int Cout, int relu, int mode,
-                    cudaStream_t st);
-
-// 0 = auto (TMEM-operand kernel where it applies, else the shared-memory-operand kernel), 1 = shared-memory-operand kernel only,
-// 2 = TMEM-operand kernel only (shapes it does not take are refused).  SMAAT_DS_IMPL presets it.
+// Where the A operand (the depthwise result) goes to the tensor core: 0 = auto (the register form), 1 = read by wgmma from
+// shared memory through a descriptor, 2 = loaded into registers first.  SMAAT_DS_IMPL presets it.  Auto takes the register
+// form: bench.py's B = 32, 12 x 288 x 288 forward ran at 2 365-2 369 frames/s with it and 2 187-2 194 with the shared-memory
+// form (H100 80GB HBM3 SXM, 700 W power limit, two alternated runs each); the scalar K-major stores of the shared-memory form
+// cost the producers more than the register form's fragment loads cost the consumers.
 static std::atomic<int> g_ds_impl{-1};
 static int ds_impl() {
   int v = g_ds_impl.load(std::memory_order_relaxed);
@@ -582,18 +516,14 @@ static int ds_impl() {
 using namespace smaat;
 
 extern "C" int smaat_set_dsconv_impl(int impl) {
-  SMAAT_REQUIRE(impl >= 0 && impl <= 2, "set_dsconv_impl: 0 = auto, 1 = shared-memory A operand, 2 = TMEM A operand");
+  SMAAT_REQUIRE(impl >= 0 && impl <= 2, "set_dsconv_impl: 0 = auto, 1 = A operand from shared memory, 2 = A operand from registers");
   g_ds_impl.store(impl, std::memory_order_relaxed);
   return SMAAT_OK;
 }
 
 extern "C" int smaat_dsconv_eligible2(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                                       const float* pw_w, int H, int W, int k, int Cout, int with_stats) {
-  const int impl = ds_impl();
-  // batch statistics in the epilogue exist in the shared-memory-operand kernel only
-  if (impl != 1 && !with_stats && dsconv_tmem_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, H, W, k, Cout)) return 1;
-  if (impl == 2) return 0;
-  return ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, H, W, k, Cout) ? 1 : 0;
+  return ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, H, W, k, Cout, with_stats != 0, false) ? 1 : 0;
 }
 
 extern "C" int smaat_dsconv_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
@@ -612,11 +542,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   SMAAT_REQUIRE(mode != SMAAT_PW_TF32X3 || pw_w_lo, "dsconv: TF32X3 needs pw_w_lo (see smaat_split_tf32)");
   SMAAT_REQUIRE(oc_y || y_bstride >= (int64_t)Cout * H * W, "dsconv: y batch stride too small");
   SMAAT_REQUIRE(!oc_y || (oc_w && !stats), "dsconv+outconv: needs the OutConv weight and no batch statistics");
-  const int impl = ds_impl();
-  if (impl != 1 && !stats && dsconv_tmem_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, pw_w_lo, H, W, k, Cout))
-    return dsconv_tmem_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, oc_w, oc_b, oc_y,
-                           B, H, W, Cout, relu, mode, (cudaStream_t)stream);
-  if (impl == 2 || !ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, pw_w_lo, H, W, k, Cout))
+  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, pw_w_lo, H, W, k, Cout, stats != nullptr, oc_y != nullptr))
     return fail(SMAAT_E_UNSUPPORTED, "dsconv: shape not taken by the fused kernel (k=%d Cout=%d H=%d W=%d); use dw3x3 + pw1x1", k,
                 Cout, H, W);
   cudaStream_t st = (cudaStream_t)stream;
@@ -625,6 +551,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   const int n_tile = Cout > 64 ? 128 : 64;
   const int cc = TC_BK / k;
   const bool x3 = mode == SMAAT_PW_TF32X3;
+  const bool a_smem = ds_impl() == 1;
   const int K = k * (C0 + C1);
 
   CUtensorMap m0, m1, mw, mwl;
@@ -657,14 +584,14 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   DsParams p;
   p.dw_w = dw_w; p.dw_b = dw_b; p.scale = scale; p.shift = shift; p.y = y; p.y_bstride = y_bstride; p.stats = stats;
   p.oc_w = oc_w; p.oc_b = oc_b; p.oc_y = oc_y;
-  static const int timing_on = [] { const char* e = getenv("SMAAT_DSCONV_TIMING"); return e ? atoi(e) : 0; }();
-  p.timing = timing_on;
   p.C0 = C0; p.C1 = C1; p.H = H; p.W = W; p.Cout = Cout; p.relu = relu; p.K = K;
-  p.tiles_x = p.tiles_y = p.total_tiles = p.nchunks = 0;
+  p.tiles_x = p.tiles_y = p.npass = p.total_tiles = p.nchunks = 0;
 
-#define DS_DISPATCH(NT, KP, PWv)                                                   \
-  return x3 ? launch_ds<NT, KP, PWv, true>(m0, m1, mw, mwl, p, B, st)              \
-            : launch_ds<NT, KP, PWv, false>(m0, m1, mw, mwl, p, B, st)
+#define DS_DISPATCH(NT, KP, PWv)                                                                           \
+  return x3 ? (a_smem ? launch_ds<NT, KP, PWv, true, true>(m0, m1, mw, mwl, p, B, st)                       \
+                      : launch_ds<NT, KP, PWv, true, false>(m0, m1, mw, mwl, p, B, st))                     \
+            : (a_smem ? launch_ds<NT, KP, PWv, false, true>(m0, m1, mw, mwl, p, B, st)                      \
+                      : launch_ds<NT, KP, PWv, false, false>(m0, m1, mw, mwl, p, B, st))
   if (n_tile == 64) {
     if (k == 2) { if (pw == 32) { DS_DISPATCH(64, 2, 32); } else { DS_DISPATCH(64, 2, 16); } }
     else        { if (pw == 32) { DS_DISPATCH(64, 1, 32); } else { DS_DISPATCH(64, 1, 16); } }
@@ -685,8 +612,8 @@ extern "C" int smaat_dsconv_fwd(const float* x0, int C0, int64_t x0_bstride, con
 }
 
 /* The network's last two modules in one kernel: DS conv -> BN/ReLU -> OutConv(Cout -> 1) (reference models/SmaAt_UNet.py:55-56,
- * unet_parts.py:67-73).  The Cout-channel activation never reaches HBM: each epilogue thread owns one pixel's Cout values
- * (TMEM lane = pixel) and reduces them against oc_w.  logits: (B, 1, H, W). */
+ * unet_parts.py:67-73).  The Cout-channel activation never reaches HBM: the four lanes of a fragment group hold one pixel's
+ * Cout <= 128 accumulators and reduce them against oc_w.  logits: (B, 1, H, W). */
 extern "C" int smaat_dsconv_outconv_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                                         const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
                                         const float* scale, const float* shift, const float* oc_w, const float* oc_b,
@@ -694,16 +621,4 @@ extern "C" int smaat_dsconv_outconv_fwd(const float* x0, int C0, int64_t x0_bstr
   SMAAT_REQUIRE(oc_w && logits, "dsconv+outconv: null pointer");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
                     logits, B, H, W, k, Cout, relu, mode, stream);
-}
-
-/* Debug hook: copies the fused kernel's stage timers of CTA 0 (16 counters, clock64 cycles; layout in dsconv_fused.cu)
- * to `out` and clears them.  Synchronises the device. */
-extern "C" int smaat_debug_dsconv_timing(unsigned long long* out) {
-  SMAAT_REQUIRE(out, "debug_dsconv_timing: null pointer");
-  cudaError_t e = cudaMemcpyFromSymbol(out, g_ds_timing, sizeof(g_ds_timing));
-  if (e != cudaSuccess) return fail(SMAAT_E_CUDA, "debug_dsconv_timing: %s", cudaGetErrorString(e));
-  unsigned long long z[16] = {0};
-  e = cudaMemcpyToSymbol(g_ds_timing, z, sizeof(z));
-  if (e != cudaSuccess) return fail(SMAAT_E_CUDA, "debug_dsconv_timing: %s", cudaGetErrorString(e));
-  return SMAAT_OK;
 }

@@ -1,5 +1,5 @@
 // pw1x1.cu -- C-ABI entry for the pointwise 1x1 conv: validates, then routes to the exact
-// CUDA-core GEMM (pw1x1_simt.cu) or the tcgen05 tensor-core GEMM (pw1x1_tc.cu).
+// CUDA-core GEMM (pw1x1_simt.cu) or the wgmma tensor-core GEMM (pw1x1_tc.cu).
 #include "common.cuh"
 
 namespace smaat {
@@ -31,7 +31,7 @@ extern "C" int smaat_pw1x1_fwd(const float* x, const float* w, const float* w_lo
   }
 }
 
-/* 1 if (x, w, K, Cout, P) can take the tcgen05 path, else 0 (caller then uses SMAAT_PW_FP32_SIMT). */
+/* 1 if (x, w, K, Cout, P) can take the tensor-core path, else 0 (caller then uses SMAAT_PW_FP32_SIMT). */
 extern "C" int smaat_pw1x1_tc_eligible(const float* x, const float* w, int K, int Cout, int P) {
   return pw1x1_tc_eligible(x, w, nullptr, K, Cout, P) ? 1 : 0;
 }

@@ -4,7 +4,7 @@
 // Replaces DepthwiseSeparableConv.pointwise + eval BatchNorm2d + ReLU
 // (reference models/layers.py:45,49; parts_ds.py:25-26,34-35) in SMAAT_PW_FP32_SIMT mode.
 // This is the exact-product path: the strict-tolerance parity anchor on the GPU, and the
-// kernel for shapes the tcgen05 path does not take (P % 4 != 0, K % 4 != 0).  The fast path
+// kernel for shapes the tensor-core path does not take (P % 4 != 0, K % 4 != 0).  The fast path
 // is pw1x1_tc.cu.  Per image: Y[Cout x P] = W[Cout x K] * X[K x P].
 #include "common.cuh"
 

@@ -1,39 +1,28 @@
-// pw1x1_tc.cu -- pointwise 1x1 conv on the 5th-gen tensor cores (tcgen05, TMEM accumulators),
-// fused with the per-channel affine (+ReLU) epilogue and optional BatchNorm statistics.
+// pw1x1_tc.cu -- pointwise 1x1 conv on the Hopper tensor cores (wgmma, tf32, fp32 accumulate in registers), fused with the
+// per-channel affine (+ReLU) epilogue and optional BatchNorm statistics.
 //
 // Replaces DepthwiseSeparableConv.pointwise + eval BatchNorm2d + ReLU
 // (reference models/layers.py:45,49; parts_ds.py:25-26,34-35): the only dense contraction
 // on the SmaAt-UNet forward path.
 //
 // Mapping (per image b):  D[128 pixels x N_TILE channels] += A[128 px x 8] * B[N_TILE x 8]^T
-//   A = activations X[b] ([K][P], pixels contiguous)  -> "MN-major" smem operand: the NCHW
-//       tensor is consumed as it lies in HBM, no transpose.  TMA boxes of 32 k-rows x 32 px
-//       (4 boxes = 128 pixels) with the 128B-span / 32B-atom swizzle, the only swizzled layout
-//       the hardware takes for MN-major 32-bit operands (UMMA layout type SWIZZLE_128B_BASE32B);
-//   B = weights W ([Cout][K], K contiguous)           -> K-major operand, one TMA box
-//       of N_TILE rows x 32 k with the plain 128B swizzle;
-//   D in TMEM: lane = pixel, column = output channel, so tcgen05.ld.32x32b hands every warp
-//       32 consecutive pixels of one channel per register -> fully coalesced NCHW stores with
-//       no smem staging.  kind::tf32, fp32 accumulate.
-// TF32X3 mode (fp32-grade accuracy): activations are split in smem into a tf32 "hi" part and
-// the "lo" remainder by 4 transform warps; weights arrive pre-split; three MMAs
-// (hi*hi + lo*hi + hi*lo) per k-step accumulate into the same TMEM tile.
+//   A = activations X[b] ([K][P], pixels contiguous): consumed as it lies in HBM, no transpose.  TMA boxes of 32 k-rows x
+//       32 px (4 boxes = 128 pixels) with the 128-byte swizzle; each consumer thread loads its A fragment into registers
+//       (tf32 wgmma reads only K-major operands from shared memory, this one is MN-major) -- conflict-free, see tc_common.cuh;
+//   B = weights W ([Cout][K], K contiguous) -> K-major SW128 operand, one TMA box of N_TILE rows x 32 k;
+//   D in registers of two consumer warpgroups (64 pixels each).
+// TF32X3 mode (fp32-grade accuracy): the activations are split into a tf32 "hi" part and the "lo" remainder in registers,
+// the weights arrive pre-split; three MMAs (hi*hi + lo*hi + hi*lo) per k-step accumulate into the same registers.
 //
-// Persistent, warp-specialised: one CTA per SM loops over output tiles (tile = blockIdx.x +
-// i*gridDim.x; consecutive tiles share the activation tile and differ in the channel tile so the
-// re-read hits L2).  warp 0 = TMA producer (runs ahead across tile boundaries through a
-// STAGES-deep smem ring), warp 1 = TMEM alloc + MMA issuer (one elected lane), warps 2-5 =
-// epilogue (warp w owns TMEM lanes 32*(w%4)..+31), warps 6-9 = hi/lo transform (X3 only).
-// Two accumulator stages in TMEM (2 x N_TILE columns) let the epilogue of tile i overlap the
-// MMAs of tile i+1.  mbarriers: full/empty per smem stage, xform per stage (X3),
-// tmem_full/tmem_empty per accumulator stage; tcgen05.commit releases smem stages and
-// publishes finished accumulators.
+// Persistent: one CTA per SM loops over output tiles (tile = blockIdx.x + i*gridDim.x; consecutive tiles share the activation
+// tile and differ in the channel tile, so the re-read hits L2).  Warp 0 = TMA producer, running ahead across tile boundaries
+// through a STAGES-deep shared-memory ring, so the loads of the next tile overlap the epilogue of this one; warpgroups 1-2 =
+// MMA + epilogue.  mbarriers: full (TMA bytes) / empty (8 consumer warps done reading) per stage.
 #include <stdlib.h>
 
 #include "tc_common.cuh"
 
 namespace smaat {
-
 
 struct PwTcParams {
   const float* scale;
@@ -45,57 +34,35 @@ struct PwTcParams {
   int tiles_m, tiles_n, total_tiles;
 };
 
-// ATM (TF32X3, N_TILE = 256 only): the hi / lo split of the activations is written to TENSOR MEMORY (tcgen05.st, lane = pixel)
-// and the MMAs take their A operand from TMEM: per k-chunk that removes the 32 KB the split wrote to shared memory and the
-// 48 KB the three MMA passes read back (272 -> 192 KB through the 128 B/clk port, which bounded this shape at 65 % tensor-pipe
-// activity in round 1).  TMEM: one 256-column accumulator + a 4-stage A ring of 64 columns (hi | lo).
-template <int N_TILE, int STAGES, bool X3, bool ATM = false>
+template <int N_TILE, int STAGES, bool X3>
 struct PwTcCfg {
-  static_assert(!ATM || (X3 && N_TILE == 256), "A-operand-in-TMEM variant: TF32X3, N_TILE = 256");
   static constexpr int A_BYTES = TC_BM * TC_BK * 4;   // 16 KB: 4 blocks x (32 k-rows x 128 B)
   static constexpr int B_BYTES = N_TILE * TC_BK * 4;  // N_TILE rows x 128 B
-  static constexpr int STAGE_BYTES = ATM ? (A_BYTES + 2 * B_BYTES) : (X3 ? 2 : 1) * (A_BYTES + B_BYTES);
-  static constexpr int OFF_ALO = A_BYTES;  // X3 only
-  static constexpr int OFF_B = (X3 && !ATM ? 2 : 1) * A_BYTES;
-  static constexpr int OFF_BLO = OFF_B + B_BYTES;  // X3 only
-  static constexpr int AT_STAGES = 4, AT_COLS = 64;   // ATM: TMEM A ring
-  static constexpr int BAR_BYTES = 512;
+  static constexpr int STAGE_BYTES = A_BYTES + (X3 ? 2 : 1) * B_BYTES;
+  static constexpr int OFF_B = A_BYTES;
+  static constexpr int OFF_BLO = A_BYTES + B_BYTES;  // X3 only
+  static constexpr int BAR_BYTES = 256;
   static constexpr int AFF_N = 512;                                      // per-channel epilogue affine staged in smem
-  static constexpr int SACC_BYTES = 4 * 2 * N_TILE * 8;                  // per-epilogue-warp fp64 BatchNorm partial sums
+  static constexpr int SACC_BYTES = 8 * 2 * N_TILE * 8;                  // per-consumer-warp fp64 BatchNorm partial sums
   static constexpr int TOTAL = STAGES * STAGE_BYTES + BAR_BYTES + 2 * AFF_N * 4 + SACC_BYTES + 1024;  // + alignment slack
   static constexpr uint32_t TX_BYTES = A_BYTES + (X3 ? 2 : 1) * B_BYTES;
-  static constexpr int THREADS = X3 ? 320 : 192;
-  // TF32X3 with N_TILE <= 128: the stage holds the weight rows as [hi | lo] contiguously, so one N = 2*N_TILE MMA computes
-  // A_hi*[B_hi | B_lo] into 2*N_TILE accumulator columns and a second N = N_TILE MMA adds A_lo*B_hi to the first half --
-  // 2 instead of 3 MMAs per k-step (every MMA re-reads its 4 KB A slice from shared memory whatever N is); the epilogue
-  // adds the two halves.  N_TILE = 256 keeps three MMAs (an accumulator stage is limited to 256 of the 512 columns).
-  static constexpr bool WIDE = X3 && N_TILE <= 128;
-  static constexpr int ACC_COLS = WIDE ? 2 * N_TILE : N_TILE;
-  static constexpr int ACC_STAGES = ATM ? 1 : 2;
-  static constexpr int TMEM_COLS = ATM ? 512 : 2 * ACC_COLS;  // two accumulator stages (ATM: one + the A ring)
-  static_assert(TMEM_COLS <= 512 && (TMEM_COLS & (TMEM_COLS - 1)) == 0, "TMEM allocation must be a power of two <= 512");
+  static constexpr int THREADS = 384;
   static_assert(TOTAL <= 227 * 1024, "shared memory budget");
 };
 
-template <int N_TILE, int STAGES, bool X3, bool ATM = false>
-__global__ void __launch_bounds__(PwTcCfg<N_TILE, STAGES, X3, ATM>::THREADS, 1)
+template <int N_TILE, int STAGES, bool X3>
+__global__ void __launch_bounds__(384, 1)
     pw1x1_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
                     const __grid_constant__ CUtensorMap map_wlo, const PwTcParams p) {
-  using L = PwTcCfg<N_TILE, STAGES, X3, ATM>;
+  using L = PwTcCfg<N_TILE, STAGES, X3>;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
-  // 1 KB alignment: swizzle atoms (8 x 128 B for the weights, 4 x 128 B for the activations).  Offset arithmetic
-  // on the __shared__ array (not a uintptr_t round trip) keeps the accesses LDS/STS instead of generic LD/ST.
+  // 1 KB alignment: 128-byte swizzle atoms.  Offset arithmetic on the __shared__ array (not a uintptr_t round trip) keeps the
+  // accesses LDS/STS instead of generic LD/ST.
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * L::STAGE_BYTES);
   float* aff = reinterpret_cast<float*>(smem + STAGES * L::STAGE_BYTES + L::BAR_BYTES);  // [2][AFF_N] scale | shift
-  uint64_t* full_bar = bars;                         // [STAGES] TMA bytes landed
-  uint64_t* empty_bar = bars + STAGES;               // [STAGES] MMAs that read the stage retired
-  uint64_t* xform_bar = bars + 2 * STAGES;           // [STAGES] hi/lo split done (X3)
-  uint64_t* tmem_full_bar = bars + 3 * STAGES;       // [2] accumulator complete
-  uint64_t* tmem_empty_bar = bars + 3 * STAGES + 2;  // [2] accumulator drained by the epilogue
-  uint64_t* ta_full = bars + 3 * STAGES + 4;         // [AT_STAGES] ATM: hi/lo split of a chunk is in TMEM (128 arrivals)
-  uint64_t* ta_empty = ta_full + L::AT_STAGES;       // [AT_STAGES] ATM: the MMAs reading it retired
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(ta_empty + L::AT_STAGES);
+  uint64_t* full_bar = bars;            // [STAGES] TMA bytes landed
+  uint64_t* empty_bar = bars + STAGES;  // [STAGES] the 8 consumer warps finished with the stage
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler too
   const int lane = threadIdx.x & 31;
@@ -107,35 +74,17 @@ __global__ void __launch_bounds__(PwTcCfg<N_TILE, STAGES, X3, ATM>::THREADS, 1)
     if (X3) tma_prefetch_desc(&map_wlo);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], ATM ? 129 : 1);       // ATM: the MMAs' commit (weights) + the 128 split threads (activations)
-      mbar_init(&xform_bar[s], 128);
-    }
-    for (int s = 0; s < L::AT_STAGES; ++s) {
-      mbar_init(&ta_full[s], 128);
-      mbar_init(&ta_empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full_bar[a], 1);
-      mbar_init(&tmem_empty_bar[a], 128);
+      mbar_init(&empty_bar[s], 8);
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)),
-                 "r"((uint32_t)L::TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   // epilogue affine of the channels this CTA can touch (padded with identity; all-identity when no affine is given,
-  // which is why indices may wrap for Cout > AFF_N), read back as LDS.128 broadcasts
+  // which is why indices may wrap for Cout > AFF_N)
   for (int c = threadIdx.x; c < L::AFF_N; c += blockDim.x) {
     aff[c] = (c < p.Cout && p.scale) ? __ldg(p.scale + c) : 1.f;
     aff[L::AFF_N + c] = (c < p.Cout && p.shift) ? __ldg(p.shift + c) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   if (warp == 0) {
     // ===== TMA producer =====
@@ -161,266 +110,130 @@ __global__ void __launch_bounds__(PwTcCfg<N_TILE, STAGES, X3, ATM>::THREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer: the whole warp walks the loop (warp-uniform control flow, descriptors in uniform registers), one
-    // elected lane issues; descriptors are built once per stage and advanced by constant adds per k-step =====
-    constexpr uint32_t idesc = make_idesc_tf32(N_TILE);
-    constexpr uint32_t idesc_wide = make_idesc_tf32(L::WIDE ? 2 * N_TILE : N_TILE);
-    constexpr uint32_t idesc_ts = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N_TILE >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-    uint32_t it = 0, tcount = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++tcount) {
-      const uint32_t acc = ATM ? 0u : (tcount & 1u);
-      const uint32_t acc_ph = ATM ? (tcount & 1u) : ((tcount >> 1) & 1u);
-      mbar_wait(&tmem_empty_bar[acc], acc_ph ^ 1u);  // epilogue has drained this accumulator stage
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * L::ACC_COLS;
-      for (int i = 0; i < nk; ++i, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1u;
-        if (ATM) {
-          const int ts = it % L::AT_STAGES;
-          mbar_wait(&full_bar[s], ph);                               // weights of this chunk landed
-          mbar_wait(&ta_full[ts], (it / L::AT_STAGES) & 1u);         // activations split into TMEM
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
-            const uint64_t bd0 = make_smem_desc(a_addr + L::OFF_B, 16, 1024, LAYOUT_SW128);
-            const uint64_t bl0 = make_smem_desc(a_addr + L::OFF_BLO, 16, 1024, LAYOUT_SW128);
-            const uint32_t a_hi = tmem_base + (uint32_t)L::ACC_COLS + (uint32_t)(ts * L::AT_COLS);
-            const int kc = min(TC_BK, p.K - i * TC_BK);
-            const int nmma = (kc + 7) >> 3;
-            auto tstep = [&](int kk) {
-              const uint32_t accum = (i > 0 || kk > 0) ? 1u : 0u;
-              const uint64_t bd = bd0 + (uint64_t)(kk * 2), bl = bl0 + (uint64_t)(kk * 2);
-              asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem), "r"(a_hi + 8u * kk), "l"(bd), "r"(idesc_ts), "r"(accum) : "memory");
-              asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem), "r"(a_hi + 32u + 8u * kk), "l"(bd), "r"(idesc_ts), "r"(1u) : "memory");
-              asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem), "r"(a_hi + 8u * kk), "l"(bl), "r"(idesc_ts), "r"(1u) : "memory");
-            };
-            if (nmma == TC_BK / 8) {
-#pragma unroll
-              for (int kk = 0; kk < TC_BK / 8; ++kk) tstep(kk);
-            } else {
-              for (int kk = 0; kk < nmma; ++kk) tstep(kk);
-            }
-            umma_commit(&empty_bar[s]);
-            umma_commit(&ta_empty[ts]);
-            if (i == nk - 1) umma_commit(&tmem_full_bar[acc]);
-          }
-          __syncwarp();
-          continue;
-        }
-        mbar_wait(X3 ? &xform_bar[s] : &full_bar[s], ph);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
-          // A (MN-major tf32, SW128 with 32 B atoms): one k-row = 128 B of pixels; 4-row swizzle groups 512 B apart (SBO),
-          // 8 k-rows per MMA = +1 KB per k-step (+64 in the descriptor's >>4 address field); 32-pixel blocks 4 KB apart (LBO)
-          const uint64_t ad0 = make_smem_desc(a_addr, TC_BK * 128, 512, LAYOUT_SW128_BASE32B);
-          const uint64_t al0 = make_smem_desc(a_addr + L::OFF_ALO, TC_BK * 128, 512, LAYOUT_SW128_BASE32B);
-          // B (K-major, SW128): 8 tf32 = 32 B along the swizzled 128 B row (+2 per k-step); 8-row groups 1 KB apart (SBO)
-          const uint64_t bd0 = make_smem_desc(a_addr + L::OFF_B, 16, 1024, LAYOUT_SW128);
-          const uint64_t bl0 = make_smem_desc(a_addr + L::OFF_BLO, 16, 1024, LAYOUT_SW128);
-          const int kc = min(TC_BK, p.K - i * TC_BK);
-          auto step = [&](int kk, uint32_t accum) {
-            const uint64_t ad = ad0 + (uint64_t)(kk * 64), bd = bd0 + (uint64_t)(kk * 2);
-            if (L::WIDE) {
-              umma_tf32(d_tmem, ad, bd, idesc_wide, accum);                       // A_hi * [B_hi | B_lo]
-              umma_tf32(d_tmem, al0 + (uint64_t)(kk * 64), bd, idesc, 1u);         // A_lo * B_hi
-            } else {
-              umma_tf32(d_tmem, ad, bd, idesc, accum);
-              if (X3) {
-                umma_tf32(d_tmem, al0 + (uint64_t)(kk * 64), bd, idesc, 1u);
-                umma_tf32(d_tmem, ad, bl0 + (uint64_t)(kk * 2), idesc, 1u);
-              }
-            }
-          };
-          if (kc == TC_BK) {
-#pragma unroll
-            for (int kk = 0; kk < TC_BK / 8; ++kk) step(kk, (kk > 0) ? 1u : (i > 0 ? 1u : 0u));
-          } else {
-            const int nmma = (kc + 7) >> 3;
-            for (int kk = 0; kk < nmma; ++kk) step(kk, (i > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[s]);  // implicit tcgen05.fence::before_thread_sync
-          if (i == nk - 1) umma_commit(&tmem_full_bar[acc]);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 6) {
-    // ===== epilogue warps 2..5: TMEM -> registers -> affine/ReLU -> coalesced NCHW stores =====
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const float act_lo = p.relu ? 0.f : -INFINITY;  // ReLU as a branch-free max()
-    // BatchNorm batch statistics: this warp's fp64 partial sums [2][N_TILE] live in shared memory across the CTA's
-    // tiles (lane j owns columns j, j+32, ...: no atomics, no sync) and reach HBM once per n-tile change / at the end
-    double* sacc = reinterpret_cast<double*>(smem + STAGES * L::STAGE_BYTES + L::BAR_BYTES + 2 * L::AFF_N * 4) + q * 2 * N_TILE;
-    int stat_n0 = -1;
-    if (p.stats) {
-      for (int c = lane; c < 2 * N_TILE; c += 32) sacc[c] = 0.0;
-      __syncwarp();
-    }
-    double stat_npix = 0.0;   // valid pixels this warp has accumulated since the last flush (warp-uniform)
-    auto flush_stats = [&](int n0f) {
-      __syncwarp();
-      for (int c = lane; c < N_TILE; c += 32) {
-        if (n0f + c < p.Cout) {
-          // z = sc * acc + sh:  sum z = sc*S1 + n*sh,  sum z^2 = sc^2*S2 + 2*sc*sh*S1 + n*sh^2
-          const double sc = (double)aff[(n0f + c) & (L::AFF_N - 1)], sh = (double)aff[L::AFF_N + ((n0f + c) & (L::AFF_N - 1))];
-          const double S1 = sacc[c], S2 = sacc[N_TILE + c];
-          atomicAdd(p.stats + n0f + c, sc * S1 + stat_npix * sh);
-          atomicAdd(p.stats + p.Cout + n0f + c, sc * sc * S2 + 2.0 * sc * sh * S1 + stat_npix * sh * sh);
-        }
-        sacc[c] = 0.0;
-        sacc[N_TILE + c] = 0.0;
-      }
-      stat_npix = 0.0;
-      __syncwarp();
-    };
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++tcount) {
-      const int tn = tile % p.tiles_n;
-      const int rest = tile / p.tiles_n;
-      const int tm = rest % p.tiles_m;
-      const int b = rest / p.tiles_m;
-      const int n0 = tn * N_TILE;
-      if (p.stats && n0 != stat_n0) {
-        if (stat_n0 >= 0) flush_stats(stat_n0);
-        stat_n0 = n0;
-      }
-      const uint32_t acc = ATM ? 0u : (tcount & 1u);
-      const uint32_t acc_ph = ATM ? (tcount & 1u) : ((tcount >> 1) & 1u);
-      mbar_wait(&tmem_full_bar[acc], acc_ph);
-      tc_fence_after();
-      const int pix = tm * TC_BM + q * 32 + lane;
-      const bool pvalid = pix < p.P;
-      float* ypix = p.y + (int64_t)b * p.y_bstride + pix;
-#pragma unroll 1
-      for (int c0 = 0; c0 < N_TILE; c0 += 32) {
-        if (n0 + c0 >= p.Cout) break;
-        uint32_t r[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * L::ACC_COLS + (uint32_t)c0;
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-              "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-              "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-              "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-            : "r"(taddr));
-        float scv[32], shv[32];
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          const float4 a = *reinterpret_cast<const float4*>(aff + ((n0 + c0 + 4 * j4) & (L::AFF_N - 1)));
-          const float4 t = *reinterpret_cast<const float4*>(aff + L::AFF_N + ((n0 + c0 + 4 * j4) & (L::AFF_N - 1)));
-          scv[4 * j4] = a.x; scv[4 * j4 + 1] = a.y; scv[4 * j4 + 2] = a.z; scv[4 * j4 + 3] = a.w;
-          shv[4 * j4] = t.x; shv[4 * j4 + 1] = t.y; shv[4 * j4 + 2] = t.z; shv[4 * j4 + 3] = t.w;
-        }
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (L::WIDE) {   // second half of the accumulator: the A_hi*B_lo term
-          uint32_t r2[32];
-          tmem_ld32(taddr + N_TILE, r2);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(r2[j]));
-        }
-        const int nch = min(32, p.Cout - (n0 + c0));  // warp-uniform
-        float* yp = ypix + (int64_t)(n0 + c0) * p.P;
-        if (nch == 32) {
-          // hot path: 5 instructions per channel (FFMA, FMNMX, 64-bit pointer bump, predicated STG), no branches
-          if (pvalid) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              *yp = fmaxf(fmaf(__uint_as_float(r[j]), scv[j], shv[j]), act_lo);
-              yp += p.P;
-            }
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (pvalid && j < nch) yp[(int64_t)j * p.P] = fmaxf(fmaf(__uint_as_float(r[j]), scv[j], shv[j]), act_lo);
-        }
-        if (p.stats) {
-          // BatchNorm batch statistics from the RAW accumulators, re-read from TMEM in fragment layout (several pixels per
-          // thread: 14 shuffles per 32 channels).  Pixels past P and channels past Cout are exact zeros (TMA zero fill),
-          // so no masks; the epilogue affine is applied analytically when the sums are flushed.
-          float s1, s2;
-          tmem_colsum32<L::WIDE ? N_TILE : 0>(taddr, lane, s1, s2);
-          const int col = c0 + tmem_colsum32_col(lane);
-          sacc[col] += (double)s1;
-          sacc[N_TILE + col] += (double)s2;
-        }
-      }
-      if (p.stats) stat_npix += (double)max(0, min(32, p.P - (tm * TC_BM + q * 32)));
-      tc_fence_before();
-      mbar_arrive(&tmem_empty_bar[acc]);  // 128 arrivals release the accumulator stage to the MMA warp
-    }
-    if (p.stats && stat_n0 >= 0) flush_stats(stat_n0);
-  } else if (X3) {
-    // ===== warps 6..9: split the landed activations into tf32 hi (in place) and lo =====
-    const int et = threadIdx.x - 192;  // 0..127
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      for (int i = 0; i < nk; ++i, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1u;
-        mbar_wait(&full_bar[s], ph);
-        if (ATM) {
-          // thread = pixel = TMEM lane 32 q + lane (q = warp % 4: the lane quarter this warp may write); its 32 k values sit in
-          // the MN-major tile at a_tile_offset(k, m): for a fixed k the warp reads one 128-byte row -- conflict-free
-          const int q = warp & 3, m = q * 32 + lane;
-          const unsigned char* at = smem + s * L::STAGE_BYTES;
-          uint32_t hi[32], lo[32];
-#pragma unroll
-          for (int k = 0; k < 32; ++k) {
-            const float v = *reinterpret_cast<const float*>(at + a_tile_offset(k, m));
-            const float h = tf32_hi(v);
-            hi[k] = __float_as_uint(h);
-            lo[k] = __float_as_uint(v - h);
-          }
-          mbar_arrive(&empty_bar[s]);                      // the activations of this stage are in registers
-          const int ts = it % L::AT_STAGES;
-          mbar_wait(&ta_empty[ts], ((it / L::AT_STAGES) & 1u) ^ 1u);
-          tc_fence_after();
-          const uint32_t t0 = tmem_base + (uint32_t)L::ACC_COLS + (uint32_t)(ts * L::AT_COLS) + ((uint32_t)(q * 32) << 16);
-          tmem_st32(t0, hi);
-          tmem_st32(t0 + 32u, lo);
-          asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-          tc_fence_before();
-          mbar_arrive(&ta_full[ts]);
-          continue;
-        }
-        float4* a4 = reinterpret_cast<float4*>(smem + s * L::STAGE_BYTES);
-        float4* l4 = reinterpret_cast<float4*>(smem + s * L::STAGE_BYTES + L::OFF_ALO);
-#pragma unroll
-        for (int itx = 0; itx < L::A_BYTES / 16 / 128; ++itx) {
-          const int idx = et + itx * 128;
-          const float4 v = a4[idx];
-          float4 h, l;
-          h.x = __uint_as_float(__float_as_uint(v.x) & 0xffffe000u);
-          h.y = __uint_as_float(__float_as_uint(v.y) & 0xffffe000u);
-          h.z = __uint_as_float(__float_as_uint(v.z) & 0xffffe000u);
-          h.w = __uint_as_float(__float_as_uint(v.w) & 0xffffe000u);
-          l.x = v.x - h.x; l.y = v.y - h.y; l.z = v.z - h.z; l.w = v.w - h.w;
-          a4[idx] = h;
-          l4[idx] = l;
-        }
-        fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor-core (async) proxy
-        mbar_arrive(&xform_bar[s]);
-      }
-    }
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
+  if (warp < 4) return;
+
+  // ===== consumer warpgroups 1, 2: MMAs into register accumulators, then affine/ReLU -> NCHW stores =====
+  const int wg = (warp >> 2) - 1, wq = warp & 3, cw = warp - 4;   // cw: consumer warp 0..7
+  const int g = lane >> 2, t = lane & 3;
+  const int m0 = tc_row_pixel(wg, wq, 0, g), m1 = tc_row_pixel(wg, wq, 1, g);
+  const float act_lo = p.relu ? 0.f : -INFINITY;  // ReLU as a branch-free max()
+  // BatchNorm batch statistics: this warp's fp64 partial sums [2][N_TILE] live in shared memory across the CTA's tiles
+  // (lanes 0..3 own the columns of their fragment group: no atomics) and reach HBM once per n-tile change / at the end
+  double* sacc = reinterpret_cast<double*>(smem + STAGES * L::STAGE_BYTES + L::BAR_BYTES + 2 * L::AFF_N * 4) + cw * 2 * N_TILE;
+  int stat_n0 = -1;
+  if (p.stats) {
+    for (int c = lane; c < 2 * N_TILE; c += 32) sacc[c] = 0.0;
     __syncwarp();
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)L::TMEM_COLS) : "memory");
   }
+  double stat_npix = 0.0;   // valid pixels this warp has accumulated since the last flush (warp-uniform)
+  auto flush_stats = [&](int n0f) {
+    __syncwarp();
+    for (int c = lane; c < N_TILE; c += 32) {
+      if (n0f + c < p.Cout) {
+        // z = sc * acc + sh:  sum z = sc*S1 + n*sh,  sum z^2 = sc^2*S2 + 2*sc*sh*S1 + n*sh^2
+        const double sc = (double)aff[(n0f + c) & (L::AFF_N - 1)], sh = (double)aff[L::AFF_N + ((n0f + c) & (L::AFF_N - 1))];
+        const double S1 = sacc[c], S2 = sacc[N_TILE + c];
+        atomicAdd(p.stats + n0f + c, sc * S1 + stat_npix * sh);
+        atomicAdd(p.stats + p.Cout + n0f + c, sc * sc * S2 + 2.0 * sc * sh * S1 + stat_npix * sh * sh);
+      }
+      sacc[c] = 0.0;
+      sacc[N_TILE + c] = 0.0;
+    }
+    stat_npix = 0.0;
+    __syncwarp();
+  };
+
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    const int tn = tile % p.tiles_n;
+    const int rest = tile / p.tiles_n;
+    const int tm = rest % p.tiles_m;
+    const int b = rest / p.tiles_m;
+    const int n0 = tn * N_TILE;
+    if (p.stats && n0 != stat_n0) {
+      if (stat_n0 >= 0) flush_stats(stat_n0);
+      stat_n0 = n0;
+    }
+    float acc[N_TILE / 2];
+#pragma unroll
+    for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < nk; ++i, ++it) {
+      const int s = it % STAGES;
+      mbar_wait(&full_bar[s], (it / STAGES) & 1u);
+      const unsigned char* st = smem + s * L::STAGE_BYTES;
+      const uint64_t bd0 = make_kmajor_desc(smem_u32(st + L::OFF_B));
+      const uint64_t bl0 = make_kmajor_desc(smem_u32(st + L::OFF_BLO));
+#pragma unroll
+      for (int kk = 0; kk < TC_BK / 8; ++kk) {
+        float v[4];
+        load_a_frag(st, kk, t, m0, m1, v);
+        uint32_t ahi[4], alo[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float h = X3 ? tf32_hi(v[e]) : v[e];
+          ahi[e] = __float_as_uint(h);
+          alo[e] = __float_as_uint(v[e] - h);
+        }
+        wgmma_fence();
+        Wgmma<N_TILE>::rs(acc, ahi, bd0 + (uint64_t)(2 * kk), 1u);
+        if (X3) {
+          Wgmma<N_TILE>::rs(acc, alo, bd0 + (uint64_t)(2 * kk), 1u);
+          Wgmma<N_TILE>::rs(acc, ahi, bl0 + (uint64_t)(2 * kk), 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait0();
+      wgmma_keep(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[s]);
+    }
+
+    // ----- epilogue: rows g / g + 8 are pixels m0 / m1, columns n0 + 8j + 2t + {0, 1}
+    const int pix0 = tm * TC_BM + m0, pix1 = tm * TC_BM + m1;
+    const bool v0 = pix0 < p.P, v1 = pix1 < p.P;
+    float* yb = p.y + (int64_t)b * p.y_bstride;
+#pragma unroll
+    for (int j = 0; j < N_TILE / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int c = n0 + 8 * j + 2 * t + e;
+        if (c < p.Cout) {
+          const float sc = aff[c & (L::AFF_N - 1)], sh = aff[L::AFF_N + (c & (L::AFF_N - 1))];
+          float* yc = yb + (int64_t)c * p.P;
+          if (v0) yc[pix0] = fmaxf(fmaf(acc[4 * j + e], sc, sh), act_lo);
+          if (v1) yc[pix1] = fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo);
+        }
+      }
+    }
+    if (p.stats) {
+      // BatchNorm batch statistics from the RAW accumulators.  Pixels past P and channels past Cout are exact zeros (TMA zero
+      // fill), so no masks; the epilogue affine is applied analytically when the sums are flushed.
+#pragma unroll
+      for (int j = 0; j < N_TILE / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float a = acc[4 * j + e], bb = acc[4 * j + 2 + e];
+          const float s1 = frag_colsum(a + bb), s2 = frag_colsum(fmaf(a, a, bb * bb));
+          if (lane < 4) {
+            const int col = 8 * j + 2 * t + e;
+            sacc[col] += (double)s1;
+            sacc[N_TILE + col] += (double)s2;
+          }
+        }
+      }
+      const int nv = __popc(__ballot_sync(0xffffffffu, v0)) + __popc(__ballot_sync(0xffffffffu, v1));
+      stat_npix += (double)(nv / 4);   // each pixel row is held by the 4 lanes of its fragment group
+    }
+  }
+  if (p.stats && stat_n0 >= 0) flush_stats(stat_n0);
 }
 
-template <int N_TILE, int STAGES, bool X3, bool ATM = false>
+template <int N_TILE, int STAGES, bool X3>
 static int launch_tc(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mwl, PwTcParams p, int B, cudaStream_t st) {
-  using L = PwTcCfg<N_TILE, STAGES, X3, ATM>;
-  auto kern = pw1x1_tc_kernel<N_TILE, STAGES, X3, ATM>;
+  using L = PwTcCfg<N_TILE, STAGES, X3>;
+  auto kern = pw1x1_tc_kernel<N_TILE, STAGES, X3>;
   static std::atomic<uint64_t> attr_mask{0};   // cudaFuncSetAttribute is per device
   if (first_use_on_device(attr_mask)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
@@ -446,18 +259,16 @@ int pw1x1_tc_launch(const float* x, const float* w, const float* w_lo, const flo
   SMAAT_REQUIRE(pw1x1_tc_eligible(x, w, w_lo, K, Cout, P), "pw1x1(tc): needs P %% 4 == 0, K %% 4 == 0 and 16-byte aligned x/w");
   SMAAT_REQUIRE(!x3 || w_lo, "pw1x1(tc): TF32X3 needs w_lo (see smaat_split_tf32)");
   SMAAT_REQUIRE(Cout <= 512 || (!scale && !shift), "pw1x1(tc): Cout=%d > 512 with an epilogue affine (smem staging holds 512 channels)", Cout);
-  // the tile shape depends on the layer only, never on the batch: results stay bit-identical across batch sizes
-  // ... with one exception that still depends on the layer alone: tiny planes (P <= 512, the 18 x 18 bottleneck) have only 3 pixel
-  // tiles per image; at N_TILE = 256 the B = 32 forward is 192 tiles on 148 SMs (2 rounds, 65 % filled), at 128 it is 384 tiles of
-  // half the work (3 rounds = 1.5 of the former)
-  const int n_tile = Cout > 128 ? (P <= 512 ? 128 : 256) : (Cout > 64 ? 128 : 64);
+  // the tile shape depends on the layer only, never on the batch: results stay bit-identical across batch sizes.  N_TILE is
+  // at most 128: the accumulators of a 64 x N_TILE warpgroup tile live in registers (N_TILE / 2 per thread).
+  const int n_tile = Cout > 64 ? 128 : 64;
 
   CUtensorMap mx, mw, mwl;
   {
     const uint64_t dims[3] = {(uint64_t)P, (uint64_t)K, (uint64_t)B};
     const uint64_t str[3] = {0, (uint64_t)P * 4, (uint64_t)K * P * 4};
     const uint32_t box[3] = {32u, (uint32_t)TC_BK, 1u};
-    int r = make_tmap_f32(&mx, x, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, "pw1x1(x)");
+    int r = make_tmap_f32(&mx, x, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, "pw1x1(x)");
     if (r) return r;
   }
   {
@@ -477,20 +288,13 @@ int pw1x1_tc_launch(const float* x, const float* w, const float* w_lo, const flo
   p.K = K; p.Cout = Cout; p.P = P; p.relu = relu;
   p.tiles_m = p.tiles_n = p.total_tiles = 0;
 
-  // one persistent CTA per SM: the smem ring takes ~192 KB of the 227 KB
+  // one persistent CTA per SM: the smem ring takes ~150-200 KB of the 227 KB
   if (x3) {
-    if (n_tile == 256) {
-      // SMAAT_PW_ATMEM=0 keeps the round-1 variant (split written to shared memory) for A/B measurements
-      static const bool atm = [] { const char* e = getenv("SMAAT_PW_ATMEM"); return !(e && e[0] == '0'); }();
-      if (atm) return launch_tc<256, 2, true, true>(mx, mw, mwl, p, B, st);
-      return launch_tc<256, 2, true>(mx, mw, mwl, p, B, st);  // activations split once per 256 channels
-    }
     if (n_tile == 128) return launch_tc<128, 3, true>(mx, mw, mwl, p, B, st);
-    return launch_tc<64, 4, true>(mx, mw, mwl, p, B, st);
+    return launch_tc<64, 5, true>(mx, mw, mwl, p, B, st);
   }
-  if (n_tile == 256) return launch_tc<256, 4, false>(mx, mw, mwl, p, B, st);
-  if (n_tile == 128) return launch_tc<128, 6, false>(mx, mw, mwl, p, B, st);
-  return launch_tc<64, 8, false>(mx, mw, mwl, p, B, st);
+  if (n_tile == 128) return launch_tc<128, 5, false>(mx, mw, mwl, p, B, st);
+  return launch_tc<64, 6, false>(mx, mw, mwl, p, B, st);
 }
 
 }  // namespace smaat

@@ -1,28 +1,24 @@
-// pw1x1_wgrad_tc.cu -- pointwise 1x1 weight gradient on the tensor cores:
+// pw1x1_wgrad_tc.cu -- pointwise 1x1 weight gradient on the Hopper tensor cores (wgmma, tf32):
 //   dW[o][c] += sum_{b,p} dz[b,o,p] * d[b,c,p]        (Cout x K outputs, reduction over B*H*W pixels)
 //
 // Backward of DepthwiseSeparableConv.pointwise (reference models/layers.py:45,49).  Both operands have
-// the reduction dimension (pixels) contiguous in NCHW, i.e. both are K-major for the MMA:
-//   A = dz viewed [B*Cout rows][P]  -> TMA box 128 rows x 32 px, SWIZZLE_128B
+// the reduction dimension (pixels) contiguous in NCHW, i.e. both are K-major for the MMA and both are read by
+// the tensor core straight from shared memory:
+//   A = dz viewed [B*Cout rows][P]  -> TMA box 128 rows x 32 px, SWIZZLE_128B (two consumer warpgroups x 64 rows)
 //   B = d  viewed [B*K    rows][P]  -> TMA box N_TILE rows x 32 px, SWIZZLE_128B
-//   D[128 x N_TILE] in TMEM accumulates over this CTA's slice of the (image, 32-pixel chunk) list;
+//   D[128 x N_TILE] in registers accumulates over this CTA's slice of the (image, 32-pixel chunk) list;
 // the slice results are merged into dW with fp32 atomics (split-K over pixels: the output is tiny,
 // the reduction is B*P = millions long).  Rows of A beyond Cout / rows of B beyond K inside a box
 // belong to neighbouring channels or images: they only produce D rows/columns that are never stored.
-// TF32X3: the 4 transform warps split BOTH landed tiles into tf32 hi (in place) + lo, three MMAs per
+// TF32X3: the consumer warpgroups split BOTH landed tiles into tf32 hi (in place) + lo, three MMAs per
 // k-step (hi*hi + lo*hi + hi*lo) -> fp32-grade gradients; TF32: one MMA on the raw fp32 tiles.
 #include "tc_common.cuh"
 
 namespace smaat {
 
-// both operands K-major here
-__host__ __device__ constexpr uint32_t make_idesc_tf32_kk(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (0u << 15) | (0u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-}
-
-// A = the operand on the M side (TMEM lanes), B = the operand on the N side (TMEM columns).  Normally A = dz (Cout rows per
+// A = the operand on the M side (rows), B = the operand on the N side (columns).  Normally A = dz (Cout rows per
 // image) and B = d (K rows); for Cout <= 64 the roles are swapped so the 128-row A box is not half empty (transposed = 1:
-// D is dW^T and lanes map to consecutive dW addresses).
+// D is dW^T).
 struct WgParams {
   float* dW;
   int K, Cout, P, B;       // K = rows of the B-side operand per image, Cout = rows of the A-side operand per image
@@ -40,12 +36,12 @@ struct WgCfg {
   static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 6 ? 6 : (200 * 1024) / STAGE_BYTES;
   static constexpr int TOTAL = STAGES * STAGE_BYTES + 512 + 1024;
   static constexpr uint32_t TX = A_BYTES + B_BYTES;
-  static constexpr int THREADS = X3 ? 320 : 192;
+  static constexpr int THREADS = 384;
   static_assert(STAGES >= 2, "pipeline depth");
 };
 
 template <int N_TILE, bool X3>
-__global__ void __launch_bounds__(WgCfg<N_TILE, X3>::THREADS, 1)
+__global__ void __launch_bounds__(384, 1)
     pw1x1_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_constant__ CUtensorMap map_d, const WgParams p) {
   using L = WgCfg<N_TILE, X3>;
   constexpr int STAGES = L::STAGES;
@@ -54,9 +50,6 @@ __global__ void __launch_bounds__(WgCfg<N_TILE, X3>::THREADS, 1)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * L::STAGE_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* xform_bar = bars + 2 * STAGES;
-  uint64_t* done_bar = bars + 3 * STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 3 * STAGES + 1);
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
   // work item: (o tile, c tile, pixel split)
@@ -73,17 +66,11 @@ __global__ void __launch_bounds__(WgCfg<N_TILE, X3>::THREADS, 1)
     tma_prefetch_desc(&map_d);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-      mbar_init(&xform_bar[s], 128);
+      mbar_init(&empty_bar[s], 8);
     }
-    mbar_init(done_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, N_TILE < 32 ? 32 : N_TILE);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   if (warp == 0) {
     if (lane == 0) {
@@ -99,70 +86,26 @@ __global__ void __launch_bounds__(WgCfg<N_TILE, X3>::THREADS, 1)
         tma_load_2d(st + L::OFF_B, &map_d, &full_bar[s], p0, b * p.K + c0);
       }
     }
-  } else if (warp == 1) {
-    // MMA issuer: whole warp in the loop (warp-uniform control flow, descriptors in uniform registers), one elected lane
-    // issues; both operands are K-major SW128 (8 tf32 = 32 B per k-step = +2 in the descriptor's >>4 address field)
-    constexpr uint32_t idesc = make_idesc_tf32_kk(N_TILE);
-    for (int i = 0; i < nchunks; ++i) {
-      const int s = i % STAGES;
-      mbar_wait(X3 ? &xform_bar[s] : &full_bar[s], (i / STAGES) & 1u);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
-        const uint64_t ad0 = make_b_desc(a_addr), bd0 = make_b_desc(a_addr + L::OFF_B);
-        const uint64_t al0 = make_b_desc(a_addr + L::OFF_LO), bl0 = make_b_desc(a_addr + L::OFF_LO + L::OFF_B);
+    return;
+  }
+  if (warp < 4 || nchunks <= 0) return;
+
+  // ===== consumer warpgroups 1, 2: warpgroup wg owns D rows 64 wg .. 64 wg + 63 =====
+  const int wg = (warp >> 2) - 1, wq = warp & 3;
+  const int ct = threadIdx.x - 128;   // 0..255
+  float acc[N_TILE / 2];
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint64_t ad = ad0 + (uint64_t)(kk * 2), bd = bd0 + (uint64_t)(kk * 2);
-          umma_tf32(tmem_base, ad, bd, idesc, (kk > 0) ? 1u : (i > 0 ? 1u : 0u));
-          if (X3) {
-            umma_tf32(tmem_base, al0 + (uint64_t)(kk * 2), bd, idesc, 1u);
-            umma_tf32(tmem_base, ad, bl0 + (uint64_t)(kk * 2), idesc, 1u);
-          }
-        }
-        umma_commit(&empty_bar[s]);
-        if (i == nchunks - 1) umma_commit(done_bar);
-      }
-      __syncwarp();
-    }
-  } else if (warp < 6) {
-    // epilogue: TMEM lane = output channel o, column = input channel c
-    if (nchunks > 0) {
-      mbar_wait(done_bar, 0);
-      tc_fence_after();
-      const int q = warp & 3;
-      const int o = o0 + q * 32 + lane;
-#pragma unroll 1
-      for (int cc = 0; cc < N_TILE; cc += 32) {
-        if (c0 + cc >= p.K) break;
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)cc, r);
-        tmem_ld_wait();
-        if (o < p.Cout) {
-          if (p.transposed) {   // D[o][c] = dW[c][o]: a warp's 32 lanes hit 32 consecutive floats
-            float* dst = p.dW + (int64_t)(c0 + cc) * p.ldw + o;
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (c0 + cc + j < p.K) atomicAdd(dst + (int64_t)j * p.ldw, __uint_as_float(r[j]));
-          } else {
-            float* dst = p.dW + (int64_t)o * p.ldw + c0 + cc;
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (c0 + cc + j < p.K) atomicAdd(dst + j, __uint_as_float(r[j]));
-          }
-        }
-      }
-      tc_fence_before();
-    }
-  } else if (X3) {
-    const int et = threadIdx.x - 192;
-    for (int i = 0; i < nchunks; ++i) {
-      const int s = i % STAGES;
-      mbar_wait(&full_bar[s], (i / STAGES) & 1u);
-      float4* a4 = reinterpret_cast<float4*>(smem + s * L::STAGE_BYTES);
-      float4* l4 = reinterpret_cast<float4*>(smem + s * L::STAGE_BYTES + L::OFF_LO);
+  for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.f;
+  for (int i = 0; i < nchunks; ++i) {
+    const int s = i % STAGES;
+    mbar_wait(&full_bar[s], (i / STAGES) & 1u);
+    unsigned char* st = smem + s * L::STAGE_BYTES;
+    if (X3) {
+      // split [A | B] into hi (in place) and lo; the named barrier makes the whole B split visible to both warpgroups
+      float4* a4 = reinterpret_cast<float4*>(st);
+      float4* l4 = reinterpret_cast<float4*>(st + L::OFF_LO);
 #pragma unroll 4
-      for (int idx = et; idx < (L::A_BYTES + L::B_BYTES) / 16; idx += 128) {
+      for (int idx = ct; idx < (L::A_BYTES + L::B_BYTES) / 16; idx += 256) {
         const float4 v = a4[idx];
         float4 h, l;
         h.x = tf32_hi(v.x); h.y = tf32_hi(v.y); h.z = tf32_hi(v.z); h.w = tf32_hi(v.w);
@@ -170,15 +113,45 @@ __global__ void __launch_bounds__(WgCfg<N_TILE, X3>::THREADS, 1)
         a4[idx] = h;
         l4[idx] = l;
       }
-      fence_proxy_async_smem();
-      mbar_arrive(&xform_bar[s]);
+      fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor-core (async) proxy
+      consumer_sync();
     }
-  }
-  __syncthreads();
-  if (warp == 1) {
+    const uint32_t a_addr = smem_u32(st) + (uint32_t)(wg * 64 * 128);
+    const uint64_t ad0 = make_kmajor_desc(a_addr), bd0 = make_kmajor_desc(smem_u32(st + L::OFF_B));
+    const uint64_t al0 = make_kmajor_desc(a_addr + L::OFF_LO), bl0 = make_kmajor_desc(smem_u32(st + L::OFF_LO + L::OFF_B));
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      Wgmma<N_TILE>::ss(acc, ad0 + (uint64_t)(2 * kk), bd0 + (uint64_t)(2 * kk), 1u);
+      if (X3) {
+        Wgmma<N_TILE>::ss(acc, al0 + (uint64_t)(2 * kk), bd0 + (uint64_t)(2 * kk), 1u);
+        Wgmma<N_TILE>::ss(acc, ad0 + (uint64_t)(2 * kk), bl0 + (uint64_t)(2 * kk), 1u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait0();
+    wgmma_keep(acc);
     __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, N_TILE < 32 ? 32 : N_TILE);
+    if (lane == 0) mbar_arrive(&empty_bar[s]);
+  }
+
+  // epilogue: D row = output channel o, column = input channel c
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int e2 = 0; e2 < 2; ++e2) {
+    const int o = o0 + 64 * wg + 16 * wq + g + 8 * e2;
+    if (o >= p.Cout) continue;
+#pragma unroll
+    for (int j = 0; j < N_TILE / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int c = c0 + 8 * j + 2 * t + e;
+        if (c >= p.K) continue;
+        const float v = acc[4 * j + 2 * e2 + e];
+        if (p.transposed) atomicAdd(p.dW + (int64_t)c * p.ldw + o, v);   // D[o][c] = dW[c][o]
+        else atomicAdd(p.dW + (int64_t)o * p.ldw + c, v);
+      }
+    }
   }
 }
 
@@ -220,7 +193,7 @@ int pw1x1_wgrad_tc_launch(const float* dz, const float* d, float* dW, int B, int
     const int ti = K; K = Cout; Cout = ti;
     transposed = 1;
   }
-  const int n_tile = K > 128 ? 256 : (K > 64 ? 128 : 64);
+  const int n_tile = K > 64 ? 128 : 64;   // accumulators in registers: N_TILE / 2 per thread
   {
     const uint64_t dims[2] = {(uint64_t)P, (uint64_t)B * Cout};
     const uint64_t str[2] = {0, (uint64_t)P * 4};
@@ -239,11 +212,9 @@ int pw1x1_wgrad_tc_launch(const float* dz, const float* d, float* dW, int B, int
   p.dW = dW; p.K = K; p.Cout = Cout; p.P = P; p.B = B; p.ldw = ldw; p.transposed = transposed;
   p.chunks_per_img = p.total_chunks = p.chunks_per_split = p.tiles_o = p.tiles_c = 0;
   if (x3) {
-    if (n_tile == 256) return launch_wg<256, true>(mz, md, p, st);
     if (n_tile == 128) return launch_wg<128, true>(mz, md, p, st);
     return launch_wg<64, true>(mz, md, p, st);
   }
-  if (n_tile == 256) return launch_wg<256, false>(mz, md, p, st);
   if (n_tile == 128) return launch_wg<128, false>(mz, md, p, st);
   return launch_wg<64, false>(mz, md, p, st);
 }

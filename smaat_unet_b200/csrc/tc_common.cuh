@@ -1,195 +1,81 @@
-// tc_common.cuh -- tcgen05 / TMEM helpers shared by the tensor-core kernels (pw1x1_tc.cu, dsconv_fused.cu).
+// tc_common.cuh -- Hopper warpgroup-MMA (wgmma) helpers shared by the tensor-core kernels (pw1x1_tc.cu, pw1x1_wgrad_tc.cu,
+// dsconv_fused.cu).
+//
+// tf32 wgmma takes shared-memory operands only K-major.  The activations of the forward kernels lie pixels-contiguous (NCHW),
+// i.e. MN-major for the pixel-rows operand, so that operand goes through registers: each thread loads its A fragment from a
+// 128B-swizzled [k][32 px] tile (what TMA SWIZZLE_128B writes, or what the depthwise producers write) and issues the RS form.
+// (The fused DS conv's producers can instead write their result K-major, for the tensor core to read: kmajor_offset.)
+// The weights ([Cout][K], K contiguous) are the K-major B operand, read by the tensor core through a descriptor.
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace smaat {
 
-constexpr int TC_BM = 128;  // pixels per tile (UMMA M)
-constexpr int TC_BK = 32;   // k per stage (one 128-byte swizzle row of fp32 on the weight side)
+constexpr int TC_BM = 128;  // pixels per tile: two consumer warpgroups x m64
+constexpr int TC_BK = 32;   // k per stage (one 128-byte swizzle row of fp32)
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_keep(float (&d)[N]) {   // accumulators are live across the asynchronous MMAs
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
-// smem matrix descriptor (cute::UMMA::SmemDescriptor layout): addr>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout_type [61,64): 2 = SWIZZLE_128B (16-byte chunks,
-// 8-row atom), 1 = SWIZZLE_128B_BASE32B (32-byte chunks, 4-row atom) -- the only swizzled layout
-// the hardware accepts for MN-major 32-bit (tf32) operands.
-constexpr uint32_t LAYOUT_SW128 = 2, LAYOUT_SW128_BASE32B = 1;
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
+// Shared-memory matrix descriptor (sm_90 GMMA layout): addr>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout [62,64)
+// with 1 = SWIZZLE_128B.  K-major SW128 operand: rows of 128 B (32 tf32), 8-row atoms 1 KB apart (SBO); one k8 step is 32 B
+// along the row = +2 in the address field.  The tile base must be 1 KB aligned.
+__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3fffu);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout << 61;
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// A operand: activations, MN-major tf32.  One k-row = 128 B (32 pixels); 4-row swizzle groups 512 B apart
-// (SBO); 8 k-rows per MMA (+1 KB per k-step); 32-pixel blocks `lbo` bytes apart.
-__device__ __forceinline__ uint64_t make_a_desc(uint32_t saddr, uint32_t lbo) {
-  return make_smem_desc(saddr, lbo, 512, LAYOUT_SW128_BASE32B);
-}
-// B operand: weights, K-major SW128.  8 tf32 = 32 B along the swizzled 128 B row; 8-row groups 1 KB apart.
-__device__ __forceinline__ uint64_t make_b_desc(uint32_t saddr) { return make_smem_desc(saddr, 16, 1024, LAYOUT_SW128); }
 
-// Byte offset of activation element (k-row kr, pixel m) inside one A tile stored as 4 blocks of
-// [32 k-rows][32 px] with the 128B-span / 32B-atom swizzle (what TMA SWIZZLE_128B_ATOM_32B writes):
-// 32-byte chunk index (bits 5-6) XOR k-row (bits 7-8).
+// Byte offset of activation element (k-row kr, pixel m) inside one A tile stored as 4 blocks of [32 k-rows][32 px] with the
+// 128-byte swizzle (16-byte chunk index XOR k-row % 8) -- the layout TMA SWIZZLE_128B writes for a 32 px x 32 k box.
 __device__ __forceinline__ uint32_t a_tile_offset(int kr, int m) {
   const int j = m >> 5, col = m & 31;
-  return (uint32_t)(j * (TC_BK * 128) + kr * 128 + ((((col >> 3) ^ (kr & 3)) << 5) | ((col & 7) << 2)));
+  return (uint32_t)(j * (TC_BK * 128) + kr * 128 + ((((col >> 2) ^ (kr & 7)) << 4) | ((col & 3) << 2)));
 }
 
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32=1 [4,6), a/b_format TF32=2
-// [7,10)/[10,13), a_major MN=1 [15], b_major K=0 [16], N>>3 [17,23), M>>4 [24,29).
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (0u << 16) | ((uint32_t)(n >> 3) << 17) |
-         ((uint32_t)(TC_BM >> 4) << 24);
+// Byte offset of element (row, k) of a K-major operand tile with 128-byte rows (32 tf32 of k) and the 128-byte swizzle
+// (16-byte chunk index XOR row % 8): the layout make_kmajor_desc describes.
+__device__ __forceinline__ uint32_t kmajor_offset(int row, int k) {
+  return (uint32_t)(row * 128 + ((((k >> 2) ^ (row & 7)) << 4) | ((k & 3) << 2)));
 }
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-// One lane of the (converged) warp: the single-thread tcgen05 issue slot.  Unlike `if (lane == 0)` it keeps the
-// surrounding control flow warp-uniform for the compiler.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t cols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t base, uint32_t cols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(cols) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (lane = TMEM lane = pixel)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-// 32 lanes x 32 consecutive fp32 columns <- 32 registers per thread (lane = TMEM lane): the A operand written by its producers
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Fragment-shaped TMEM read: 16 lanes x 32 columns.  Thread T gets, for i = 0..3 and e = 0,1:
-//   f[4i + e]     = lane T/4,     column 8i + 2(T%4) + e
-//   f[4i + 2 + e] = lane T/4 + 8, column 8i + 2(T%4) + e
-// (the mma m16n8 accumulator layout, repeated over 4 column groups).  Several pixels (lanes) per thread make a
-// reduction over pixels mostly register-local -- see tmem_colsum32.
-__device__ __forceinline__ void tmem_ld_16x256b_x4(uint32_t taddr, uint32_t (&f)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.16x256b.x4.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(f[0]), "=r"(f[1]), "=r"(f[2]), "=r"(f[3]), "=r"(f[4]), "=r"(f[5]), "=r"(f[6]), "=r"(f[7]), "=r"(f[8]),
-        "=r"(f[9]), "=r"(f[10]), "=r"(f[11]), "=r"(f[12]), "=r"(f[13]), "=r"(f[14]), "=r"(f[15])
-      : "r"(taddr));
+// Pixel (0..127 of the tile) of accumulator row g + 8e of warp wq in consumer warpgroup wg.  A warp's 16 rows are half of a
+// 32-pixel block; the 8 rows a fragment register covers are pixels {c..c+3, c+16..c+19}: with the swizzle above, the 32
+// lanes of one fragment load (4 k-rows x those 8 pixels) then fall on 32 different banks.
+__device__ __forceinline__ int tc_row_pixel(int wg, int wq, int e, int g) {
+  return 64 * wg + 32 * (wq >> 1) + 4 * (2 * (wq & 1) + e) + (g & 3) + 16 * (g >> 2);
 }
 
-// Column sums (s1) and sums of squares (s2) over the 32 TMEM lanes of this warp's quarter for the 32 columns at
-// taddr (lane field = first lane of the quarter).  On return lane T holds the totals of column tmem_colsum32_col(T).
-// 2 fragment loads + 14 shuffles instead of a 62-shuffle register transpose.
-__device__ __forceinline__ int tmem_colsum32_col(int lane) {
-  return 8 * (((lane >> 4) & 1) * 2 + ((lane >> 3) & 1)) + 2 * (lane & 3) + ((lane >> 2) & 1);
-}
-// SECOND > 0: the value of a column is the sum of the accumulators at taddr and taddr + SECOND (split accumulation).
-// row_mask: bit l = TMEM lane l of this quarter takes part (rows whose accumulators are not exact zeros but must not count).
-template <int SECOND = 0>
-__device__ __forceinline__ void tmem_colsum32(uint32_t taddr, int lane, float& sum, float& sumsq, uint32_t row_mask = 0xffffffffu) {
-  float s1[8], s2[8];
-#pragma unroll
-  for (int v = 0; v < 8; ++v) s1[v] = s2[v] = 0.f;
-#pragma unroll
-  for (int half = 0; half < 2; ++half) {
-    uint32_t f[16];
-    tmem_ld_16x256b_x4(taddr + ((uint32_t)(16 * half) << 16), f);
-    if (SECOND > 0) {
-      uint32_t f2[16];
-      tmem_ld_16x256b_x4(taddr + (uint32_t)SECOND + ((uint32_t)(16 * half) << 16), f2);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 16; ++i) f[i] = __float_as_uint(__uint_as_float(f[i]) + __uint_as_float(f2[i]));
-    }
-    tmem_ld_wait();
-    const bool va = (row_mask >> (16 * half + (lane >> 2))) & 1u, vb = (row_mask >> (16 * half + (lane >> 2) + 8)) & 1u;
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const float a = va ? __uint_as_float(f[4 * i + e]) : 0.f, b = vb ? __uint_as_float(f[4 * i + 2 + e]) : 0.f;
-        s1[2 * i + e] += a + b;
-        s2[2 * i + e] = fmaf(a, a, fmaf(b, b, s2[2 * i + e]));
-      }
-  }
-#pragma unroll
-  for (int s = 4; s >= 1; s >>= 1) {   // lanes differing in bits 4, 3, 2 hold the other rows of the same columns
-    const int x = s * 4;
-    const bool up = (lane & x) != 0;
-#pragma unroll
-    for (int v = 0; v < s; ++v) {
-      const float k1 = up ? s1[v + s] : s1[v], d1 = up ? s1[v] : s1[v + s];
-      const float k2 = up ? s2[v + s] : s2[v], d2 = up ? s2[v] : s2[v + s];
-      s1[v] = k1 + __shfl_xor_sync(0xffffffffu, d1, x);
-      s2[v] = k2 + __shfl_xor_sync(0xffffffffu, d2, x);
-    }
-  }
-  sum = s1[0];
-  sumsq = s2[0];
+// The thread's A fragment of k-step kk (8 k-rows) from an A tile at `at`: rows m0 / m1 (its two pixels), k-rows 8kk + t, + 4.
+__device__ __forceinline__ void load_a_frag(const unsigned char* at, int kk, int t, int m0, int m1, float (&v)[4]) {
+  const int k0 = 8 * kk + t;
+  v[0] = *reinterpret_cast<const float*>(at + a_tile_offset(k0, m0));
+  v[1] = *reinterpret_cast<const float*>(at + a_tile_offset(k0, m1));
+  v[2] = *reinterpret_cast<const float*>(at + a_tile_offset(k0 + 4, m0));
+  v[3] = *reinterpret_cast<const float*>(at + a_tile_offset(k0 + 4, m1));
 }
 
 __device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float(__float_as_uint(v) & 0xffffe000u); }
 
-// v[j] = this lane's value for channel j (32 channels).  Returns, in lane L, the sum over the 32 lanes of
-// channel L: a butterfly that halves the live channels per step -- 16+8+4+2+1 = 31 shuffles instead of
-// 32 x 5 for 32 independent warp reductions.  (Train-mode BatchNorm statistics in the GEMM epilogues.)
-__device__ __forceinline__ float warp_transpose_sum32(float (&v)[32], int lane) {
-#pragma unroll
-  for (int s = 16; s >= 1; s >>= 1) {
-    const bool up = (lane & s) != 0;
-#pragma unroll
-    for (int i = 0; i < s; ++i) {
-      const float keep = up ? v[i + s] : v[i];
-      const float send = up ? v[i] : v[i + s];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, s);
-    }
-  }
-  return v[0];
+// Sums over the 8 lanes of a fragment column group (lanes with equal t): afterwards lanes 0..3 hold the totals.
+__device__ __forceinline__ float frag_colsum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 4);
+  v += __shfl_xor_sync(0xffffffffu, v, 8);
+  v += __shfl_xor_sync(0xffffffffu, v, 16);
+  return v;
 }
+
+// Named barrier over the two consumer warpgroups (256 threads); id 0 is __syncthreads.
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 }  // namespace smaat

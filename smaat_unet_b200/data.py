@@ -1,8 +1,8 @@
-"""Input pipeline for the B200 path (SURVEY 8 f3): pre-decompressed shards + a pinned, threaded batch loader.
+"""Input pipeline for the GPU path (SURVEY 8 f3): pre-decompressed shards + a pinned, threaded batch loader.
 
 The reference reads gzip-9 HDF5 sample by sample through one DataLoader worker (utils/dataset_precip.py:23-44,63-77,
-models/regression_lightning.py:177-199) -- a few hundred frames/s at best, while one B200 consumes ~900 frames/s in
-training and ~4 600 frames/s in inference.  This module keeps the reference's *indexing semantics* and removes the
+models/regression_lightning.py:177-199) -- a few hundred frames/s at best, far below what the GPU path consumes in
+training and in inference.  This module keeps the reference's *indexing semantics* and removes the
 decompression and the per-sample Python overhead from the step:
 
   * ``write_shard`` / ``convert_h5`` -- one-off conversion of ``<file>[train|test]["images"]`` into a raw float32

@@ -167,7 +167,7 @@ def pw_bwd(dz, d, weight, dW, db, need_input=True):
     P = H * W
     lib = _lib.load()
     m = ops.PW_MODES[ops.get_pointwise_mode()]
-    if m != 0 and P % 4 == 0 and K >= 8 and Cout >= 8:      # tensor cores: split-K over pixels, TMEM accumulation, fp32 atomics to merge
+    if m != 0 and P % 4 == 0 and K >= 8 and Cout >= 8:      # tensor cores: split-K over pixels, register accumulators, fp32 atomics to merge
         _call(f"smaat_pw1x1_bwd_weight_tc[K{K}_N{Cout}_P{P}]", 4 * B * P * (K + Cout), 2 * B * P * K * Cout, lib.smaat_pw1x1_bwd_weight_tc,
               _ptr(dz), _ptr(d), _ptr(dW), _ptr(db), B, K, Cout, P, m, _stream())
     else:

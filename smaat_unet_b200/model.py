@@ -1,4 +1,4 @@
-"""SmaAt-UNet assembled from the B200 drop-in blocks.
+"""SmaAt-UNet assembled from the H100 drop-in blocks.
 
 Same constructor, attribute names (hence state_dict keys) and forward graph as the
 reference's ``models/SmaAt_UNet.py:7-57``; provided so the full model can be built where the

@@ -11,7 +11,7 @@ constructor signatures, forward signatures and ``state_dict`` keys as
 so checkpoints trained with the reference load unchanged (``calc_metrics_test_set.py:114``).
 The parameter containers are ordinary torch modules (``nn.Conv2d`` / ``nn.BatchNorm2d`` /
 ``nn.Linear`` -> identical default initialisation and key names) but their ``forward`` is
-never called: all arithmetic runs in libsmaat_b200.so (sm_100a kernels) through ``ops``.
+never called: all arithmetic runs in libsmaat_b200.so (sm_90a kernels) through ``ops``.
 There is no PyTorch / CPU fallback; unsupported requests raise.
 """
 from __future__ import annotations
@@ -252,7 +252,7 @@ class UpDS(_CachingModule):
 
     The concat is never materialised: the first depthwise kernel reads [skip, up] as a virtual concat.
     ``bilinear=False`` (ConvTranspose2d(in, in // 2, 2, stride=2), :72-73): kernel = stride, so the transposed conv is one
-    tcgen05 pointwise GEMM to the 4 packed taps + a pixel shuffle (csrc/convt.cu).
+    wgmma pointwise GEMM to the 4 packed taps + a pixel shuffle (csrc/convt.cu).
     """
 
     def __init__(self, in_channels, out_channels, bilinear=True, kernels_per_layer=1):
@@ -343,8 +343,8 @@ class ChannelAttention(nn.Module):
         """sigmoid(MLP(avg) + MLP(max)) as a (B, C) tensor.  ``with_maxpool``: also return MaxPool2d(2)(x) (or None), computed
         in the same read of x as the global pools."""
         l1, l2 = self.MLP[1], self.MLP[3]
-        # 512 channels: the MLP run by the last-arriving pooling CTA of each image measured SLOWER than a second launch
-        # (tools/time_cbam_pool.py, B = 32: 57.6 vs 24.5 us at 18 x 18, 49.8 vs 37.7 us at 36 x 36; equal from 72 x 72 up)
+        # 512 channels: the MLP runs as a second launch instead of in the last-arriving pooling CTA of each image, whose
+        # serial 512-channel MLP sits on the critical path of these small planes
         one = None if x.shape[1] >= 512 else ops.cbam_pool_mlp(x, l1.weight.detach(), l1.bias.detach(), l2.weight.detach(), l2.bias.detach(),
                                                                with_maxpool=with_maxpool)
         if one is not None:          # pools + MLP + sigmoid (+ the 2x2 max-pool) in one launch

@@ -18,7 +18,7 @@ assert _pw_mode in PW_MODES, f"SMAAT_PW_MODE must be one of {list(PW_MODES)}"
 
 
 def set_pointwise_mode(mode: str) -> None:
-    """'tf32x3' (default; tcgen05 3xTF32 split, fp32-grade), 'tf32' (tcgen05 single pass; what
+    """'tf32x3' (default; wgmma 3xTF32 split, fp32-grade), 'tf32' (wgmma single pass; what
     cuDNN's allow_tf32=True default gives the reference on a GPU), 'fp32' (CUDA-core exact)."""
     global _pw_mode
     if mode not in PW_MODES:
@@ -157,7 +157,7 @@ def pw1x1(x, weight, scale, shift, relu, mode=None, w_split=None, stats=None, ou
     """Pointwise 1x1 + per-channel affine (+ReLU) (layers.py:45,49 + parts_ds.py:25-26).
 
     weight: (Cout, K[,1,1]).  mode None = module-level default.  w_split = cached (hi, lo) for
-    'tf32x3'.  Falls to the exact CUDA-core kernel for shapes the tcgen05 path does not take.
+    'tf32x3'.  Falls to the exact CUDA-core kernel for shapes the tensor-core path does not take.
     """
     x = _dense(x, "x")
     B, K, H, W = x.shape
@@ -193,9 +193,9 @@ def set_fused_dsconv(enabled: bool) -> None:
 
 
 def set_dsconv_impl(impl: str) -> None:
-    """Which fused DS-conv kernel runs: 'auto' (TMEM-operand kernel where it applies, else the shared-memory-operand one),
-    'smem' (round-1 kernel only) or 'tmem' (TMEM-operand kernel only; other shapes fall back to dw3x3 + pw1x1)."""
-    _lib.check(_lib.load().smaat_set_dsconv_impl({"auto": 0, "smem": 1, "tmem": 2}[impl]), "smaat_set_dsconv_impl")
+    """How the fused DS-conv kernel feeds the depthwise result to the tensor core: 'auto', 'smem' (wgmma reads it from shared
+    memory) or 'regs' (loaded into registers first)."""
+    _lib.check(_lib.load().smaat_set_dsconv_impl({"auto": 0, "smem": 1, "regs": 2}[impl]), "smaat_set_dsconv_impl")
 
 
 def dsconv_takes(x, x1, pw_weight, k, mode=None, stats=False) -> bool:
@@ -230,6 +230,8 @@ def dsconv(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, mod
     assert K == k * (C0 + C1), f"pointwise weight {tuple(pw_weight.shape)} does not match k*Cin={k * (C0 + C1)}"
     lib = _lib.load()
     if not lib.smaat_dsconv_eligible2(_ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(w2d), H, W, k, Cout, int(stats is not None)):
+        return None
+    if outconv is not None and Cout > 128:     # the fused OutConv needs all channels in one pass (smaat_dsconv_outconv_fwd)
         return None
     wlo = None
     if PW_MODES[mode] == 2:

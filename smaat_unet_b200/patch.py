@@ -1,10 +1,10 @@
-"""Rebind the reference's block classes to the B200 drop-ins, in place.
+"""Rebind the reference's block classes to the H100 drop-ins, in place.
 
 The reference has no plugin registry: ``models/SmaAt_UNet.py:2-4`` and
 ``models/unet_precip_regression_lightning.py:1-3`` import the block classes by name.
 ``patch_reference()`` swaps those names in the already-importable reference modules so that
 ``SmaAt_UNet`` and the Lightning variants (UNetDS, UNetDSAttention, UNetDSAttention4CBAMs,
-UNetAttention's CBAMs) are constructed from B200 blocks with no change to reference code.
+UNetAttention's CBAMs) are constructed from H100 blocks with no change to reference code.
 """
 from __future__ import annotations
 

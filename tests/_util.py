@@ -4,8 +4,8 @@ import torch
 
 # Tolerances (relative to max|reference|), stated per pointwise arithmetic mode:
 #   fp32   : CUDA-core FFMA, exact fp32 products, fp32 accumulate
-#   tf32x3 : tcgen05 3xTF32 split; products carry ~2^-21 relative error
-#   tf32   : tcgen05 single TF32 pass (10-bit mantissa inputs) -- what cuDNN gives the reference by default on a GPU
+#   tf32x3 : wgmma 3xTF32 split; products carry ~2^-21 relative error
+#   tf32   : wgmma single TF32 pass (10-bit mantissa inputs) -- what cuDNN gives the reference by default on a GPU
 PW_TOL = {"fp32": 2e-5, "tf32x3": 3e-5, "tf32": 4e-3}
 # end-to-end (18 pointwise layers + BN scaling) tolerances for the full network
 NET_TOL = {"fp32": 1e-4, "tf32x3": 1e-4, "tf32": 2e-2}

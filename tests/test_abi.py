@@ -34,7 +34,7 @@ def test_binding_table_matches_header():
 
 def test_abi_version_and_error_string():
     lib = S._lib.load()
-    assert lib.smaat_abi_version() == 1
+    assert lib.smaat_abi_version() == 2
     # argument validation happens on the host before any CUDA call: usable without a GPU
     rc = lib.smaat_maxpool2_fwd(None, None, 1, 4, 4, None)
     assert rc == -1 and b"maxpool2" in lib.smaat_last_error()
@@ -92,9 +92,94 @@ def test_product_package_never_imports_oracle():
             assert "oracle" not in src.replace("# oracle", ""), f"{fn} references the oracle"
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/models"), reason="reference checkout only exists in the build container")
-def test_patch_reference_rebinds_names():
-    done = S.patch_reference("/root/reference")
+# A stand-in for the reference's `models` package with its import structure: every module imports the block classes BY NAME
+# (models/SmaAt_UNet.py:2-4, unet_precip_regression_lightning.py:1-3), and the placeholder blocks refuse to be constructed,
+# so a model built after patch_reference() proves that each module's names were rebound.  The assemblies restate the
+# constructors the repository already restates in smaat_unet_b200/model.py.
+_PLACEHOLDER = """from torch import nn
+
+
+def _placeholder(name):
+    def __init__(self, *args, **kwargs):
+        raise AssertionError(f"{name}: the unpatched block was constructed")
+    return type(name, (nn.Module,), {"__init__": __init__})
+
+
+"""
+_STANDIN = {
+    "__init__.py": "",
+    "layers.py": _PLACEHOLDER + "\n".join(f'{n} = _placeholder("{n}")' for n in ("DepthwiseSeparableConv", "ChannelAttention", "SpatialAttention", "CBAM")),
+    "unet_parts.py": _PLACEHOLDER + "\n".join(f'{n} = _placeholder("{n}")' for n in ("DoubleConv", "Down", "Up", "OutConv")),
+    "unet_parts_depthwise_separable.py": "from models.layers import DepthwiseSeparableConv  # noqa: F401\n" + _PLACEHOLDER
+    + "\n".join(f'{n} = _placeholder("{n}")' for n in ("DoubleConvDS", "DownDS", "UpDS")),
+    "_assemble.py": """def assemble(m, g, n_channels, n_classes, k, bilinear, r, n_cbams):
+    # g: the globals of the calling module, i.e. the block names as that module sees them
+    factor = 2 if bilinear else 1
+    widths = (64, 128, 256, 512, 1024 // factor)
+    m.inc = g["DoubleConvDS"](n_channels, 64, kernels_per_layer=k)
+    for lvl in range(5):
+        if lvl > 0:
+            setattr(m, f"down{lvl}", g["DownDS"](widths[lvl - 1], widths[lvl], kernels_per_layer=k))
+        if lvl < n_cbams:
+            setattr(m, f"cbam{lvl + 1}", g["CBAM"](widths[lvl], reduction_ratio=r))
+    for i, (cin, cout) in enumerate(zip((1024, 512, 256, 128), (512 // factor, 256 // factor, 128 // factor, 64))):
+        setattr(m, f"up{i + 1}", g["UpDS"](cin, cout, bilinear, kernels_per_layer=k))
+    m.outc = g["OutConv"](64, n_classes)
+""",
+    "SmaAt_UNet.py": """from torch import nn
+from models.unet_parts import OutConv  # noqa: F401
+from models.unet_parts_depthwise_separable import DoubleConvDS, UpDS, DownDS  # noqa: F401
+from models.layers import CBAM  # noqa: F401
+from models._assemble import assemble
+
+
+class SmaAt_UNet(nn.Module):
+    def __init__(self, n_channels, n_classes, kernels_per_layer=2, bilinear=True, reduction_ratio=16):
+        super().__init__()
+        assemble(self, globals(), n_channels, n_classes, kernels_per_layer, bilinear, reduction_ratio, 5)
+""",
+    "unet_precip_regression_lightning.py": """from torch import nn
+from models.unet_parts import Down, DoubleConv, Up, OutConv  # noqa: F401
+from models.unet_parts_depthwise_separable import DoubleConvDS, UpDS, DownDS  # noqa: F401
+from models.layers import CBAM  # noqa: F401
+from models._assemble import assemble
+
+
+def _wrapper(n_cbams):
+    def __init__(self, hparams):
+        nn.Module.__init__(self)
+        h = hparams
+        assemble(self, globals(), h.n_channels, h.n_classes, h.kernels_per_layer, h.bilinear, h.reduction_ratio, n_cbams)
+    return __init__
+
+
+UNetDS = type("UNetDS", (nn.Module,), {"__init__": _wrapper(0)})
+UNetDSAttention = type("UNetDSAttention", (nn.Module,), {"__init__": _wrapper(5)})
+UNetDSAttention4CBAMs = type("UNetDSAttention4CBAMs", (nn.Module,), {"__init__": _wrapper(4)})
+""",
+}
+
+
+@pytest.fixture
+def standin_reference(tmp_path):
+    import sys
+    root = tmp_path / "reference"
+    (root / "models").mkdir(parents=True)
+    for name, src in _STANDIN.items():
+        (root / "models" / name).write_text(src)
+    saved = {k: v for k, v in sys.modules.items() if k == "models" or k.startswith("models.")}
+    for k in saved:
+        del sys.modules[k]
+    yield str(root)
+    for k in [k for k in sys.modules if k == "models" or k.startswith("models.")]:
+        del sys.modules[k]
+    sys.modules.update(saved)
+    if str(root) in sys.path:
+        sys.path.remove(str(root))
+
+
+def test_patch_reference_rebinds_names(standin_reference):
+    done = S.patch_reference(standin_reference)
     assert "models.SmaAt_UNet" in done
     import models.SmaAt_UNet as msu
     m = msu.SmaAt_UNet(12, 1)
@@ -102,15 +187,12 @@ def test_patch_reference_rebinds_names():
     assert len(m.state_dict()) == 214
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/models"), reason="reference checkout only exists in the build container")
-def test_patch_reference_reaches_the_lightning_wrappers():
+def test_patch_reference_reaches_the_lightning_wrappers(standin_reference):
     """The Lightning wrapper classes (models/unet_precip_regression_lightning.py:86-208) import the block classes by name;
-    after patch_reference() their UNCHANGED constructors build B200 blocks and keep the reference's state_dict schema.
-    `lightning` / `torchmetrics` / `h5py` are not installed here: oracle/ref_stubs.py stands in for those imports only."""
+    after patch_reference() their constructors build H100 blocks and keep the reference's state_dict schema."""
     from oracle import ref_stubs
     from oracle.cases import smaat_unet_schema
-    ref_stubs.install()
-    done = S.patch_reference("/root/reference", strict=True)
+    done = S.patch_reference(standin_reference, strict=True)
     assert "models.unet_precip_regression_lightning" in done
     import models.unet_precip_regression_lightning as L
     for cls, n_cbams in (("UNetDSAttention", 5), ("UNetDSAttention4CBAMs", 4), ("UNetDS", 0)):

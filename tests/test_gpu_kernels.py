@@ -204,27 +204,18 @@ DS_CASES = [
     (1, 8, 0, 36, 52, 2, 16),      # ragged patches in x and y
     (1, 128, 128, 16, 16, 2, 64),  # K = 512: many chunks, both producer groups, concat boundary mid-loop
     (3, 24, 0, 8, 96, 2, 40),      # odd chunk count (3 per tile) -> groups alternate across tiles
-    (8, 16, 0, 128, 128, 2, 64),   # 512 tile pairs: 3-4 per CTA -> both accumulator pair buffers reused (TMEM-operand kernel)
-    (8, 16, 0, 128, 64, 2, 128),   # 256 pairs, N_TILE 128: the single accumulator pair is handed back by the epilogue
-    (2, 32, 32, 40, 72, 2, 96),    # 16 x 16 pairs with ragged right / bottom halves, concat, Cout between the tile sizes
-    (2, 32, 0, 32, 32, 2, 256),    # Cout = 256: two output-channel passes of 128 over the same pairs (TMEM-operand kernel)
+    (8, 16, 0, 128, 128, 2, 64),   # 1024 tiles: 7-8 per CTA -> every ring wraps many times across tiles
+    (8, 16, 0, 128, 64, 2, 128),   # 512 tiles, N_TILE 128: one producer group feeds several tiles per CTA
+    (2, 32, 32, 40, 72, 2, 96),    # ragged right / bottom patches, concat, Cout between the tile sizes
+    (2, 32, 0, 32, 32, 2, 256),    # Cout = 256: two output-channel passes of 128 over the same patches
     (1, 48, 16, 16, 64, 2, 512),   # Cout = 512: four passes, concat
 ]
 
 
-def _tmem_takes(H, W, k, Cout):
-    """dsconv_tmem_eligible restated: k = 2, 8 <= Cout <= 128 or Cout in {256, 384, 512}, W % 4 == 0, and 32 x 8 / 16 x 16 tile
-    pairs waste <= 35 %."""
-    if k != 2 or Cout < 8 or Cout > 512 or (Cout > 128 and Cout % 128) or W % 4:
-        return False
-    cd = lambda a, b: -(-a // b)   # noqa: E731
-    return min((cd(W, pw) * pw / W) * (cd(H, php) * php / H) for pw, php in ((32, 8), (16, 16))) <= 1.35
-
-
-@pytest.fixture(params=["smem", "tmem"])
+@pytest.fixture(params=["smem", "regs"])
 def ds_impl(request):
-    """Both generations of the fused kernel behind the same ABI entry: A operand staged in shared memory (dsconv_fused.cu,
-    all k) / written to tensor memory (dsconv_tmem.cu, k = 2, no batch statistics)."""
+    """Both ways the fused kernel hands the depthwise result to the tensor core behind the same ABI entry: K-major tiles
+    that wgmma reads from shared memory / tiles loaded into registers for wgmma's register-A form."""
     ops.set_dsconv_impl(request.param)
     yield request.param
     ops.set_dsconv_impl("auto")
@@ -234,10 +225,6 @@ def ds_impl(request):
 @pytest.mark.parametrize("case", DS_CASES)
 def test_dsconv_fused_matches_oracle(case, mode, ds_impl):
     B, C0, C1, H, W, k, Cout = case
-    if ds_impl == "tmem" and not _tmem_takes(H, W, k, Cout):
-        pytest.skip("not a shape of the TMEM-operand kernel (k = 2, tile-pair waste <= 35 %)")
-    if ds_impl == "smem" and Cout > 128:
-        pytest.skip("the shared-memory-operand kernel takes Cout <= 128")
     C = C0 + C1
     x = rnd(B, C, H, W)
     dw_w, dw_b = rnd(k * C, 1, 3, 3), rnd(k * C)
@@ -252,9 +239,9 @@ def test_dsconv_fused_matches_oracle(case, mode, ds_impl):
     assert y is not None, f"fused kernel refused an eligible shape {case}"
     torch.cuda.synchronize()
     assert_close(y, ref, PW_TOL[mode], f"dsconv {mode} {case}")
-    # no bias / no affine / no relu (+ statistics: shared-memory-operand kernel only)
+    # no bias / no affine / no relu (+ statistics: Cout <= 128, all channels in one pass)
     pre = O.pointwise1x1(O.depthwise3x3(x.astype(np.float64), dw_w, None, k), pw_w, None)
-    if ds_impl == "tmem":
+    if Cout > 128:
         y2 = ops.dsconv(x0, dev(dw_w), None, k, dev(pw_w), None, None, False, x1=x1, mode=mode)
         assert_close(y2, pre, PW_TOL[mode], f"dsconv plain {mode} {case}")
         return
@@ -269,8 +256,6 @@ def test_dsconv_fused_matches_oracle(case, mode, ds_impl):
 def test_dsconv_with_fused_outconv_matches_oracle(case, mode, ds_impl):
     """smaat_dsconv_outconv_fwd: DS conv -> BN/ReLU -> OutConv(Cout -> 1) with the activation kept in registers."""
     B, C0, C1, H, W, k, Cout = case
-    if ds_impl == "tmem" and not _tmem_takes(H, W, k, Cout):
-        pytest.skip("not a shape of the TMEM-operand kernel")
     C = C0 + C1
     x = rnd(B, C, H, W)
     dw_w, dw_b = rnd(k * C, 1, 3, 3), rnd(k * C)
@@ -292,6 +277,10 @@ def test_dsconv_with_fused_outconv_matches_oracle(case, mode, ds_impl):
 def test_dsconv_ineligible_shapes_fall_back():
     # Cout > 128 / tiny planes are not fused: ops.dsconv says so and the module path still gives the right answer
     assert ops.dsconv(dev(rnd(1, 16, 8, 8)), dev(rnd(32, 1, 3, 3)), None, 2, dev(rnd(256, 32, 1, 1)), None, None, False) is None
+    # Cout = 256 is fused in passes of 128, but the fused OutConv needs every channel in one pass: declined, not an error
+    x32, w256 = dev(rnd(1, 16, 32, 32)), dev(rnd(256, 32, 1, 1))
+    assert ops.dsconv(x32, dev(rnd(32, 1, 3, 3)), None, 2, w256, None, None, True) is not None
+    assert ops.dsconv(x32, dev(rnd(32, 1, 3, 3)), None, 2, w256, None, None, True, outconv=(dev(rnd(1, 256, 1, 1)), None)) is None
     m = S.DepthwiseSeparableConv(16, 256, 3, padding=1, kernels_per_layer=2).cuda().eval()
     x = rnd(1, 16, 18, 18)
     sd = {k_: v.detach().cpu().numpy() for k_, v in m.state_dict().items()}
@@ -301,8 +290,8 @@ def test_dsconv_ineligible_shapes_fall_back():
 
 
 def test_dsconv_with_batch_statistics_only_where_a_kernel_has_them():
-    """smaat_dsconv_eligible2(with_stats): the TMEM-operand kernel has no batch-statistics epilogue, so a request with `stats`
-    is either taken by the shared-memory-operand kernel (Cout <= 128) or declined (Cout = 256) -- never an error -- and
+    """smaat_dsconv_eligible2(with_stats): batch statistics need all channels in one pass, so a request with `stats` is
+    either taken by the fused kernel (Cout <= 128) or declined (Cout = 256, passes of 128) -- never an error -- and
     DepthwiseSeparableConv.run(stats=...) gives the same result and the same sums either way."""
     for cout, fused in ((64, True), (256, False)):
         m = S.DepthwiseSeparableConv(16, cout, 3, padding=1, kernels_per_layer=2).cuda().eval()

@@ -144,7 +144,7 @@ def test_gradients_match_cpu_autograd(name, train):
 
 def test_training_step_reduces_loss_and_matches_cpu_one_step():
     """One Adam step on the reference's loss (regression_lightning.py:57-65: mse(sum)/B) moves the parameters the same
-    way on the B200 path and on the CPU port."""
+    way on the GPU path and on the CPU port."""
     name = "unet_12_1_k2_train"
     sd_np, xs_np = case_tensors(name, np.float64)
     tgt = np.random.default_rng(5).uniform(0, 1, (xs_np[0].shape[0], 32, 32))

@@ -1,4 +1,4 @@
-"""BASELINE configs[4]: high-res 576x576 inference, batch 8, one B200 (same pixel count per step as 32 x 288^2)."""
+"""BASELINE configs[4]: high-res 576x576 inference, batch 8, one GPU (same pixel count per step as 32 x 288^2)."""
 import json, sys, torch
 sys.path.insert(0, ".")
 import smaat_unet_b200 as S
@@ -16,5 +16,5 @@ for mode in ("tf32x3", "tf32"):
     for i in range(20): sess.forward(xs[i % 2])
     e1.record(); torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / 20
-    print(json.dumps({"workload": "configs[4]: SmaAt-UNet forward (eval), batch=8, 12->1ch 576x576, 1xB200", "pointwise": mode,
+    print(json.dumps({"workload": "configs[4]: SmaAt-UNet forward (eval), batch=8, 12->1ch 576x576, 1 GPU", "pointwise": mode,
                       "frames_per_s": 8 / (ms * 1e-3), "ms_per_step": ms, "launches_per_forward": int(sess.launches_per_forward)}))

@@ -1,4 +1,4 @@
-"""Run one kernel shape a few times (for ncu).  usage: prof_one.py dsconv|pw|dw <mode>"""
+"""Run one kernel shape a few times (for a profiler).  usage: prof_one.py dsconv|pw|dw <mode>"""
 import sys, torch
 sys.path.insert(0, ".")
 import smaat_unet_b200 as S
