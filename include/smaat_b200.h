@@ -279,6 +279,31 @@ int smaat_pixel_shuffle2_pad_fwd(const float* t, const float* bias, float* y, in
                                  int Wo, void* stream);
 int smaat_pixel_shuffle2_pad_bwd(const float* g, int64_t g_bstride, float* dt, int B, int Cout, int H, int W, int Ho, int Wo, void* stream);
 
+/* ---- dense 3x3 conv, padding 1: nn.Conv2d(Cin, Cout, 3, padding=1) of DoubleConv (models/unet_parts.py:16,19), with the
+ * eval BatchNorm2d + ReLU that follow it (:17-18, 20-21) in the epilogue, over the virtual concat [x0, x1] of Up
+ * (unet_parts.py:63, torch.cat never materialised).
+ * smaat_conv3x3_pack_weight: w (Cout, C0 + C1, 3, 3) -> wp (Cout, 9, C0p + C1p), Cxp = Cx rounded up to 32, zero padded:
+ *   wp[o][3 dy + dx][c] = w[o][c][dy][dx] with x1's channels at offset C0p.  flip_transpose != 0 packs the input-gradient
+ *   weight instead: wp (C0 + C1, 9, Coutp), wp[c][3 dy + dx][o] = w[o][c][2 - dy][2 - dx]; run it through smaat_conv3x3_fwd
+ *   with x0 = dz (Cout channels, C1 = 0) and Cout = C0 + C1 to get dX (split [dx0 | dx1] by channel).
+ * smaat_conv3x3_fwd: y[b,o,p] = act(scale[o] * sum_{c,dy,dx} w[o,c,dy,dx] in[b,c,p+(dy-1,dx-1)] + shift[o]), zero outside the
+ *   image; scale/shift/stats/relu/y_bstride as smaat_pw1x1_fwd (affine for Cout <= 1024).  mode: SMAAT_PW_FP32_SIMT (CUDA
+ *   cores, any shape), SMAAT_PW_TF32 / SMAAT_PW_TF32X3 (wgmma implicit GEMM; wp_lo = the lo parts of smaat_split_tf32 of wp in
+ *   TF32X3, wp the hi parts).  The tensor-core modes return SMAAT_E_UNSUPPORTED unless W % 4 == 0, Cout >= 8, x0 / x1 / wp
+ *   16-byte aligned and the batch strides multiples of 4; smaat_conv3x3_tc_eligible answers the same test (1/0).
+ * smaat_conv3x3_bwd_weight: dW (Cout, C0 + C1, 3, 3) += sum_{b,p} dz[b,o,p] in[b,c,p+(dy-1,dx-1)], in the nn.Conv2d layout.
+ *   dz: (B, Cout, H, W) dense.  mode: SMAAT_PW_FP32_SIMT (CUDA cores, any shape) or SMAAT_PW_TF32 / SMAAT_PW_TF32X3 (wgmma,
+ *   split over pixel chunks; SMAAT_E_UNSUPPORTED unless W % 4 == 0, dz / x0 / x1 16-byte aligned and the batch strides
+ *   multiples of 4).  The bias gradient is the dz_sum of smaat_bn_bwd_coeffs. */
+int smaat_conv3x3_pack_weight(const float* w, float* wp, int Cout, int C0, int C1, int flip_transpose, void* stream);
+int smaat_conv3x3_tc_eligible(const float* x0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                              const float* wp, int W, int Cout);
+int smaat_conv3x3_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                      const float* wp, const float* wp_lo, const float* scale, const float* shift, float* y, int64_t y_bstride,
+                      double* stats, int B, int H, int W, int Cout, int relu, int mode, void* stream);
+int smaat_conv3x3_bwd_weight(const float* dz, const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1,
+                             int64_t x1_bstride, float* dW, int B, int H, int W, int Cout, int mode, void* stream);
+
 /* ---- optimizer step (reference models/regression_lightning.py:47-48, train_SmaAtUNet.py:25: torch.optim.Adam with its
  * defaults) over flat fp32 buffers of n floats (n % 4 == 0, 16-byte aligned; parameters, gradients, first and second moment
  * share one layout; padding must carry zero gradients).  lr and step are DEVICE scalars (fp32; step = completed steps,

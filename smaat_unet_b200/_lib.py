@@ -67,6 +67,10 @@ SIGNATURES = {
     "smaat_pixel_shuffle2_pad_fwd": [_p, _p, _p, _l, _i, _i, _i, _i, _i, _i, _p],
     "smaat_pixel_shuffle2_pad_bwd": [_p, _l, _p, _i, _i, _i, _i, _i, _i, _p],
     "smaat_adam_step": [_p, _p, _p, _p, _l, _p, _p, C.c_double, C.c_double, C.c_double, _p],
+    "smaat_conv3x3_pack_weight": [_p, _p, _i, _i, _i, _i, _p],
+    "smaat_conv3x3_tc_eligible": [_p, _l, _p, _i, _l, _p, _i, _i],
+    "smaat_conv3x3_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _p],
+    "smaat_conv3x3_bwd_weight": [_p, _p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _p],
 }
 _SPECIAL = {
     "smaat_abi_version": ([], _i),

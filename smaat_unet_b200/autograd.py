@@ -56,6 +56,41 @@ class DoubleConvDSFn(torch.autograd.Function):
         return (None, dx if need[1] else None, dx1 if need[2] else None, *pg)
 
 
+class DoubleConvFn(torch.autograd.Function):
+    """(Conv2d 3x3 => BN => ReLU) * 2 over the virtual concat [x, x1] (unet_parts.py:8-25)."""
+
+    @staticmethod
+    def params(mod):
+        c0, bn0, c1, bn1 = mod.double_conv[0], mod.double_conv[1], mod.double_conv[3], mod.double_conv[4]
+        out = []
+        for p in (c0.weight, c0.bias, bn0.weight, bn0.bias, c1.weight, c1.bias, bn1.weight, bn1.bias):
+            if p is None:
+                raise NotImplementedError("DoubleConv without conv bias / BN affine parameters is not supported in the autograd path")
+            out.append(p)
+        return out
+
+    @staticmethod
+    def run(mod, x, x1=None):
+        return DoubleConvFn.apply(mod, x, x1, *DoubleConvFn.params(mod))
+
+    @staticmethod
+    def forward(ctx, mod, x, x1, *params):
+        x = ops._dense(x, "x")
+        x1 = ops._dense(x1, "x1") if x1 is not None else None
+        out, saved = Fn.dense_double_conv_fwd(mod, x, x1)
+        ctx.mod, ctx.saved = mod, saved
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        need = ctx.needs_input_grad
+        _check_saved(ctx, "DoubleConv")
+        dx, dx1, pg = Fn.dense_double_conv_bwd(ctx.mod, ctx.saved, g, need_x=need[1], need_x1=need[2])
+        ctx.saved = None
+        pg = [pgi if (need[3 + i] and not Fn.is_sunk(prm)) else None for i, (pgi, prm) in enumerate(zip(pg, DoubleConvFn.params(ctx.mod)))]
+        return (None, dx if need[1] else None, dx1 if need[2] else None, *pg)
+
+
 class DSConvFn(torch.autograd.Function):
     """A standalone DepthwiseSeparableConv (layers.py:47-50): depthwise then pointwise, both biases, no BN/activation."""
 

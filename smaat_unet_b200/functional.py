@@ -7,6 +7,7 @@ PyTorch arithmetic fallback; torch supplies memory, streams and the autograd tap
 
 Reference semantics restated (file:line under /root/reference):
   DoubleConvDS  models/unet_parts_depthwise_separable.py:17-36   CBAM  models/layers.py:90-141
+  DoubleConv    models/unet_parts.py:15-22
   BatchNorm2d train mode: batch mean / biased variance normalise, running stats get the unbiased
   variance with momentum 0.1 (SURVEY 8a row a4).
 """
@@ -79,6 +80,24 @@ def double_conv_fwd(mod, x, x1=None):
     sc1, sh1, m1, i1 = bn_scale_shift(bn1, S1, n)
     out = ops.affine_act(z1, sc1, sh1, "relu")
     saved = dict(x=x, x1=x1, d0=d0, z0=z0, sc0=sc0, sh0=sh0, m0=m0, i0=i0, d1=d1, z1=z1, sc1=sc1, sh1=sh1, m1=m1, i1=i1, n=n)
+    return out, saved
+
+
+def dense_double_conv_fwd(mod, x, x1=None):
+    """DoubleConv forward (unet_parts.py:15-22) over [x, x1] with explicit BatchNorm (batch statistics in train mode).
+    The second conv's input relu(BN0(z0)) is materialised (affine_act): its weight gradient needs it.  Returns (out, saved)."""
+    bn0, bn1 = mod.double_conv[1], mod.double_conv[4]
+    B, _, H, W = x.shape
+    n = B * H * W
+    S0 = ops.new_stats(bn0.num_features, x.device)
+    S1 = ops.new_stats(bn1.num_features, x.device)
+    z0 = mod.conv(0, x, x1, shift=_p(mod.double_conv[0].bias), stats=S0)
+    sc0, sh0, m0, i0 = bn_scale_shift(bn0, S0, n)
+    a0 = ops.affine_act(z0, sc0, sh0, "relu")
+    z1 = mod.conv(3, a0, shift=_p(mod.double_conv[3].bias), stats=S1)
+    sc1, sh1, m1, i1 = bn_scale_shift(bn1, S1, n)
+    out = ops.affine_act(z1, sc1, sh1, "relu")
+    saved = dict(x=x, x1=x1, z0=z0, a0=a0, sc0=sc0, sh0=sh0, m0=m0, i0=i0, z1=z1, sc1=sc1, sh1=sh1, m1=m1, i1=i1, n=n)
     return out, saved
 
 
@@ -233,6 +252,39 @@ def double_conv_bwd(mod, saved, g, need_x=True, need_x1=True):
     del d0
     dx, dx1 = dw_bwd(dd0, ds0.depthwise.weight, s["x"], s["x1"], None, None, k, g0[0], g0[1], need_input=need_in)
     return dx, dx1, g0 + g1
+
+
+def conv3x3_bwd(mod, idx, dz, x0, x1, dW, need_input=True):
+    """Backward of DoubleConv conv ``idx`` over [x0, x1]: accumulates dW; returns (dx0, dx1).  The input gradient is the
+    forward kernel on dz with the flipped, transposed weight; it splits over the virtual concat as channel views."""
+    ops.conv3x3_bwd_weight(dz, x0, x1, dW)
+    if not need_input:
+        return None, None
+    C0, C1 = x0.shape[1], (x1.shape[1] if x1 is not None else 0)
+    wt, hi, lo = mod.packed(idx, C0, C1, flip_transpose=True)
+    dx = ops.conv3x3(dz, wt, C0 + C1, None, None, False, w_split=(hi, lo) if hi is not None else None)
+    return (dx[:, :C0], dx[:, C0:]) if C1 else (dx, None)
+
+
+def dense_double_conv_bwd(mod, saved, g, need_x=True, need_x1=True):
+    """Backward of dense_double_conv_fwd.  Returns (dx, dx1, [8 parameter grads in DoubleConvFn.PARAMS order])."""
+    c0, bn0, c1, bn1 = mod.double_conv[0], mod.double_conv[1], mod.double_conv[3], mod.double_conv[4]
+    s = saved
+    n = s["n"]
+    g = ops._dense(g, "grad_output")
+    pg = [_zeros_like_param(p) for p in (c0.weight, c0.bias, bn0.weight, bn0.bias, c1.weight, c1.bias, bn1.weight, bn1.bias)]
+    tr0 = bn0.training or not bn0.track_running_stats
+    tr1 = bn1.training or not bn1.track_running_stats
+    # second conv: out = relu(BN1(z1)), z1 = conv(a0) + b1; the conv bias gradient is sum dz1, from the BN sums
+    dz1 = bn_act_bwd(g, s["z1"], s["sc1"], s["sh1"], bn1.weight.detach(), s["m1"], s["i1"], n, tr1, 1, pg[6], pg[7], dz_sum=pg[5])
+    da0, _ = conv3x3_bwd(mod, 3, dz1, s["a0"], None, pg[4])
+    del dz1
+    # first conv: a0 = relu(BN0(z0)), z0 = conv([x, x1]) + b0
+    dz0 = bn_act_bwd(da0, s["z0"], s["sc0"], s["sh0"], bn0.weight.detach(), s["m0"], s["i0"], n, tr0, 1, pg[2], pg[3], dz_sum=pg[1])
+    del da0
+    need_in = need_x or (s["x1"] is not None and need_x1)
+    dx, dx1 = conv3x3_bwd(mod, 0, dz0, s["x"], s["x1"], pg[0], need_input=need_in)
+    return dx, dx1, pg
 
 
 def cbam_bwd(mod, saved, g):

@@ -1,4 +1,4 @@
-"""SmaAt-UNet assembled from the H100 drop-in blocks.
+"""SmaAt-UNet and the paper's dense baselines (UNet, UNetAttention) assembled from the H100 drop-in blocks.
 
 Same constructor, attribute names (hence state_dict keys) and forward graph as the
 reference's ``models/SmaAt_UNet.py:7-57``; provided so the full model can be built where the
@@ -10,7 +10,7 @@ from __future__ import annotations
 
 from torch import nn
 
-from .modules import CBAM, DoubleConvDS, DownDS, OutConv, UpDS
+from .modules import CBAM, DoubleConv, DoubleConvDS, Down, DownDS, OutConv, Up, UpDS
 
 _ENC = (64, 128, 256, 512)
 
@@ -60,3 +60,78 @@ class SmaAt_UNet(nn.Module):
         for i in range(3):
             y = getattr(self, f"up{i + 1}")(y, att[3 - i])
         return self.up4(y, att[0], outconv=self.outc)
+
+
+class UNet(nn.Module):
+    """The dense baseline of ``models/unet_precip_regression_lightning.py:7-38`` (the Lightning class without its training
+    plumbing): same attribute names (hence the reference's 128 state_dict keys with ``bilinear=True``) and forward order."""
+
+    def __init__(self, n_channels, n_classes, bilinear=True):
+        super().__init__()
+        self.n_channels, self.n_classes, self.bilinear = n_channels, n_classes, bilinear
+        self.inc = DoubleConv(n_channels, 64)
+        self.down1 = Down(64, 128)
+        self.down2 = Down(128, 256)
+        self.down3 = Down(256, 512)
+        factor = 2 if bilinear else 1
+        self.down4 = Down(512, 1024 // factor)
+        self.up1 = Up(1024, 512 // factor, bilinear)
+        self.up2 = Up(512, 256 // factor, bilinear)
+        self.up3 = Up(256, 128 // factor, bilinear)
+        self.up4 = Up(128, 64, bilinear)
+        self.outc = OutConv(64, n_classes)
+
+    def forward(self, x):
+        x1 = self.inc(x)
+        x2 = self.down1(x1)
+        x3 = self.down2(x2)
+        x4 = self.down3(x3)
+        x5 = self.down4(x4)
+        x = self.up1(x5, x4)
+        x = self.up2(x, x3)
+        x = self.up3(x, x2)
+        x = self.up4(x, x1)
+        return self.outc(x)
+
+
+class UNetAttention(nn.Module):
+    """``models/unet_precip_regression_lightning.py:41-83``: UNet with a CBAM on every skip (178 state_dict keys with
+    ``bilinear=True``).  ``downN`` runs on the un-attended map right after ``cbamN`` did, so the CBAM hands it its 2x2 max-pool."""
+
+    def __init__(self, n_channels, n_classes, bilinear=True, reduction_ratio=16):
+        super().__init__()
+        self.n_channels, self.n_classes, self.bilinear = n_channels, n_classes, bilinear
+        r = reduction_ratio
+        self.inc = DoubleConv(n_channels, 64)
+        self.cbam1 = CBAM(64, reduction_ratio=r)
+        self.down1 = Down(64, 128)
+        self.cbam2 = CBAM(128, reduction_ratio=r)
+        self.down2 = Down(128, 256)
+        self.cbam3 = CBAM(256, reduction_ratio=r)
+        self.down3 = Down(256, 512)
+        self.cbam4 = CBAM(512, reduction_ratio=r)
+        factor = 2 if bilinear else 1
+        self.down4 = Down(512, 1024 // factor)
+        self.cbam5 = CBAM(1024 // factor, reduction_ratio=r)
+        self.up1 = Up(1024, 512 // factor, bilinear)
+        self.up2 = Up(512, 256 // factor, bilinear)
+        self.up3 = Up(256, 128 // factor, bilinear)
+        self.up4 = Up(128, 64, bilinear)
+        self.outc = OutConv(64, n_classes)
+
+    def forward(self, x):
+        x1 = self.inc(x)
+        x1Att = self.cbam1(x1)
+        x2 = self.down1(x1)
+        x2Att = self.cbam2(x2)
+        x3 = self.down2(x2)
+        x3Att = self.cbam3(x3)
+        x4 = self.down3(x3)
+        x4Att = self.cbam4(x4)
+        x5 = self.down4(x4)
+        x5Att = self.cbam5(x5)
+        x = self.up1(x5Att, x4Att)
+        x = self.up2(x, x3Att)
+        x = self.up3(x, x2Att)
+        x = self.up4(x, x1Att)
+        return self.outc(x)

@@ -6,7 +6,7 @@ constructor signatures, forward signatures and ``state_dict`` keys as
 * ``models/layers.py``: DepthwiseSeparableConv (:34-50), ChannelAttention (:90-111),
   SpatialAttention (:114-129), CBAM (:132-141)
 * ``models/unet_parts_depthwise_separable.py``: DoubleConvDS (:10-39), DownDS (:42-53), UpDS (:56-86)
-* ``models/unet_parts.py``: OutConv (:67-73)
+* ``models/unet_parts.py``: DoubleConv (:8-25), Down (:28-36), Up (:39-64), OutConv (:67-73)
 
 so checkpoints trained with the reference load unchanged (``calc_metrics_test_set.py:114``).
 The parameter containers are ordinary torch modules (``nn.Conv2d`` / ``nn.BatchNorm2d`` /
@@ -247,24 +247,9 @@ class DownDS(nn.Module):
         return self.maxpool_conv[1].run(pooled)
 
 
-class UpDS(_CachingModule):
-    """models/unet_parts_depthwise_separable.py:56-86 -- upsample x2, pad to the skip, concat, DoubleConvDS.
-
-    The concat is never materialised: the first depthwise kernel reads [skip, up] as a virtual concat.
-    ``bilinear=False`` (ConvTranspose2d(in, in // 2, 2, stride=2), :72-73): kernel = stride, so the transposed conv is one
-    wgmma pointwise GEMM to the 4 packed taps + a pixel shuffle (csrc/convt.cu).
-    """
-
-    def __init__(self, in_channels, out_channels, bilinear=True, kernels_per_layer=1):
-        super().__init__()
-        self.bilinear = bilinear
-        if bilinear:
-            self.up = nn.Upsample(scale_factor=2, mode="bilinear", align_corners=True)
-            self.conv = DoubleConvDS(in_channels, out_channels, in_channels // 2, kernels_per_layer=kernels_per_layer)
-        else:
-            self.up = nn.ConvTranspose2d(in_channels, in_channels // 2, kernel_size=2, stride=2)
-            self.conv = DoubleConvDS(in_channels, out_channels, kernels_per_layer=kernels_per_layer)
-        self._packed = None
+class _TransposedUp(_CachingModule):
+    """ConvTranspose2d(Cin, Cin // 2, kernel_size=2, stride=2) + F.pad of Up / UpDS (``bilinear=False``): kernel = stride, so the
+    transposed conv is one wgmma pointwise GEMM to the 4 packed taps + a pixel shuffle (csrc/convt.cu)."""
 
     def _drop_caches(self):
         self._packed = None
@@ -284,13 +269,34 @@ class UpDS(_CachingModule):
     def _up_transposed(self, x1, Ho, Wo):
         up = self.up
         if (up.kernel_size, up.stride, up.padding, up.output_padding, up.dilation, up.groups) != ((2, 2), (2, 2), (0, 0), (0, 0), (1, 1), 1):
-            raise NotImplementedError("UpDS: only the reference's ConvTranspose2d(kernel_size=2, stride=2) is implemented (parts_ds.py:72)")
+            raise NotImplementedError(f"{type(self).__name__}: only the reference's ConvTranspose2d(kernel_size=2, stride=2) is implemented "
+                                      "(parts_ds.py:72, unet_parts.py:50)")
         wp, split = self._packed_weight()
         if _needs_grad(up, x1):
             from .autograd import ConvT2x2PadFn
             return ConvT2x2PadFn.apply(x1, up.weight, up.bias, Ho, Wo, wp, split)
         t = ops.pw1x1(x1, wp, None, None, False, w_split=split)
         return ops.pixel_shuffle2_pad(t, up.bias.detach() if up.bias is not None else None, up.out_channels, Ho, Wo)
+
+
+class UpDS(_TransposedUp):
+    """models/unet_parts_depthwise_separable.py:56-86 -- upsample x2, pad to the skip, concat, DoubleConvDS.
+
+    The concat is never materialised: the first depthwise kernel reads [skip, up] as a virtual concat.
+    ``bilinear=False`` (ConvTranspose2d(in, in // 2, 2, stride=2), :72-73): kernel = stride, so the transposed conv is one
+    wgmma pointwise GEMM to the 4 packed taps + a pixel shuffle (csrc/convt.cu).
+    """
+
+    def __init__(self, in_channels, out_channels, bilinear=True, kernels_per_layer=1):
+        super().__init__()
+        self.bilinear = bilinear
+        if bilinear:
+            self.up = nn.Upsample(scale_factor=2, mode="bilinear", align_corners=True)
+            self.conv = DoubleConvDS(in_channels, out_channels, in_channels // 2, kernels_per_layer=kernels_per_layer)
+        else:
+            self.up = nn.ConvTranspose2d(in_channels, in_channels // 2, kernel_size=2, stride=2)
+            self.conv = DoubleConvDS(in_channels, out_channels, kernels_per_layer=kernels_per_layer)
+        self._packed = None
 
     def forward(self, x1, x2, outconv=None):
         if not self.bilinear:
@@ -301,6 +307,148 @@ class UpDS(_CachingModule):
         else:
             up = ops.upsample2x_pad(x1, x2.shape[2], x2.shape[3])
         return self.conv.run(x2, x1=up, outconv=outconv)
+
+
+class DoubleConv(_CachingModule):
+    """models/unet_parts.py:8-25 -- (Conv2d 3x3 => BN => ReLU) * 2, the dense block of UNet / UNetAttention.
+
+    Eval mode runs 2 kernels: conv3x3 (+folded BN +ReLU) twice (csrc/conv3x3_tc.cu; the exact CUDA-core kernel in 'fp32'
+    mode and for the shapes the tensor-core kernel declines).  ``run(x, x1)`` reads the virtual concat [x, x1].
+    """
+
+    def __init__(self, in_channels, out_channels, mid_channels=None):
+        super().__init__()
+        if not mid_channels:
+            mid_channels = out_channels
+        self.double_conv = nn.Sequential(
+            nn.Conv2d(in_channels, mid_channels, kernel_size=3, padding=1),
+            nn.BatchNorm2d(mid_channels),
+            nn.ReLU(inplace=True),
+            nn.Conv2d(mid_channels, out_channels, kernel_size=3, padding=1),
+            nn.BatchNorm2d(out_channels),
+            nn.ReLU(inplace=True),
+        )
+        self._fold = {}
+        self._packed = {}
+
+    def _drop_caches(self):
+        self._fold = {}
+        self._packed = {}
+
+    def _check(self):
+        for idx in (0, 3):
+            c = self.double_conv[idx]
+            if (c.kernel_size, c.padding, c.stride, c.dilation, c.groups) != ((3, 3), (1, 1), (1, 1), (1, 1), 1) or c.padding_mode != "zeros":
+                raise NotImplementedError("smaat_unet_b200 implements the dense conv the reference uses: 3x3, padding=1, stride 1, "
+                                          "groups=1 (unet_parts.py:16,19)")
+
+    def packed(self, idx, C0, C1=0, flip_transpose=False):
+        """(packed weight, tf32 hi, tf32 lo) of conv ``idx`` for inputs [C0 | C1] (hi/lo None unless 'tf32x3'); with
+        ``flip_transpose`` the input-gradient form.  Cached on the weight's version; re-derived inside a training capture."""
+        w = self.double_conv[idx].weight
+        mode = ops.get_pointwise_mode()
+        key = (_versions(w), mode)
+        slot = (idx, C0, C1, bool(flip_transpose))
+        in_train_capture = self.training and torch.cuda.is_current_stream_capturing()
+        hit = self._packed.get(slot)
+        if in_train_capture or hit is None or hit[0] != key:
+            with torch.no_grad():
+                wp = ops.conv3x3_pack_weight(w.detach(), C0, C1, flip_transpose)
+                hi, lo = ops.split_tf32(wp) if mode == "tf32x3" else (None, None)
+            hit = (None if in_train_capture else key, (wp, hi, lo))
+            self._packed[slot] = hit
+        return hit[1]
+
+    def conv(self, idx, x, x1=None, scale=None, shift=None, relu=False, stats=None):
+        """Conv ``idx`` (0 or 3) over [x, x1] with the epilogue y = act(scale * acc + shift)."""
+        self._check()
+        C0, C1 = x.shape[1], (x1.shape[1] if x1 is not None else 0)
+        wp, hi, lo = self.packed(idx, C0, C1)
+        return ops.conv3x3(x, wp, self.double_conv[idx].out_channels, scale, shift, relu, x1=x1,
+                           w_split=(hi, lo) if hi is not None else None, stats=stats)
+
+    def _folded(self, idx):
+        """(scale, shift) of eval BatchNorm idx+1 folded with the bias of conv idx; cached."""
+        conv, bn = self.double_conv[idx], self.double_conv[idx + 1]
+        key = _versions(bn.weight, bn.bias, bn.running_mean, bn.running_var, conv.bias)
+        hit = self._fold.get(idx)
+        if hit is None or hit[0] != key:
+            with torch.no_grad():
+                sc_sh = ops.bn_fold(bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var,
+                                    conv.bias.detach() if conv.bias is not None else None, bn.eps)
+            self._fold[idx] = (key, sc_sh)
+            hit = self._fold[idx]
+        return hit[1]
+
+    def run(self, x, x1=None):
+        ops._req(x, "input", 4)
+        if x1 is not None:
+            ops._req(x1, "input", 4)
+        self._check()
+        if _needs_grad(self, x, x1):
+            from .autograd import DoubleConvFn
+            return DoubleConvFn.run(self, x, x1)
+        bns = (self.double_conv[1], self.double_conv[4])
+        if self.training or any(not bn.track_running_stats or bn.running_mean is None for bn in bns):
+            from . import functional as Fn       # batch statistics (and running-stat update), no tape
+            return Fn.dense_double_conv_fwd(self, x, x1)[0]
+        s0, t0 = self._folded(0)
+        y = self.conv(0, x, x1, scale=s0, shift=t0, relu=True)
+        s1, t1 = self._folded(3)
+        return self.conv(3, y, scale=s1, shift=t1, relu=True)
+
+    def forward(self, x):
+        return self.run(x)
+
+
+class Down(nn.Module):
+    """models/unet_parts.py:28-36 -- MaxPool2d(2) then DoubleConv."""
+
+    def __init__(self, in_channels, out_channels):
+        super().__init__()
+        self.maxpool_conv = nn.Sequential(nn.MaxPool2d(2), DoubleConv(in_channels, out_channels))
+
+    def forward(self, x, pooled=None):
+        """``pooled``: MaxPool2d(2)(x) when the caller already has it; a plain call takes the one a preceding ``CBAM(x)``
+        left behind (UNetAttention's ``cbamN(x)`` -> ``downN(x)``, unet_precip_regression_lightning.py:68-77), as DownDS does."""
+        if pooled is None:
+            pooled = _take_stashed_maxpool(x)
+        if pooled is None:
+            if _needs_grad(self, x):
+                from .autograd import MaxPool2Fn
+                pooled = MaxPool2Fn.apply(x) if x.requires_grad else ops.maxpool2(x)
+            else:
+                pooled = ops.maxpool2(ops._dense(x, "input"))
+        return self.maxpool_conv[1].run(pooled)
+
+
+class Up(_TransposedUp):
+    """models/unet_parts.py:39-64 -- upsample x2 (bilinear, or ConvTranspose2d), pad to the skip, concat, DoubleConv.
+
+    The concat is never materialised: the first 3x3 conv reads [skip, up] as a virtual concat."""
+
+    def __init__(self, in_channels, out_channels, bilinear=True):
+        super().__init__()
+        self.bilinear = bilinear
+        if bilinear:
+            self.up = nn.Upsample(scale_factor=2, mode="bilinear", align_corners=True)
+            self.conv = DoubleConv(in_channels, out_channels, in_channels // 2)
+        else:
+            self.up = nn.ConvTranspose2d(in_channels, in_channels // 2, kernel_size=2, stride=2)
+            self.conv = DoubleConv(in_channels, out_channels)
+        self._packed = None
+
+    def forward(self, x1, x2):
+        ops._req(x1, "x1", 4)
+        ops._req(x2, "x2", 4)
+        if not self.bilinear:
+            return self.conv.run(x2, x1=self._up_transposed(x1, x2.shape[2], x2.shape[3]))
+        if torch.is_grad_enabled() and x1.requires_grad:
+            from .autograd import Upsample2xPadFn
+            up = Upsample2xPadFn.apply(x1, x2.shape[2], x2.shape[3])
+        else:
+            up = ops.upsample2x_pad(x1, x2.shape[2], x2.shape[3])
+        return self.conv.run(x2, x1=up)
 
 
 class OutConv(nn.Module):
@@ -451,6 +599,11 @@ def cached_tensors(model):
         elif isinstance(m, DoubleConvDS):
             for _, pair in m._fold.values():
                 out.extend(pair)
+        elif isinstance(m, DoubleConv):
+            for _, pair in m._fold.values():
+                out.extend(pair)
+            for _, trio in m._packed.values():
+                out.extend(t for t in trio if t is not None)
         elif isinstance(m, SpatialAttention) and m._fold is not None:
             out.append(m._fold[1])
     return out

@@ -253,6 +253,89 @@ def dsconv(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, mod
     return y
 
 
+def _pad32(c):
+    return (c + 31) // 32 * 32
+
+
+def conv3x3_pack_weight(w, C0, C1=0, flip_transpose=False):
+    """nn.Conv2d 3x3 weight (Cout, C0 + C1, 3, 3) -> the packed K-major GEMM matrix of smaat_conv3x3_fwd: (Cout, 9 (C0p + C1p)),
+    or with ``flip_transpose`` the input-gradient matrix (C0 + C1, 9 Coutp) (csrc/conv3x3_simt.cu)."""
+    w = _dense(w, "conv.weight")
+    Cout = w.shape[0]
+    assert tuple(w.shape) == (Cout, C0 + C1, 3, 3), f"conv weight {tuple(w.shape)} does not match Cin={C0 + C1}"
+    shape = (C0 + C1, 9 * _pad32(Cout)) if flip_transpose else (Cout, 9 * (_pad32(C0) + _pad32(C1)))
+    wp = torch.empty(shape, device=w.device, dtype=torch.float32)
+    _call("smaat_conv3x3_pack_weight", 8 * wp.numel(), 0, _lib.load().smaat_conv3x3_pack_weight, _ptr(w), _ptr(wp), Cout, C0, C1,
+          int(bool(flip_transpose)), _stream())
+    return wp
+
+
+def conv3x3_takes(x, x1, wp, Cout, mode=None) -> bool:
+    """True when ``conv3x3`` runs the tensor-core kernel for these inputs in ``mode`` (else the CUDA-core one)."""
+    mode = mode or _pw_mode
+    if PW_MODES[mode] == 0:
+        return False
+    x, bs0 = _nchw_bstride(x, "x")
+    C1, bs1 = 0, 0
+    if x1 is not None:
+        x1, bs1 = _nchw_bstride(x1, "x1")
+        C1 = x1.shape[1]
+    return bool(_lib.load().smaat_conv3x3_tc_eligible(_ptr(x), bs0, _ptr(x1), C1, bs1, _ptr(wp), x.shape[3], Cout))
+
+
+def conv3x3(x, wp, Cout, scale, shift, relu, x1=None, mode=None, w_split=None, stats=None):
+    """nn.Conv2d(Cin, Cout, 3, padding=1) over the virtual concat [x, x1] + per-channel affine (+ReLU) (unet_parts.py:16-21,63).
+
+    wp: ``conv3x3_pack_weight`` of the weight; w_split: its cached tf32 (hi, lo) for 'tf32x3'.  Shapes the tensor-core kernel
+    does not take (W % 4 != 0, Cout < 8) run on the exact CUDA-core kernel."""
+    x, bs0 = _nchw_bstride(x, "x")
+    B, C0, H, W = x.shape
+    C1, bs1 = 0, 0
+    if x1 is not None:
+        x1, bs1 = _nchw_bstride(x1, "x1")
+        assert x1.shape[0] == B and x1.shape[2:] == x.shape[2:], "concat inputs must agree in B, H, W"
+        C1 = x1.shape[1]
+    assert wp.shape == (Cout, 9 * (_pad32(C0) + _pad32(C1))), f"packed weight {tuple(wp.shape)} does not match Cin={C0}+{C1}"
+    mode = mode or _pw_mode
+    m = PW_MODES[mode]
+    lib = _lib.load()
+    if m != 0 and not lib.smaat_conv3x3_tc_eligible(_ptr(x), bs0, _ptr(x1), C1, bs1, _ptr(wp), W, Cout):
+        m = 0
+    wlo = None
+    if m == 2:
+        wp, wlo = w_split if w_split is not None else split_tf32(wp)
+    y = torch.empty((B, Cout, H, W), device=x.device, dtype=torch.float32)
+    name = "smaat_conv3x3_fwd" if m else "smaat_conv3x3_fwd_simt"
+    Cin = C0 + C1
+    _call(f"{name}[C{Cin}_N{Cout}_S{H}x{W}]", 4 * B * H * W * (Cin + Cout) + 36 * Cin * Cout, 18 * B * H * W * Cin * Cout, lib.smaat_conv3x3_fwd,
+          _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(wp), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(y), Cout * H * W, _ptr(stats),
+          B, H, W, Cout, int(bool(relu)), m, _stream())
+    return y
+
+
+def conv3x3_bwd_weight(dz, x, x1, dW, mode=None):
+    """dW (Cout, Cin, 3, 3) += the weight gradient of ``conv3x3`` over [x, x1] for output gradient dz (unet_parts.py:16,19).
+    Tensor cores in 'tf32' / 'tf32x3' where the shape allows (W % 4 == 0, aligned), else the exact CUDA-core kernel."""
+    dz = _dense(dz, "dz")
+    x, bs0 = _nchw_bstride(x, "x")
+    B, C0, H, W = x.shape
+    C1, bs1 = 0, 0
+    if x1 is not None:
+        x1, bs1 = _nchw_bstride(x1, "x1")
+        C1 = x1.shape[1]
+    Cout = dz.shape[1]
+    assert tuple(dW.shape) == (Cout, C0 + C1, 3, 3) and dW.is_contiguous()
+    m = PW_MODES[mode or _pw_mode]
+    tc_ok = W % 4 == 0 and bs0 % 4 == 0 and bs1 % 4 == 0 and all(t.data_ptr() % 16 == 0 for t in (dz, x) + ((x1,) if C1 else ()))
+    if not tc_ok:
+        m = 0
+    Cin = C0 + C1
+    name = "smaat_conv3x3_bwd_weight" if m else "smaat_conv3x3_bwd_weight_simt"
+    _call(f"{name}[C{Cin}_N{Cout}_S{H}x{W}]", 4 * B * H * W * (Cin + Cout), 18 * B * H * W * Cin * Cout,
+          _lib.load().smaat_conv3x3_bwd_weight, _ptr(dz), _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(dW), B, H, W, Cout, m, _stream())
+    return dW
+
+
 def bn_fold(gamma, beta, running_mean, running_var, conv_bias, eps):
     """Eval BatchNorm2d -> (scale, shift) for the pw epilogue (parts_ds.py:25,34)."""
     Cn = gamma.numel()

@@ -3,8 +3,8 @@
 The reference has no plugin registry: ``models/SmaAt_UNet.py:2-4`` and
 ``models/unet_precip_regression_lightning.py:1-3`` import the block classes by name.
 ``patch_reference()`` swaps those names in the already-importable reference modules so that
-``SmaAt_UNet`` and the Lightning variants (UNetDS, UNetDSAttention, UNetDSAttention4CBAMs,
-UNetAttention's CBAMs) are constructed from H100 blocks with no change to reference code.
+``SmaAt_UNet`` and the Lightning variants (UNet, UNetAttention, UNetDS, UNetDSAttention,
+UNetDSAttention4CBAMs) are constructed from H100 blocks with no change to reference code.
 """
 from __future__ import annotations
 
@@ -16,10 +16,10 @@ from . import modules as M
 _TARGETS = {
     "models.layers": ("DepthwiseSeparableConv", "ChannelAttention", "SpatialAttention", "CBAM"),
     "models.unet_parts_depthwise_separable": ("DepthwiseSeparableConv", "DoubleConvDS", "DownDS", "UpDS"),
-    "models.unet_parts": ("OutConv",),
+    "models.unet_parts": ("DoubleConv", "Down", "Up", "OutConv"),
     "models.SmaAt_UNet": ("OutConv", "DoubleConvDS", "UpDS", "DownDS", "CBAM"),
     # needs `lightning`; patched only if it imports
-    "models.unet_precip_regression_lightning": ("OutConv", "DoubleConvDS", "UpDS", "DownDS", "CBAM"),
+    "models.unet_precip_regression_lightning": ("Down", "DoubleConv", "Up", "OutConv", "DoubleConvDS", "UpDS", "DownDS", "CBAM"),
 }
 
 
