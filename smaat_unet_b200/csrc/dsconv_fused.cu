@@ -16,18 +16,24 @@
 //               (cp.async.bulk.prefetch.tensor) made bench.py's B = 32 forward slower: 2 220 vs 2 346-2 369 frames/s (H100
 //               80GB HBM3 SXM, 700 W; two runs with, six without), so there is none
 //   warp 1      prefetches the weight chunks (K-major SW128, [hi rows | lo rows]) into their own ring
+//               (warpgroup 0 runs on 24 registers per thread: setmaxnreg hands the rest to the consumers)
 //   warps 4-11  two consumer warpgroups (64 pixels each): wgmma (TF32X3: A_hi B_hi + A_lo B_hi + A_hi B_lo per k-step) into
 //               register accumulators, with the A operand either read by the tensor core from the A ring (A_SMEM) or
-//               loaded into registers from it first, then the epilogue:
-//               scale/shift/ReLU -> NCHW stores (or the fused 1-class OutConv dot product; or BatchNorm batch statistics)
+//               loaded into registers from it first (and split into tf32 hi / lo there in TF32X3 mode), then the epilogue:
+//               scale/shift/ReLU -> NCHW stores (or the fused 1-class OutConv dot product; or BatchNorm batch statistics).
+//               The main loop is pipelined: a chunk's MMAs are committed as one group (two half-chunk groups in the
+//               register form at N_TILE 64 in TF32X3, where registers are short), the wait leaves the newest group in
+//               flight, and the previous chunk's A and B stages are released once it retires.  The register form
+//               alternates two fragment sets so that the set a group in flight reads is never overwritten
 //   warps 12..  NG depthwise producer groups (128 threads each; group g takes every NG-th chunk): 3x3 stencil
 //               from the staged tile with a sliding register window (one LDS.128 per row, edge columns from the
-//               neighbouring quads by shuffle), then write the result into an AS-stage A ring -- as hi and lo tf32 parts
-//               in TF32X3 mode (the split is free here: values are in registers) -- in one of two layouts:
+//               neighbouring quads by shuffle), then write the result into an AS-stage A ring in one of two layouts:
 //                 A_SMEM   [pixel][k] 128B-swizzled K-major tiles, the layout wgmma reads through a descriptor (one scalar
-//                          store per value: a thread's 4 pixels are 4 rows);
-//                 !A_SMEM  [k][pixel] 128B-swizzled tiles (one 16-byte store per 4 pixels), which the consumers load into
-//                          registers conflict-free (tc_common.cuh) and feed to wgmma's register-A form
+//                          store per value: a thread's 4 pixels are 4 rows), as hi and lo tf32 parts in TF32X3 mode;
+//                 !A_SMEM  [k][pixel] 128B-swizzled fp32 tiles (one 16-byte store per 4 pixels), which the consumers load
+//                          into registers conflict-free (tc_common.cuh) and feed to wgmma's register-A form.  Storing fp32
+//                          once instead of hi and lo halves the A ring's shared-memory traffic in TF32X3 mode; the split
+//                          in the consumer is the same tf32_hi / v - hi on the same value, so results are unchanged
 // Which one runs is smaat_set_dsconv_impl's choice (csrc/dsconv_fused.cu, below).
 #include <stdlib.h>
 
@@ -50,7 +56,7 @@ struct DsParams {
   int tiles_x, tiles_y, npass, total_tiles, nchunks;
 };
 
-template <int N_TILE, int KPL, int PW, bool X3>
+template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
 struct DsCfg {
   static constexpr int PH = TC_BM / PW;
   static constexpr int BW = PW + 8, BH = PH + 2;
@@ -58,16 +64,22 @@ struct DsCfg {
   static constexpr int IN_BYTES = CC * BH * BW * 4;            // multiple of 128 for PW in {16,32}
   static constexpr int A_BYTES = TC_BM * TC_BK * 4;            // 16 KB
   static constexpr int B_BYTES = N_TILE * TC_BK * 4;
-  static constexpr int AST_BYTES = (X3 ? 2 : 1) * A_BYTES;     // A ring stage: hi [+ lo]
+  // A ring stage: fp32 (register form: the consumers split hi / lo after loading), or hi [+ lo] (A_SMEM: the tensor core reads
+  // the parts)
+  static constexpr int AST_BYTES = (X3 && A_SMEM ? 2 : 1) * A_BYTES;
   static constexpr int BST_BYTES = (X3 ? 2 : 1) * B_BYTES;     // B ring stage: hi [+ lo]
   static constexpr int OFF_ALO = A_BYTES;
   static constexpr int OFF_BLO = B_BYTES;
-  static constexpr int AS = X3 ? (N_TILE > 64 ? 2 : 3) : 4;     // A ring (the input ring must stay deep enough to cover HBM latency)
   // depthwise producer groups (128 threads each), sized by the register file: the consumers hold N_TILE / 2 accumulators
   // per thread.  NG <= AS always: the per-stage a_empty barriers are tested by phase parity, which is only unambiguous while
   // a group can never be two hand-backs of a stage behind
   static constexpr int NG = N_TILE > 64 ? 1 : 2;
-  static constexpr int BS = X3 ? 2 : 4;                         // weight ring, prefetched by its own warp
+  // A ring and weight ring (prefetched by its own warp).  The consumers hold two stages of each (chunk i in flight, chunk i - 1
+  // retiring); the producers write NG more, the weight loader runs one ahead.  The input ring gets the rest (it must stay deep
+  // enough to cover HBM latency).  TF32X3 in the A_SMEM form (32 KB A stages) keeps two-deep rings at N_TILE 128: deeper ones
+  // leave too little for the input ring
+  static constexpr int AS = X3 ? (A_SMEM ? (N_TILE > 64 ? 2 : 3) : 2 + NG) : 4;
+  static constexpr int BS = X3 ? (A_SMEM && N_TILE > 64 ? 2 : 3) : 4;
   static constexpr int AFF_N = 512;                            // scale | shift | OutConv weights of up to 512 channels
   static constexpr int BAR_BYTES = 512;
   static constexpr int IS_FIT = (224 * 1024 - 1024 - BAR_BYTES - 3 * AFF_N * 4 - AS * AST_BYTES - BS * BST_BYTES) / IN_BYTES;
@@ -80,6 +92,18 @@ struct DsCfg {
   static constexpr uint32_t B_TX = BST_BYTES;
   static constexpr int PROD_WARP = 12;                         // first producer warp
   static constexpr int THREADS = 384 + 128 * NG;               // TMA, loader, 2 idle | 2 consumer warpgroups | producers
+  // setmaxnreg split of the registers a CTA launches with (__launch_bounds__(THREADS, 1), 128 or 96 per thread): warpgroup 0
+  // gives up all but REGS_TMA, the producer group gives some back at N_TILE 128 (its stencil fits in 104 without spills), the
+  // consumers (accumulators + two register-A fragment sets) take the rest: 192 at N_TILE 128, 128 at N_TILE 64
+  static constexpr int REGS_LAUNCH = (65536 / THREADS) / 8 * 8;
+  static constexpr int REGS_TMA = 24;
+  static constexpr int REGS_PROD = N_TILE > 64 ? 104 : REGS_LAUNCH;
+  static constexpr int REGS_MMA = ((THREADS / 128 * REGS_LAUNCH - REGS_TMA - NG * REGS_PROD) / 2) / 8 * 8;
+  static constexpr int REGS_SUM = REGS_TMA + 2 * REGS_MMA + NG * REGS_PROD;
+  static_assert(REGS_SUM <= THREADS / 128 * REGS_LAUNCH && REGS_MMA >= REGS_LAUNCH, "register budget");
+  // k-steps per MMA commit group in the register form.  A whole chunk (4) holds 2 x 32 fragment registers in TF32X3; at
+  // N_TILE 64 the consumers' 128 registers cannot (ptxas would serialise the MMAs), so groups are half chunks there
+  static constexpr int KS = (X3 && N_TILE == 64) ? 2 : TC_BK / 8;
   static_assert(IS >= 2, "input ring");
   static_assert(NG <= AS, "phase-parity barriers");
   static_assert(IN_BYTES % 128 == 0, "TMA destination alignment");
@@ -87,11 +111,11 @@ struct DsCfg {
 };
 
 template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
-__global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
+__global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1)
     dsconv_fused_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
                         const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
                         const DsParams p) {
-  using L = DsCfg<N_TILE, KPL, PW, X3>;
+  using L = DsCfg<N_TILE, KPL, PW, X3, A_SMEM>;
   constexpr int PH = L::PH, BW = L::BW, BH = L::BH, CC = L::CC, IS = L::IS, AS = L::AS, BS = L::BS;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
@@ -149,9 +173,11 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
   }
   __syncthreads();
 
-  if (warp == 0) {
+  if (warp < 4) {
+    // warpgroup 0 keeps few registers: the consumers' two register-A fragment sets need them (all four warps reallocate)
+    regs_dealloc<L::REGS_TMA>();
     // ===== TMA: input halo boxes, running ahead through the IS-deep ring =====
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       uint32_t gc = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         int b, ty, tx, np;
@@ -173,11 +199,8 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
         }
       }
     }
-    return;
-  }
-  if (warp == 1) {
     // ===== weight-ring loader: K-major SW128 chunks (hi [+lo]) of this tile's channel pass, decoupled from the input ring =====
-    if (lane == 0) {
+    if (warp == 1 && lane == 0) {
       uint32_t gc = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         int b, ty, tx, np;
@@ -193,9 +216,9 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
     }
     return;
   }
-  if (warp < 4) return;
 
   if (warp < L::PROD_WARP) {
+    regs_alloc<L::REGS_MMA>();
     // ===== consumer warpgroups: MMAs into register accumulators, then the epilogue =====
     const int wg = (warp >> 2) - 1, wq = warp & 3;
     const int g = lane >> 2, t = lane & 3;
@@ -211,14 +234,28 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
       float acc[N_TILE / 2];
 #pragma unroll
       for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.f;
-      for (int i = 0; i < nch; ++i, ++gc) {
+      // Pipelined k loop: chunk i's MMAs are issued as one group, then the wait leaves that group in flight and retires chunk
+      // i - 1, whose A and B stages go back to the producers and the weight loader.
+      auto release = [&](uint32_t c) {
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&a_empty[c % AS]);
+          mbar_arrive(&b_empty[c % BS]);
+        }
+      };
+      auto wait_stages = [&](const unsigned char*& ast, uint64_t& bd, uint64_t& bl) {
         const int sa = gc % AS, sb = gc % BS;
         mbar_wait(&a_full[sa], (gc / AS) & 1u);
         mbar_wait(&b_full[sb], (gc / BS) & 1u);
-        const unsigned char* ast = a_base + sa * L::AST_BYTES;
-        const uint64_t bd0 = make_kmajor_desc(smem_u32(b_base + sb * L::BST_BYTES));
-        const uint64_t bl0 = make_kmajor_desc(smem_u32(b_base + sb * L::BST_BYTES + L::OFF_BLO));
-        if (A_SMEM) {
+        ast = a_base + sa * L::AST_BYTES;
+        bd = make_kmajor_desc(smem_u32(b_base + sb * L::BST_BYTES));
+        bl = make_kmajor_desc(smem_u32(b_base + sb * L::BST_BYTES + L::OFF_BLO));
+      };
+      if (A_SMEM) {
+        for (int i = 0; i < nch; ++i, ++gc) {
+          const unsigned char* ast;
+          uint64_t bd0, bl0;
+          wait_stages(ast, bd0, bl0);
           const uint32_t a_addr = smem_u32(ast) + (uint32_t)(wg * 64 * 128);   // this warpgroup's 64 rows: 8 swizzle atoms
           const uint64_t ad0 = make_kmajor_desc(a_addr), al0 = make_kmajor_desc(a_addr + L::OFF_ALO);
           wgmma_fence();
@@ -230,35 +267,46 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
               Wgmma<N_TILE>::ss(acc, ad0 + (uint64_t)(2 * kk), bl0 + (uint64_t)(2 * kk), 1u);
             }
           }
-        } else {
-#pragma unroll
-        for (int kk = 0; kk < TC_BK / 8; ++kk) {
-          float vh[4], vl[4];
-          load_a_frag(ast, kk, t, m0, m1, vh);
-          if (X3) load_a_frag(ast + L::OFF_ALO, kk, t, m0, m1, vl);
-          uint32_t ahi[4], alo[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            ahi[e] = __float_as_uint(vh[e]);
-            alo[e] = X3 ? __float_as_uint(vl[e]) : 0u;
-          }
-          wgmma_fence();
-          Wgmma<N_TILE>::rs(acc, ahi, bd0 + (uint64_t)(2 * kk), 1u);
-          if (X3) {
-            Wgmma<N_TILE>::rs(acc, alo, bd0 + (uint64_t)(2 * kk), 1u);
-            Wgmma<N_TILE>::rs(acc, ahi, bl0 + (uint64_t)(2 * kk), 1u);
-          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (i > 0) release(gc - 1);
         }
-        }
-        wgmma_commit();
         wgmma_wait0();
-        wgmma_keep(acc);
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(&a_empty[sa]);
-          mbar_arrive(&b_empty[sb]);
+      } else {
+        // Chunk i's fragments must stay untouched until it retires, so two fragment sets alternate (the loop is unrolled by 2;
+        // no control-flow path may load a set whose chunk is still in flight, or ptxas serialises the MMAs: the odd tail is
+        // outside the loop)
+        // A commit group is KS k-steps: GPC groups per chunk.  Chunk i - 1 has retired once the first group of chunk i is
+        // issued and the wait leaves only that one in flight
+        constexpr int KS = L::KS, GPC = (TC_BK / 8) / KS;
+        const unsigned char* ast = nullptr;
+        uint64_t bd0 = 0, bl0 = 0;
+        auto group = [&](AFrags<X3, KS>& cur, AFrags<X3, KS>& prev, int q) {
+          const int part = q % GPC;
+          if (part == 0) wait_stages(ast, bd0, bl0);
+          load_a_frags<X3, KS>(ast, part * KS, t, m0, m1, cur);
+          mma_a_frags<N_TILE, X3, KS>(acc, cur, bd0, bl0, part * KS);
+          wgmma_wait<1>();
+          wgmma_keep(prev);
+          if (part == 0 && q > 0) release(gc - 1);
+          if (part == GPC - 1) ++gc;
+        };
+        AFrags<X3, KS> fa, fb;
+        const int ngrp = nch * GPC;
+        int q = 0;
+        for (; q + 1 < ngrp; q += 2) {
+          group(fa, fb, q);
+          group(fb, fa, q + 1);
         }
+        if (q < ngrp) group(fa, fb, q);
+        wgmma_wait0();
+        wgmma_keep(fa);
+        wgmma_keep(fb);
       }
+      // the tile's last chunk has retired; its stages are released before the epilogue, so that TMA, the weight loader and
+      // the producers run on through it
+      wgmma_keep(acc);
+      release(gc - 1);
 
       // ----- epilogue: rows g / g + 8 are patch pixels m0 / m1, columns n0 + 8j + 2t + {0, 1}
       const int n0 = np * N_TILE;
@@ -331,6 +379,7 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
 
   {
     // ===== depthwise producer groups: NG groups of 4 warps (warps 12 ..), group g takes every NG-th chunk =====
+    if (L::REGS_PROD < L::REGS_LAUNCH) regs_dealloc<L::REGS_PROD>();
     const int g = (warp - L::PROD_WARP) >> 2;
     const int t = threadIdx.x - 32 * L::PROD_WARP - 128 * g;  // 0..127
     const int Cin = p.C0 + p.C1;
@@ -424,14 +473,8 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
                 }
                 continue;
               }
-              const uint32_t off = a_tile_offset(ci * KPL + kk, m);
-              if (X3) {
-                const float4 h = make_float4(tf32_hi(o4[0]), tf32_hi(o4[1]), tf32_hi(o4[2]), tf32_hi(o4[3]));
-                *reinterpret_cast<float4*>(my_op + off) = h;
-                *reinterpret_cast<float4*>(my_op + L::OFF_ALO + off) = make_float4(o4[0] - h.x, o4[1] - h.y, o4[2] - h.z, o4[3] - h.w);
-              } else {
-                *reinterpret_cast<float4*>(my_op + off) = make_float4(o4[0], o4[1], o4[2], o4[3]);
-              }
+              // fp32 in both modes: the consumers split TF32X3's hi / lo parts after loading (one pass through shared memory)
+              *reinterpret_cast<float4*>(my_op + a_tile_offset(ci * KPL + kk, m)) = make_float4(o4[0], o4[1], o4[2], o4[3]);
             }
           }
         }
@@ -446,12 +489,14 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3>::THREADS, 1)
 template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
 static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl, DsParams p,
                      int B, cudaStream_t st) {
-  using L = DsCfg<N_TILE, KPL, PW, X3>;
+  using L = DsCfg<N_TILE, KPL, PW, X3, A_SMEM>;
   auto kern = dsconv_fused_kernel<N_TILE, KPL, PW, X3, A_SMEM>;
   static std::atomic<uint64_t> attr_mask{0};   // cudaFuncSetAttribute is per device
   if (first_use_on_device(attr_mask)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
     if (e != cudaSuccess) return fail(SMAAT_E_CUDA, "dsconv: smem attribute (%d B): %s", L::TOTAL, cudaGetErrorString(e));
+    int r = check_reg_budget((const void*)kern, L::THREADS, L::REGS_SUM, "dsconv");
+    if (r) return r;
   }
   p.tiles_x = ceil_div(p.W, PW);
   p.tiles_y = ceil_div(p.H, L::PH);

@@ -17,7 +17,9 @@
 // Persistent: one CTA per SM loops over output tiles (tile = blockIdx.x + i*gridDim.x; consecutive tiles share the activation
 // tile and differ in the channel tile, so the re-read hits L2).  Warp 0 = TMA producer, running ahead across tile boundaries
 // through a STAGES-deep shared-memory ring, so the loads of the next tile overlap the epilogue of this one; warpgroups 1-2 =
-// MMA + epilogue.  mbarriers: full (TMA bytes) / empty (8 consumer warps done reading) per stage.
+// MMA + epilogue.  mbarriers: full (TMA bytes) / empty (8 consumer warps done reading) per stage.  The k loop keeps one
+// chunk's MMAs in flight while the previous chunk retires and its stage is released (two register-A fragment sets in turn;
+// setmaxnreg moves warpgroup 0's spare registers to the consumers for them).
 #include <stdlib.h>
 
 #include "tc_common.cuh"
@@ -47,6 +49,11 @@ struct PwTcCfg {
   static constexpr int TOTAL = STAGES * STAGE_BYTES + BAR_BYTES + 2 * AFF_N * 4 + SACC_BYTES + 1024;  // + alignment slack
   static constexpr uint32_t TX_BYTES = A_BYTES + (X3 ? 2 : 1) * B_BYTES;
   static constexpr int THREADS = 384;
+  // setmaxnreg split of the 3 x 168 registers per thread the CTA launches with (__launch_bounds__(384, 1))
+  static constexpr int REGS_TMA = 40, REGS_MMA = 232;
+  static_assert(REGS_TMA + 2 * REGS_MMA <= 3 * 168, "register budget");
+  // the consumers hold two stages (chunk i in flight, chunk i - 1 retiring): the TMA warp needs a third to run ahead
+  static_assert(STAGES >= 3, "ring depth");
   static_assert(TOTAL <= 227 * 1024, "shared memory budget");
 };
 
@@ -86,9 +93,11 @@ __global__ void __launch_bounds__(384, 1)
   }
   __syncthreads();
 
-  if (warp == 0) {
+  if (warp < 4) {
+    // warpgroup 0 keeps few registers: the consumers' two register-A fragment sets need them (all four warps reallocate)
+    regs_dealloc<L::REGS_TMA>();
     // ===== TMA producer =====
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         const int tn = tile % p.tiles_n;
@@ -112,7 +121,7 @@ __global__ void __launch_bounds__(384, 1)
     }
     return;
   }
-  if (warp < 4) return;
+  regs_alloc<L::REGS_MMA>();
 
   // ===== consumer warpgroups 1, 2: MMAs into register accumulators, then affine/ReLU -> NCHW stores =====
   const int wg = (warp >> 2) - 1, wq = warp & 3, cw = warp - 4;   // cw: consumer warp 0..7
@@ -159,36 +168,39 @@ __global__ void __launch_bounds__(384, 1)
     float acc[N_TILE / 2];
 #pragma unroll
     for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.f;
-    for (int i = 0; i < nk; ++i, ++it) {
+    // Pipelined k loop: chunk i's MMAs are issued as one group, then the wait leaves that group in flight and retires chunk
+    // i - 1, whose stage goes back to the TMA warp.  Chunk i's fragments must stay untouched until it retires, so two
+    // fragment sets alternate (the loop is unrolled by 2; no control-flow path may load a set whose chunk is still in
+    // flight, or ptxas serialises the MMAs: the odd tail is outside the loop)
+    auto release = [&](uint32_t c) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[c % STAGES]);
+    };
+    auto chunk = [&](AFrags<X3>& cur, AFrags<X3>& prev, int i) {
       const int s = it % STAGES;
       mbar_wait(&full_bar[s], (it / STAGES) & 1u);
       const unsigned char* st = smem + s * L::STAGE_BYTES;
-      const uint64_t bd0 = make_kmajor_desc(smem_u32(st + L::OFF_B));
-      const uint64_t bl0 = make_kmajor_desc(smem_u32(st + L::OFF_BLO));
-#pragma unroll
-      for (int kk = 0; kk < TC_BK / 8; ++kk) {
-        float v[4];
-        load_a_frag(st, kk, t, m0, m1, v);
-        uint32_t ahi[4], alo[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float h = X3 ? tf32_hi(v[e]) : v[e];
-          ahi[e] = __float_as_uint(h);
-          alo[e] = __float_as_uint(v[e] - h);
-        }
-        wgmma_fence();
-        Wgmma<N_TILE>::rs(acc, ahi, bd0 + (uint64_t)(2 * kk), 1u);
-        if (X3) {
-          Wgmma<N_TILE>::rs(acc, alo, bd0 + (uint64_t)(2 * kk), 1u);
-          Wgmma<N_TILE>::rs(acc, ahi, bl0 + (uint64_t)(2 * kk), 1u);
-        }
-      }
-      wgmma_commit();
-      wgmma_wait0();
-      wgmma_keep(acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[s]);
+      load_a_frags<X3, TC_BK / 8>(st, 0, t, m0, m1, cur);
+      mma_a_frags<N_TILE, X3, TC_BK / 8>(acc, cur, make_kmajor_desc(smem_u32(st + L::OFF_B)),
+                                         make_kmajor_desc(smem_u32(st + L::OFF_BLO)), 0);
+      wgmma_wait<1>();
+      wgmma_keep(prev);
+      if (i > 0) release(it - 1);
+      ++it;
+    };
+    AFrags<X3> fa, fb;
+    int i = 0;
+    for (; i + 1 < nk; i += 2) {
+      chunk(fa, fb, i);
+      chunk(fb, fa, i + 1);
     }
+    if (i < nk) chunk(fa, fb, i);
+    // the tile's last chunk retires before the epilogue; its stage is released first, so TMA runs on through the epilogue
+    wgmma_wait0();
+    wgmma_keep(acc);
+    wgmma_keep(fa);
+    wgmma_keep(fb);
+    release(it - 1);
 
     // ----- epilogue: rows g / g + 8 are pixels m0 / m1, columns n0 + 8j + 2t + {0, 1}
     const int pix0 = tm * TC_BM + m0, pix1 = tm * TC_BM + m1;
@@ -238,6 +250,8 @@ static int launch_tc(const CUtensorMap& mx, const CUtensorMap& mw, const CUtenso
   if (first_use_on_device(attr_mask)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
     if (e != cudaSuccess) return fail(SMAAT_E_CUDA, "pw1x1(tc): smem attribute (%d B): %s", L::TOTAL, cudaGetErrorString(e));
+    int r = check_reg_budget((const void*)kern, L::THREADS, L::REGS_TMA + 2 * L::REGS_MMA, "pw1x1(tc)");
+    if (r) return r;
   }
   p.tiles_m = ceil_div(p.P, TC_BM);
   p.tiles_n = ceil_div(p.Cout, N_TILE);
@@ -290,7 +304,7 @@ int pw1x1_tc_launch(const float* x, const float* w, const float* w_lo, const flo
 
   // one persistent CTA per SM: the smem ring takes ~150-200 KB of the 227 KB
   if (x3) {
-    if (n_tile == 128) return launch_tc<128, 3, true>(mx, mw, mwl, p, B, st);
+    if (n_tile == 128) return launch_tc<128, 4, true>(mx, mw, mwl, p, B, st);
     return launch_tc<64, 5, true>(mx, mw, mwl, p, B, st);
   }
   if (n_tile == 128) return launch_tc<128, 5, false>(mx, mw, mwl, p, B, st);

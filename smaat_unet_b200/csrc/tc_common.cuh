@@ -18,10 +18,46 @@ constexpr int TC_BK = 32;   // k per stage (one 128-byte swizzle row of fp32)
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Wait until at most N committed MMA groups of this warpgroup are still pending.  The pipelined main loops commit one group
+// per k-chunk (or half chunk) and wait with N = 1: the previous group has retired (the shared-memory stages of a chunk whose
+// groups have all retired may be handed back) while the newest one runs.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_keep(float (&d)[N]) {   // accumulators are live across the asynchronous MMAs
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// The same for register-A fragments: placed after the wait that retires the MMAs reading them, it keeps them live (and
+// unmodified) until then, so ptxas neither reuses their registers early nor serialises the MMAs.
+template <int P, int K>
+__device__ __forceinline__ void wgmma_keep(uint32_t (&a)[P][K][4]) {
+#pragma unroll
+  for (int p = 0; p < P; ++p)
+#pragma unroll
+    for (int k = 0; k < K; ++k)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) asm volatile("" : "+r"(a[p][k][e])::"memory");
+}
+
+// Warpgroup register reallocation (setmaxnreg): every warp of the warpgroup executes the same value.  Warpgroups that only
+// issue TMA give registers back, the MMA warpgroups take them, within the CTA's launch allocation.
+template <int R>
+__device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// Host check, once per device before a launch: the sum of the warpgroups' setmaxnreg targets (`regs_sum`, registers per
+// thread summed over the CTA's warpgroups) must fit in what the CTA is launched with, or an increase would wait forever.
+inline int check_reg_budget(const void* kern, int threads, int regs_sum, const char* who) {
+  cudaFuncAttributes a;
+  cudaError_t e = cudaFuncGetAttributes(&a, kern);
+  if (e != cudaSuccess) return fail(SMAAT_E_CUDA, "%s: cudaFuncGetAttributes: %s", who, cudaGetErrorString(e));
+  const int launched = ((a.numRegs + 7) / 8) * 8 * (threads / 128);
+  if (launched < regs_sum)
+    return fail(SMAAT_E_CUDA, "%s: built with %d registers per thread, the warpgroups' register split needs %d per 128 threads > %d",
+                who, a.numRegs, regs_sum, launched);
+  return SMAAT_OK;
 }
 
 // Shared-memory matrix descriptor (sm_90 GMMA layout): addr>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout [62,64)
@@ -66,6 +102,45 @@ __device__ __forceinline__ void load_a_frag(const unsigned char* at, int kk, int
 }
 
 __device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float(__float_as_uint(v) & 0xffffe000u); }
+
+// Register-A fragments of KS k-steps (one commit group; TC_BK / 8 = 4 k-steps make a k-chunk): f[0][kk] = the values (tf32)
+// or their tf32 hi parts (TF32X3), f[1][kk] = the lo remainders v - hi (TF32X3 only).  MMAs in flight read them until
+// their group retires.
+template <bool X3, int KS = TC_BK / 8>
+using AFrags = uint32_t[X3 ? 2 : 1][KS][4];
+
+// Loads k-steps kk0 .. kk0 + KS - 1 from an fp32 A tile at `at` and splits them in registers.
+template <bool X3, int KS>
+__device__ __forceinline__ void load_a_frags(const unsigned char* at, int kk0, int t, int m0, int m1, AFrags<X3, KS>& f) {
+#pragma unroll
+  for (int kk = 0; kk < KS; ++kk) {
+    float v[4];
+    load_a_frag(at, kk0 + kk, t, m0, m1, v);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float h = X3 ? tf32_hi(v[e]) : v[e];
+      f[0][kk][e] = __float_as_uint(h);
+      if (X3) f[X3 ? 1 : 0][kk][e] = __float_as_uint(v[e] - h);
+    }
+  }
+}
+
+// One fence, the MMAs of k-steps kk0 .. kk0 + KS - 1 (TF32X3: A_hi B_hi + A_lo B_hi + A_hi B_lo per k-step) and one commit.
+// bd / bl: descriptors of the chunk's B hi / lo tiles.
+template <int N_TILE, bool X3, int KS>
+__device__ __forceinline__ void mma_a_frags(float (&acc)[N_TILE / 2], const AFrags<X3, KS>& f, uint64_t bd, uint64_t bl, int kk0) {
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < KS; ++kk) {
+    const uint64_t k2 = (uint64_t)(2 * (kk0 + kk));
+    Wgmma<N_TILE>::rs(acc, f[0][kk], bd + k2, 1u);
+    if (X3) {
+      Wgmma<N_TILE>::rs(acc, f[X3 ? 1 : 0][kk], bd + k2, 1u);
+      Wgmma<N_TILE>::rs(acc, f[0][kk], bl + k2, 1u);
+    }
+  }
+  wgmma_commit();
+}
 
 // Sums over the 8 lanes of a fragment column group (lanes with equal t): afterwards lanes 0..3 hold the totals.
 __device__ __forceinline__ float frag_colsum(float v) {
