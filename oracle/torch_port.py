@@ -62,10 +62,13 @@ def cbam(x, sd, p, training=False):
     def mlp(v):
         return F.linear(F.relu(F.linear(v, sd[ca + ".1.weight"], sd[ca + ".1.bias"])), sd[ca + ".3.weight"], sd[ca + ".3.bias"])
 
-    s = torch.sigmoid(mlp(x.mean(dim=(2, 3))) + mlp(x.amax(dim=(2, 3))))
+    # The max pools use the reference's ops (AdaptiveMaxPool2d(1), torch.max(dim=1)), not Tensor.amax: the forward values
+    # agree, but on tied maxima (exact zeros after a ReLU are common) amax splits the gradient evenly among the ties while
+    # these send all of it to one index, as the reference's backward does.
+    s = torch.sigmoid(mlp(x.mean(dim=(2, 3))) + mlp(F.adaptive_max_pool2d(x, 1).flatten(1)))
     x = x * s[:, :, None, None]
     w = sd[p + ".spatial_att.conv.weight"]
-    m = torch.cat([x.mean(dim=1, keepdim=True), x.amax(dim=1, keepdim=True)], dim=1)
+    m = torch.cat([x.mean(dim=1, keepdim=True), torch.max(x, dim=1, keepdim=True)[0]], dim=1)
     a = _bn(F.conv2d(m, w, None, padding=w.shape[-1] // 2), sd, p + ".spatial_att.bn", training)
     return x * torch.sigmoid(a)
 
