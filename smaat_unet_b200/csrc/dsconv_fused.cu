@@ -20,7 +20,8 @@
 //   warps 4-11  two consumer warpgroups (64 pixels each): wgmma (TF32X3: A_hi B_hi + A_lo B_hi + A_hi B_lo per k-step) into
 //               register accumulators, with the A operand either read by the tensor core from the A ring (A_SMEM) or
 //               loaded into registers from it first (and split into tf32 hi / lo there in TF32X3 mode), then the epilogue:
-//               scale/shift/ReLU -> NCHW stores (or the fused 1-class OutConv dot product; or BatchNorm batch statistics).
+//               scale/shift/ReLU -> NCHW (staged per 32-channel slice in shared memory and written by TMA tensor stores),
+//               or the fused 1-class OutConv dot product; [+ BatchNorm batch statistics].
 //               The main loop is pipelined: a chunk's MMAs are committed as one group (two half-chunk groups in the
 //               register form at N_TILE 64 in TF32X3, where registers are short), the wait leaves the newest group in
 //               flight, and the previous chunk's A and B stages are released once it retires.  The register form
@@ -82,11 +83,25 @@ struct DsCfg {
   static constexpr int BS = X3 ? (A_SMEM && N_TILE > 64 ? 2 : 3) : 4;
   static constexpr int AFF_N = 512;                            // scale | shift | OutConv weights of up to 512 channels
   static constexpr int BAR_BYTES = 512;
-  static constexpr int IS_FIT = (224 * 1024 - 1024 - BAR_BYTES - 3 * AFF_N * 4 - AS * AST_BYTES - BS * BST_BYTES) / IN_BYTES;
+  static constexpr int FREE = 224 * 1024 - 1024 - BAR_BYTES - 3 * AFF_N * 4 - AS * AST_BYTES - BS * BST_BYTES;
+  // Output staging: per consumer warpgroup ST_BUFS buffers of one 32-channel x 64-pixel TMA store box (8 KB), taken from the
+  // input ring.  Two, so that a slice's store overlaps the staging of the next: in 3xTF32 with k = 2 the input ring goes
+  // 6 -> 4 at N_TILE 64 and 4 -> 2 at N_TILE 128 (one buffer there, with a 3-deep input ring, measured 1-6 % slower per
+  // layer: DESIGN §6).  Where two would leave the input ring under 2 stages one is used, and where even one would (k = 1 at
+  // N_TILE 128 in 3xTF32: 30 KB boxes), the instance keeps the direct-store epilogue (ST_BUFS = 0)
+  static constexpr int ST_BOX = 32 * 64 * 4;
+  static constexpr int ST_WANT = 2;
+  static constexpr int ST_BUFS = (FREE - 2 * ST_WANT * ST_BOX) / IN_BYTES >= 2 ? ST_WANT
+                                 : (FREE - 2 * ST_BOX) / IN_BYTES >= 2     ? 1
+                                                                           : 0;
+  static constexpr int ST_BYTES = 2 * ST_BUFS * ST_BOX;
+  static_assert(ST_BUFS > 0 || (FREE - 2 * ST_BOX) / IN_BYTES < 2, "staging falls back only where one buffer does not fit");
+  static constexpr int IS_FIT = (FREE - ST_BYTES) / IN_BYTES;
   static constexpr int IS = IS_FIT > 8 ? 8 : IS_FIT;           // input ring: as deep as shared memory allows
   static constexpr int OFF_A = ((IS * IN_BYTES + 1023) / 1024) * 1024;
   static constexpr int OFF_BR = OFF_A + AS * AST_BYTES;
-  static constexpr int OFF_BAR = OFF_BR + BS * BST_BYTES;
+  static constexpr int OFF_ST = OFF_BR + BS * BST_BYTES;       // 1 KB aligned: the 128-byte swizzle repeats every 1 KB
+  static constexpr int OFF_BAR = OFF_ST + ST_BYTES;
   static_assert((IS * NG + IS + 2 * AS + 2 * BS) * 8 <= BAR_BYTES, "barrier block");
   static constexpr int TOTAL = OFF_BAR + BAR_BYTES + 3 * AFF_N * 4 + 1024;
   static constexpr uint32_t B_TX = BST_BYTES;
@@ -110,11 +125,41 @@ struct DsCfg {
   static_assert(TOTAL <= 227 * 1024, "shared memory budget");
 };
 
+// ----- staged output epilogue: TMA tensor stores of 32-channel x 64-pixel boxes from shared memory -----
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed bulk stores may still be reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// 4 x 4 transpose across the 4 lanes of a fragment group with equal t (lanes 4q + t, q = 0..3; quad lane q = g & 3): on entry
+// v[s] is slot s at quad pixel q, on exit v[p] is slot q at quad pixel p.  Two butterfly stages (lanes 8 apart, then 4 apart)
+__device__ __forceinline__ void quad_transpose(float (&v)[4], int q) {
+  const bool h1 = q & 2, h0 = q & 1;
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const float r = __shfl_xor_sync(0xffffffffu, h1 ? v[e] : v[e + 2], 8);
+    if (h1) v[e] = r; else v[e + 2] = r;
+  }
+#pragma unroll
+  for (int e = 0; e < 4; e += 2) {
+    const float r = __shfl_xor_sync(0xffffffffu, h0 ? v[e] : v[e + 1], 4);
+    if (h0) v[e] = r; else v[e + 1] = r;
+  }
+}
+
 template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
 __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1)
     dsconv_fused_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
                         const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
-                        const DsParams p) {
+                        const __grid_constant__ CUtensorMap map_y, const DsParams p) {
   using L = DsCfg<N_TILE, KPL, PW, X3, A_SMEM>;
   constexpr int PH = L::PH, BW = L::BW, BH = L::BH, CC = L::CC, IS = L::IS, AS = L::AS, BS = L::BS;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
@@ -152,6 +197,7 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
     tma_prefetch_desc(&map_in1);
     tma_prefetch_desc(&map_w);
     if (X3) tma_prefetch_desc(&map_wlo);
+    if (L::ST_BUFS && !p.oc_y) tma_prefetch_desc(&map_y);
     for (int s = 0; s < IS; ++s) {
       for (int g = 0; g < L::NG; ++g) mbar_init(&in_full[s * L::NG + g], 1);
       mbar_init(&in_empty[s], 128);
@@ -227,6 +273,25 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
     const int m1 = A_SMEM ? m0 + 8 : tc_row_pixel(wg, wq, 1, g);
     const float act_lo = p.relu ? 0.f : -INFINITY;
     const int64_t P = (int64_t)p.H * p.W;
+    // Staged epilogue.  This warpgroup's patch pixels 64 wg .. 64 wg + 63 (both A forms) are the PW x PH / 2 half-patch its
+    // TMA store box covers, so each warpgroup stages and stores on its own.  The box lies [channel][pixel] in shared memory
+    // with the TMA swizzle of its row length (128 B at PW 32, 64 B at PW 16).  A warp holds 16 pixels of every channel, and
+    // unswizzled channels are 256 B apart: any store order would be at least 2-way bank-conflicted.  So the 4 lanes of a
+    // fragment group with equal t (quad pixels q = 0..3 of two pixel quads and channels 2t, 2t + 1) transpose their values
+    // (quad_transpose): each lane then stores 4 consecutive pixels of one channel with one STS.128, slot q ^ (t & 2)
+    // (slot s: channel 2t + (s & 1), quad of accumulator row s >> 1).  The t & 2 twist puts the lanes t and t + 2 of one
+    // quarter-warp on different swizzle phases.  In the register form that makes every STS.128 conflict-free at PW 32; at
+    // PW 16 the 64-byte swizzle spans 4 bank groups and a quarter-warp's pixels only 4, so it stays 2-way there (and in the
+    // shared-memory form, whose rows are consecutive pixels, 2-way at PW 32 and 4-way at PW 16).
+    constexpr int SW_MASK = PW == 32 ? 7 : 3;      // 16-byte chunk bits [4, 7) / [4, 6) ^= address bits [7, 10) / [7, 9)
+    const int quad = g & 3, slot = quad ^ (t & 2);
+    const int st_ch = 2 * t + (slot & 1);           // channel of this lane's stores within an 8-channel fragment column
+    const int st_px = ((slot & 2) ? m1 : m0) - quad - 64 * wg;   // first of its 4 pixels within the half-patch
+    const uint32_t st_a0 = (uint32_t)(st_ch * 256 + st_px * 4);
+    const uint32_t st_off = st_a0 ^ (((st_a0 >> 7) & SW_MASK) << 4);   // + 2 KB per fragment column: the swizzle phase repeats
+    const uint32_t st_base = smem_u32(smem + L::OFF_ST) + (uint32_t)(wg * L::ST_BUFS * L::ST_BOX);
+    const bool st_leader = (threadIdx.x & 127) == 0;
+    uint32_t st_n = 0;                              // this warpgroup's staged boxes so far (buffer st_n % ST_BUFS)
     uint32_t gc = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       int b, ty, tx, np;
@@ -357,6 +422,40 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
           if (v0) p.oc_y[(int64_t)b * P + o0] = d0 + ob;
           if (v1) p.oc_y[(int64_t)b * P + o1] = d1 + ob;
         }
+      } else if (L::ST_BUFS) {
+        // One 32-channel slice at a time: wait until the buffer's previous store has been read out, stage the slice (the same
+        // fmaxf(fmaf(acc, sc, sh), act_lo) as the direct stores: bit-identical), hand it to the async proxy and store it as
+        // one box.  TMA clips what lies outside W, H or Cout; slices wholly past Cout are skipped
+        const int y_half = ty * PH + wg * (PH / 2);
+#pragma unroll
+        for (int s = 0; s < N_TILE / 32; ++s) {
+          if (n0 + 32 * s >= p.Cout) break;
+          const uint32_t buf = st_base + (st_n % L::ST_BUFS) * L::ST_BOX;
+          if (st_leader) bulk_wait_read<L::ST_BUFS - 1>();
+          wg_sync(2 + wg);
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * s + jj;
+            float v[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) v[q] = (t & 2) ? acc[4 * j + (q ^ 2)] : acc[4 * j + q];
+            quad_transpose(v, quad);
+            const int c = n0 + 8 * j + st_ch;
+            const float sc = aff[c], sh = aff[L::AFF_N + c];
+            const float4 o = make_float4(fmaxf(fmaf(v[0], sc, sh), act_lo), fmaxf(fmaf(v[1], sc, sh), act_lo),
+                                         fmaxf(fmaf(v[2], sc, sh), act_lo), fmaxf(fmaf(v[3], sc, sh), act_lo));
+            asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(buf + st_off + 2048u * jj), "f"(o.x), "f"(o.y),
+                         "f"(o.z), "f"(o.w)
+                         : "memory");
+          }
+          fence_proxy_async_smem();
+          wg_sync(2 + wg);
+          if (st_leader) {
+            tma_store_4d(&map_y, buf, tx * PW, y_half, n0 + 32 * s, b);
+            bulk_commit();
+          }
+          ++st_n;
+        }
       } else {
         float* yb = p.y + (int64_t)b * p.y_bstride;
 #pragma unroll
@@ -374,6 +473,7 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
         }
       }
     }
+    if (L::ST_BUFS && st_leader) bulk_wait_all();   // the stores have read their boxes before the CTA's shared memory goes
     return;
   }
 
@@ -487,8 +587,8 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
 }
 
 template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
-static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl, DsParams p,
-                     int B, cudaStream_t st) {
+static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl,
+                     const CUtensorMap& my, DsParams p, int B, cudaStream_t st) {
   using L = DsCfg<N_TILE, KPL, PW, X3, A_SMEM>;
   auto kern = dsconv_fused_kernel<N_TILE, KPL, PW, X3, A_SMEM>;
   static std::atomic<uint64_t> attr_mask{0};   // cudaFuncSetAttribute is per device
@@ -506,7 +606,7 @@ static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtenso
   p.total_tiles = (int)total;
   p.nchunks = ceil_div(p.C0 + p.C1, L::CC);
   const int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
-  kern<<<grid, L::THREADS, L::TOTAL, st>>>(m0, m1, mw, mwl, p);
+  kern<<<grid, L::THREADS, L::TOTAL, st>>>(m0, m1, mw, mwl, my, p);
   SMAAT_LAUNCH_CHECK("smaat_dsconv_fwd");
   return SMAAT_OK;
 }
@@ -527,9 +627,13 @@ static int pick_pw(int H, int W) {
   return best <= 1.35 ? pw : 0;
 }
 
+// y: the activation output, or null where it is not known yet (smaat_dsconv_eligible*) or not written (the fused OutConv).  The
+// epilogue stores it by TMA, which needs a 16-byte aligned base and 16-byte multiples as strides
 static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* pw_w,
-                        const float* pw_w_lo, int H, int W, int k, int Cout, bool stats, bool outconv) {
+                        const float* pw_w_lo, const float* y, int64_t y_bstride, int H, int W, int k, int Cout, bool stats,
+                        bool outconv) {
   if (k != 1 && k != 2) return false;
+  if (y && (!aligned16(y) || y_bstride % 4 != 0)) return false;
   // Cout > 128: whole passes of 128 channels; batch statistics and the fused OutConv need all channels in one pass
   if (Cout < 8 || Cout > 512 || (Cout > 128 && (Cout % 128 != 0 || stats || outconv))) return false;
   if (W % 4 != 0 || !aligned16(x0) || bs0 % 4 != 0) return false;
@@ -568,7 +672,8 @@ extern "C" int smaat_set_dsconv_impl(int impl) {
 
 extern "C" int smaat_dsconv_eligible2(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                                       const float* pw_w, int H, int W, int k, int Cout, int with_stats) {
-  return ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, H, W, k, Cout, with_stats != 0, false) ? 1 : 0;
+  return ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, with_stats != 0, false) ? 1
+                                                                                                                                : 0;
 }
 
 extern "C" int smaat_dsconv_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
@@ -587,9 +692,12 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   SMAAT_REQUIRE(mode != SMAAT_PW_TF32X3 || pw_w_lo, "dsconv: TF32X3 needs pw_w_lo (see smaat_split_tf32)");
   SMAAT_REQUIRE(oc_y || y_bstride >= (int64_t)Cout * H * W, "dsconv: y batch stride too small");
   SMAAT_REQUIRE(!oc_y || (oc_w && !stats), "dsconv+outconv: needs the OutConv weight and no batch statistics");
-  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, pw_w_lo, H, W, k, Cout, stats != nullptr, oc_y != nullptr))
-    return fail(SMAAT_E_UNSUPPORTED, "dsconv: shape not taken by the fused kernel (k=%d Cout=%d H=%d W=%d); use dw3x3 + pw1x1", k,
-                Cout, H, W);
+  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, pw_w_lo, oc_y ? nullptr : y, y_bstride, H, W, k, Cout,
+                   stats != nullptr, oc_y != nullptr))
+    return fail(SMAAT_E_UNSUPPORTED,
+                "dsconv: shape or output layout not taken by the fused kernel (k=%d Cout=%d H=%d W=%d, y 16-byte aligned with a "
+                "batch stride that is a multiple of 4); use dw3x3 + pw1x1",
+                k, Cout, H, W);
   cudaStream_t st = (cudaStream_t)stream;
   const int pw = pick_pw(H, W);
   const int ph = TC_BM / pw;
@@ -626,6 +734,15 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
       if (r) return r;
     }
   }
+  // the staged epilogue's store box: one warpgroup's half-patch (PW x PH / 2 pixels) x 32 channels, swizzled by its row length
+  CUtensorMap my = m0;
+  if (!oc_y) {
+    const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)Cout, (uint64_t)B};
+    const uint64_t str[4] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4, (uint64_t)y_bstride * 4};
+    const uint32_t ybox[4] = {(uint32_t)pw, (uint32_t)(ph / 2), 32u, 1u};
+    int r = make_tmap_f32(&my, y, 4, dims, str, ybox, pw == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, "dsconv(y)");
+    if (r) return r;
+  }
   DsParams p;
   p.dw_w = dw_w; p.dw_b = dw_b; p.scale = scale; p.shift = shift; p.y = y; p.y_bstride = y_bstride; p.stats = stats;
   p.oc_w = oc_w; p.oc_b = oc_b; p.oc_y = oc_y;
@@ -633,10 +750,10 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   p.tiles_x = p.tiles_y = p.npass = p.total_tiles = p.nchunks = 0;
 
 #define DS_DISPATCH(NT, KP, PWv)                                                                           \
-  return x3 ? (a_smem ? launch_ds<NT, KP, PWv, true, true>(m0, m1, mw, mwl, p, B, st)                       \
-                      : launch_ds<NT, KP, PWv, true, false>(m0, m1, mw, mwl, p, B, st))                     \
-            : (a_smem ? launch_ds<NT, KP, PWv, false, true>(m0, m1, mw, mwl, p, B, st)                      \
-                      : launch_ds<NT, KP, PWv, false, false>(m0, m1, mw, mwl, p, B, st))
+  return x3 ? (a_smem ? launch_ds<NT, KP, PWv, true, true>(m0, m1, mw, mwl, my, p, B, st)                   \
+                      : launch_ds<NT, KP, PWv, true, false>(m0, m1, mw, mwl, my, p, B, st))                 \
+            : (a_smem ? launch_ds<NT, KP, PWv, false, true>(m0, m1, mw, mwl, my, p, B, st)                  \
+                      : launch_ds<NT, KP, PWv, false, false>(m0, m1, mw, mwl, my, p, B, st))
   if (n_tile == 64) {
     if (k == 2) { if (pw == 32) { DS_DISPATCH(64, 2, 32); } else { DS_DISPATCH(64, 2, 16); } }
     else        { if (pw == 32) { DS_DISPATCH(64, 1, 32); } else { DS_DISPATCH(64, 1, 16); } }

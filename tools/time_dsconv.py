@@ -1,0 +1,115 @@
+"""Time the fused DS conv alone at bench.py's shapes with Cout <= 128 (B = 32, 3xTF32, k = 2), with CUDA events (a tool, not a
+test).
+
+For each shape it times two entry points over the same tiles, main loop and affine:
+  smaat_dsconv_fwd          writes the Cout-channel activation (the layer as the forward runs it);
+  smaat_dsconv_outconv_fwd  writes one float per pixel (the fused 1-class OutConv) instead of Cout.
+Their difference bounds what the output stores cost.  Each timing is 5 warm-up launches, then 40 launches between two CUDA
+events.  `hbm_ms` is the algorithmic HBM floor: input + output bytes at 3.35 TB/s (H100 SXM data sheet).
+
+  python tools/time_dsconv.py [--tree DIR] [--mode tf32x3|tf32] [--json]
+
+--tree imports smaat_unet_b200 from another checkout (a built one), to compare two builds in one session."""
+import argparse
+import json
+import os
+import sys
+
+ap = argparse.ArgumentParser()
+ap.add_argument("--tree", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ap.add_argument("--mode", default="tf32x3", choices=["tf32", "tf32x3"])
+ap.add_argument("--json", action="store_true", help="one JSON line per shape instead of a table")
+args = ap.parse_args()
+sys.path.insert(0, os.path.abspath(args.tree))
+
+import torch  # noqa: E402
+
+from smaat_unet_b200 import _lib, ops  # noqa: E402
+
+B, K_PL = 32, 2
+# (C0, C1, S, Cout): C1 > 0 is Up's concat, read virtually.  Each runs once per SmaAt-UNet forward
+SHAPES = [
+    (12, 0, 288, 64),
+    (64, 0, 288, 64),
+    (64, 64, 288, 64),
+    (64, 0, 144, 128),
+    (128, 0, 144, 128),
+    (128, 128, 144, 128),
+    (128, 0, 144, 64),
+    (256, 0, 72, 128),
+]
+WARMUP, ITERS = 5, 40
+HBM_BPS = 3.35e12
+
+
+def timed(fn):
+    for _ in range(WARMUP):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(ITERS):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / ITERS
+
+
+def main():
+    assert torch.cuda.is_available(), "time_dsconv.py needs a GPU"
+    lib = _lib.load()
+    mode = ops.PW_MODES[args.mode]
+    g = torch.Generator(device="cuda").manual_seed(7)
+    p = ops._ptr
+    st = ops._stream()
+    rows = []
+    for C0, C1, S, Cout in SHAPES:
+        Cin = C0 + C1
+        K = K_PL * Cin
+        x0 = torch.rand(B, C0, S, S, device="cuda", generator=g)
+        x1 = torch.rand(B, C1, S, S, device="cuda", generator=g) if C1 else None
+        dw_w = torch.randn(K, 1, 3, 3, device="cuda", generator=g) * 0.3
+        dw_b = torch.randn(K, device="cuda", generator=g) * 0.1
+        pw_w = torch.randn(Cout, K, device="cuda", generator=g) * 0.1
+        scale = torch.rand(Cout, device="cuda", generator=g) + 0.5
+        shift = torch.randn(Cout, device="cuda", generator=g) * 0.1
+        oc_w = torch.randn(Cout, device="cuda", generator=g) * 0.1
+        oc_b = torch.randn(1, device="cuda", generator=g)
+        hi, lo = ops.split_tf32(pw_w) if args.mode == "tf32x3" else (pw_w, None)
+        y = torch.empty(B, Cout, S, S, device="cuda")
+        logits = torch.empty(B, 1, S, S, device="cuda")
+        bs0, bs1 = C0 * S * S, C1 * S * S
+
+        def fwd():
+            _lib.check(lib.smaat_dsconv_fwd(p(x0), C0, bs0, p(x1), C1, bs1, p(dw_w), p(dw_b), p(hi), p(lo), p(scale), p(shift),
+                                            p(y), Cout * S * S, None, B, S, S, K_PL, Cout, 1, mode, st), "smaat_dsconv_fwd")
+
+        def outconv():
+            _lib.check(lib.smaat_dsconv_outconv_fwd(p(x0), C0, bs0, p(x1), C1, bs1, p(dw_w), p(dw_b), p(hi), p(lo), p(scale),
+                                                    p(shift), p(oc_w), p(oc_b), p(logits), B, S, S, K_PL, Cout, 1, mode, st),
+                       "smaat_dsconv_outconv_fwd")
+
+        ms_fwd = timed(fwd)
+        ms_oc = timed(outconv)
+        hbm = 4.0 * B * S * S * (Cin + Cout) / HBM_BPS * 1e3
+        name = f"C{Cin}->{Cout} {S}^2" + (" (concat)" if C1 else "")
+        rows.append({"layer": name, "fwd_ms": round(ms_fwd, 4), "outconv_ms": round(ms_oc, 4), "gap_ms": round(ms_fwd - ms_oc, 4),
+                     "hbm_ms": round(hbm, 4)})
+        del x0, x1, y
+    total_gap = sum(r["gap_ms"] for r in rows)
+    dev = torch.cuda.get_device_name()
+    if args.json:
+        for r in rows:
+            print(json.dumps(r))
+        print(json.dumps({"device": dev, "mode": args.mode, "sum_fwd_ms": round(sum(r["fwd_ms"] for r in rows), 4),
+                          "sum_gap_ms": round(total_gap, 4)}))
+        return
+    print(f"{dev}, {args.mode}, B = {B}, k = {K_PL}; {WARMUP} warm-up + {ITERS} timed launches per entry point")
+    print(f"{'layer':28s} {'fwd ms':>8s} {'outconv ms':>10s} {'gap ms':>8s} {'HBM floor ms':>12s}")
+    for r in rows:
+        print(f"{r['layer']:28s} {r['fwd_ms']:8.3f} {r['outconv_ms']:10.3f} {r['gap_ms']:8.3f} {r['hbm_ms']:12.3f}")
+    print(f"sum of gaps (each layer runs once per forward): {total_gap:.3f} ms")
+
+
+if __name__ == "__main__":
+    main()
