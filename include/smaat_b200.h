@@ -255,6 +255,26 @@ int smaat_mse_metrics_fwd(const float* pred, const float* target, int64_t n, flo
                           int denormalize, double* batch_acc, float* dpred, float grad_scale, void* stream);
 int smaat_metrics_commit(const double* batch_acc, double* totals, int batch_size, int denormalize, void* stream);
 
+/* ---- multi-class cross-entropy + confusion matrix of one segmentation step, one pass, no host sync ----------------
+ * Replaces nn.CrossEntropyLoss() of train_SmaAtUNet.py:54,182 (log_softmax + nll_loss) and the per-batch host histogram
+ * behind metric.iou.IoU.add (metric/iou.py:38-62, metric/confusionmatrix.py:40-69).
+ * smaat_ce_fwd: logits (B, K, P) fp32 NCHW dense, target (B, P) int64 class indices, 2 <= K <= 1024 (larger K:
+ *   SMAAT_E_UNSUPPORTED).  A pixel whose label equals ignore_index (only when use_ignore != 0) is skipped; a label outside
+ *   [0, K) that is not ignored is INVALID: counted, never used as an index, no loss, no gradient, no confusion entry.
+ *   batch_acc: double[3], overwritten: [0] sum over counted pixels of logsumexp_c(l) - l_target (fp32 terms, fp64 sum)
+ *                                      [1] counted pixels   [2] invalid labels
+ *   dlogits (nullable): (B, K, P), softmax(l) - onehot(target), unscaled; exactly 0 on ignored and invalid pixels.
+ *   conf (nullable): int64 K x K, ADDED INTO: conf[target][argmax_c l] += 1 per counted pixel; ties go to the first index.
+ *   NaN logits: the pixel's loss term and gradient are NaN (so is the loss, as in torch); its argmax is the first NaN
+ *   channel, as torch.argmax / np.argmax return, and the pixel is counted in conf under that column.
+ *   128-bit loads when P % 4 == 0 and logits / target / dlogits are 16-byte aligned, a scalar kernel otherwise.
+ * smaat_confusion_add: conf[target[i]][pred[i]] += 1 over n int64 (pred, target) pairs; a pair with either value outside
+ *   [0, K) is skipped and added to *invalid (int64 device counter, nullable). */
+int smaat_ce_fwd(const float* logits, const int64_t* target, int B, int K, int64_t P, int64_t ignore_index, int use_ignore,
+                 double* batch_acc, float* dlogits, int64_t* conf, void* stream);
+int smaat_confusion_add(const int64_t* pred, const int64_t* target, int64_t n, int K, int64_t* conf, int64_t* invalid,
+                        void* stream);
+
 /* CBAM in three launches (reference models/layers.py:90-141).
  * smaat_cbam_pool_mlp_fwd: ChannelAttention's global pools AND its shared MLP + sigmoid (layers.py:98-109): the last pooling
  *   CTA of each image finishes the MLP; pooled != NULL also emits MaxPool2d(2)(x) from the same read (parts_ds.py:48).

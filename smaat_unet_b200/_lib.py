@@ -62,6 +62,8 @@ SIGNATURES = {
     "smaat_cbam_mlp_bwd": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p],
     "smaat_mse_metrics_fwd": [_p, _p, _l, _f, _f, _i, _p, _p, _f, _p],
     "smaat_metrics_commit": [_p, _p, _i, _i, _p],
+    "smaat_ce_fwd": [_p, _p, _i, _i, _l, _l, _i, _p, _p, _p, _p],
+    "smaat_confusion_add": [_p, _p, _l, _i, _p, _p, _p],
     "smaat_convt2x2_pack_weight": [_p, _p, _i, _i, _p],
     "smaat_convt2x2_unpack_wgrad": [_p, _p, _p, _p, _i, _i, _p],
     "smaat_pixel_shuffle2_pad_fwd": [_p, _p, _p, _l, _i, _i, _i, _i, _i, _i, _p],

@@ -12,6 +12,8 @@ decompression and the per-sample Python overhead from the step:
     constructor arguments, ``__len__`` and ``__getitem__`` results of the reference's
     ``precipitation_maps_oversampled_h5`` (utils/dataset_precip.py:47-77) and ``precipitation_maps_h5`` (:6-44):
     ``imgs = images[index]`` (resp. ``images[index : index + seq]``), ``input = imgs[:num_input]``, ``target = imgs[-1]``.
+  * ``precipitation_maps_classification_shard`` -- ``precipitation_maps_classification_h5`` (:83-127): the same sliding
+    window with the target frame bucketed into 8 rain-rate classes (int64).
   * ``PinnedBatchLoader`` -- a background thread gathers whole batches straight into pinned host buffers (a small
     ring), in the order of a sampler (sequential, seeded shuffle, or an explicit index list such as the reference's
     train/valid split), sharded across ranks like ``DistributedSampler``; it yields ``(x, y)`` pinned tensors that
@@ -133,6 +135,54 @@ class precipitation_maps_shard(Dataset):
         return (self.num_input, self.nx, self.ny), (self.nx, self.ny)
 
 
+class precipitation_maps_classification_shard(Dataset):
+    """Same samples as ``precipitation_maps_classification_h5`` (utils/dataset_precip.py:83-127) over an (n_images, H, W)
+    shard: the sliding window of ``precipitation_maps_shard`` with the target frame turned into 8 rain-rate classes,
+    ``np.digitize(target * 47.83 * 12, [0, 0.5, 1, 2, 5, 10, 30], right=True)`` (mm/h bins of the de-normalised frame),
+    as int64 class indices for ``CrossEntropyLoss`` / ``TrainSession(loss="cross_entropy")``."""
+
+    target_dtype = torch.int64
+    num_classes = 8
+
+    def __init__(self, in_file, num_input_images, img_to_predict, train=True, transform=None):
+        super().__init__()
+        self.file_name = in_file
+        self.dataset = _open(in_file)
+        self.n_images, self.nx, self.ny = self.dataset.shape
+        self.num_input = num_input_images
+        self.img_to_predict = img_to_predict
+        self.sequence_length = num_input_images + img_to_predict
+        self.bins = np.array([0.0, 0.5, 1, 2, 5, 10, 30])
+        self.train = train
+        self.size_dataset = self.n_images - (num_input_images + img_to_predict)
+        self.transform = transform
+
+    def _buckets(self, target_img):
+        # float32 frame times Python floats stays float32 (as in the reference), then the bin search in float64
+        return np.digitize(target_img * 47.83 * 12, self.bins, right=True)
+
+    def __getitem__(self, index):
+        imgs = np.array(self.dataset[index: index + self.sequence_length], dtype="float32")
+        if self.transform is not None:
+            imgs = self.transform(imgs)
+        return imgs[: self.num_input], self._buckets(imgs[-1])
+
+    def __len__(self):
+        return self.size_dataset
+
+    def read_into(self, index, x_out, y_out):
+        if self.transform is not None:
+            x, y = self[index]
+            x_out[...] = x
+            y_out[...] = y
+            return
+        x_out[...] = self.dataset[index: index + self.num_input]
+        y_out[...] = self._buckets(np.asarray(self.dataset[index + self.sequence_length - 1], dtype=np.float32))
+
+    def sample_shapes(self):
+        return (self.num_input, self.nx, self.ny), (self.nx, self.ny)
+
+
 # ------------------------------------------------------------------------------------------------ loader
 def shard_indices(indices, rank, world, drop_last=False):
     """This rank's share of ``indices`` with ``DistributedSampler`` semantics: padded by wrapping around (or truncated
@@ -177,8 +227,9 @@ class PinnedBatchLoader:
         self.epoch = 0
         pin = torch.cuda.is_available() if pin_memory is None else bool(pin_memory)
         xs, ys = dataset.sample_shapes()
+        ydt = getattr(dataset, "target_dtype", torch.float32)      # int64 class indices for the classification shard
         self._x = [torch.empty((self.batch_size,) + tuple(xs), dtype=torch.float32, pin_memory=pin) for _ in range(self.ring)]
-        self._y = [torch.empty((self.batch_size,) + tuple(ys), dtype=torch.float32, pin_memory=pin) for _ in range(self.ring)]
+        self._y = [torch.empty((self.batch_size,) + tuple(ys), dtype=ydt, pin_memory=pin) for _ in range(self.ring)]
         self._guard = [None] * self.ring      # per slot: event that must complete before the slot is refilled
         self._held = None
 

@@ -19,6 +19,17 @@ The gradient bucket is all-reduced (average) by NCCL over NVLink in TWO pieces s
 backward pass: the decoder's slice (its gradients are final once the backward pass has reached the attention maps) is
 reduced on a side stream while the encoder's backward is still running; the encoder's slice follows.  BatchNorm statistics
 stay per rank, as in the reference (no SyncBatchNorm).
+
+Segmentation (train_SmaAtUNet.py:139-199): ``loss="cross_entropy"`` trains with ``nn.CrossEntropyLoss()`` semantics instead
+of the default ``"mse"``.  The target buffer is then int64 (B, H, W) class indices, the step's loss + gradient + IoU update
+is ``segmentation.ce_step`` (one kernel pass), ``metrics`` defaults to ``IoU(K)`` with K the logits' channel count (pass
+``metrics=None`` for none), and ``step`` returns the mean cross-entropy over the pixels not labelled -100.  With several
+ranks the averaged per-rank mean gradients equal the gradient of the global mean only when every rank counts the same
+number of pixels (no ignored or invalid labels, equal shards) -- the same caveat as the MSE path's sum / B_local.
+
+    sess = TrainSession(SmaAt_UNet(3, 21), batch=8, in_shape=(3, 224, 224), loss="cross_entropy")
+    loss = sess.step(x, y)          # y: (B, H, W) int64
+    iou, miou = sess.metrics.value()
 """
 from __future__ import annotations
 
@@ -31,13 +42,18 @@ from . import _lib, ops
 from . import functional as Fn
 from .metrics import PrecipitationMetrics, step_loss
 from .modules import CBAM
+from .segmentation import IoU, ce_step
 
 _ALIGN = 64          # floats: every parameter starts on a 256-byte boundary of the flat buffers (TMA needs 16)
+_DEFAULT = object()  # metrics argument not given: the loss's own default metric
 
 
 class TrainSession:
-    def __init__(self, model, batch, in_shape, lr=1e-3, device=None, use_graph=True, metrics=None, warmup=3,
-                 betas=(0.9, 0.999), eps=1e-8, overlap_allreduce=True, recompute_depthwise=False):
+    def __init__(self, model, batch, in_shape, lr=1e-3, device=None, use_graph=True, metrics=_DEFAULT, warmup=3,
+                 betas=(0.9, 0.999), eps=1e-8, overlap_allreduce=True, recompute_depthwise=False, loss="mse"):
+        if loss not in ("mse", "cross_entropy"):
+            raise ValueError(f"TrainSession: loss={loss!r}; 'mse' or 'cross_entropy'")
+        self.loss_kind = loss
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self.model = model.to(self.device).train()
         self.batch, self.in_shape = int(batch), tuple(in_shape)
@@ -52,9 +68,13 @@ class TrainSession:
                     dist.broadcast(t, src=0)
         self.params = [p for p in self.model.parameters() if p.requires_grad]
         self._flatten()
-        self.metrics = metrics if metrics is not None else PrecipitationMetrics(device=self.device)
         self.x = torch.zeros((self.batch,) + self.in_shape, device=self.device, dtype=torch.float32)
-        self.y = torch.zeros((self.batch,) + self.in_shape[1:], device=self.device, dtype=torch.float32)
+        if loss == "mse":
+            self.metrics = metrics if metrics is not None and metrics is not _DEFAULT else PrecipitationMetrics(device=self.device)
+            self.y = torch.zeros((self.batch,) + self.in_shape[1:], device=self.device, dtype=torch.float32)
+        else:
+            self.metrics = IoU(self._n_classes(), device=self.device) if metrics is _DEFAULT else metrics
+            self.y = torch.zeros((self.batch,) + self.in_shape[1:], device=self.device, dtype=torch.int64)
         self.loss = torch.zeros((), device=self.device, dtype=torch.float32)
         self.lr = torch.full((), float(lr), device=self.device, dtype=torch.float32)      # device scalar: graphs follow set_lr()
         self.opt_step = torch.zeros((), device=self.device, dtype=torch.float32)          # completed optimizer steps
@@ -76,6 +96,16 @@ class TrainSession:
         self.record_comm_timing = False
         self.skip_allreduce = False         # measurement only (bench.py: step time without the collective); replicas diverge
         self._build(warmup)
+
+    def _n_classes(self):
+        """Channel count of the model's logits, from one eval-mode forward of a single zero sample (no statistics move)."""
+        with torch.no_grad(), torch.cuda.device(self.device):
+            self.model.eval()
+            try:
+                out = self.model(self.x[:1])
+            finally:
+                self.model.train()
+        return int(out.shape[1])
 
     # ---- flat buffers ------------------------------------------------------------------------------------
     def _flatten(self):
@@ -127,6 +157,8 @@ class TrainSession:
             pred = self.model(self.x)
         finally:
             Fn.set_recompute_depthwise(old)
+        if self.loss_kind == "cross_entropy":
+            return ce_step(pred, self.y, self.metrics)    # nn.CrossEntropyLoss + IoU.add in one pass (segmentation.py)
         return step_loss(pred, self.y, self.metrics)      # loss_func + metrics.update in one pass (metrics.py)
 
     def _phase1(self):
@@ -179,7 +211,8 @@ class TrainSession:
             self.exp_avg.zero_()
             self.exp_avg_sq.zero_()
             self.opt_step.zero_()
-        self.metrics.load_totals(self._metrics_snap)      # warm-up must not disturb totals the caller already holds
+        if self.metrics is not None:
+            self.metrics.load_totals(self._metrics_snap)  # warm-up must not disturb totals the caller already holds
         ops.bump_weights_generation()
 
     def _verify_split(self):
@@ -227,7 +260,7 @@ class TrainSession:
 
     def _build(self, warmup):
         snap = self._snapshot()          # warm-up steps must not change the model the caller handed in
-        self._metrics_snap = self.metrics.totals_snapshot()
+        self._metrics_snap = self.metrics.totals_snapshot() if self.metrics is not None else None
         self._sink_keys = Fn.add_grad_sinks(self.params, self._views)
         weakref.finalize(self, Fn.remove_grad_sinks, self._sink_keys)
         cur = torch.cuda.current_stream(self.device)
