@@ -107,6 +107,24 @@ int smaat_dsconv_outconv_fwd(const float* x0, int C0, int64_t x0_bstride, const 
                              const float* scale, const float* shift, const float* oc_w, const float* oc_b, float* logits,
                              int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
 
+/* The fused DS conv with the CBAM fusions of the serving forward (models/layers.py:90-141 around the DS blocks of
+ * models/SmaAt_UNet.py:41-57); arguments as smaat_dsconv_fwd, without batch statistics.
+ *   gate_sc (B, C0), gate_sa (B, 1, H, W), both or neither: x0 is read as the CBAM output (x0 * gate_sc) * gate_sa, bit for bit
+ *     what smaat_cbam_scale_fwd writes (zero padding stays zero), so the CBAM output of a skip is never materialised.
+ *   pool_sum, pool_max (B, npart, Cout) and pooled (B, Cout, H / 2, W / 2), all or none: the epilogue also writes per half-patch
+ *     partial sums / maxima of y (npart = smaat_dsconv_pool_parts(H, W); smaat_cbam_mlp_partials_fwd finishes the channel
+ *     gate from them) and MaxPool2d(2)(y) (parts_ds.py:48; floor for odd H).  Fixed layout and order: no atomics.
+ * smaat_dsconv_cbam_eligible: 1 if smaat_dsconv_cbam_fwd takes this request in `mode` (the pools need an instance with the
+ *   staged epilogue), else 0. */
+int smaat_dsconv_cbam_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                               const float* pw_w, int H, int W, int k, int Cout, int mode, int with_gate, int with_pools);
+int smaat_dsconv_pool_parts(int H, int W);
+int smaat_dsconv_cbam_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                          const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
+                          const float* scale, const float* shift, float* y, int64_t y_bstride,
+                          const float* gate_sc, const float* gate_sa, float* pool_sum, float* pool_max, float* pooled,
+                          int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
+
 /* How the fused DS conv (smaat_dsconv_fwd / smaat_dsconv_outconv_fwd, same reference lines, models/layers.py:47-50) hands the
  * depthwise result to the tensor core: 0 = auto (default; 2, the faster of the two on an H100), 1 = K-major tiles in shared memory that wgmma reads
  * through a descriptor, 2 = tiles the consumers load into registers for wgmma's register-A form.  Same results up to
@@ -286,6 +304,12 @@ int smaat_cbam_pool_mlp_fwd(const float* x, float* avg, float* mx, float* pooled
                             const float* b2, float* sc, int* counters, int B, int C, int H, int W, int hidden, void* stream);
 int smaat_cbam_gate_scale_fwd(const float* pooled, const float* wsp, const float* bn_affine, const float* x, const float* sc, float* y,
                               int64_t y_bstride, int B, int C, int H, int W, int ks, void* stream);
+/* smaat_cbam_mlp_partials_fwd: the channel gate of a map whose producer (smaat_dsconv_cbam_fwd) already pooled it: reduces
+ *   psum / pmax (B, npart, C) per (b, c) in a fixed order to avg = sum / (H * W) and mx, then the shared MLP + sigmoid as
+ *   smaat_cbam_pool_mlp_fwd (same counters).  C % 16 == 0, C <= 512, hidden <= 64 (else SMAAT_E_UNSUPPORTED). */
+int smaat_cbam_mlp_partials_fwd(const float* psum, const float* pmax, int npart, float* avg, float* mx, const float* w1,
+                                const float* b1, const float* w2, const float* b2, float* sc, int* counters, int B, int C,
+                                int H, int W, int hidden, void* stream);
 
 /* ---- UpDS(bilinear=False): nn.ConvTranspose2d(in, in // 2, 2, stride=2) + F.pad (reference
  * models/unet_parts_depthwise_separable.py:72-73, 76-81).  Kernel = stride = 2: no overlapping taps, so the transposed conv is ONE

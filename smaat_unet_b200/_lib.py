@@ -27,6 +27,9 @@ SIGNATURES = {
     "smaat_set_dsconv_impl": [_i],
     "smaat_dsconv_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_outconv_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
+    "smaat_dsconv_cbam_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _i, _i],
+    "smaat_dsconv_pool_parts": [_i, _i],
+    "smaat_dsconv_cbam_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _l, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_split_tf32": [_p, _p, _p, _l, _p],
     "smaat_bn_fold": [_p, _p, _p, _p, _p, _f, _p, _p, _i, _p],
     "smaat_channel_stats": [_p, _p, _i, _i, _i, _p],
@@ -42,6 +45,7 @@ SIGNATURES = {
     "smaat_cbam_scale_fwd": [_p, _p, _p, _p, _l, _i, _i, _i, _p],
     "smaat_cbam_pool_mlp_fwd": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p],
     "smaat_cbam_gate_scale_fwd": [_p, _p, _p, _p, _p, _p, _l, _i, _i, _i, _i, _i, _p],
+    "smaat_cbam_mlp_partials_fwd": [_p, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p],
     "smaat_outconv_fwd": [_p, _p, _p, _p, _i, _i, _i, _i, _p],
     # ---- backward
     "smaat_bn_act_bwd_reduce": [_p, _p, _p, _p, _p, _i, _i, _i, _i, _p],

@@ -448,6 +448,44 @@ __global__ void __launch_bounds__(256) cbam_pool_maxpool_kernel(const float* __r
   }
 }
 
+// ---- channel gate from the partial pools the producing DS conv wrote in its epilogue (smaat_dsconv_cbam_fwd) ---------------
+// psum / pmax: (B, npart, C).  CTA (channel block, image) reduces MP_CB channels: thread (group j, channel quad q) folds parts
+// j, j + MP_NJ, ... with 128-bit loads, then one thread per quad folds the groups in order -- a fixed order, so the result
+// does not depend on timing.  The last CTA of an image runs the MLP (cbam_pool_finish), as in cbam_pool_kernel.
+constexpr int MP_CB = 16, MP_NQ = MP_CB / 4, MP_NJ = 256 / MP_NQ;
+__global__ void __launch_bounds__(256) cbam_mlp_partials_kernel(const float* __restrict__ psum, const float* __restrict__ pmax,
+                                                                int npart, float* __restrict__ avg, float* __restrict__ mx, int P,
+                                                                const MlpTail tail) {
+  __shared__ float4 rs[MP_NJ][MP_NQ], rm[MP_NJ][MP_NQ];
+  const int b = blockIdx.y, c0 = blockIdx.x * MP_CB;
+  const int q = threadIdx.x % MP_NQ, j = threadIdx.x / MP_NQ;
+  const int64_t step = tail.C / 4;                               // float4s per part
+  const int64_t base = ((int64_t)b * npart * tail.C + c0) / 4 + q;
+  const float4* s4 = reinterpret_cast<const float4*>(psum) + base;
+  const float4* m4 = reinterpret_cast<const float4*>(pmax) + base;
+  float4 s = make_float4(0.f, 0.f, 0.f, 0.f), m = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
+#pragma unroll 4
+  for (int i = j; i < npart; i += MP_NJ) {
+    const float4 a = __ldg(s4 + i * step), e = __ldg(m4 + i * step);
+    s.x += a.x; s.y += a.y; s.z += a.z; s.w += a.w;
+    m.x = fmaxf(m.x, e.x); m.y = fmaxf(m.y, e.y); m.z = fmaxf(m.z, e.z); m.w = fmaxf(m.w, e.w);
+  }
+  rs[j][q] = s;
+  rm[j][q] = m;
+  __syncthreads();
+  if (threadIdx.x < MP_NQ) {
+    for (int jj = 1; jj < MP_NJ; ++jj) {
+      const float4 a = rs[jj][q], e = rm[jj][q];
+      s.x += a.x; s.y += a.y; s.z += a.z; s.w += a.w;
+      m.x = fmaxf(m.x, e.x); m.y = fmaxf(m.y, e.y); m.z = fmaxf(m.z, e.z); m.w = fmaxf(m.w, e.w);
+    }
+    const int64_t o = (int64_t)b * tail.C + c0 + 4 * q;
+    avg[o] = s.x / (float)P; avg[o + 1] = s.y / (float)P; avg[o + 2] = s.z / (float)P; avg[o + 3] = s.w / (float)P;
+    mx[o] = m.x; mx[o + 1] = m.y; mx[o + 2] = m.z; mx[o + 3] = m.w;
+  }
+  cbam_pool_finish(tail, b, MP_CB, avg, mx);
+}
+
 // ---- spatial gate + scale in one kernel: y = (x * sc) * sigmoid(BN(conv kxk(pooled))) --------------------------------------
 // The gate of a 32 x 32 pixel tile is computed exactly as cbam_gate_kernel does (staged 2-channel tile with halo), then the
 // same thread walks its 4 pixels through the CTA's slice of the channels: the 1-channel gate map never reaches HBM and
@@ -599,6 +637,24 @@ extern "C" int smaat_cbam_pool_mlp_fwd(const float* x, float* avg, float* mx, fl
     }
   }
   SMAAT_LAUNCH_CHECK("smaat_cbam_pool_mlp_fwd");
+  return SMAAT_OK;
+}
+
+/* ChannelAttention's pools finished from the partial sums / maxima smaat_dsconv_cbam_fwd wrote for the map x (B, C, H, W), and its
+ * shared MLP + sigmoid (layers.py:98-109): avg, mx, sc (B, C).  psum / pmax: (B, npart, C).  counters as smaat_cbam_pool_mlp_fwd.
+ * Needs C % 16 == 0, C <= 512, hidden <= 64 and 16-byte aligned psum / pmax: SMAAT_E_UNSUPPORTED otherwise. */
+extern "C" int smaat_cbam_mlp_partials_fwd(const float* psum, const float* pmax, int npart, float* avg, float* mx, const float* w1,
+                                           const float* b1, const float* w2, const float* b2, float* sc, int* counters, int B, int C,
+                                           int H, int W, int hidden, void* stream) {
+  SMAAT_REQUIRE(psum && pmax && avg && mx && w1 && b1 && w2 && b2 && sc && counters && npart > 0 && B > 0 && C > 0 && H > 0 && W > 0 &&
+                    hidden > 0,
+                "cbam_mlp_partials: bad arguments");
+  SMAAT_REQUIRE(B <= 65535, "cbam_mlp_partials: batch too large for grid.y");
+  if (C % MP_CB != 0 || C > 512 || hidden > 64 || !aligned16(psum) || !aligned16(pmax))
+    return fail(SMAAT_E_UNSUPPORTED, "cbam_mlp_partials: needs C %% %d == 0, C <= 512, hidden <= 64, aligned partials", MP_CB);
+  MlpTail t{w1, b1, w2, b2, sc, counters, C, hidden};
+  cbam_mlp_partials_kernel<<<dim3(C / MP_CB, B), 256, 0, (cudaStream_t)stream>>>(psum, pmax, npart, avg, mx, H * W, t);
+  SMAAT_LAUNCH_CHECK("smaat_cbam_mlp_partials_fwd");
   return SMAAT_OK;
 }
 

@@ -38,6 +38,8 @@
 // Which one runs is smaat_set_dsconv_impl's choice (csrc/dsconv_fused.cu, below).
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "tc_common.cuh"
 
 namespace smaat {
@@ -53,6 +55,14 @@ struct DsParams {
   const float* oc_w;   // fused OutConv (1 class): logits = sum_c oc_w[c] * act[c] + oc_b, written instead of y
   const float* oc_b;
   float* oc_y;
+  // CBAM fusions of the serving forward (smaat_dsconv_cbam_fwd).  gate_sc (B, C0): x0 is read as the CBAM output
+  // (x0 * gate_sc[b, c]) * gate_sa[b, p], gate_sa coming in by its own TMA map.  pool_sum / pool_max (B, npart, Cout): per
+  // half-patch partial sums / maxima of the output for the channel gate's pools; pooled (B, Cout, H / 2, W / 2): its 2x2 max-pool
+  const float* gate_sc;
+  float* pool_sum;
+  float* pool_max;
+  float* pooled;
+  int npart;
   int C0, C1, H, W, Cout, relu, K;
   int tiles_x, tiles_y, npass, total_tiles, nchunks;
 };
@@ -98,7 +108,12 @@ struct DsCfg {
   static_assert(ST_BUFS > 0 || (FREE - 2 * ST_BOX) / IN_BYTES < 2, "staging falls back only where one buffer does not fit");
   static constexpr int IS_FIT = (FREE - ST_BYTES) / IN_BYTES;
   static constexpr int IS = IS_FIT > 8 ? 8 : IS_FIT;           // input ring: as deep as shared memory allows
-  static constexpr int OFF_A = ((IS * IN_BYTES + 1023) / 1024) * 1024;
+  // beside each input stage, the CBAM spatial gate's one-channel halo box (gated chunks only), in what the ring leaves over
+  static constexpr int SA_TX = BH * BW * 4;
+  static constexpr int SA_BYTES = (SA_TX + 127) / 128 * 128;
+  static_assert(IS * (IN_BYTES + SA_BYTES) + ST_BYTES <= FREE, "gate boxes fit beside the input ring");
+  static constexpr int OFF_SA = IS * IN_BYTES;
+  static constexpr int OFF_A = ((OFF_SA + IS * SA_BYTES + 1023) / 1024) * 1024;
   static constexpr int OFF_BR = OFF_A + AS * AST_BYTES;
   static constexpr int OFF_ST = OFF_BR + BS * BST_BYTES;       // 1 KB aligned: the 128-byte swizzle repeats every 1 KB
   static constexpr int OFF_BAR = OFF_ST + ST_BYTES;
@@ -159,7 +174,8 @@ template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
 __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1)
     dsconv_fused_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
                         const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
-                        const __grid_constant__ CUtensorMap map_y, const DsParams p) {
+                        const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_sa,
+                        const DsParams p) {
   using L = DsCfg<N_TILE, KPL, PW, X3, A_SMEM>;
   constexpr int PH = L::PH, BW = L::BW, BH = L::BH, CC = L::CC, IS = L::IS, AS = L::AS, BS = L::BS;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
@@ -198,6 +214,7 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
     tma_prefetch_desc(&map_w);
     if (X3) tma_prefetch_desc(&map_wlo);
     if (L::ST_BUFS && !p.oc_y) tma_prefetch_desc(&map_y);
+    if (p.gate_sc) tma_prefetch_desc(&map_sa);
     for (int s = 0; s < IS; ++s) {
       for (int g = 0; g < L::NG; ++g) mbar_init(&in_full[s * L::NG + g], 1);
       mbar_init(&in_empty[s], 128);
@@ -233,8 +250,11 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
           const int s = gc % IS;
           mbar_wait(&in_empty[s], ((gc / IS) & 1u) ^ 1u);
           uint64_t* full = &in_full[s * L::NG + (int)(gc % (uint32_t)L::NG)];      // the barrier of the group that reads this chunk
-          mbar_arrive_expect_tx(full, L::IN_BYTES);
           const int cb = i * CC;
+          const bool gated = p.gate_sc && cb < p.C0;
+          mbar_arrive_expect_tx(full, L::IN_BYTES + (gated ? L::SA_TX : 0));
+          // the gate's halo box: same origin and extent as the input box, one channel; zero fill outside the image
+          if (gated) tma_load_3d(smem + L::OFF_SA + s * L::SA_BYTES, &map_sa, full, x0 - 4, y0 - 1, b);
           const CUtensorMap* m = (cb < p.C0) ? &map_in0 : &map_in1;
           const int cc = (cb < p.C0) ? cb : cb - p.C0;
           asm volatile(
@@ -454,6 +474,53 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
             tma_store_4d(&map_y, buf, tx * PW, y_half, n0 + 32 * s, b);
             bulk_commit();
           }
+          if (p.pool_sum) {
+            // The CBAM channel gate's pools and the next level's MaxPool2d(2), read back from the staged slice (the stored values
+            // bit for bit; the store reads the buffer too, and nothing writes it before the next wg_sync).  4 threads per
+            // channel, 2 items each: an item is 4 columns of a row pair, i.e. two 2 x 2 windows (the half-patch origin is even
+            // and PH / 2 is even, so no window straddles it).  Pixels outside H or W are masked; an odd last row goes into the
+            // pools but not the max-pool (floor, as MaxPool2d)
+            const int pt = threadIdx.x & 127, pch = pt >> 2, pq = pt & 3;
+            const int c = n0 + 32 * s + pch;
+            float psum = 0.f, pmax = -INFINITY;
+#pragma unroll
+            for (int it = 0; it < 2; ++it) {
+              constexpr int NQ = PW / 4;
+              const int item = pq + 4 * it, rp = item / NQ, qd = item % NQ;   // lanes pq = 0..3: 4 adjacent items, 32 B of max-pool
+              const int px = 2 * rp * PW + 4 * qd;
+              const uint32_t a0 = (uint32_t)(pch * 256 + px * 4), a1 = a0 + (uint32_t)(PW * 4);
+              float4 u, v;
+              asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(u.x), "=f"(u.y), "=f"(u.z), "=f"(u.w)
+                           : "r"(buf + (a0 ^ (((a0 >> 7) & SW_MASK) << 4))));
+              asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+                           : "r"(buf + (a1 ^ (((a1 >> 7) & SW_MASK) << 4))));
+              const int gy = y_half + 2 * rp, gx = tx * PW + 4 * qd;      // W % 4 == 0: a quad is all in or all out
+              const bool in0 = gx < p.W && gy < p.H, in1 = gx < p.W && gy + 1 < p.H;
+              if (in0) {
+                psum += (u.x + u.y) + (u.z + u.w);
+                pmax = fmaxf(pmax, fmaxf(fmaxf(u.x, u.y), fmaxf(u.z, u.w)));
+              }
+              if (in1) {
+                psum += (v.x + v.y) + (v.z + v.w);
+                pmax = fmaxf(pmax, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
+                if (c < p.Cout) {
+                  const int hw = p.W >> 1;
+                  const float2 m2 = make_float2(fmaxf(fmaxf(u.x, u.y), fmaxf(v.x, v.y)), fmaxf(fmaxf(u.z, u.w), fmaxf(v.z, v.w)));
+                  *reinterpret_cast<float2*>(p.pooled + ((int64_t)b * p.Cout + c) * (int64_t)(p.H >> 1) * hw +
+                                             (int64_t)(gy >> 1) * hw + (gx >> 1)) = m2;
+                }
+              }
+            }
+            psum += __shfl_xor_sync(0xffffffffu, psum, 1);
+            psum += __shfl_xor_sync(0xffffffffu, psum, 2);
+            pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 1));
+            pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 2));
+            if (pq == 0 && c < p.Cout) {
+              const int64_t o = ((int64_t)b * p.npart + 2 * (ty * p.tiles_x + tx) + wg) * p.Cout + c;
+              p.pool_sum[o] = psum;
+              p.pool_max[o] = pmax;
+            }
+          }
           ++st_n;
         }
       } else {
@@ -485,11 +552,15 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
     const int Cin = p.C0 + p.C1;
     uint32_t gc = 0, iph = 0;       // iph: phase bit per input stage of this group's fill barriers
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      const int b = tile / tiles_per_img;
       for (int i = 0; i < nch; ++i, ++gc) {
         if ((int)(gc % (uint32_t)L::NG) != g) continue;
         const int s = gc % IS;
+        // chunks of x0 under a CBAM gate: each staged value is read as (x * sc[b, c]) * sa[b, p], the two rounded products of
+        // cbam_gate_scale_kernel in its order, so the stencil sees exactly the materialised CBAM output
+        const bool gated = p.gate_sc && i * CC < p.C0;
         // depthwise weights of this thread's (first) task: issued before the ring waits so that their latency hides there
-        float wr[KPL][9], br[KPL];
+        float wr[KPL][9], br[KPL], gsc = 0.f;
         auto task_channel = [&](int task) { return (PW == 32) ? (task >> 3) : (((task >> 4) << 1) | ((task >> 2) & 1)); };
         auto load_weights = [&](int task) {
           const int gch = i * CC + task_channel(task);
@@ -501,6 +572,7 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
             for (int w9 = 0; w9 < 9; ++w9) wr[kk][w9] = chv ? __ldg(p.dw_w + (int64_t)gk * 9 + w9) : 0.f;
             br[kk] = (chv && p.dw_b) ? __ldg(p.dw_b + gk) : 0.f;
           }
+          if (gated) gsc = gch < p.C0 ? __ldg(p.gate_sc + (int64_t)b * p.C0 + gch) : 0.f;
         };
         load_weights(t);
         mbar_wait(&in_full[s * L::NG + g], (iph >> s) & 1u);
@@ -509,75 +581,90 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
         mbar_wait(&a_empty[sa], ((gc / AS) & 1u) ^ 1u);  // the MMAs that read this A stage AS chunks ago retired
         unsigned char* my_op = a_base + sa * L::AST_BYTES;
         const float* in_stage = reinterpret_cast<const float*>(smem + s * L::IN_BYTES);
+        const float* sa_stage = reinterpret_cast<const float*>(smem + L::OFF_SA + s * L::SA_BYTES);
+        // the gated and the plain stencil are compiled apart, so that chunks without the gate run the plain loop unchanged
+        auto stencil = [&](auto gate_c) {
+          constexpr bool G = decltype(gate_c)::value;
 #pragma unroll 1
-        for (int task = t; task < CC * 8; task += 128) {
-          // task -> (input channel ci, column quad qc, row group rg).  A quarter-warp (8 lanes: one 128-bit shared-memory
-          // wavefront) must touch 8 different 16-byte bank groups: PW = 32 -> the 8 quads of one channel row; PW = 16 ->
-          // the 4 quads of TWO channels (16 words apart in the input tile, and 2 k-rows apart = a different
-          // swizzle phase in the A operand).  Pairing the two row groups of one channel instead (rows 4 apart: 96 words in
-          // the input tile, 4 KB in the A operand) put both halves on the same banks: every LDS.128 / STS.128 2-way.
-          int ci, qc, rg;
-          if (PW == 32) {
-            ci = task >> 3; qc = task & 7; rg = 0;
-          } else {
-            qc = task & 3; ci = ((task >> 4) << 1) | ((task >> 2) & 1); rg = (task >> 3) & 1;
-          }
-          constexpr int NQ = PW / 4;
-          const int c0 = qc << 2, r0 = rg << 2;
-          if (task != t) load_weights(task);   // KPL = 1: a second task per chunk
-          // smem column of patch column c (dx = -1..1) is c + 4 + dx: the 4 outputs read cols c0+3 .. c0+8
-          const float* trow = in_stage + (ci * BH + r0) * BW + c0 + 3;
-          float win[3][6];
-          // one LDS.128 per row; the two edge values come from the neighbouring quads' registers (lane -1 / +1 hold columns
-          // c0-4..c0-1 / c0+4..c0+7 of the same channel row), only the first / last quad of a patch row reads the halo
-          // column -- the 32 lanes' scalar loads would all fall on 8 banks (stride 4 words): a 4-way conflict each
-          const bool lb = (qc == 0), rb = (qc == NQ - 1);
-          const int edge = lb ? 0 : 5;
-          auto load_row = [&](float* wl, int r) {
-            const float4 a = *reinterpret_cast<const float4*>(trow + r * BW + 1);
-            float left = __shfl_up_sync(0xffffffffu, a.w, 1), right = __shfl_down_sync(0xffffffffu, a.x, 1);
-            if (lb | rb) {
-              const float e = trow[r * BW + edge];
-              if (lb) left = e; else right = e;
+          for (int task = t; task < CC * 8; task += 128) {
+            // task -> (input channel ci, column quad qc, row group rg).  A quarter-warp (8 lanes: one 128-bit shared-memory
+            // wavefront) must touch 8 different 16-byte bank groups: PW = 32 -> the 8 quads of one channel row; PW = 16 ->
+            // the 4 quads of TWO channels (16 words apart in the input tile, and 2 k-rows apart = a different
+            // swizzle phase in the A operand).  Pairing the two row groups of one channel instead (rows 4 apart: 96 words in
+            // the input tile, 4 KB in the A operand) put both halves on the same banks: every LDS.128 / STS.128 2-way.
+            int ci, qc, rg;
+            if (PW == 32) {
+              ci = task >> 3; qc = task & 7; rg = 0;
+            } else {
+              qc = task & 3; ci = ((task >> 4) << 1) | ((task >> 2) & 1); rg = (task >> 3) & 1;
             }
-            wl[0] = left; wl[1] = a.x; wl[2] = a.y; wl[3] = a.z; wl[4] = a.w; wl[5] = right;
-          };
-#pragma unroll
-          for (int r = 0; r < 2; ++r) load_row(win[r], r);
-#pragma unroll
-          for (int rr = 0; rr < 4; ++rr) {
-            load_row(win[(rr + 2) % 3], rr + 2);
-            const float* w0 = win[rr % 3];
-            const float* w1 = win[(rr + 1) % 3];
-            const float* w2 = win[(rr + 2) % 3];
-            const int m = (r0 + rr) * PW + c0;
-#pragma unroll
-            for (int kk = 0; kk < KPL; ++kk) {
-              float o4[4];
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                float a = br[kk];
-                a = fmaf(wr[kk][0], w0[j], a); a = fmaf(wr[kk][1], w0[j + 1], a); a = fmaf(wr[kk][2], w0[j + 2], a);
-                a = fmaf(wr[kk][3], w1[j], a); a = fmaf(wr[kk][4], w1[j + 1], a); a = fmaf(wr[kk][5], w1[j + 2], a);
-                a = fmaf(wr[kk][6], w2[j], a); a = fmaf(wr[kk][7], w2[j + 1], a); a = fmaf(wr[kk][8], w2[j + 2], a);
-                o4[j] = a;
+            constexpr int NQ = PW / 4;
+            const int c0 = qc << 2, r0 = rg << 2;
+            if (task != t) load_weights(task);   // KPL = 1: a second task per chunk
+            // smem column of patch column c (dx = -1..1) is c + 4 + dx: the 4 outputs read cols c0+3 .. c0+8
+            const float* trow = in_stage + (ci * BH + r0) * BW + c0 + 3;
+            const float* srow = sa_stage + r0 * BW + c0 + 3;
+            float win[3][6];
+            // one LDS.128 per row; the two edge values come from the neighbouring quads' registers (lane -1 / +1 hold columns
+            // c0-4..c0-1 / c0+4..c0+7 of the same channel row), only the first / last quad of a patch row reads the halo
+            // column -- the 32 lanes' scalar loads would all fall on 8 banks (stride 4 words): a 4-way conflict each
+            const bool lb = (qc == 0), rb = (qc == NQ - 1);
+            const int edge = lb ? 0 : 5;
+            auto load_row = [&](float* wl, int r) {
+              float4 a = *reinterpret_cast<const float4*>(trow + r * BW + 1);
+              if (G) {
+                const float4 ga = *reinterpret_cast<const float4*>(srow + r * BW + 1);
+                a.x = __fmul_rn(__fmul_rn(a.x, gsc), ga.x);
+                a.y = __fmul_rn(__fmul_rn(a.y, gsc), ga.y);
+                a.z = __fmul_rn(__fmul_rn(a.z, gsc), ga.z);
+                a.w = __fmul_rn(__fmul_rn(a.w, gsc), ga.w);
               }
-              if (A_SMEM) {
-                const int kr = ci * KPL + kk;
+              float left = __shfl_up_sync(0xffffffffu, a.w, 1), right = __shfl_down_sync(0xffffffffu, a.x, 1);
+              if (lb | rb) {
+                float e = trow[r * BW + edge];
+                if (G) e = __fmul_rn(__fmul_rn(e, gsc), srow[r * BW + edge]);
+                if (lb) left = e; else right = e;
+              }
+              wl[0] = left; wl[1] = a.x; wl[2] = a.y; wl[3] = a.z; wl[4] = a.w; wl[5] = right;
+            };
+#pragma unroll
+            for (int r = 0; r < 2; ++r) load_row(win[r], r);
+#pragma unroll
+            for (int rr = 0; rr < 4; ++rr) {
+              load_row(win[(rr + 2) % 3], rr + 2);
+              const float* w0 = win[rr % 3];
+              const float* w1 = win[(rr + 1) % 3];
+              const float* w2 = win[(rr + 2) % 3];
+              const int m = (r0 + rr) * PW + c0;
+#pragma unroll
+              for (int kk = 0; kk < KPL; ++kk) {
+                float o4[4];
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
-                  const uint32_t off = kmajor_offset(m + j, kr);
-                  const float h = X3 ? tf32_hi(o4[j]) : o4[j];
-                  *reinterpret_cast<float*>(my_op + off) = h;
-                  if (X3) *reinterpret_cast<float*>(my_op + L::OFF_ALO + off) = o4[j] - h;
+                  float a = br[kk];
+                  a = fmaf(wr[kk][0], w0[j], a); a = fmaf(wr[kk][1], w0[j + 1], a); a = fmaf(wr[kk][2], w0[j + 2], a);
+                  a = fmaf(wr[kk][3], w1[j], a); a = fmaf(wr[kk][4], w1[j + 1], a); a = fmaf(wr[kk][5], w1[j + 2], a);
+                  a = fmaf(wr[kk][6], w2[j], a); a = fmaf(wr[kk][7], w2[j + 1], a); a = fmaf(wr[kk][8], w2[j + 2], a);
+                  o4[j] = a;
                 }
-                continue;
+                if (A_SMEM) {
+                  const int kr = ci * KPL + kk;
+#pragma unroll
+                  for (int j = 0; j < 4; ++j) {
+                    const uint32_t off = kmajor_offset(m + j, kr);
+                    const float h = X3 ? tf32_hi(o4[j]) : o4[j];
+                    *reinterpret_cast<float*>(my_op + off) = h;
+                    if (X3) *reinterpret_cast<float*>(my_op + L::OFF_ALO + off) = o4[j] - h;
+                  }
+                  continue;
+                }
+                // fp32 in both modes: the consumers split TF32X3's hi / lo parts after loading (one pass through shared memory)
+                *reinterpret_cast<float4*>(my_op + a_tile_offset(ci * KPL + kk, m)) = make_float4(o4[0], o4[1], o4[2], o4[3]);
               }
-              // fp32 in both modes: the consumers split TF32X3's hi / lo parts after loading (one pass through shared memory)
-              *reinterpret_cast<float4*>(my_op + a_tile_offset(ci * KPL + kk, m)) = make_float4(o4[0], o4[1], o4[2], o4[3]);
             }
           }
-        }
+        };
+        if (gated) stencil(std::true_type{}); else stencil(std::false_type{});
         if (A_SMEM) fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
         mbar_arrive(&a_full[sa]);
         mbar_arrive(&in_empty[s]);
@@ -588,9 +675,11 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
 
 template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
 static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl,
-                     const CUtensorMap& my, DsParams p, int B, cudaStream_t st) {
+                     const CUtensorMap& my, const CUtensorMap& msa, DsParams p, int B, cudaStream_t st) {
   using L = DsCfg<N_TILE, KPL, PW, X3, A_SMEM>;
   auto kern = dsconv_fused_kernel<N_TILE, KPL, PW, X3, A_SMEM>;
+  // the pools are read back from the staging buffers: instances with the direct-store epilogue do not take them
+  if (p.pool_sum && !L::ST_BUFS) return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools need the staged epilogue");
   static std::atomic<uint64_t> attr_mask{0};   // cudaFuncSetAttribute is per device
   if (first_use_on_device(attr_mask)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
@@ -605,8 +694,9 @@ static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtenso
   SMAAT_REQUIRE(total < (1ll << 31), "dsconv: too many tiles");
   p.total_tiles = (int)total;
   p.nchunks = ceil_div(p.C0 + p.C1, L::CC);
+  p.npart = 2 * p.tiles_x * p.tiles_y;
   const int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
-  kern<<<grid, L::THREADS, L::TOTAL, st>>>(m0, m1, mw, mwl, my, p);
+  kern<<<grid, L::THREADS, L::TOTAL, st>>>(m0, m1, mw, mwl, my, msa, p);
   SMAAT_LAUNCH_CHECK("smaat_dsconv_fwd");
   return SMAAT_OK;
 }
@@ -641,6 +731,21 @@ static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, i
   const int K = k * (C0 + C1);
   if (K % 4 != 0 || !aligned16(pw_w) || (pw_w_lo && !aligned16(pw_w_lo))) return false;
   return pick_pw(H, W) != 0;
+}
+
+// Whether the instance dsconv_run dispatches to has the staged epilogue (ST_BUFS > 0), which the CBAM pools are read from
+template <int N_TILE, int KPL, int PW>
+static bool ds_staged_t(bool x3, bool a_smem) {
+  return (x3 ? (a_smem ? DsCfg<N_TILE, KPL, PW, true, true>::ST_BUFS : DsCfg<N_TILE, KPL, PW, true, false>::ST_BUFS)
+             : (a_smem ? DsCfg<N_TILE, KPL, PW, false, true>::ST_BUFS : DsCfg<N_TILE, KPL, PW, false, false>::ST_BUFS)) > 0;
+}
+static bool ds_staged(int n_tile, int k, int pw, bool x3, bool a_smem) {
+  if (n_tile == 64) {
+    if (k == 2) return pw == 32 ? ds_staged_t<64, 2, 32>(x3, a_smem) : ds_staged_t<64, 2, 16>(x3, a_smem);
+    return pw == 32 ? ds_staged_t<64, 1, 32>(x3, a_smem) : ds_staged_t<64, 1, 16>(x3, a_smem);
+  }
+  if (k == 2) return pw == 32 ? ds_staged_t<128, 2, 32>(x3, a_smem) : ds_staged_t<128, 2, 16>(x3, a_smem);
+  return pw == 32 ? ds_staged_t<128, 1, 32>(x3, a_smem) : ds_staged_t<128, 1, 16>(x3, a_smem);
 }
 
 // Where the A operand (the depthwise result) goes to the tensor core: 0 = auto (the register form), 1 = read by wgmma from
@@ -681,11 +786,30 @@ extern "C" int smaat_dsconv_eligible(const float* x0, int C0, int64_t x0_bstride
   return smaat_dsconv_eligible2(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout, 0);
 }
 
+extern "C" int smaat_dsconv_cbam_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                                          const float* pw_w, int H, int W, int k, int Cout, int mode, int with_gate, int with_pools) {
+  if (mode != SMAAT_PW_TF32 && mode != SMAAT_PW_TF32X3) return 0;
+  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, false, false)) return 0;
+  (void)with_gate;   // every fused instance takes the gate
+  if (with_pools && !ds_staged(Cout > 64 ? 128 : 64, k, pick_pw(H, W), mode == SMAAT_PW_TF32X3, ds_impl() == 1)) return 0;
+  return 1;
+}
+
+extern "C" int smaat_dsconv_pool_parts(int H, int W) {
+  const int pw = (H > 0 && W > 0) ? pick_pw(H, W) : 0;
+  return pw ? 2 * ceil_div(W, pw) * ceil_div(H, TC_BM / pw) : 0;
+}
+
 static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride, const float* dw_w,
                       const float* dw_b, const float* pw_w, const float* pw_w_lo, const float* scale, const float* shift, float* y,
-                      int64_t y_bstride, double* stats, const float* oc_w, const float* oc_b, float* oc_y, int B, int H, int W,
-                      int k, int Cout, int relu, int mode, void* stream) {
+                      int64_t y_bstride, double* stats, const float* oc_w, const float* oc_b, float* oc_y, const float* gate_sc,
+                      const float* gate_sa, float* pool_sum, float* pool_max, float* pooled, int B, int H, int W, int k, int Cout,
+                      int relu, int mode, void* stream) {
   SMAAT_REQUIRE(x0 && dw_w && pw_w && (y || oc_y), "dsconv: null pointer");
+  SMAAT_REQUIRE(!gate_sc == !gate_sa, "dsconv: the CBAM gate needs both sc and sa");
+  SMAAT_REQUIRE(!gate_sa || aligned16(gate_sa), "dsconv: the CBAM gate map must be 16-byte aligned");
+  SMAAT_REQUIRE(!pool_sum || (pool_max && pooled && y && !oc_y && !stats), "dsconv: the CBAM pools need sum, max and max-pool outputs and y");
+  SMAAT_REQUIRE(!pooled || (reinterpret_cast<uintptr_t>(pooled) & 7u) == 0, "dsconv: the max-pool output must be 8-byte aligned");
   SMAAT_REQUIRE(B > 0 && C0 > 0 && C1 >= 0 && H > 0 && W > 0 && Cout > 0, "dsconv: bad shape");
   SMAAT_REQUIRE(C1 == 0 || x1, "dsconv: C1=%d but x1 is null", C1);
   SMAAT_REQUIRE(mode == SMAAT_PW_TF32 || mode == SMAAT_PW_TF32X3, "dsconv: mode must be SMAAT_PW_TF32 or SMAAT_PW_TF32X3");
@@ -743,17 +867,27 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
     int r = make_tmap_f32(&my, y, 4, dims, str, ybox, pw == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, "dsconv(y)");
     if (r) return r;
   }
+  // the CBAM spatial gate sa (B, 1, H, W): one-channel halo boxes at the input boxes' origin
+  CUtensorMap msa = m0;
+  if (gate_sa) {
+    const uint64_t dims[3] = {(uint64_t)W, (uint64_t)H, (uint64_t)B};
+    const uint64_t str[3] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4};
+    const uint32_t sbox[3] = {(uint32_t)(pw + 8), (uint32_t)(ph + 2), 1u};
+    int r = make_tmap_f32(&msa, gate_sa, 3, dims, str, sbox, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(gate sa)");
+    if (r) return r;
+  }
   DsParams p;
   p.dw_w = dw_w; p.dw_b = dw_b; p.scale = scale; p.shift = shift; p.y = y; p.y_bstride = y_bstride; p.stats = stats;
   p.oc_w = oc_w; p.oc_b = oc_b; p.oc_y = oc_y;
+  p.gate_sc = gate_sc; p.pool_sum = pool_sum; p.pool_max = pool_max; p.pooled = pooled; p.npart = 0;
   p.C0 = C0; p.C1 = C1; p.H = H; p.W = W; p.Cout = Cout; p.relu = relu; p.K = K;
   p.tiles_x = p.tiles_y = p.npass = p.total_tiles = p.nchunks = 0;
 
 #define DS_DISPATCH(NT, KP, PWv)                                                                           \
-  return x3 ? (a_smem ? launch_ds<NT, KP, PWv, true, true>(m0, m1, mw, mwl, my, p, B, st)                   \
-                      : launch_ds<NT, KP, PWv, true, false>(m0, m1, mw, mwl, my, p, B, st))                 \
-            : (a_smem ? launch_ds<NT, KP, PWv, false, true>(m0, m1, mw, mwl, my, p, B, st)                  \
-                      : launch_ds<NT, KP, PWv, false, false>(m0, m1, mw, mwl, my, p, B, st))
+  return x3 ? (a_smem ? launch_ds<NT, KP, PWv, true, true>(m0, m1, mw, mwl, my, msa, p, B, st)                   \
+                      : launch_ds<NT, KP, PWv, true, false>(m0, m1, mw, mwl, my, msa, p, B, st))                 \
+            : (a_smem ? launch_ds<NT, KP, PWv, false, true>(m0, m1, mw, mwl, my, msa, p, B, st)                  \
+                      : launch_ds<NT, KP, PWv, false, false>(m0, m1, mw, mwl, my, msa, p, B, st))
   if (n_tile == 64) {
     if (k == 2) { if (pw == 32) { DS_DISPATCH(64, 2, 32); } else { DS_DISPATCH(64, 2, 16); } }
     else        { if (pw == 32) { DS_DISPATCH(64, 1, 32); } else { DS_DISPATCH(64, 1, 16); } }
@@ -770,7 +904,7 @@ extern "C" int smaat_dsconv_fwd(const float* x0, int C0, int64_t x0_bstride, con
                                 int W, int k, int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(y, "dsconv: null output");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, stats, nullptr,
-                    nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
+                    nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
 }
 
 /* The network's last two modules in one kernel: DS conv -> BN/ReLU -> OutConv(Cout -> 1) (reference models/SmaAt_UNet.py:55-56,
@@ -782,5 +916,20 @@ extern "C" int smaat_dsconv_outconv_fwd(const float* x0, int C0, int64_t x0_bstr
                                         float* logits, int B, int H, int W, int k, int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(oc_w && logits, "dsconv+outconv: null pointer");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
-                    logits, B, H, W, k, Cout, relu, mode, stream);
+                    logits, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
+}
+
+/* The fused DS conv of the serving forward with the CBAM fusions around it (models/layers.py:90-141, SmaAt_UNet.py:41-57).
+ * gate_sc (B, C0) and gate_sa (B, 1, H, W), both or neither: x0 is read as the CBAM output (x0 * sc) * sa, exactly as
+ * smaat_cbam_gate_scale_fwd / smaat_cbam_scale_fwd would have written it.  pool_sum / pool_max (B, npart, Cout) and pooled
+ * (B, Cout, H / 2, W / 2), all or none: the epilogue also writes per half-patch partial sums and maxima of y for the channel
+ * gate's pools (npart = smaat_dsconv_pool_parts(H, W); smaat_cbam_mlp_partials_fwd finishes them) and MaxPool2d(2)(y). */
+extern "C" int smaat_dsconv_cbam_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                                     const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
+                                     const float* scale, const float* shift, float* y, int64_t y_bstride, const float* gate_sc,
+                                     const float* gate_sa, float* pool_sum, float* pool_max, float* pooled, int B, int H, int W, int k,
+                                     int Cout, int relu, int mode, void* stream) {
+  SMAAT_REQUIRE(y, "dsconv_cbam: null output");
+  return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, nullptr, nullptr,
+                    nullptr, nullptr, gate_sc, gate_sa, pool_sum, pool_max, pooled, B, H, W, k, Cout, relu, mode, stream);
 }

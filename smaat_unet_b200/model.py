@@ -10,7 +10,7 @@ from __future__ import annotations
 
 from torch import nn
 
-from .modules import CBAM, DoubleConv, DoubleConvDS, Down, DownDS, OutConv, Up, UpDS
+from .modules import CBAM, DoubleConv, DoubleConvDS, Down, DownDS, OutConv, Up, UpDS, _needs_grad
 
 _ENC = (64, 128, 256, 512)
 
@@ -48,18 +48,33 @@ class SmaAt_UNet(nn.Module):
         return self.outc(y)
 
     def forward_serving(self, x):
-        """Same graph with the one fusion the plain-call API cannot express: up4's last DS conv applies the 1-class OutConv
-        in its epilogue (SmaAt_UNet.py:55-56), so the 64-channel activation never reaches HBM.  Used by
-        ``engine.InferenceSession`` (inference only; falls back to the plain calls under autograd / train mode)."""
-        f = self.inc(x)
-        att = [self.cbam1(f)]
-        for lvl in range(1, 5):
-            f = getattr(self, f"down{lvl}")(f)
-            att.append(getattr(self, f"cbam{lvl + 1}")(f))
-        y = att[4]
+        """Same graph with the fusions the plain-call API cannot express (``engine.InferenceSession``; inference only, the
+        plain calls under autograd / train mode):
+        * up4's last DS conv applies the 1-class OutConv in its epilogue (SmaAt_UNet.py:55-56), so the 64-channel activation
+          never reaches HBM;
+        * the three large CBAMs (levels 1-3) never write their output: they compute only their two gates, and the first DS
+          conv of up2 / up3 / up4 applies them as it loads the skip, with the products the CBAM's own kernel would have used
+          (bit for bit the same logits).  Levels 4-5 run the plain calls."""
+        if self.training or _needs_grad(self, x):
+            return self.forward(x)
+        skips, f = [], self.inc(x)
+        for lvl in range(5):
+            if lvl > 0:
+                f = getattr(self, f"down{lvl}")(f, pooled=pooled)
+            cbam = getattr(self, f"cbam{lvl + 1}")
+            bn = cbam.spatial_att.bn
+            if lvl < 3 and not bn.training and bn.track_running_stats:
+                sc, sa, pooled = cbam.serving_gates(f)
+                skips.append((f, (sc, sa)))
+            else:
+                skips.append((cbam(f), None))       # a plain call leaves its max-pool for the DownDS that follows
+                pooled = None
+        y = skips[4][0]
         for i in range(3):
-            y = getattr(self, f"up{i + 1}")(y, att[3 - i])
-        return self.up4(y, att[0], outconv=self.outc)
+            skip, gate = skips[3 - i]
+            y = getattr(self, f"up{i + 1}")(y, skip, gate=gate)
+        skip, gate = skips[0]
+        return self.up4(y, skip, outconv=self.outc, gate=gate)
 
 
 class UNet(nn.Module):

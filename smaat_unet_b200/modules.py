@@ -113,6 +113,22 @@ class DepthwiseSeparableConv(_CachingModule):
         d = ops.dw3x3(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, x1=x1, in_scale=in_scale, in_shift=in_shift)
         return ops.pw1x1(d, self.pointwise.weight.detach(), scale, shift, relu, mode=mode, w_split=split, stats=stats)
 
+    def cbam_takes(self, x, x1=None, gate=False, pools=False) -> bool:
+        """Whether ``run_cbam`` takes this input: the fused kernel with the serving forward's CBAM fusions."""
+        return ops.dsconv_cbam_takes(x, x1, self.pointwise.weight.detach(), self.kernels_per_layer, gate=gate, pools=pools)
+
+    def run_cbam(self, x, x1=None, scale=None, shift=None, relu=False, gate=None, pools=False):
+        """``run`` in one fused kernel that reads x as the CBAM output (x * sc) * sa (``gate=(sc, sa)``) and / or also returns
+        the channel gate's partial pools and the 2x2 max-pool of its output (``pools``): see ``ops.dsconv_cbam``."""
+        self._check()
+        dw_b = self.depthwise.bias.detach() if self.depthwise.bias is not None else None
+        if shift is None:
+            shift = self.pointwise.bias.detach() if self.pointwise.bias is not None else None
+        mode = ops.get_pointwise_mode()
+        split = self.pw_split() if mode == "tf32x3" else None
+        return ops.dsconv_cbam(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(),
+                               scale, shift, relu, x1=x1, mode=mode, w_split=split, gate=gate, pools=pools)
+
     def forward(self, x):
         if _needs_grad(self, x):
             from .autograd import DSConvFn
@@ -158,13 +174,23 @@ class DoubleConvDS(_CachingModule):
             hit = self._fold[idx]
         return hit[1]
 
-    def run(self, x, x1=None, outconv=None):
+    def _eval_folded(self, *inputs):
+        """True when this call runs the eval fast path: folded BatchNorm, no batch statistics, no autograd tape."""
+        bns = (self.double_conv[1], self.double_conv[4])
+        return not (_needs_grad(self, *inputs) or self.training
+                    or any(not bn.track_running_stats or bn.running_mean is None for bn in bns))
+
+    def run(self, x, x1=None, outconv=None, gate=None):
         """``outconv`` (an OutConv module with one class, inference only): fold it into the last kernel's epilogue and
-        return the logits -- the block's own output is then never materialised (models/SmaAt_UNet.py:55-56)."""
+        return the logits -- the block's own output is then never materialised (models/SmaAt_UNet.py:55-56).
+        ``gate=(sc, sa)``: x is the un-attended skip and the block's input is the CBAM output (x * sc) * sa, which the first
+        DS conv computes as it loads x (inference only; materialised first where that kernel does not take it)."""
         ops._req(x, "input", 4)
+        if gate is not None and not (self._eval_folded(x, x1) and self.double_conv[0].cbam_takes(x, x1, gate=True)):
+            x, gate = ops.cbam_scale(x, gate[0], gate[1]), None
         if outconv is not None:
-            y = self._run_with_outconv(x, x1, outconv)
-            return y if y is not None else outconv(self.run(x, x1))
+            y = self._run_with_outconv(x, x1, outconv, gate)
+            return y if y is not None else outconv(self.run(x, x1, gate=gate))
         if _needs_grad(self, x, x1):
             from .autograd import DoubleConvDSFn
             return DoubleConvDSFn.run(self, x, x1)
@@ -172,19 +198,23 @@ class DoubleConvDS(_CachingModule):
         if self.training or any(not bn.track_running_stats or bn.running_mean is None for bn in bns):
             from . import functional as Fn       # batch statistics (and running-stat update), no tape
             return Fn.double_conv_fwd(self, x, x1)[0]
-        s0, t0 = self._folded(0)
-        y = self.double_conv[0].run(x, x1=x1, scale=s0, shift=t0, relu=True)
+        y = self._first_conv(x, x1, gate)
         s1, t1 = self._folded(3)
         return self.double_conv[3].run(y, scale=s1, shift=t1, relu=True)
 
-    def _run_with_outconv(self, x, x1, outconv):
+    def _first_conv(self, x, x1, gate):
+        s0, t0 = self._folded(0)
+        if gate is not None:
+            return self.double_conv[0].run_cbam(x, x1=x1, scale=s0, shift=t0, relu=True, gate=gate)
+        return self.double_conv[0].run(x, x1=x1, scale=s0, shift=t0, relu=True)
+
+    def _run_with_outconv(self, x, x1, outconv, gate=None):
         bns = (self.double_conv[1], self.double_conv[4])
         oc = outconv.conv
         if (_needs_grad(self, x, x1) or _needs_grad(outconv, x) or self.training or oc.out_channels != 1
                 or any(not bn.track_running_stats or bn.running_mean is None for bn in bns)):
             return None
-        s0, t0 = self._folded(0)
-        y = self.double_conv[0].run(x, x1=x1, scale=s0, shift=t0, relu=True)
+        y = self._first_conv(x, x1, gate)
         s1, t1 = self._folded(3)
         ob = oc.bias.detach() if oc.bias is not None else None
         z = self.double_conv[3].run(y, scale=s1, shift=t1, relu=True, outconv=(oc.weight.detach(), ob))
@@ -298,15 +328,17 @@ class UpDS(_TransposedUp):
             self.conv = DoubleConvDS(in_channels, out_channels, kernels_per_layer=kernels_per_layer)
         self._packed = None
 
-    def forward(self, x1, x2, outconv=None):
+    def forward(self, x1, x2, outconv=None, gate=None):
+        """``gate=(sc, sa)`` (serving forward, inference only): x2 is the un-attended skip, and the block reads the CBAM output
+        (x2 * sc) * sa as it loads it (DoubleConvDS.run)."""
         if not self.bilinear:
-            return self.conv.run(x2, x1=self._up_transposed(x1, x2.shape[2], x2.shape[3]), outconv=outconv)
+            return self.conv.run(x2, x1=self._up_transposed(x1, x2.shape[2], x2.shape[3]), outconv=outconv, gate=gate)
         if torch.is_grad_enabled() and x1.requires_grad:
             from .autograd import Upsample2xPadFn
             up = Upsample2xPadFn.apply(x1, x2.shape[2], x2.shape[3])
         else:
             up = ops.upsample2x_pad(x1, x2.shape[2], x2.shape[3])
-        return self.conv.run(x2, x1=up, outconv=outconv)
+        return self.conv.run(x2, x1=up, outconv=outconv, gate=gate)
 
 
 class DoubleConv(_CachingModule):
@@ -587,6 +619,14 @@ class CBAM(nn.Module):
             sa = ops.cbam_gate(red, self.spatial_att.conv.weight.detach(), self.spatial_att.bn_affine())
             y = ops.cbam_scale(x, sc, sa, out=out)
         return (y, pooled) if with_maxpool else y
+
+    def serving_gates(self, x):
+        """Serving forward, inference only: CBAM(x)'s two gates (sc (B, C), sa (B, 1, H, W)) and MaxPool2d(2)(x) (or None),
+        without writing CBAM(x): pools + MLP (+ max-pool), channel reduce, k x k gate -- the same launches and values as
+        ``forward``.  The consumer applies (x * sc) * sa as it loads x (``UpDS.forward(..., gate=(sc, sa))``)."""
+        sc, pooled = self.channel_att.gate(x, with_maxpool=True)
+        red = ops.cbam_reduce(x, sc)
+        return sc, ops.cbam_gate(red, self.spatial_att.conv.weight.detach(), self.spatial_att.bn_affine()), pooled
 
 
 def cached_tensors(model):

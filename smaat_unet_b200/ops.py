@@ -212,6 +212,63 @@ def dsconv_takes(x, x1, pw_weight, k, mode=None, stats=False) -> bool:
     return bool(_lib.load().smaat_dsconv_eligible2(_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2], x.shape[3], k, w2d.shape[0], int(bool(stats))))
 
 
+def dsconv_cbam_takes(x, x1, pw_weight, k, gate=False, pools=False, mode=None) -> bool:
+    """True when ``dsconv_cbam`` runs on these inputs: the fused kernel, reading x as a CBAM output (``gate``) and / or writing
+    the channel gate's partial pools and the 2x2 max-pool of its output (``pools``)."""
+    mode = mode or _pw_mode
+    if not _fuse_ds or PW_MODES[mode] == 0:
+        return False
+    x, bs0 = _nchw_bstride(x, "x")
+    C1, bs1 = 0, 0
+    if x1 is not None:
+        x1, bs1 = _nchw_bstride(x1, "x1")
+        C1 = x1.shape[1]
+    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
+    return bool(_lib.load().smaat_dsconv_cbam_eligible(_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2], x.shape[3], k,
+                                                       w2d.shape[0], PW_MODES[mode], int(bool(gate)), int(bool(pools))))
+
+
+def dsconv_cbam(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, mode=None, w_split=None, gate=None, pools=False):
+    """``dsconv`` in the serving forward's CBAM fusions (smaat_dsconv_cbam_fwd).  ``gate=(sc (B, C0), sa (B, 1, H, W))``: x is read as
+    the CBAM output (x * sc) * sa.  ``pools``: also returns the channel gate's partial sums / maxima (B, npart, Cout) and
+    MaxPool2d(2) of the output: (y, psum, pmax, pooled).  Raises where ``dsconv_cbam_takes`` is False."""
+    mode = mode or _pw_mode
+    if not dsconv_cbam_takes(x, x1, pw_weight, k, gate is not None, pools, mode):
+        raise RuntimeError("smaat_unet_b200: dsconv_cbam called on a request the fused kernel does not take (check dsconv_cbam_takes)")
+    x, bs0 = _nchw_bstride(x, "x")
+    B, C0, H, W = x.shape
+    C1, bs1 = 0, 0
+    if x1 is not None:
+        x1, bs1 = _nchw_bstride(x1, "x1")
+        C1 = x1.shape[1]
+    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
+    Cout, K = w2d.shape
+    assert K == k * (C0 + C1), f"pointwise weight {tuple(pw_weight.shape)} does not match k*Cin={k * (C0 + C1)}"
+    lib = _lib.load()
+    wlo = None
+    if PW_MODES[mode] == 2:
+        w2d, wlo = w_split if w_split is not None else split_tf32(w2d)
+    sc = sa = None
+    if gate is not None:
+        sc, sa = _dense(gate[0], "gate sc"), _dense(gate[1], "gate sa")
+        assert sc.numel() == B * C0 and sa.numel() == B * H * W, "CBAM gate: sc (B, C0), sa (B, 1, H, W)"
+    psum = pmax = pooled = None
+    if pools:
+        npart = lib.smaat_dsconv_pool_parts(H, W)
+        psum = torch.empty((B, npart, Cout), device=x.device, dtype=torch.float32)
+        pmax = torch.empty_like(psum)
+        pooled = torch.empty((B, Cout, H // 2, W // 2), device=x.device, dtype=torch.float32)
+    y = torch.empty((B, Cout, H, W), device=x.device, dtype=torch.float32)
+    Cin = C0 + C1
+    extra = (4 * B * H * W * C0 if gate is not None else 0) + (4 * B * Cout * (H // 2) * (W // 2) + 8 * psum.numel() if pools else 0)
+    _call(f"smaat_dsconv_fwd[C{Cin}_N{Cout}_S{H}]",
+          4 * B * H * W * (Cin + Cout) + 4 * K * Cout + extra, 2 * B * H * W * K * (Cout + 9),
+          lib.smaat_dsconv_cbam_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(_dense(dw_weight, "depthwise.weight")), _ptr(dw_bias),
+          _ptr(w2d), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(y), Cout * H * W, _ptr(sc), _ptr(sa), _ptr(psum), _ptr(pmax), _ptr(pooled),
+          B, H, W, k, Cout, int(bool(relu)), PW_MODES[mode], _stream())
+    return (y, psum, pmax, pooled) if pools else y
+
+
 def dsconv(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, mode=None, w_split=None, stats=None, outconv=None):
     """Fused DepthwiseSeparableConv (layers.py:47-50) + affine (+ReLU); returns None when the fused kernel
     does not take this shape/mode (caller then runs dw3x3 + pw1x1).  ``outconv=(weight (1, Cout[,1,1]), bias or None)``
@@ -486,6 +543,24 @@ def cbam_pool_mlp(x, w1, b1, w2, b2, with_maxpool=False):
     _call(f"smaat_cbam_pool_mlp_fwd[C{Cc}_S{H}]", (5 if want_pool else 4) * B * Cc * H * W, 0, _lib.load().smaat_cbam_pool_mlp_fwd, _ptr(x), _ptr(avg), _ptr(mx),
           _ptr(pooled), _ptr(_dense(w1, "w1")), _ptr(b1), _ptr(_dense(w2, "w2")), _ptr(b2), _ptr(sc), _ptr(cnt), B, Cc, H, W, hidden, _stream())
     return sc, avg, mx, pooled
+
+
+def cbam_mlp_partials(psum, pmax, H, W, w1, b1, w2, b2):
+    """ChannelAttention gate from the partial pools ``dsconv_cbam(..., pools=True)`` wrote for an (H, W) map, in one launch:
+    (sc, avg, mx), each (B, C); None when the shape is not taken (C % 16, C > 512, hidden > 64) -- callers then pool the map
+    itself (``cbam_pool_mlp``)."""
+    B, npart, Cc = psum.shape
+    hidden = w1.shape[0]
+    if Cc % 16 != 0 or Cc > 512 or hidden > 64:
+        return None
+    avg = torch.empty((B, Cc), device=psum.device, dtype=torch.float32)
+    mx = torch.empty_like(avg)
+    sc = torch.empty_like(avg)
+    cnt = _counters(psum.device, B)
+    _call(f"smaat_cbam_mlp_partials_fwd[C{Cc}_S{H}]", 8 * psum.numel() + 12 * B * Cc, 0, _lib.load().smaat_cbam_mlp_partials_fwd,
+          _ptr(_dense(psum, "psum")), _ptr(_dense(pmax, "pmax")), npart, _ptr(avg), _ptr(mx), _ptr(_dense(w1, "w1")), _ptr(b1),
+          _ptr(_dense(w2, "w2")), _ptr(b2), _ptr(sc), _ptr(cnt), B, Cc, H, W, hidden, _stream())
+    return sc, avg, mx
 
 
 def cbam_gate_scale(x, sc, pooled, wsp, bn_affine, out=None):

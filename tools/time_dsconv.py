@@ -7,7 +7,11 @@ For each shape it times two entry points over the same tiles, main loop and affi
 Their difference bounds what the output stores cost.  Each timing is 5 warm-up launches, then 40 launches between two CUDA
 events.  `hbm_ms` is the algorithmic HBM floor: input + output bytes at 3.35 TB/s (H100 SXM data sheet).
 
-  python tools/time_dsconv.py [--tree DIR] [--mode tf32x3|tf32] [--json]
+With --cbam it times instead the serving forward's CBAM fusions (smaat_dsconv_cbam_fwd) against the plain fused conv on the same
+tiles: the second DS conv of inc / down1 / down2 with and without the epilogue pools (partial sums / maxima + 2x2 max-pool), and
+the first DS conv of up4 / up3 / up2 with and without the gate applied on load.
+
+  python tools/time_dsconv.py [--tree DIR] [--mode tf32x3|tf32] [--json] [--cbam]
 
 --tree imports smaat_unet_b200 from another checkout (a built one), to compare two builds in one session."""
 import argparse
@@ -19,6 +23,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--tree", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 ap.add_argument("--mode", default="tf32x3", choices=["tf32", "tf32x3"])
 ap.add_argument("--json", action="store_true", help="one JSON line per shape instead of a table")
+ap.add_argument("--cbam", action="store_true", help="time the CBAM fusions (epilogue pools, gate on load) instead")
 args = ap.parse_args()
 sys.path.insert(0, os.path.abspath(args.tree))
 
@@ -55,8 +60,55 @@ def timed(fn):
     return e0.elapsed_time(e1) / ITERS
 
 
+# (C0, C1, S, Cout, what): producers of the CBAM level 1-3 maps (pools) and the up-block convs reading them (gate)
+CBAM_SHAPES = [
+    (64, 0, 288, 64, "pools"),
+    (128, 0, 144, 128, "pools"),
+    (256, 0, 72, 256, "pools"),
+    (64, 64, 288, 64, "gate"),
+    (128, 128, 144, 128, "gate"),
+    (256, 256, 72, 256, "gate"),
+]
+
+
+def main_cbam():
+    g = torch.Generator(device="cuda").manual_seed(7)
+    rows = []
+    for C0, C1, S, Cout, what in CBAM_SHAPES:
+        Cin = C0 + C1
+        K = K_PL * Cin
+        x0 = torch.rand(B, C0, S, S, device="cuda", generator=g)
+        x1 = torch.rand(B, C1, S, S, device="cuda", generator=g) if C1 else None
+        dw_w = torch.randn(K, 1, 3, 3, device="cuda", generator=g) * 0.3
+        dw_b = torch.randn(K, device="cuda", generator=g) * 0.1
+        pw_w = torch.randn(Cout, K, device="cuda", generator=g) * 0.1
+        scale = torch.rand(Cout, device="cuda", generator=g) + 0.5
+        shift = torch.randn(Cout, device="cuda", generator=g) * 0.1
+        split = ops.split_tf32(pw_w) if args.mode == "tf32x3" else None
+        gate = (torch.rand(B, C0, device="cuda", generator=g), torch.rand(B, 1, S, S, device="cuda", generator=g)) if what == "gate" else None
+        common = (dw_w, dw_b, K_PL, pw_w, scale, shift, True)
+        ms_plain = timed(lambda: ops.dsconv(x0, *common, x1=x1, mode=args.mode, w_split=split))
+        ms_fused = timed(lambda: ops.dsconv_cbam(x0, *common, x1=x1, mode=args.mode, w_split=split, gate=gate, pools=what == "pools"))
+        name = f"C{Cin}->{Cout} {S}^2" + (" (concat)" if C1 else "")
+        rows.append({"layer": name, "fusion": what, "plain_ms": round(ms_plain, 4), "fused_ms": round(ms_fused, 4),
+                     "extra_ms": round(ms_fused - ms_plain, 4)})
+        del x0, x1
+    dev = torch.cuda.get_device_name()
+    if args.json:
+        for r in rows:
+            print(json.dumps(r))
+        print(json.dumps({"device": dev, "mode": args.mode}))
+        return
+    print(f"{dev}, {args.mode}, B = {B}, k = {K_PL}; {WARMUP} warm-up + {ITERS} timed launches each")
+    print(f"{'layer':28s} {'fusion':>6s} {'plain ms':>9s} {'fused ms':>9s} {'extra ms':>9s}")
+    for r in rows:
+        print(f"{r['layer']:28s} {r['fusion']:>6s} {r['plain_ms']:9.3f} {r['fused_ms']:9.3f} {r['extra_ms']:9.3f}")
+
+
 def main():
     assert torch.cuda.is_available(), "time_dsconv.py needs a GPU"
+    if args.cbam:
+        return main_cbam()
     lib = _lib.load()
     mode = ops.PW_MODES[args.mode]
     g = torch.Generator(device="cuda").manual_seed(7)
