@@ -106,6 +106,21 @@ int smaat_dsconv_outconv_fwd(const float* x0, int C0, int64_t x0_bstride, const 
                              const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
                              const float* scale, const float* shift, const float* oc_w, const float* oc_b, float* logits,
                              int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
+/* The same kernel for a K-class OutConv, ending in the class map the reference's validation loop predicts
+ * (pred_class = torch.argmax(softmax(y_pred), dim=1), train_SmaAtUNet.py:76; softmax keeps the order).  oc_w: (K, Cout),
+ * oc_b: (K) or NULL; logits: (B, K, H, W) or NULL; classes: (B, H, W) int64 or NULL, not both NULL.  Class j's logit is bit for
+ * bit what smaat_dsconv_outconv_fwd writes with oc_w row j and oc_b[j]; classes[b, p] is the argmax of the K logits, ties to
+ * the first index, a NaN logit wins (torch.argmax), identical whether or not logits are written.  Neither the Cout-channel
+ * activation nor (with logits NULL) the K logit planes reach HBM.  Eligibility: that of smaat_dsconv_outconv_fwd (Cout <= 128,
+ * no batch statistics) and 1 <= K <= 32 (K <= 22 for Cout > 64: the class weights live in the shared memory the kernel
+ * leaves free); SMAAT_E_UNSUPPORTED otherwise (callers then run smaat_dsconv_fwd or dw3x3 + pw1x1,
+ * smaat_outconv_fwd and smaat_argmax_channels_fwd).  smaat_dsconv_classify_eligible returns 1/0 for the same test in `mode`. */
+int smaat_dsconv_classify_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                                   const float* pw_w, int H, int W, int k, int Cout, int K, int mode);
+int smaat_dsconv_classify_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                              const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
+                              const float* scale, const float* shift, const float* oc_w, const float* oc_b, int K,
+                              float* logits, int64_t* classes, int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
 
 /* The fused DS conv with the CBAM fusions of the serving forward (models/layers.py:90-141 around the DS blocks of
  * models/SmaAt_UNet.py:41-57); arguments as smaat_dsconv_fwd, without batch statistics.
@@ -292,6 +307,11 @@ int smaat_ce_fwd(const float* logits, const int64_t* target, int B, int K, int64
                  double* batch_acc, float* dlogits, int64_t* conf, void* stream);
 int smaat_confusion_add(const int64_t* pred, const int64_t* target, int64_t n, int K, int64_t* conf, int64_t* invalid,
                         void* stream);
+/* smaat_argmax_channels_fwd: the class map of any (B, K, P) logits, classes[b, p] = argmax_c x[b, c, p] (int64), in one read:
+ *   ties go to the first index and a NaN logit wins, as torch.argmax (and smaat_ce_fwd's confusion column).  1 <= K <= 1024
+ *   (larger K: SMAAT_E_UNSUPPORTED).  128-bit loads when P % 4 == 0 and x / classes are 16-byte aligned, a scalar kernel
+ *   otherwise.  Serves every model output smaat_dsconv_classify_fwd does not produce. */
+int smaat_argmax_channels_fwd(const float* x, int64_t* classes, int B, int K, int64_t P, void* stream);
 
 /* CBAM in three launches (reference models/layers.py:90-141).
  * smaat_cbam_pool_mlp_fwd: ChannelAttention's global pools AND its shared MLP + sigmoid (layers.py:98-109): the last pooling

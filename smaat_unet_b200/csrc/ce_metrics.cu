@@ -203,6 +203,41 @@ __global__ void __launch_bounds__(CE_THREADS) confusion_add_kernel(const int64_t
   }
 }
 
+// Channel argmax: the class map of (B, K, P) logits in one read, NPX consecutive pixels of one image per thread (NPX = 4: 128-bit
+// loads and two 128-bit stores of the int64 classes).  The first strictly larger value wins, and a NaN wins and stays: the
+// answer of torch.argmax, and of ce_fwd_kernel's argmax above.
+template <int NPX>
+__global__ void __launch_bounds__(CE_THREADS) argmax_channels_kernel(const float* __restrict__ x, int64_t* __restrict__ classes, int K,
+                                                                     int64_t P, int64_t groups) {
+  const int64_t gpi = P / NPX;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += stride) {
+    const int64_t b = g / gpi;
+    const int64_t p0 = (g - b * gpi) * NPX;
+    const float* base = x + b * (int64_t)K * P + p0;
+    float m[NPX];
+    int am[NPX];
+#pragma unroll
+    for (int j = 0; j < NPX; ++j) { m[j] = -INFINITY; am[j] = 0; }
+    for (int c = 0; c < K; ++c) {
+      float v[NPX];
+      load_px_last<NPX>(base + (int64_t)c * P, v);
+#pragma unroll
+      for (int j = 0; j < NPX; ++j) {
+        if (m[j] == m[j] && (v[j] > m[j] || v[j] != v[j])) { m[j] = v[j]; am[j] = c; }
+      }
+    }
+    int64_t* out = classes + b * P + p0;
+    if constexpr (NPX == 4) {
+      reinterpret_cast<longlong2*>(out)[0] = make_longlong2(am[0], am[1]);
+      reinterpret_cast<longlong2*>(out)[1] = make_longlong2(am[2], am[3]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < NPX; ++j) out[j] = am[j];
+    }
+  }
+}
+
 static int64_t l2_bytes() {
   int dev = 0, l2 = 0;
   cudaGetDevice(&dev);
@@ -249,6 +284,25 @@ extern "C" int smaat_ce_fwd(const float* logits, const int64_t* target, int B, i
     else      ce_fwd_kernel<1, false><<<g, CE_THREADS, 0, st>>>(logits, target, K, P, groups, ignore_index, use_ignore, batch_acc, dlogits, cf);
   }
   SMAAT_LAUNCH_CHECK("smaat_ce_fwd");
+  return SMAAT_OK;
+}
+
+extern "C" int smaat_argmax_channels_fwd(const float* x, int64_t* classes, int B, int K, int64_t P, void* stream) {
+  SMAAT_REQUIRE(x && classes && B > 0 && P > 0, "argmax_channels: bad arguments (B=%d, P=%lld)", B, (long long)P);
+  SMAAT_REQUIRE(K >= 1, "argmax_channels: K=%d classes", K);
+  if (K > 1024) return fail(SMAAT_E_UNSUPPORTED, "argmax_channels: K=%d classes, this build supports at most 1024", K);
+  SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(x) & 3u) == 0 && (reinterpret_cast<uintptr_t>(classes) & 7u) == 0,
+                "argmax_channels: logits must be 4-byte and classes 8-byte aligned");
+  const bool vec = P % 4 == 0 && aligned16(x) && aligned16(classes);
+  const int npx = vec ? 4 : 1;
+  const int64_t groups = (int64_t)B * (P / npx);
+  int64_t blocks = ceil_div64(groups, CE_THREADS);
+  const int64_t cap = (int64_t)num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (vec) argmax_channels_kernel<4><<<(unsigned)blocks, CE_THREADS, 0, st>>>(x, classes, K, P, groups);
+  else     argmax_channels_kernel<1><<<(unsigned)blocks, CE_THREADS, 0, st>>>(x, classes, K, P, groups);
+  SMAAT_LAUNCH_CHECK("smaat_argmax_channels_fwd");
   return SMAAT_OK;
 }
 

@@ -63,9 +63,15 @@ struct DsParams {
   float* pool_max;
   float* pooled;
   int npart;
+  // K-class OutConv + argmax (smaat_dsconv_classify_fwd): ncls > 0 classes, oc_w (ncls, Cout), oc_b (ncls) or null, oc_y the
+  // (B, ncls, H, W) logits or null, cls the (B, H, W) class map or null
+  int ncls;
+  int64_t* cls;
   int C0, C1, H, W, Cout, relu, K;
   int tiles_x, tiles_y, npass, total_tiles, nchunks;
 };
+
+constexpr int DS_MAX_CLASSES = 32;   // classes of the fused K-class OutConv + argmax (smaat_dsconv_classify_fwd)
 
 template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
 struct DsCfg {
@@ -119,6 +125,16 @@ struct DsCfg {
   static constexpr int OFF_BAR = OFF_ST + ST_BYTES;
   static_assert((IS * NG + IS + 2 * AS + 2 * BS) * 8 <= BAR_BYTES, "barrier block");
   static constexpr int TOTAL = OFF_BAR + BAR_BYTES + 3 * AFF_N * 4 + 1024;
+  // The K-class OutConv of smaat_dsconv_classify_fwd keeps its weights ([class][N_TILE], zero past Cout) and biases in the shared
+  // memory the rings leave under the 227 KB limit (11.5-29.5 KB), appended after the affine block and requested only by class
+  // launches: as many classes as fit, at most DS_MAX_CLASSES (32 at N_TILE 64, 22 at N_TILE 128).  Read through the L1 the
+  // weights were a cache miss per class (the carveout leaves little L1 beside 213 KB of shared memory)
+  static constexpr int OFF_CLS = OFF_BAR + BAR_BYTES + 3 * AFF_N * 4;
+  static constexpr int CLS_FIT = (227 * 1024 - TOTAL) / ((N_TILE + 1) * 4);
+  static constexpr int MAX_CLASSES = CLS_FIT < DS_MAX_CLASSES ? CLS_FIT : DS_MAX_CLASSES;
+  static constexpr int CLS_SMEM = MAX_CLASSES * (N_TILE + 1) * 4;
+  static_assert(MAX_CLASSES >= 21, "the class weights of a 21-class model fit beside the rings");
+  static_assert(TOTAL + CLS_SMEM <= 227 * 1024, "the class weights take no shared memory from the rings");
   static constexpr uint32_t B_TX = BST_BYTES;
   static constexpr int PROD_WARP = 12;                         // first producer warp
   static constexpr int THREADS = 384 + 128 * NG;               // TMA, loader, 2 idle | 2 consumer warpgroups | producers
@@ -233,6 +249,15 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
     aff[c] = (c < p.Cout && p.scale) ? __ldg(p.scale + c) : 1.f;
     aff[L::AFF_N + c] = (c < p.Cout && p.shift) ? __ldg(p.shift + c) : 0.f;
     aff[2 * L::AFF_N + c] = (c < p.Cout && p.oc_w) ? __ldg(p.oc_w + c) : 0.f;
+  }
+  float* cls_w = reinterpret_cast<float*>(smem + L::OFF_CLS);   // [ncls][N_TILE] (class launches only), then ncls biases
+  float* cls_b = cls_w + L::MAX_CLASSES * N_TILE;
+  if (p.ncls) {
+    for (int i = threadIdx.x; i < p.ncls * N_TILE; i += blockDim.x) {
+      const int cl = i / N_TILE, c = i - cl * N_TILE;
+      cls_w[i] = c < p.Cout ? __ldg(p.oc_w + (int64_t)cl * p.Cout + c) : 0.f;
+    }
+    for (int cl = threadIdx.x; cl < p.ncls; cl += blockDim.x) cls_b[cl] = p.oc_b ? __ldg(p.oc_b + cl) : 0.f;
   }
   __syncthreads();
 
@@ -419,7 +444,57 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
           }
         }
       }
-      if (p.oc_y) {
+      if (p.ncls) {
+        // K-class OutConv + argmax.  The activations replace the accumulators in place (fmaxf(fmaf(acc, sc, sh), act_lo), as
+        // below); then, one class at a time, the one-class dot product below in its order (fmaf over the thread's channels, the
+        // two xor shuffles, + bias), so class j's logit is bit for bit what that epilogue writes with OutConv row j.  After the
+        // butterfly all 4 lanes of a fragment group hold the same logits; each keeps the same running (max, first index) per
+        // pixel -- torch.argmax's rule: a NaN wins and stays -- so the registers hold two logits whatever K is.  A lane's two
+        // channels 2t, 2t + 1 of a fragment column are one 8-byte shared-memory load (the 8 fragment groups read the same
+        // address: a broadcast, conflict-free).  Logit stores rotate over the 4 lanes
+#pragma unroll
+        for (int j = 0; j < N_TILE / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = 8 * j + 2 * t + e;
+            const float sc = aff[c], sh = aff[L::AFF_N + c];
+            acc[4 * j + e] = fmaxf(fmaf(acc[4 * j + e], sc, sh), act_lo);
+            acc[4 * j + 2 + e] = fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo);
+          }
+        }
+        float best0 = -INFINITY, best1 = -INFINITY;
+        int arg0 = 0, arg1 = 0;
+#pragma unroll 1
+        for (int cl = 0; cl < p.ncls; ++cl) {
+          const float* wr = cls_w + cl * N_TILE + 2 * t;   // zero past Cout, where the activation is 0 too
+          float d0 = 0.f, d1 = 0.f;
+#pragma unroll
+          for (int j = 0; j < N_TILE / 8; ++j) {
+            const float2 w = *reinterpret_cast<const float2*>(wr + 8 * j);
+            d0 = fmaf(acc[4 * j], w.x, d0);
+            d1 = fmaf(acc[4 * j + 2], w.x, d1);
+            d0 = fmaf(acc[4 * j + 1], w.y, d0);
+            d1 = fmaf(acc[4 * j + 3], w.y, d1);
+          }
+          d0 += __shfl_xor_sync(0xffffffffu, d0, 1);
+          d0 += __shfl_xor_sync(0xffffffffu, d0, 2);
+          d1 += __shfl_xor_sync(0xffffffffu, d1, 1);
+          d1 += __shfl_xor_sync(0xffffffffu, d1, 2);
+          const float ob = cls_b[cl];
+          const float l0 = d0 + ob, l1 = d1 + ob;
+          if (best0 == best0 && (l0 > best0 || l0 != l0)) { best0 = l0; arg0 = cl; }
+          if (best1 == best1 && (l1 > best1 || l1 != l1)) { best1 = l1; arg1 = cl; }
+          if (p.oc_y && t == (cl & 3)) {
+            float* yk = p.oc_y + ((int64_t)b * p.ncls + cl) * P;
+            if (v0) yk[o0] = l0;
+            if (v1) yk[o1] = l1;
+          }
+        }
+        if (p.cls) {
+          if (v0 && t == 0) p.cls[(int64_t)b * P + o0] = arg0;
+          if (v1 && t == 1) p.cls[(int64_t)b * P + o1] = arg1;
+        }
+      } else if (p.oc_y) {
         // fused OutConv: each pixel's dot product over all Cout <= N_TILE activations.  Channels past Cout have zero
         // accumulators, identity affine and zero OutConv weight: no mask needed
         float d0 = 0.f, d1 = 0.f;
@@ -680,10 +755,14 @@ static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtenso
   auto kern = dsconv_fused_kernel<N_TILE, KPL, PW, X3, A_SMEM>;
   // the pools are read back from the staging buffers: instances with the direct-store epilogue do not take them
   if (p.pool_sum && !L::ST_BUFS) return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools need the staged epilogue");
+  if (p.ncls > L::MAX_CLASSES)
+    return fail(SMAAT_E_UNSUPPORTED, "dsconv+classify: %d classes, this instance keeps the weights of at most %d", p.ncls, L::MAX_CLASSES);
   static std::atomic<uint64_t> attr_mask{0};   // cudaFuncSetAttribute is per device
   if (first_use_on_device(attr_mask)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
-    if (e != cudaSuccess) return fail(SMAAT_E_CUDA, "dsconv: smem attribute (%d B): %s", L::TOTAL, cudaGetErrorString(e));
+    // class launches append the class weights (CLS_SMEM); every other launch requests TOTAL, as before
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL + L::CLS_SMEM);
+    if (e != cudaSuccess)
+      return fail(SMAAT_E_CUDA, "dsconv: smem attribute (%d B): %s", L::TOTAL + L::CLS_SMEM, cudaGetErrorString(e));
     int r = check_reg_budget((const void*)kern, L::THREADS, L::REGS_SUM, "dsconv");
     if (r) return r;
   }
@@ -696,7 +775,7 @@ static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtenso
   p.nchunks = ceil_div(p.C0 + p.C1, L::CC);
   p.npart = 2 * p.tiles_x * p.tiles_y;
   const int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
-  kern<<<grid, L::THREADS, L::TOTAL, st>>>(m0, m1, mw, mwl, my, msa, p);
+  kern<<<grid, L::THREADS, L::TOTAL + (p.ncls ? L::CLS_SMEM : 0), st>>>(m0, m1, mw, mwl, my, msa, p);
   SMAAT_LAUNCH_CHECK("smaat_dsconv_fwd");
   return SMAAT_OK;
 }
@@ -739,6 +818,21 @@ static bool ds_staged_t(bool x3, bool a_smem) {
   return (x3 ? (a_smem ? DsCfg<N_TILE, KPL, PW, true, true>::ST_BUFS : DsCfg<N_TILE, KPL, PW, true, false>::ST_BUFS)
              : (a_smem ? DsCfg<N_TILE, KPL, PW, false, true>::ST_BUFS : DsCfg<N_TILE, KPL, PW, false, false>::ST_BUFS)) > 0;
 }
+// The most classes whose OutConv weights the instance dsconv_run dispatches to keeps in shared memory (DsCfg::MAX_CLASSES)
+template <int N_TILE, int KPL, int PW>
+static int ds_max_classes_t(bool x3, bool a_smem) {
+  return x3 ? (a_smem ? DsCfg<N_TILE, KPL, PW, true, true>::MAX_CLASSES : DsCfg<N_TILE, KPL, PW, true, false>::MAX_CLASSES)
+            : (a_smem ? DsCfg<N_TILE, KPL, PW, false, true>::MAX_CLASSES : DsCfg<N_TILE, KPL, PW, false, false>::MAX_CLASSES);
+}
+static int ds_max_classes(int n_tile, int k, int pw, bool x3, bool a_smem) {
+  if (n_tile == 64) {
+    if (k == 2) return pw == 32 ? ds_max_classes_t<64, 2, 32>(x3, a_smem) : ds_max_classes_t<64, 2, 16>(x3, a_smem);
+    return pw == 32 ? ds_max_classes_t<64, 1, 32>(x3, a_smem) : ds_max_classes_t<64, 1, 16>(x3, a_smem);
+  }
+  if (k == 2) return pw == 32 ? ds_max_classes_t<128, 2, 32>(x3, a_smem) : ds_max_classes_t<128, 2, 16>(x3, a_smem);
+  return pw == 32 ? ds_max_classes_t<128, 1, 32>(x3, a_smem) : ds_max_classes_t<128, 1, 16>(x3, a_smem);
+}
+
 static bool ds_staged(int n_tile, int k, int pw, bool x3, bool a_smem) {
   if (n_tile == 64) {
     if (k == 2) return pw == 32 ? ds_staged_t<64, 2, 32>(x3, a_smem) : ds_staged_t<64, 2, 16>(x3, a_smem);
@@ -802,10 +896,12 @@ extern "C" int smaat_dsconv_pool_parts(int H, int W) {
 
 static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride, const float* dw_w,
                       const float* dw_b, const float* pw_w, const float* pw_w_lo, const float* scale, const float* shift, float* y,
-                      int64_t y_bstride, double* stats, const float* oc_w, const float* oc_b, float* oc_y, const float* gate_sc,
-                      const float* gate_sa, float* pool_sum, float* pool_max, float* pooled, int B, int H, int W, int k, int Cout,
-                      int relu, int mode, void* stream) {
-  SMAAT_REQUIRE(x0 && dw_w && pw_w && (y || oc_y), "dsconv: null pointer");
+                      int64_t y_bstride, double* stats, const float* oc_w, const float* oc_b, float* oc_y, int ncls, int64_t* cls,
+                      const float* gate_sc, const float* gate_sa, float* pool_sum, float* pool_max, float* pooled, int B, int H, int W,
+                      int k, int Cout, int relu, int mode, void* stream) {
+  // head: an OutConv in the epilogue (one class, or ncls classes with the argmax) replaces the activation output
+  const bool head = oc_y || ncls > 0;
+  SMAAT_REQUIRE(x0 && dw_w && pw_w && (y || oc_y || cls), "dsconv: null pointer");
   SMAAT_REQUIRE(!gate_sc == !gate_sa, "dsconv: the CBAM gate needs both sc and sa");
   SMAAT_REQUIRE(!gate_sa || aligned16(gate_sa), "dsconv: the CBAM gate map must be 16-byte aligned");
   SMAAT_REQUIRE(!pool_sum || (pool_max && pooled && y && !oc_y && !stats), "dsconv: the CBAM pools need sum, max and max-pool outputs and y");
@@ -814,10 +910,10 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   SMAAT_REQUIRE(C1 == 0 || x1, "dsconv: C1=%d but x1 is null", C1);
   SMAAT_REQUIRE(mode == SMAAT_PW_TF32 || mode == SMAAT_PW_TF32X3, "dsconv: mode must be SMAAT_PW_TF32 or SMAAT_PW_TF32X3");
   SMAAT_REQUIRE(mode != SMAAT_PW_TF32X3 || pw_w_lo, "dsconv: TF32X3 needs pw_w_lo (see smaat_split_tf32)");
-  SMAAT_REQUIRE(oc_y || y_bstride >= (int64_t)Cout * H * W, "dsconv: y batch stride too small");
-  SMAAT_REQUIRE(!oc_y || (oc_w && !stats), "dsconv+outconv: needs the OutConv weight and no batch statistics");
-  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, pw_w_lo, oc_y ? nullptr : y, y_bstride, H, W, k, Cout,
-                   stats != nullptr, oc_y != nullptr))
+  SMAAT_REQUIRE(head || y_bstride >= (int64_t)Cout * H * W, "dsconv: y batch stride too small");
+  SMAAT_REQUIRE(!head || (oc_w && !stats),"dsconv+outconv: needs the OutConv weight and no batch statistics");
+  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, pw_w_lo, head ? nullptr : y, y_bstride, H, W, k, Cout,
+                   stats != nullptr, head))
     return fail(SMAAT_E_UNSUPPORTED,
                 "dsconv: shape or output layout not taken by the fused kernel (k=%d Cout=%d H=%d W=%d, y 16-byte aligned with a "
                 "batch stride that is a multiple of 4); use dw3x3 + pw1x1",
@@ -860,7 +956,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   }
   // the staged epilogue's store box: one warpgroup's half-patch (PW x PH / 2 pixels) x 32 channels, swizzled by its row length
   CUtensorMap my = m0;
-  if (!oc_y) {
+  if (!head) {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)Cout, (uint64_t)B};
     const uint64_t str[4] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4, (uint64_t)y_bstride * 4};
     const uint32_t ybox[4] = {(uint32_t)pw, (uint32_t)(ph / 2), 32u, 1u};
@@ -878,7 +974,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   }
   DsParams p;
   p.dw_w = dw_w; p.dw_b = dw_b; p.scale = scale; p.shift = shift; p.y = y; p.y_bstride = y_bstride; p.stats = stats;
-  p.oc_w = oc_w; p.oc_b = oc_b; p.oc_y = oc_y;
+  p.oc_w = oc_w; p.oc_b = oc_b; p.oc_y = oc_y; p.ncls = ncls; p.cls = cls;
   p.gate_sc = gate_sc; p.pool_sum = pool_sum; p.pool_max = pool_max; p.pooled = pooled; p.npart = 0;
   p.C0 = C0; p.C1 = C1; p.H = H; p.W = W; p.Cout = Cout; p.relu = relu; p.K = K;
   p.tiles_x = p.tiles_y = p.npass = p.total_tiles = p.nchunks = 0;
@@ -904,7 +1000,7 @@ extern "C" int smaat_dsconv_fwd(const float* x0, int C0, int64_t x0_bstride, con
                                 int W, int k, int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(y, "dsconv: null output");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, stats, nullptr,
-                    nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
+                    nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
 }
 
 /* The network's last two modules in one kernel: DS conv -> BN/ReLU -> OutConv(Cout -> 1) (reference models/SmaAt_UNet.py:55-56,
@@ -916,7 +1012,36 @@ extern "C" int smaat_dsconv_outconv_fwd(const float* x0, int C0, int64_t x0_bstr
                                         float* logits, int B, int H, int W, int k, int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(oc_w && logits, "dsconv+outconv: null pointer");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
-                    logits, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
+                    logits, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
+}
+
+extern "C" int smaat_dsconv_classify_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                                              const float* pw_w, int H, int W, int k, int Cout, int K, int mode) {
+  if (mode != SMAAT_PW_TF32 && mode != SMAAT_PW_TF32X3) return 0;
+  if (K < 1 || K > DS_MAX_CLASSES) return 0;
+  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, false, true)) return 0;
+  // the class weights must fit the shared memory the instance leaves free: 32 classes at Cout <= 64, 22 up to Cout = 128
+  return K <= ds_max_classes(Cout > 64 ? 128 : 64, k, pick_pw(H, W), mode == SMAAT_PW_TF32X3, ds_impl() == 1) ? 1 : 0;
+}
+
+/* The network's last two modules for a K-class model, ending in the class map: DS conv -> BN/ReLU -> OutConv(Cout -> K) ->
+ * argmax over the K logits of each pixel (the reference's torch.argmax(softmax(y_pred), dim=1), train_SmaAtUNet.py:76; softmax
+ * keeps the order).  Neither the Cout-channel activation nor, unless asked for, the K logit planes reach HBM. */
+extern "C" int smaat_dsconv_classify_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                                         const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
+                                         const float* scale, const float* shift, const float* oc_w, const float* oc_b, int K,
+                                         float* logits, int64_t* classes, int B, int H, int W, int k, int Cout, int relu, int mode,
+                                         void* stream) {
+  SMAAT_REQUIRE(oc_w && (logits || classes), "dsconv+classify: needs the OutConv weight and a logits or a classes output");
+  SMAAT_REQUIRE(K >= 1, "dsconv+classify: K=%d classes", K);
+  if (K > DS_MAX_CLASSES)
+    return fail(SMAAT_E_UNSUPPORTED, "dsconv+classify: K=%d classes, the fused epilogue takes at most %d; use smaat_dsconv_fwd + "
+                                     "smaat_outconv_fwd + smaat_argmax_channels_fwd", K, DS_MAX_CLASSES);
+  SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(oc_w) & 3u) == 0 && (reinterpret_cast<uintptr_t>(logits) & 3u) == 0 &&
+                    (reinterpret_cast<uintptr_t>(classes) & 7u) == 0,
+                "dsconv+classify: weights / logits must be 4-byte and classes 8-byte aligned");
+  return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
+                    logits, K, classes, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
 }
 
 /* The fused DS conv of the serving forward with the CBAM fusions around it (models/layers.py:90-141, SmaAt_UNet.py:41-57).
@@ -931,5 +1056,5 @@ extern "C" int smaat_dsconv_cbam_fwd(const float* x0, int C0, int64_t x0_bstride
                                      int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(y, "dsconv_cbam: null output");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, nullptr, nullptr,
-                    nullptr, nullptr, gate_sc, gate_sa, pool_sum, pool_max, pooled, B, H, W, k, Cout, relu, mode, stream);
+                    nullptr, nullptr, 0, nullptr, gate_sc, gate_sa, pool_sum, pool_max, pooled, B, H, W, k, Cout, relu, mode, stream);
 }

@@ -19,10 +19,17 @@ from . import _lib
 
 
 class InferenceSession:
-    def __init__(self, model, batch, in_shape, device=None, use_graph=True, slots=2, serving_fusions=True):
+    def __init__(self, model, batch, in_shape, device=None, use_graph=True, slots=2, serving_fusions=True, output="logits"):
+        """``output="logits"`` (default): the model's fp32 output.  ``output="classes"``: the (batch, H, W) int64 class map
+        argmax over its channels (the reference's ``torch.argmax(softmax(y_pred), dim=1)``, train_SmaAtUNet.py:76), computed
+        inside the captured graph: ``model.forward_classes`` where the model has it (SmaAt_UNet: OutConv and argmax in the last
+        kernel's epilogue), otherwise ``model(x)`` followed by the channel argmax kernel.  Only the class map crosses PCIe."""
+        if output not in ("logits", "classes"):
+            raise ValueError(f"InferenceSession: output must be 'logits' or 'classes', got {output!r}")
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self.model = model.to(self.device).eval()
         self.batch, self.in_shape = batch, tuple(in_shape)
+        self.output = output
         self.use_graph = use_graph
         self.compute = torch.cuda.Stream(self.device)
         self.h2d = torch.cuda.Stream(self.device)
@@ -31,23 +38,28 @@ class InferenceSession:
         self.launches_per_forward = 0
         self.graph = None
         # the serving forward may fuse what plain module calls cannot express (OutConv in the last epilogue, model.py);
-        # serving_fusions=False captures exactly the reference-API call sequence
-        self._fwd = getattr(self.model, "forward_serving", None) if serving_fusions else None
+        # serving_fusions=False captures exactly the reference-API call sequence (+ the argmax kernel for class maps)
+        name = "forward_classes" if output == "classes" else "forward_serving"
+        self._fwd = getattr(self.model, name, None) if serving_fusions else None
         if self._fwd is None:
-            self._fwd = self.model
+            self._fwd = self.model if output == "logits" else self._model_then_argmax
         self._capture()
         self.out_shape = tuple(self.static_out.shape)
         # staging slots (device side) so H2D of step i+1 and D2H of step i-1 overlap compute of step i
         self.slots = slots
         self.in_stage = [torch.empty_like(self.static_in) for _ in range(slots)]
         self.out_stage = [torch.empty_like(self.static_out) for _ in range(slots)]
-        self.out_host = [torch.empty(self.out_shape, dtype=torch.float32, pin_memory=True) for _ in range(slots)]
+        self.out_host = [torch.empty(self.out_shape, dtype=self.static_out.dtype, pin_memory=True) for _ in range(slots)]
         self._h2d_done = [torch.cuda.Event() for _ in range(slots)]
         self._in_free = [torch.cuda.Event() for _ in range(slots)]
         self._out_ready = [torch.cuda.Event() for _ in range(slots)]
         self._d2h_done = [torch.cuda.Event() for _ in range(slots)]
         self._pending = collections.deque()
         self._step = 0
+
+    def _model_then_argmax(self, x):
+        from . import ops
+        return ops.argmax_channels(self.model(x))
 
     def _capture(self):
         with torch.cuda.device(self.device), torch.no_grad():
@@ -139,8 +151,8 @@ class InferenceSession:
 
     @property
     def h2d_bytes_per_step(self):
-        return self.static_in.numel() * 4
+        return self.static_in.numel() * self.static_in.element_size()
 
     @property
     def d2h_bytes_per_step(self):
-        return self.static_out.numel() * 4
+        return self.static_out.numel() * self.static_out.element_size()

@@ -8,11 +8,19 @@ reference checkout is not importable (e.g. the GPU box).  With the reference on
 """
 from __future__ import annotations
 
+import torch
 from torch import nn
 
+from . import ops
 from .modules import CBAM, DoubleConv, DoubleConvDS, Down, DownDS, OutConv, Up, UpDS, _needs_grad
 
 _ENC = (64, 128, 256, 512)
+
+
+def _classes_of(model, x):
+    """The class map of ``model(x)``'s logits: the plain forward, then the channel argmax kernel (ops.argmax_channels)."""
+    with torch.no_grad():
+        return ops.argmax_channels(model(x))
 
 
 class SmaAt_UNet(nn.Module):
@@ -55,6 +63,20 @@ class SmaAt_UNet(nn.Module):
         * the three large CBAMs (levels 1-3) never write their output: they compute only their two gates, and the first DS
           conv of up2 / up3 / up4 applies them as it loads the skip, with the products the CBAM's own kernel would have used
           (bit for bit the same logits).  Levels 4-5 run the plain calls."""
+        return self._serving(x, classes=False)
+
+    def forward_classes(self, x):
+        """``forward_serving``'s graph ending in the (B, H, W) int64 class map the reference predicts from the logits
+        (``torch.argmax(softmax(y_pred), dim=1)``, train_SmaAtUNet.py:76): up4's last DS conv applies the n_classes-class
+        OutConv and the argmax in its epilogue (n_classes <= 32), so neither its 64-channel activation nor the logits reach
+        HBM.  Each class's logit there is the one-class fused OutConv's arithmetic, which sums in another order than the
+        unfused OutConv of the logits route: pixels whose top two logits lie within rounding of each other may pick the other
+        class.  Inference only; in train mode or under autograd the plain forward followed by the argmax kernel."""
+        if self.training or _needs_grad(self, x):
+            return _classes_of(self, x)
+        return self._serving(x, classes=True)
+
+    def _serving(self, x, classes):
         if self.training or _needs_grad(self, x):
             return self.forward(x)
         skips, f = [], self.inc(x)
@@ -74,7 +96,7 @@ class SmaAt_UNet(nn.Module):
             skip, gate = skips[3 - i]
             y = getattr(self, f"up{i + 1}")(y, skip, gate=gate)
         skip, gate = skips[0]
-        return self.up4(y, skip, outconv=self.outc, gate=gate)
+        return self.up4(y, skip, outconv=self.outc, gate=gate, classes=classes)
 
 
 class UNet(nn.Module):
@@ -107,6 +129,10 @@ class UNet(nn.Module):
         x = self.up3(x, x2)
         x = self.up4(x, x1)
         return self.outc(x)
+
+    def forward_classes(self, x):
+        """The (B, H, W) int64 class map of ``forward``'s logits (train_SmaAtUNet.py:76): the forward, then the argmax kernel."""
+        return _classes_of(self, x)
 
 
 class UNetAttention(nn.Module):
@@ -150,3 +176,7 @@ class UNetAttention(nn.Module):
         x = self.up3(x, x2Att)
         x = self.up4(x, x1Att)
         return self.outc(x)
+
+    def forward_classes(self, x):
+        """The (B, H, W) int64 class map of ``forward``'s logits (train_SmaAtUNet.py:76): the forward, then the argmax kernel."""
+        return _classes_of(self, x)

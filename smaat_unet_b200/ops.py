@@ -310,6 +310,84 @@ def dsconv(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, mod
     return y
 
 
+_fuse_classify = os.environ.get("SMAAT_FUSE_CLASSIFY", "1") != "0"
+
+
+def set_fused_classify(enabled: bool) -> None:
+    """Enable/disable the K-class OutConv + argmax in the last DS conv's epilogue (default on; off = that conv, OutConv and
+    the channel argmax kernel as separate launches).  For A/B measurements (tools/bench_classes.py)."""
+    global _fuse_classify
+    _fuse_classify = bool(enabled)
+
+
+def dsconv_classify_takes(x, x1, pw_weight, k, n_classes, mode=None) -> bool:
+    """True when ``dsconv_classify`` runs on these inputs: the fused kernel with a ``n_classes``-class OutConv and argmax in its
+    epilogue (smaat_dsconv_classify_eligible: Cout <= 128, 1 <= n_classes <= 32 -- 22 for Cout > 64 -- the fused DS conv's
+    shapes), and neither set_fused_dsconv(False) nor set_fused_classify(False)."""
+    mode = mode or _pw_mode
+    if not _fuse_ds or not _fuse_classify or PW_MODES[mode] == 0:
+        return False
+    x, bs0 = _nchw_bstride(x, "x")
+    C1, bs1 = 0, 0
+    if x1 is not None:
+        x1, bs1 = _nchw_bstride(x1, "x1")
+        C1 = x1.shape[1]
+    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
+    return bool(_lib.load().smaat_dsconv_classify_eligible(_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2], x.shape[3],
+                                                           k, w2d.shape[0], int(n_classes), PW_MODES[mode]))
+
+
+def dsconv_classify(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, x1=None, mode=None, w_split=None,
+                    want_logits=False):
+    """``dsconv`` followed by OutConv(Cout -> K) and the channel argmax, all in the fused kernel's epilogue
+    (smaat_dsconv_classify_fwd).  oc_weight (K, Cout[,1,1]), oc_bias (K) or None.  Returns the (B, H, W) int64 class map, or
+    (classes, (B, K, H, W) logits) with ``want_logits``; class j's logits are bit for bit those of ``dsconv(..., outconv=(oc_weight[j],
+    oc_bias[j]))``.  Returns None where ``dsconv_classify_takes`` is False (the caller then runs the layers apart)."""
+    mode = mode or _pw_mode
+    ow = _dense(oc_weight, "outconv.weight")
+    K = ow.shape[0]
+    if not dsconv_classify_takes(x, x1, pw_weight, k, K, mode):
+        return None
+    x, bs0 = _nchw_bstride(x, "x")
+    B, C0, H, W = x.shape
+    C1, bs1 = 0, 0
+    if x1 is not None:
+        x1, bs1 = _nchw_bstride(x1, "x1")
+        C1 = x1.shape[1]
+    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
+    Cout, Kd = w2d.shape
+    assert Kd == k * (C0 + C1), f"pointwise weight {tuple(pw_weight.shape)} does not match k*Cin={k * (C0 + C1)}"
+    assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
+    ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
+    assert ob is None or ob.numel() == K, f"OutConv bias {tuple(oc_bias.shape)} does not match K={K}"
+    wlo = None
+    if PW_MODES[mode] == 2:
+        w2d, wlo = w_split if w_split is not None else split_tf32(w2d)
+    classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64)
+    logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
+    Cin = C0 + C1
+    _call(f"smaat_dsconv_classify_fwd[C{Cin}_N{Cout}_K{K}_S{H}]",
+          4 * B * H * W * (Cin + (K if want_logits else 0) + 2) + 4 * Kd * Cout, 2 * B * H * W * (Kd * (Cout + 9) + K * Cout),
+          _lib.load().smaat_dsconv_classify_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(_dense(dw_weight, "depthwise.weight")),
+          _ptr(dw_bias), _ptr(w2d), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, _ptr(logits), _ptr(classes),
+          B, H, W, k, Cout, int(bool(relu)), PW_MODES[mode], _stream())
+    return (classes, logits) if want_logits else classes
+
+
+def argmax_channels(x):
+    """The class map of (B, K, H, W) logits: int64 (B, H, W), torch.argmax(x, 1) exactly -- ties to the first index, a NaN
+    wins (smaat_argmax_channels_fwd, 1 <= K <= 1024)."""
+    x = _dense(x, "logits")
+    if x.dim() < 2:
+        raise RuntimeError(f"smaat_unet_b200: logits must be (B, K, ...), got shape {tuple(x.shape)}")
+    B, K = x.shape[0], x.shape[1]
+    P = x[0, 0].numel()
+    classes = torch.empty((B,) + tuple(x.shape[2:]), device=x.device, dtype=torch.int64)
+    _call(f"smaat_argmax_channels_fwd[K{K}]", 4 * B * K * P + 8 * B * P, 0, _lib.load().smaat_argmax_channels_fwd, _ptr(x), _ptr(classes),
+          B, K, P, _stream())
+    return classes
+
+
 def _pad32(c):
     return (c + 31) // 32 * 32
 
