@@ -307,6 +307,32 @@ int smaat_ce_fwd(const float* logits, const int64_t* target, int B, int K, int64
                  double* batch_acc, float* dlogits, int64_t* conf, void* stream);
 int smaat_confusion_add(const int64_t* pred, const int64_t* target, int64_t n, int K, int64_t* conf, int64_t* invalid,
                         void* stream);
+/* smaat_cross_entropy_fwd: F.cross_entropy with the options smaat_ce_fwd leaves out, in the same single pass (a separate
+ *   kernel, so the plain path keeps its registers).  Logits as smaat_ce_fwd; EXACTLY ONE of
+ *     target      (B, P) int64 class indices (ignore_index / use_ignore and invalid labels as smaat_ce_fwd), or
+ *     target_prob (B, K, P) fp32 probabilities (use_ignore must be 0: torch rejects ignore_index for them).
+ *   weight (nullable): K fp32 class weights on the device (NULL: all ones); label_smoothing eps in [0, 1].
+ *   With W = sum_k w_k, lse = logsumexp_c(l), p = softmax(l), the per-pixel loss and its gradient are
+ *     class index t:  (1 - eps) w_t (lse - l_t) + (eps / K) (W lse - sum_k w_k l_k)
+ *                     d_j = ((1 - eps) w_t + eps W / K) p_j - (1 - eps) w_t [j == t] - (eps / K) w_j
+ *     probabilities:  q' = q (1 - eps) + eps / K;  loss = lse sum_k w_k q'_k - sum_k w_k q'_k l_k;  d_j = p_j sum_k w_k q'_k - w_j q'_j
+ *   batch_acc: double[4], overwritten: [0] sum of the per-pixel losses of counted pixels (fp32 terms, fp64 sum)
+ *     [1] counted pixels (probability targets: every pixel)   [2] invalid labels; with probability targets, rows that
+ *     fail the one-hot check below (they do not affect the loss)   [3] D = sum of w_t over counted pixels (probability
+ *     targets: the pixel count) -- the divisor of torch's "mean".
+ *   loss_map (nullable): (B, P) fp32 per-pixel loss; 0 on ignored pixels, NaN on invalid labels.
+ *   dlogits (nullable): (B, K, P) unscaled per-pixel gradient; exactly 0 on ignored and invalid pixels.  With weight NULL
+ *     and eps = 0 it is bitwise smaat_ce_fwd's.
+ *   conf (nullable): as smaat_ce_fwd.  With probability targets the row is the target's first argmax, counted only when the
+ *     target row passes metric/confusionmatrix.py:57-61's checks: every value in [0, 1] and the row sums to 1 (fp32 sum in
+ *     class order; numpy's pairwise order can differ by an ulp on rows that are not one-hot).
+ *   NaN logits poison their own pixel, as in smaat_ce_fwd.
+ * smaat_onehot_classes: one-hot / probability targets (B, K, P) fp32 -> classes (B, P) int64: the row's first argmax, or -1
+ *   when the row fails the checks above, so smaat_confusion_add / the score path count it as invalid.  1 <= K <= 1024. */
+int smaat_cross_entropy_fwd(const float* logits, const int64_t* target, const float* target_prob, const float* weight, int B, int K,
+                            int64_t P, float label_smoothing, int64_t ignore_index, int use_ignore, double* batch_acc,
+                            float* loss_map, float* dlogits, int64_t* conf, void* stream);
+int smaat_onehot_classes(const float* target, int64_t* classes, int B, int K, int64_t P, void* stream);
 /* smaat_argmax_channels_fwd: the class map of any (B, K, P) logits, classes[b, p] = argmax_c x[b, c, p] (int64), in one read:
  *   ties go to the first index and a NaN logit wins, as torch.argmax (and smaat_ce_fwd's confusion column).  1 <= K <= 1024
  *   (larger K: SMAAT_E_UNSUPPORTED).  128-bit loads when P % 4 == 0 and x / classes are 16-byte aligned, a scalar kernel

@@ -9,7 +9,7 @@ from . import _lib, ops  # noqa: F401
 from .data import (PinnedBatchLoader, precipitation_maps_classification_shard, precipitation_maps_oversampled_shard,  # noqa: F401
                    precipitation_maps_shard)
 from .metrics import PrecipitationMetrics, loss_func, step_loss  # noqa: F401
-from .segmentation import ConfusionMatrix, CrossEntropyLoss, IoU, ce_step  # noqa: F401
+from .segmentation import ConfusionMatrix, CrossEntropyLoss, CrossEntropyLossWithOptions, IoU, ce_step, cross_entropy  # noqa: F401
 from .model import SmaAt_UNet, UNet, UNetAttention  # noqa: F401
 from .modules import (CBAM, ChannelAttention, DepthwiseSeparableConv, DoubleConv, DoubleConvDS, Down, DownDS,  # noqa: F401
                       OutConv, SpatialAttention, Up, UpDS)
@@ -17,4 +17,4 @@ from .ops import get_pointwise_mode, set_fused_dsconv, set_pointwise_mode  # noq
 from .patch import patch_reference  # noqa: F401
 
 __all__ = ["SmaAt_UNet", "UNet", "UNetAttention", "DoubleConv", "Down", "Up", "CBAM", "ChannelAttention", "SpatialAttention", "DepthwiseSeparableConv", "DoubleConvDS",
-           "DownDS", "UpDS", "OutConv", "patch_reference", "PrecipitationMetrics", "loss_func", "step_loss", "CrossEntropyLoss", "ConfusionMatrix", "IoU", "ce_step", "set_pointwise_mode", "get_pointwise_mode", "ops"]
+           "DownDS", "UpDS", "OutConv", "patch_reference", "PrecipitationMetrics", "loss_func", "step_loss", "CrossEntropyLoss", "CrossEntropyLossWithOptions", "ConfusionMatrix", "IoU", "ce_step", "cross_entropy", "set_pointwise_mode", "get_pointwise_mode", "ops"]

@@ -70,6 +70,8 @@ SIGNATURES = {
     "smaat_metrics_commit": [_p, _p, _i, _i, _p],
     "smaat_ce_fwd": [_p, _p, _i, _i, _l, _l, _i, _p, _p, _p, _p],
     "smaat_confusion_add": [_p, _p, _l, _i, _p, _p, _p],
+    "smaat_cross_entropy_fwd": [_p, _p, _p, _p, _i, _i, _l, _f, _l, _i, _p, _p, _p, _p, _p],
+    "smaat_onehot_classes": [_p, _p, _i, _i, _l, _p],
     "smaat_argmax_channels_fwd": [_p, _p, _i, _i, _l, _p],
     "smaat_convt2x2_pack_weight": [_p, _p, _i, _i, _p],
     "smaat_convt2x2_unpack_wgrad": [_p, _p, _p, _p, _i, _i, _p],

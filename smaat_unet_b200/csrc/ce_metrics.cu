@@ -179,6 +179,212 @@ __global__ void __launch_bounds__(CE_THREADS) ce_fwd_kernel(const float* __restr
   }
 }
 
+// One class of a probability / one-hot target row, in class order: the reference's checks (metric/confusionmatrix.py:57-61:
+// every value in [0, 1], the row sums to 1 -- summed here in fp32 in class order) and the row's first argmax.
+__device__ __forceinline__ void onehot_step(float q, int c, float& sum, float& qmax, int& qam, bool& bad) {
+  sum += q;
+  bad |= !(q >= 0.f && q <= 1.f);               // NaN fails too
+  if (q > qmax) { qmax = q; qam = c; }
+}
+
+// Cross-entropy with the options smaat_ce_fwd leaves out: class weights w, label smoothing eps, probability targets
+// (PROB) and a per-pixel loss map.  Same sweep structure as ce_fwd_kernel (logits and, with PROB, targets read once from
+// HBM; the gradient sweep re-reads them from L2); the options live here so the plain kernel keeps its registers.
+// Per pixel, with lse = logsumexp(l), W = sum_k w_k and the first logit l_0 as the shift of every difference below
+// (W * lse - sum_k w_k l_k = W * (lse - l_0) - sum_k w_k (l_k - l_0) cancels far less when the logits are large):
+//   class index t:  loss = (1 - eps) w_t (lse - l_t) + (eps / K) (W lse - sum_k w_k l_k),   D += w_t
+//                   grad_j = ((1 - eps) w_t + eps W / K) p_j - (1 - eps) w_t [j == t] - (eps / K) w_j
+//   probabilities:  q'_k = q_k (1 - eps) + eps / K,  S = sum_k w_k q'_k
+//                   loss = S lse - sum_k w_k q'_k l_k,   grad_j = S p_j - w_j q'_j,   D += 1
+// With w = 1 and eps = 0 the class-index gradient is computed by the same expression as ce_fwd_kernel's, so it is bitwise
+// the same.  With PROB the confusion row is the target's first argmax, and a row that fails the reference's one-hot checks
+// is left out and counted in acc[2] (the loss does not validate probability targets, as torch does not).
+// Class-index targets are held to 64 registers (4 CTAs of 256 threads per SM, ce_fwd_kernel's occupancy; without the bound
+// ptxas takes 75 and the streaming loop runs at 3 CTAs per SM); each thread's share of D is an fp32 sum to stay under it.
+template <int NPX, bool SMEM, bool PROB>
+__global__ void __launch_bounds__(CE_THREADS, PROB ? 2 : 4) cross_entropy_kernel(const float* __restrict__ logits, const int64_t* __restrict__ target,
+                                                                   const float* __restrict__ prob, const float* __restrict__ weight,
+                                                                   int K, int64_t P, int64_t groups, float eps, int64_t ignore_index,
+                                                                   int use_ignore, double* __restrict__ acc, float* __restrict__ loss_map,
+                                                                   float* __restrict__ dlogits, unsigned long long* __restrict__ conf) {
+  extern __shared__ unsigned sh_dyn[];
+  unsigned* sh_hist = sh_dyn;
+  float* sh_w = reinterpret_cast<float*>(sh_dyn + (SMEM ? K * K : 0));
+  __shared__ float sh_wsum;
+  if (SMEM)
+    for (int i = threadIdx.x; i < K * K; i += blockDim.x) sh_hist[i] = 0u;
+  for (int i = threadIdx.x; i < K; i += blockDim.x) sh_w[i] = weight ? __ldg(weight + i) : 1.f;
+  __syncthreads();
+  if (threadIdx.x < 32) {                       // W in a fixed order: every CTA gets the same value
+    float s = 0.f;
+    for (int i = threadIdx.x; i < K; i += 32) s += sh_w[i];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (threadIdx.x == 0) sh_wsum = s;
+  }
+  __syncthreads();
+  const float W = sh_wsum;
+  const float keep = 1.f - eps, eps_k = eps / (float)K;
+  const bool smooth = eps != 0.f;
+  const int64_t gpi = P / NPX;
+  double loss = 0.0;
+  float dsum = 0.f;                             // a thread's share of D: a few dozen weights, exact enough in fp32
+  unsigned counted = 0u, invalid = 0u;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += stride) {
+    const int64_t b = g / gpi;
+    const int64_t p0 = (g - b * gpi) * NPX;
+    const float* base = logits + b * (int64_t)K * P + p0;
+    const float* qbase = PROB ? prob + b * (int64_t)K * P + p0 : nullptr;
+    int tl[NPX];
+    bool ok[NPX];
+#pragma unroll
+    for (int j = 0; j < NPX; ++j) {
+      if (PROB) {
+        ok[j] = true;
+        tl[j] = -1;
+      } else {
+        const int64_t t = __ldg(target + b * P + p0 + j);
+        const bool ign = use_ignore && t == ignore_index;
+        ok[j] = !ign && t >= 0 && t < K;
+        invalid += (unsigned)(!ign && !ok[j]);
+        tl[j] = ok[j] ? (int)t : (ign ? -1 : -2);   // -2: invalid; never used as an index unless ok
+      }
+    }
+    float m[NPX], s[NPX], lt[NPX], l0[NPX], wd[NPX], sq[NPX], qs[NPX], qmax[NPX];
+    int am[NPX], qam[NPX];
+    bool nan_seen[NPX], qbad[NPX];
+#pragma unroll
+    for (int j = 0; j < NPX; ++j) {
+      m[j] = -INFINITY; s[j] = 0.f; lt[j] = 0.f; l0[j] = 0.f; wd[j] = 0.f; sq[j] = 0.f; qs[j] = 0.f; qmax[j] = -INFINITY;
+      am[j] = 0; qam[j] = 0; nan_seen[j] = false; qbad[j] = false;
+    }
+    for (int c = 0; c < K; ++c) {
+      float v[NPX], q[NPX];
+      load_px<NPX>(base + (int64_t)c * P, v);
+      if (PROB) load_px<NPX>(qbase + (int64_t)c * P, q);
+      const float wc = sh_w[c];
+#pragma unroll
+      for (int j = 0; j < NPX; ++j) {
+        if (v[j] > m[j]) {                      // ce_fwd_kernel's online log-sum-exp and argmax
+          s[j] = fmaf(s[j], expf(m[j] - v[j]), 1.f);
+          m[j] = v[j];
+          if (!nan_seen[j]) am[j] = c;
+        } else {
+          s[j] += expf(v[j] - m[j]);
+          if (v[j] != v[j] && !nan_seen[j]) { nan_seen[j] = true; am[j] = c; }
+        }
+        l0[j] = c == 0 ? v[j] : l0[j];
+        if (PROB) {
+          const float wq = wc * fmaf(q[j], keep, eps_k);
+          sq[j] += wq;
+          wd[j] = fmaf(wq, v[j] - l0[j], wd[j]);
+          onehot_step(q[j], c, qs[j], qmax[j], qam[j], qbad[j]);
+        } else {
+          lt[j] = (c == tl[j]) ? v[j] : lt[j];
+          if (smooth) wd[j] = fmaf(wc, v[j] - l0[j], wd[j]);
+        }
+      }
+    }
+    float inv_s[NPX], lm[NPX], ga[NPX], gb[NPX];
+#pragma unroll
+    for (int j = 0; j < NPX; ++j) {
+      const float ls = logf(s[j]);
+      const float lse0 = (m[j] - l0[j]) + ls;   // lse - l_0
+      if (PROB) {
+        lm[j] = sq[j] * lse0 - wd[j];
+        loss += (double)lm[j];
+        dsum += 1.f;
+        ++counted;
+        inv_s[j] = sq[j] / s[j];
+        const bool row_ok = !qbad[j] && qs[j] == 1.f;
+        invalid += (unsigned)!row_ok;
+        hist_add<SMEM>(row_ok ? qam[j] * K + am[j] : -1, sh_hist, conf);
+      } else {
+        const float wt = ok[j] ? sh_w[tl[j]] : 0.f;
+        gb[j] = keep * wt;
+        ga[j] = smooth ? fmaf(eps_k, W, gb[j]) : gb[j];
+        inv_s[j] = ga[j] * (1.f / s[j]);        // w = 1, eps = 0: exactly ce_fwd_kernel's 1 / s
+        if (ok[j]) {
+          float term = gb[j] * ((m[j] - lt[j]) + ls);
+          if (smooth) term = fmaf(eps_k, W * lse0 - wd[j], term);
+          lm[j] = term;
+          loss += (double)term;
+          dsum += wt;
+          ++counted;
+        } else {
+          lm[j] = tl[j] == -1 ? 0.f : NAN;      // ignored: 0; invalid label: NaN
+        }
+        hist_add<SMEM>(ok[j] ? tl[j] * K + am[j] : -1, sh_hist, conf);
+      }
+    }
+    if (loss_map) store_px<NPX>(loss_map + b * P + p0, lm);
+    if (dlogits) {
+      float* gbase = dlogits + b * (int64_t)K * P + p0;
+      for (int c = 0; c < K; ++c) {
+        float v[NPX], q[NPX], d[NPX];
+        load_px_last<NPX>(base + (int64_t)c * P, v);
+        if (PROB) load_px_last<NPX>(qbase + (int64_t)c * P, q);
+        const float wc = sh_w[c];
+#pragma unroll
+        for (int j = 0; j < NPX; ++j) {
+          if (PROB) {
+            d[j] = expf(v[j] - m[j]) * inv_s[j] - wc * fmaf(q[j], keep, eps_k);
+          } else {
+            d[j] = ok[j] ? expf(v[j] - m[j]) * inv_s[j] - (c == tl[j] ? gb[j] : 0.f) : 0.f;
+            if (smooth && ok[j]) d[j] -= eps_k * wc;
+          }
+        }
+        store_px<NPX>(gbase + (int64_t)c * P, d);
+      }
+    }
+  }
+  hist_flush<SMEM>(sh_hist, conf, K * K);
+  __shared__ double red_l[CE_THREADS / 32], red_d[CE_THREADS / 32];
+  __shared__ unsigned red_c[CE_THREADS / 32], red_i[CE_THREADS / 32];
+  const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+  loss = ce_warp_sum_f64(loss);
+  const double dsum_d = ce_warp_sum_f64((double)dsum);
+  counted = ce_warp_sum_u32(counted);
+  invalid = ce_warp_sum_u32(invalid);
+  if (lane == 0) { red_l[wp] = loss; red_d[wp] = dsum_d; red_c[wp] = counted; red_i[wp] = invalid; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double l = 0.0, dd = 0.0, c = 0.0, iv = 0.0;
+    for (int i = 0; i < CE_THREADS / 32; ++i) { l += red_l[i]; dd += red_d[i]; c += red_c[i]; iv += red_i[i]; }
+    if (c != 0.0) { atomicAdd(acc + 0, l); atomicAdd(acc + 1, c); atomicAdd(acc + 3, dd); }
+    if (iv != 0.0) atomicAdd(acc + 2, iv);
+  }
+}
+
+// One-hot / probability targets (B, K, P) -> int64 class indices (B, P): the row's first argmax, or -1 for a row that fails
+// the reference's checks (onehot_step), which smaat_confusion_add and the score path then count as invalid.
+template <int NPX>
+__global__ void __launch_bounds__(CE_THREADS) onehot_classes_kernel(const float* __restrict__ x, int64_t* __restrict__ classes, int K,
+                                                                    int64_t P, int64_t groups) {
+  const int64_t gpi = P / NPX;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += stride) {
+    const int64_t b = g / gpi;
+    const int64_t p0 = (g - b * gpi) * NPX;
+    const float* base = x + b * (int64_t)K * P + p0;
+    float sum[NPX], qmax[NPX];
+    int qam[NPX];
+    bool bad[NPX];
+#pragma unroll
+    for (int j = 0; j < NPX; ++j) { sum[j] = 0.f; qmax[j] = -INFINITY; qam[j] = 0; bad[j] = false; }
+    for (int c = 0; c < K; ++c) {
+      float v[NPX];
+      load_px_last<NPX>(base + (int64_t)c * P, v);
+#pragma unroll
+      for (int j = 0; j < NPX; ++j) onehot_step(v[j], c, sum[j], qmax[j], qam[j], bad[j]);
+    }
+    int64_t* out = classes + b * P + p0;
+#pragma unroll
+    for (int j = 0; j < NPX; ++j) out[j] = (bad[j] || sum[j] != 1.f) ? -1 : qam[j];
+  }
+}
+
 template <bool SMEM>
 __global__ void __launch_bounds__(CE_THREADS) confusion_add_kernel(const int64_t* __restrict__ pred, const int64_t* __restrict__ target,
                                                                    int64_t n, int K, unsigned long long* __restrict__ conf,
@@ -284,6 +490,77 @@ extern "C" int smaat_ce_fwd(const float* logits, const int64_t* target, int B, i
     else      ce_fwd_kernel<1, false><<<g, CE_THREADS, 0, st>>>(logits, target, K, P, groups, ignore_index, use_ignore, batch_acc, dlogits, cf);
   }
   SMAAT_LAUNCH_CHECK("smaat_ce_fwd");
+  return SMAAT_OK;
+}
+
+extern "C" int smaat_cross_entropy_fwd(const float* logits, const int64_t* target, const float* target_prob, const float* weight,
+                                       int B, int K, int64_t P, float label_smoothing, int64_t ignore_index, int use_ignore,
+                                       double* batch_acc, float* loss_map, float* dlogits, int64_t* conf, void* stream) {
+  SMAAT_REQUIRE(logits && batch_acc && B > 0 && P > 0, "cross_entropy_fwd: bad arguments (B=%d, P=%lld)", B, (long long)P);
+  SMAAT_REQUIRE((target != nullptr) != (target_prob != nullptr),
+                "cross_entropy_fwd: pass exactly one of class-index targets and probability targets");
+  SMAAT_REQUIRE(K >= 2, "cross_entropy_fwd: K=%d classes, need at least 2", K);
+  if (K > 1024) return fail(SMAAT_E_UNSUPPORTED, "cross_entropy_fwd: K=%d classes, this build supports at most 1024", K);
+  SMAAT_REQUIRE(label_smoothing >= 0.f && label_smoothing <= 1.f, "cross_entropy_fwd: label_smoothing=%g outside [0, 1]",
+                (double)label_smoothing);
+  SMAAT_REQUIRE(!(target_prob && use_ignore), "cross_entropy_fwd: ignore_index is not supported for probability targets");
+  auto a4 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; };
+  SMAAT_REQUIRE(a4(logits) && a4(target_prob) && a4(weight) && a4(loss_map) && a4(dlogits) &&
+                    (reinterpret_cast<uintptr_t>(target) & 7u) == 0 && (reinterpret_cast<uintptr_t>(batch_acc) & 7u) == 0 &&
+                    (reinterpret_cast<uintptr_t>(conf) & 7u) == 0,
+                "cross_entropy_fwd: float arrays must be 4-byte and target / batch_acc / conf 8-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaMemsetAsync(batch_acc, 0, 4 * sizeof(double), st);
+  if (e != cudaSuccess) return fail(SMAAT_E_CUDA, "cross_entropy_fwd: memset: %s", cudaGetErrorString(e));
+  const bool prob = target_prob != nullptr;
+  const bool vec = P % 4 == 0 && aligned16(logits) && (prob ? aligned16(target_prob) : aligned16(target)) &&
+                   (!dlogits || aligned16(dlogits)) && (!loss_map || aligned16(loss_map));
+  const int npx = vec ? 4 : 1;
+  const int64_t groups = (int64_t)B * (P / npx);
+  // smaat_ce_fwd's grid rule; probability targets are re-read from L2 too, so a CTA holds twice the lines
+  const int64_t per_cta = (int64_t)CE_THREADS * npx * K * 4 * (prob ? 2 : 1);
+  int64_t cap = l2_bytes() / 2 / per_cta;
+  if (cap < num_sms()) cap = num_sms();
+  if (cap > (int64_t)num_sms() * 8) cap = (int64_t)num_sms() * 8;
+  int64_t blocks = ceil_div64(groups, CE_THREADS);
+  if (blocks > cap) blocks = cap;
+  if (blocks < 1) blocks = 1;
+  const bool smem = conf && K <= CE_SMEM_HIST_MAX_K;
+  const size_t shb = ((smem ? (size_t)K * K : 0) + (size_t)K) * sizeof(unsigned);
+  auto* cf = reinterpret_cast<unsigned long long*>(conf);
+  const unsigned g = (unsigned)blocks;
+  const float eps = label_smoothing;
+#define SMAAT_XENT(NPX, SMEM, PROB)                                                                                          \
+  cross_entropy_kernel<NPX, SMEM, PROB><<<g, CE_THREADS, shb, st>>>(logits, target, target_prob, weight, K, P, groups, eps, \
+                                                                     ignore_index, use_ignore, batch_acc, loss_map, dlogits, cf)
+  if (prob) {
+    if (vec) { if (smem) SMAAT_XENT(4, true, true); else SMAAT_XENT(4, false, true); }
+    else     { if (smem) SMAAT_XENT(1, true, true); else SMAAT_XENT(1, false, true); }
+  } else {
+    if (vec) { if (smem) SMAAT_XENT(4, true, false); else SMAAT_XENT(4, false, false); }
+    else     { if (smem) SMAAT_XENT(1, true, false); else SMAAT_XENT(1, false, false); }
+  }
+#undef SMAAT_XENT
+  SMAAT_LAUNCH_CHECK("smaat_cross_entropy_fwd");
+  return SMAAT_OK;
+}
+
+extern "C" int smaat_onehot_classes(const float* target, int64_t* classes, int B, int K, int64_t P, void* stream) {
+  SMAAT_REQUIRE(target && classes && B > 0 && P > 0, "onehot_classes: bad arguments (B=%d, P=%lld)", B, (long long)P);
+  SMAAT_REQUIRE(K >= 1, "onehot_classes: K=%d classes", K);
+  if (K > 1024) return fail(SMAAT_E_UNSUPPORTED, "onehot_classes: K=%d classes, this build supports at most 1024", K);
+  SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(target) & 3u) == 0 && (reinterpret_cast<uintptr_t>(classes) & 7u) == 0,
+                "onehot_classes: target must be 4-byte and classes 8-byte aligned");
+  const bool vec = P % 4 == 0 && aligned16(target) && aligned16(classes);
+  const int npx = vec ? 4 : 1;
+  const int64_t groups = (int64_t)B * (P / npx);
+  int64_t blocks = ceil_div64(groups, CE_THREADS);
+  const int64_t cap = (int64_t)num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (vec) onehot_classes_kernel<4><<<(unsigned)blocks, CE_THREADS, 0, st>>>(target, classes, K, P, groups);
+  else     onehot_classes_kernel<1><<<(unsigned)blocks, CE_THREADS, 0, st>>>(target, classes, K, P, groups);
+  SMAAT_LAUNCH_CHECK("smaat_onehot_classes");
   return SMAAT_OK;
 }
 

@@ -30,6 +30,15 @@ number of pixels (no ignored or invalid labels, equal shards) -- the same caveat
     sess = TrainSession(SmaAt_UNet(3, 21), batch=8, in_shape=(3, 224, 224), loss="cross_entropy")
     loss = sess.step(x, y)          # y: (B, H, W) int64
     iou, miou = sess.metrics.value()
+
+``loss`` may also be a ``smaat_unet_b200.CrossEntropyLossWithOptions`` (or ``CrossEntropyLoss``) instance with reduction
+"mean" or "sum": its ``ignore_index``, ``weight`` and ``label_smoothing`` are used inside the captured step
+(``smaat_cross_entropy_fwd`` when weighted or smoothed).  They are a snapshot taken at construction -- the weight is copied to the device then, so changing the loss
+object afterwards does not change the session.  Targets are class indices: a floating-point target is rejected by
+``step``.  With several ranks each rank normalises its weighted mean by its own sum of target weights, as torch DDP does
+with a weighted ``nn.CrossEntropyLoss``.
+
+    sess = TrainSession(SmaAt_UNet(12, 8), 32, (12, 288, 288), loss=CrossEntropyLossWithOptions(weight=w, label_smoothing=0.1))
 """
 from __future__ import annotations
 
@@ -42,7 +51,7 @@ from . import _lib, ops
 from . import functional as Fn
 from .metrics import PrecipitationMetrics, step_loss
 from .modules import CBAM
-from .segmentation import IoU, ce_step
+from .segmentation import CrossEntropyLoss, CrossEntropyLossWithOptions, IoU, ce_step
 
 _ALIGN = 64          # floats: every parameter starts on a 256-byte boundary of the flat buffers (TMA needs 16)
 _DEFAULT = object()  # metrics argument not given: the loss's own default metric
@@ -51,10 +60,23 @@ _DEFAULT = object()  # metrics argument not given: the loss's own default metric
 class TrainSession:
     def __init__(self, model, batch, in_shape, lr=1e-3, device=None, use_graph=True, metrics=_DEFAULT, warmup=3,
                  betas=(0.9, 0.999), eps=1e-8, overlap_allreduce=True, recompute_depthwise=False, loss="mse"):
-        if loss not in ("mse", "cross_entropy"):
-            raise ValueError(f"TrainSession: loss={loss!r}; 'mse' or 'cross_entropy'")
+        self._ce = None          # (ignore_index, reduction, weight, label_smoothing) of a loss instance
+        if isinstance(loss, (CrossEntropyLoss, CrossEntropyLossWithOptions)):
+            if loss.reduction not in ("mean", "sum"):
+                raise ValueError(f"TrainSession: {type(loss).__name__}(reduction={loss.reduction!r}); the step needs a scalar loss, "
+                                 "'mean' or 'sum'")
+            if loss.weight is not None and loss.weight.dim() != 1:
+                raise ValueError(f"TrainSession: the loss's weight must be (K,), got {tuple(loss.weight.shape)}")
+            ce_loss, loss = loss, "cross_entropy"
+        elif isinstance(loss, str) and loss in ("mse", "cross_entropy"):
+            ce_loss = None
+        else:
+            raise ValueError(f"TrainSession: loss={loss!r}; 'mse', 'cross_entropy' or a smaat_unet_b200.CrossEntropyLossWithOptions")
         self.loss_kind = loss
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
+        if ce_loss is not None:
+            w = None if ce_loss.weight is None else ce_loss.weight.detach().to(self.device, torch.float32).clone()
+            self._ce = (int(ce_loss.ignore_index), ce_loss.reduction, w, float(ce_loss.label_smoothing))
         self.model = model.to(self.device).train()
         self.batch, self.in_shape = int(batch), tuple(in_shape)
         self.world = dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1
@@ -157,6 +179,9 @@ class TrainSession:
             pred = self.model(self.x)
         finally:
             Fn.set_recompute_depthwise(old)
+        if self._ce is not None:
+            ignore_index, reduction, weight, eps = self._ce
+            return ce_step(pred, self.y, self.metrics, ignore_index, reduction, weight=weight, label_smoothing=eps)
         if self.loss_kind == "cross_entropy":
             return ce_step(pred, self.y, self.metrics)    # nn.CrossEntropyLoss + IoU.add in one pass (segmentation.py)
         return step_loss(pred, self.y, self.metrics)      # loss_func + metrics.update in one pass (metrics.py)
@@ -363,6 +388,9 @@ class TrainSession:
     def load_batch(self, x, y):
         """Copy a batch into the static input buffers (async).  Host tensors (pinned for true overlap) are staged on a
         separate copy stream so the transfer of step i+1 hides behind the compute of step i."""
+        if self._ce is not None and y.is_floating_point():
+            raise TypeError(f"TrainSession: this session's cross-entropy loss takes int64 class-index targets, got {y.dtype}; "
+                            "probability targets go through the eager path (smaat_unet_b200.cross_entropy)")
         if x.device.type == "cpu":
             self._stage(x, y)
         else:
