@@ -121,6 +121,17 @@ int smaat_dsconv_classify_fwd(const float* x0, int C0, int64_t x0_bstride, const
                               const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
                               const float* scale, const float* shift, const float* oc_w, const float* oc_b, int K,
                               float* logits, int64_t* classes, int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
+/* The same kernel ending in the per-pixel class probabilities, softmax(y_pred) over the K logits (train_SmaAtUNet.py:76
+ * computes them before its argmax; an exceedance map such as P(rate > 1 mm/h) is a partial sum of them).  Arguments as
+ * smaat_dsconv_classify_fwd with probs: (B, K, H, W) in place of logits / classes.  The epilogue computes each class's logit
+ * twice: once for a running (max, sum of exp) per pixel, once more to write exp(l - max) / sum.  probs equals, bit for bit,
+ * smaat_softmax_channels_fwd applied to the logits smaat_dsconv_classify_fwd writes for the same inputs.  Only the K
+ * probability planes reach HBM.  Eligibility: smaat_dsconv_classify_eligible, unchanged (1 <= K <= 32, 22 for Cout > 64);
+ * SMAAT_E_UNSUPPORTED otherwise (callers then run the two convs, smaat_outconv_fwd and smaat_softmax_channels_fwd). */
+int smaat_dsconv_probs_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                           const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
+                           const float* scale, const float* shift, const float* oc_w, const float* oc_b, int K,
+                           float* probs, int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
 
 /* The fused DS conv with the CBAM fusions of the serving forward (models/layers.py:90-141 around the DS blocks of
  * models/SmaAt_UNet.py:41-57); arguments as smaat_dsconv_fwd, without batch statistics.
@@ -338,6 +349,14 @@ int smaat_onehot_classes(const float* target, int64_t* classes, int B, int K, in
  *   (larger K: SMAAT_E_UNSUPPORTED).  128-bit loads when P % 4 == 0 and x / classes are 16-byte aligned, a scalar kernel
  *   otherwise.  Serves every model output smaat_dsconv_classify_fwd does not produce. */
 int smaat_argmax_channels_fwd(const float* x, int64_t* classes, int B, int K, int64_t P, void* stream);
+/* smaat_softmax_channels_fwd: the class probabilities of any (B, K, P) logits, probs[b, c, p] = softmax_c x[b, :, p], the
+ *   softmax(y_pred) of train_SmaAtUNet.py:76 (torch.softmax(x, 1)).  One thread per pixel (4 with 128-bit loads when P % 4 == 0
+ *   and x / probs are 16-byte aligned) keeps a running (max, sum of exp) over the classes in order, then re-reads the logits,
+ *   from L2 (the grid is sized so that the lines it reads between its two sweeps fit in half of it), and writes
+ *   exp(l - max) / sum.  Non-finite logits give torch's pattern: a NaN or +inf logit makes the pixel's K probabilities NaN, a
+ *   pixel of -inf logits is NaN, a -inf logit among finite ones gets 0; K = 1 gives 1.  1 <= K <= 1024 (larger K:
+ *   SMAAT_E_UNSUPPORTED).  Serves every model output smaat_dsconv_probs_fwd does not produce. */
+int smaat_softmax_channels_fwd(const float* x, float* probs, int B, int K, int64_t P, void* stream);
 
 /* CBAM in three launches (reference models/layers.py:90-141).
  * smaat_cbam_pool_mlp_fwd: ChannelAttention's global pools AND its shared MLP + sigmoid (layers.py:98-109): the last pooling

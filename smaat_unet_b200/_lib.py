@@ -29,6 +29,7 @@ SIGNATURES = {
     "smaat_dsconv_outconv_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_classify_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _i],
     "smaat_dsconv_classify_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
+    "smaat_dsconv_probs_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_cbam_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _i, _i],
     "smaat_dsconv_pool_parts": [_i, _i],
     "smaat_dsconv_cbam_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _l, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
@@ -73,6 +74,7 @@ SIGNATURES = {
     "smaat_cross_entropy_fwd": [_p, _p, _p, _p, _i, _i, _l, _f, _l, _i, _p, _p, _p, _p, _p],
     "smaat_onehot_classes": [_p, _p, _i, _i, _l, _p],
     "smaat_argmax_channels_fwd": [_p, _p, _i, _i, _l, _p],
+    "smaat_softmax_channels_fwd": [_p, _p, _i, _i, _l, _p],
     "smaat_convt2x2_pack_weight": [_p, _p, _i, _i, _p],
     "smaat_convt2x2_unpack_wgrad": [_p, _p, _p, _p, _i, _i, _p],
     "smaat_pixel_shuffle2_pad_fwd": [_p, _p, _p, _l, _i, _i, _i, _i, _i, _i, _p],

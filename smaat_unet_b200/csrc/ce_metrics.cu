@@ -16,6 +16,7 @@
 // non-zero bin, or for larger K straight to the global matrix; either way lanes holding the same (t, argmax) pair are
 // merged with __match_any_sync first, since neighbouring pixels of a segmentation map usually share both.
 #include "common.cuh"
+#include "softmax.cuh"
 
 namespace smaat {
 
@@ -444,6 +445,34 @@ __global__ void __launch_bounds__(CE_THREADS) argmax_channels_kernel(const float
   }
 }
 
+// Channel softmax: the probabilities of (B, K, P) logits, NPX consecutive pixels of one image per thread, as
+// argmax_channels_kernel.  The first sweep feeds the classes in order to SoftmaxAcc (softmax.cuh); the second re-reads the
+// same lines, which the grid keeps in L2 (smaat_softmax_channels_fwd), and streams the probabilities out.
+template <int NPX>
+__global__ void __launch_bounds__(CE_THREADS) softmax_channels_kernel(const float* __restrict__ x, float* __restrict__ probs, int K,
+                                                                      int64_t P, int64_t groups) {
+  const int64_t gpi = P / NPX;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += stride) {
+    const int64_t b = g / gpi;
+    const int64_t off = b * (int64_t)K * P + (g - b * gpi) * NPX;
+    SoftmaxAcc acc[NPX];
+    for (int c = 0; c < K; ++c) {
+      float v[NPX];
+      load_px<NPX>(x + off + (int64_t)c * P, v);
+#pragma unroll
+      for (int j = 0; j < NPX; ++j) acc[j].add(v[j]);
+    }
+    for (int c = 0; c < K; ++c) {
+      float v[NPX];
+      load_px_last<NPX>(x + off + (int64_t)c * P, v);
+#pragma unroll
+      for (int j = 0; j < NPX; ++j) v[j] = acc[j].prob(v[j]);
+      store_px<NPX>(probs + off + (int64_t)c * P, v);
+    }
+  }
+}
+
 static int64_t l2_bytes() {
   int dev = 0, l2 = 0;
   cudaGetDevice(&dev);
@@ -580,6 +609,29 @@ extern "C" int smaat_argmax_channels_fwd(const float* x, int64_t* classes, int B
   if (vec) argmax_channels_kernel<4><<<(unsigned)blocks, CE_THREADS, 0, st>>>(x, classes, K, P, groups);
   else     argmax_channels_kernel<1><<<(unsigned)blocks, CE_THREADS, 0, st>>>(x, classes, K, P, groups);
   SMAAT_LAUNCH_CHECK("smaat_argmax_channels_fwd");
+  return SMAAT_OK;
+}
+
+extern "C" int smaat_softmax_channels_fwd(const float* x, float* probs, int B, int K, int64_t P, void* stream) {
+  SMAAT_REQUIRE(x && probs && B > 0 && P > 0, "softmax_channels: bad arguments (B=%d, P=%lld)", B, (long long)P);
+  SMAAT_REQUIRE(K >= 1, "softmax_channels: K=%d classes", K);
+  if (K > 1024) return fail(SMAAT_E_UNSUPPORTED, "softmax_channels: K=%d classes, this build supports at most 1024", K);
+  SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(x) & 3u) == 0 && (reinterpret_cast<uintptr_t>(probs) & 3u) == 0,
+                "softmax_channels: logits and probs must be 4-byte aligned");
+  const bool vec = P % 4 == 0 && aligned16(x) && aligned16(probs);
+  const int npx = vec ? 4 : 1;
+  const int64_t groups = (int64_t)B * (P / npx);
+  // smaat_ce_fwd's grid rule: the lines the grid reads between its two sweeps fit in half of the L2
+  const int64_t per_cta = (int64_t)CE_THREADS * npx * K * 4;
+  int64_t cap = l2_bytes() / 2 / per_cta;
+  if (cap < num_sms()) cap = num_sms();
+  if (cap > (int64_t)num_sms() * 8) cap = (int64_t)num_sms() * 8;
+  int64_t blocks = ceil_div64(groups, CE_THREADS);
+  if (blocks > cap) blocks = cap;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (vec) softmax_channels_kernel<4><<<(unsigned)blocks, CE_THREADS, 0, st>>>(x, probs, K, P, groups);
+  else     softmax_channels_kernel<1><<<(unsigned)blocks, CE_THREADS, 0, st>>>(x, probs, K, P, groups);
+  SMAAT_LAUNCH_CHECK("smaat_softmax_channels_fwd");
   return SMAAT_OK;
 }
 

@@ -23,9 +23,13 @@ class InferenceSession:
         """``output="logits"`` (default): the model's fp32 output.  ``output="classes"``: the (batch, H, W) int64 class map
         argmax over its channels (the reference's ``torch.argmax(softmax(y_pred), dim=1)``, train_SmaAtUNet.py:76), computed
         inside the captured graph: ``model.forward_classes`` where the model has it (SmaAt_UNet: OutConv and argmax in the last
-        kernel's epilogue), otherwise ``model(x)`` followed by the channel argmax kernel.  Only the class map crosses PCIe."""
-        if output not in ("logits", "classes"):
-            raise ValueError(f"InferenceSession: output must be 'logits' or 'classes', got {output!r}")
+        kernel's epilogue), otherwise ``model(x)`` followed by the channel argmax kernel.  Only the class map crosses PCIe.
+        ``output="probs"``: the (batch, K, H, W) fp32 softmax probabilities over the model's K output channels (the reference's
+        ``softmax(y_pred)``), likewise from ``model.forward_probs`` where the model has it, otherwise ``model(x)`` followed by
+        the channel softmax kernel; only the probabilities cross PCIe.  A model with one output channel raises ``ValueError``
+        (softmax over one channel is identically 1)."""
+        if output not in ("logits", "classes", "probs"):
+            raise ValueError(f"InferenceSession: output must be one of 'probs', 'logits' or 'classes', got {output!r}")
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self.model = model.to(self.device).eval()
         self.batch, self.in_shape = batch, tuple(in_shape)
@@ -38,11 +42,12 @@ class InferenceSession:
         self.launches_per_forward = 0
         self.graph = None
         # the serving forward may fuse what plain module calls cannot express (OutConv in the last epilogue, model.py);
-        # serving_fusions=False captures exactly the reference-API call sequence (+ the argmax kernel for class maps)
-        name = "forward_classes" if output == "classes" else "forward_serving"
+        # serving_fusions=False captures exactly the reference-API call sequence (+ the argmax / softmax kernel for class maps /
+        # probabilities)
+        name = {"logits": "forward_serving", "classes": "forward_classes", "probs": "forward_probs"}[output]
         self._fwd = getattr(self.model, name, None) if serving_fusions else None
         if self._fwd is None:
-            self._fwd = self.model if output == "logits" else self._model_then_argmax
+            self._fwd = {"logits": self.model, "classes": self._model_then_argmax, "probs": self._model_then_softmax}[output]
         self._capture()
         self.out_shape = tuple(self.static_out.shape)
         # staging slots (device side) so H2D of step i+1 and D2H of step i-1 overlap compute of step i
@@ -61,6 +66,10 @@ class InferenceSession:
         from . import ops
         return ops.argmax_channels(self.model(x))
 
+    def _model_then_softmax(self, x):
+        from . import ops
+        return ops.softmax_channels(self.model(x))
+
     def _capture(self):
         with torch.cuda.device(self.device), torch.no_grad():
             # warm-up on the compute stream: builds the folded-BN / split-weight caches (their small
@@ -70,6 +79,9 @@ class InferenceSession:
                 for _ in range(2):
                     self.static_out = self._fwd(self.static_in)
             self.compute.synchronize()
+            if self.output == "probs" and self.static_out.shape[1] == 1:
+                raise ValueError("InferenceSession(output='probs'): the model has one output channel, whose softmax is "
+                                 "identically 1; serve its logits instead")
             n0 = _lib.launch_count()
             if self.use_graph:
                 self.graph = torch.cuda.CUDAGraph()

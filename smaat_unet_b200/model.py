@@ -23,6 +23,13 @@ def _classes_of(model, x):
         return ops.argmax_channels(model(x))
 
 
+def _probs_of(model, x):
+    """The class probabilities of ``model(x)``'s logits: the plain forward, then the channel softmax kernel
+    (ops.softmax_channels), with no gradient."""
+    with torch.no_grad():
+        return ops.softmax_channels(model(x))
+
+
 class SmaAt_UNet(nn.Module):
     def __init__(self, n_channels, n_classes, kernels_per_layer=2, bilinear=True, reduction_ratio=16):
         super().__init__()
@@ -76,7 +83,17 @@ class SmaAt_UNet(nn.Module):
             return _classes_of(self, x)
         return self._serving(x, classes=True)
 
-    def _serving(self, x, classes):
+    def forward_probs(self, x):
+        """``forward_serving``'s graph ending in the (B, n_classes, H, W) fp32 class probabilities, softmax over the logits'
+        channels (the reference's ``softmax(y_pred)``, train_SmaAtUNet.py:76): up4's last DS conv applies the n_classes-class
+        OutConv and the softmax in its epilogue (n_classes <= 32), so only the probabilities reach HBM; more classes take the
+        unfused convs, OutConv and the softmax kernel.  Inference only, with no gradient: in train mode or under autograd
+        the plain forward followed by the softmax kernel, under no_grad."""
+        if self.training or _needs_grad(self, x):
+            return _probs_of(self, x)
+        return self._serving(x, probs=True)
+
+    def _serving(self, x, classes=False, probs=False):
         if self.training or _needs_grad(self, x):
             return self.forward(x)
         skips, f = [], self.inc(x)
@@ -96,7 +113,7 @@ class SmaAt_UNet(nn.Module):
             skip, gate = skips[3 - i]
             y = getattr(self, f"up{i + 1}")(y, skip, gate=gate)
         skip, gate = skips[0]
-        return self.up4(y, skip, outconv=self.outc, gate=gate, classes=classes)
+        return self.up4(y, skip, outconv=self.outc, gate=gate, classes=classes, probs=probs)
 
 
 class UNet(nn.Module):
@@ -133,6 +150,11 @@ class UNet(nn.Module):
     def forward_classes(self, x):
         """The (B, H, W) int64 class map of ``forward``'s logits (train_SmaAtUNet.py:76): the forward, then the argmax kernel."""
         return _classes_of(self, x)
+
+    def forward_probs(self, x):
+        """The class probabilities of ``forward``'s logits (train_SmaAtUNet.py:76): the forward, then the softmax kernel.
+        Inference only, with no gradient."""
+        return _probs_of(self, x)
 
 
 class UNetAttention(nn.Module):
@@ -180,3 +202,8 @@ class UNetAttention(nn.Module):
     def forward_classes(self, x):
         """The (B, H, W) int64 class map of ``forward``'s logits (train_SmaAtUNet.py:76): the forward, then the argmax kernel."""
         return _classes_of(self, x)
+
+    def forward_probs(self, x):
+        """The class probabilities of ``forward``'s logits (train_SmaAtUNet.py:76): the forward, then the softmax kernel.
+        Inference only, with no gradient."""
+        return _probs_of(self, x)

@@ -113,15 +113,19 @@ class DepthwiseSeparableConv(_CachingModule):
         d = ops.dw3x3(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, x1=x1, in_scale=in_scale, in_shift=in_shift)
         return ops.pw1x1(d, self.pointwise.weight.detach(), scale, shift, relu, mode=mode, w_split=split, stats=stats)
 
-    def run_classify(self, x, scale, shift, relu, outconv, want_logits=False):
+    def run_classify(self, x, scale, shift, relu, outconv, want_logits=False, probs=False):
         """``run`` followed by OutConv(Cout -> K) and the channel argmax in the fused kernel's epilogue (``outconv=(weight (K, Cout[,1,1]),
-        bias or None)``): the (B, H, W) int64 class map [, the logits], or None where that kernel does not take the request."""
+        bias or None)``): the (B, H, W) int64 class map [, the logits], or None where that kernel does not take the request.
+        ``probs=True``: the (B, K, H, W) softmax probabilities from that epilogue instead (``ops.dsconv_probs``)."""
         self._check()
         dw_b = self.depthwise.bias.detach() if self.depthwise.bias is not None else None
         mode = ops.get_pointwise_mode()
         split = self.pw_split() if mode == "tf32x3" else None
-        return ops.dsconv_classify(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(),
-                                   scale, shift, relu, outconv[0], outconv[1], mode=mode, w_split=split, want_logits=want_logits)
+        args = (x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(), scale, shift, relu,
+                outconv[0], outconv[1])
+        if probs:
+            return ops.dsconv_probs(*args, mode=mode, w_split=split)
+        return ops.dsconv_classify(*args, mode=mode, w_split=split, want_logits=want_logits)
 
     def cbam_takes(self, x, x1=None, gate=False, pools=False) -> bool:
         """Whether ``run_cbam`` takes this input: the fused kernel with the serving forward's CBAM fusions."""
@@ -190,20 +194,21 @@ class DoubleConvDS(_CachingModule):
         return not (_needs_grad(self, *inputs) or self.training
                     or any(not bn.track_running_stats or bn.running_mean is None for bn in bns))
 
-    def run(self, x, x1=None, outconv=None, gate=None, classes=False):
+    def run(self, x, x1=None, outconv=None, gate=None, classes=False, probs=False):
         """``outconv`` (an OutConv module with one class, inference only): fold it into the last kernel's epilogue and
         return the logits -- the block's own output is then never materialised (models/SmaAt_UNet.py:55-56).
         ``classes=True`` (with ``outconv`` of any class count): return the (B, H, W) int64 class map argmax_c OutConv(block(x))
-        instead, from the last kernel's epilogue where it takes the shape (``_run_classes``).
+        instead, from the last kernel's epilogue where it takes the shape (``_run_classes``).  ``probs=True``: the same for the
+        (B, K, H, W) softmax probabilities of OutConv(block(x)) (no gradient).
         ``gate=(sc, sa)``: x is the un-attended skip and the block's input is the CBAM output (x * sc) * sa, which the first
         DS conv computes as it loads x (inference only; materialised first where that kernel does not take it)."""
         ops._req(x, "input", 4)
         if gate is not None and not (self._eval_folded(x, x1) and self.double_conv[0].cbam_takes(x, x1, gate=True)):
             x, gate = ops.cbam_scale(x, gate[0], gate[1]), None
-        if classes:
+        if classes or probs:
             if outconv is None:
-                raise ValueError("DoubleConvDS.run(classes=True) needs the OutConv that produces the logits")
-            return self._run_classes(x, x1, outconv, gate)
+                raise ValueError("DoubleConvDS.run(classes=True / probs=True) needs the OutConv that produces the logits")
+            return self._run_classes(x, x1, outconv, gate, probs=probs)
         if outconv is not None:
             y = self._run_with_outconv(x, x1, outconv, gate)
             return y if y is not None else outconv(self.run(x, x1, gate=gate))
@@ -238,21 +243,23 @@ class DoubleConvDS(_CachingModule):
             z = outconv(self.double_conv[3].run(y, scale=s1, shift=t1, relu=True))
         return z
 
-    def _run_classes(self, x, x1, outconv, gate=None):
-        """The class map of OutConv(block(x)).  Eval fast path: the last DS conv applies the K-class OutConv and the argmax in
-        its epilogue (smaat_dsconv_classify_fwd), so neither the block's output nor the logits reach HBM; where that kernel does
-        not take the shape (K > 32, Cout > 128, ...) the same two convs run, then OutConv and the channel argmax kernel.  Under
-        autograd / batch statistics: the plain block, OutConv and the argmax."""
+    def _run_classes(self, x, x1, outconv, gate=None, probs=False):
+        """The class map of OutConv(block(x)), or with ``probs`` its softmax probabilities.  Eval fast path: the last DS conv
+        applies the K-class OutConv and the argmax / softmax in its epilogue (smaat_dsconv_classify_fwd / smaat_dsconv_probs_fwd),
+        so neither the block's output nor the logits reach HBM; where that kernel does not take the shape (K > 32, Cout > 128,
+        ...) the same two convs run, then OutConv and the channel argmax / softmax kernel.  Under autograd / batch statistics:
+        the plain block, OutConv and the argmax / softmax."""
+        head = outconv.probs if probs else outconv.classes
         if not (self._eval_folded(x, x1) and not _needs_grad(outconv, x)):
-            return outconv.classes(self.run(x, x1, gate=gate))
+            return head(self.run(x, x1, gate=gate))
         y = self._first_conv(x, x1, gate)
         s1, t1 = self._folded(3)
         oc = outconv.conv
         ob = oc.bias.detach() if oc.bias is not None else None
-        cls = self.double_conv[3].run_classify(y, s1, t1, True, (oc.weight.detach(), ob))
-        if cls is None:
-            cls = outconv.classes(self.double_conv[3].run(y, scale=s1, shift=t1, relu=True))
-        return cls
+        out = self.double_conv[3].run_classify(y, s1, t1, True, (oc.weight.detach(), ob), probs=probs)
+        if out is None:
+            out = head(self.double_conv[3].run(y, scale=s1, shift=t1, relu=True))
+        return out
 
     def forward(self, x):
         return self.run(x)
@@ -360,17 +367,19 @@ class UpDS(_TransposedUp):
             self.conv = DoubleConvDS(in_channels, out_channels, kernels_per_layer=kernels_per_layer)
         self._packed = None
 
-    def forward(self, x1, x2, outconv=None, gate=None, classes=False):
+    def forward(self, x1, x2, outconv=None, gate=None, classes=False, probs=False):
         """``gate=(sc, sa)`` (serving forward, inference only): x2 is the un-attended skip, and the block reads the CBAM output
-        (x2 * sc) * sa as it loads it (DoubleConvDS.run).  ``classes=True`` with ``outconv``: the class map of the OutConv's logits."""
+        (x2 * sc) * sa as it loads it (DoubleConvDS.run).  ``classes=True`` with ``outconv``: the class map of the OutConv's logits;
+        ``probs=True``: their softmax probabilities."""
         if not self.bilinear:
-            return self.conv.run(x2, x1=self._up_transposed(x1, x2.shape[2], x2.shape[3]), outconv=outconv, gate=gate, classes=classes)
+            return self.conv.run(x2, x1=self._up_transposed(x1, x2.shape[2], x2.shape[3]), outconv=outconv, gate=gate, classes=classes,
+                                 probs=probs)
         if torch.is_grad_enabled() and x1.requires_grad:
             from .autograd import Upsample2xPadFn
             up = Upsample2xPadFn.apply(x1, x2.shape[2], x2.shape[3])
         else:
             up = ops.upsample2x_pad(x1, x2.shape[2], x2.shape[3])
-        return self.conv.run(x2, x1=up, outconv=outconv, gate=gate, classes=classes)
+        return self.conv.run(x2, x1=up, outconv=outconv, gate=gate, classes=classes, probs=probs)
 
 
 class DoubleConv(_CachingModule):
@@ -533,6 +542,12 @@ class OutConv(nn.Module):
         train_SmaAtUNet.py:76): this module's logits, then the channel argmax kernel.  Inference only: a class map has no gradient."""
         with torch.no_grad():
             return ops.argmax_channels(self(x))
+
+    def probs(self, x):
+        """The (B, K, H, W) class probabilities softmax_c OutConv(x) (the reference's ``softmax(y_pred)``, train_SmaAtUNet.py:76):
+        this module's logits, then the channel softmax kernel.  Inference only: no gradient."""
+        with torch.no_grad():
+            return ops.softmax_channels(self(x))
 
 
 class Flatten(nn.Module):

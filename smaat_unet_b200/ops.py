@@ -314,8 +314,9 @@ _fuse_classify = os.environ.get("SMAAT_FUSE_CLASSIFY", "1") != "0"
 
 
 def set_fused_classify(enabled: bool) -> None:
-    """Enable/disable the K-class OutConv + argmax in the last DS conv's epilogue (default on; off = that conv, OutConv and
-    the channel argmax kernel as separate launches).  For A/B measurements (tools/bench_classes.py)."""
+    """Enable/disable the K-class OutConv + argmax or softmax in the last DS conv's epilogue (default on; off = that conv,
+    OutConv and the channel argmax / softmax kernel as separate launches).  For A/B measurements (tools/bench_classes.py,
+    tools/bench_probs.py)."""
     global _fuse_classify
     _fuse_classify = bool(enabled)
 
@@ -344,25 +345,12 @@ def dsconv_classify(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_
     (classes, (B, K, H, W) logits) with ``want_logits``; class j's logits are bit for bit those of ``dsconv(..., outconv=(oc_weight[j],
     oc_bias[j]))``.  Returns None where ``dsconv_classify_takes`` is False (the caller then runs the layers apart)."""
     mode = mode or _pw_mode
-    ow = _dense(oc_weight, "outconv.weight")
-    K = ow.shape[0]
+    K = _dense(oc_weight, "outconv.weight").shape[0]
     if not dsconv_classify_takes(x, x1, pw_weight, k, K, mode):
         return None
-    x, bs0 = _nchw_bstride(x, "x")
+    x, bs0, x1, C1, bs1, w2d, wlo, ow, ob = _k_class_operands(x, x1, k, pw_weight, oc_weight, oc_bias, mode, w_split)
     B, C0, H, W = x.shape
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        C1 = x1.shape[1]
-    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
     Cout, Kd = w2d.shape
-    assert Kd == k * (C0 + C1), f"pointwise weight {tuple(pw_weight.shape)} does not match k*Cin={k * (C0 + C1)}"
-    assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
-    ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
-    assert ob is None or ob.numel() == K, f"OutConv bias {tuple(oc_bias.shape)} does not match K={K}"
-    wlo = None
-    if PW_MODES[mode] == 2:
-        w2d, wlo = w_split if w_split is not None else split_tf32(w2d)
     classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64)
     logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
     Cin = C0 + C1
@@ -372,6 +360,66 @@ def dsconv_classify(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_
           _ptr(dw_bias), _ptr(w2d), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, _ptr(logits), _ptr(classes),
           B, H, W, k, Cout, int(bool(relu)), PW_MODES[mode], _stream())
     return (classes, logits) if want_logits else classes
+
+
+def _k_class_operands(x, x1, k, pw_weight, oc_weight, oc_bias, mode, w_split):
+    """The checked operands of the K-class epilogue entries (smaat_dsconv_classify_fwd, smaat_dsconv_probs_fwd):
+    (x, its batch stride, x1, C1, x1's batch stride, pointwise weight (Cout, k*Cin) [tf32 hi], its tf32 lo or None,
+    OutConv weight, OutConv bias or None)."""
+    x, bs0 = _nchw_bstride(x, "x")
+    C1, bs1 = 0, 0
+    if x1 is not None:
+        x1, bs1 = _nchw_bstride(x1, "x1")
+        C1 = x1.shape[1]
+    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
+    Cout, Kd = w2d.shape
+    assert Kd == k * (x.shape[1] + C1), f"pointwise weight {tuple(pw_weight.shape)} does not match k*Cin={k * (x.shape[1] + C1)}"
+    ow = _dense(oc_weight, "outconv.weight")
+    K = ow.shape[0]
+    assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
+    ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
+    assert ob is None or ob.numel() == K, f"OutConv bias {tuple(oc_bias.shape)} does not match K={K}"
+    wlo = None
+    if PW_MODES[mode] == 2:
+        w2d, wlo = w_split if w_split is not None else split_tf32(w2d)
+    return x, bs0, x1, C1, bs1, w2d, wlo, ow, ob
+
+
+def dsconv_probs(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, x1=None, mode=None, w_split=None):
+    """``dsconv`` followed by OutConv(Cout -> K) and the softmax over the K classes, all in the fused kernel's epilogue
+    (smaat_dsconv_probs_fwd): the (B, K, H, W) fp32 probabilities, bit for bit ``softmax_channels`` of the logits
+    ``dsconv_classify(..., want_logits=True)`` returns.  Inference only.  Returns None where ``dsconv_classify_takes`` is
+    False (the caller then runs the layers apart)."""
+    mode = mode or _pw_mode
+    K = _dense(oc_weight, "outconv.weight").shape[0]
+    if not dsconv_classify_takes(x, x1, pw_weight, k, K, mode):
+        return None
+    x, bs0, x1, C1, bs1, w2d, wlo, ow, ob = _k_class_operands(x, x1, k, pw_weight, oc_weight, oc_bias, mode, w_split)
+    B, C0, H, W = x.shape
+    Cout, Kd = w2d.shape
+    probs = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32)
+    Cin = C0 + C1
+    _call(f"smaat_dsconv_probs_fwd[C{Cin}_N{Cout}_K{K}_S{H}]",
+          4 * B * H * W * (Cin + K) + 4 * Kd * Cout, 2 * B * H * W * (Kd * (Cout + 9) + 2 * K * Cout),
+          _lib.load().smaat_dsconv_probs_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(_dense(dw_weight, "depthwise.weight")),
+          _ptr(dw_bias), _ptr(w2d), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, _ptr(probs),
+          B, H, W, k, Cout, int(bool(relu)), PW_MODES[mode], _stream())
+    return probs
+
+
+def softmax_channels(x):
+    """The class probabilities of (B, K, ...) logits: fp32 of the same shape, torch.softmax(x, 1) within fp32 rounding, with
+    torch's NaN / 0 / 1 pattern on non-finite logits (smaat_softmax_channels_fwd, 1 <= K <= 1024).  Inference only: no
+    gradient."""
+    x = _dense(x, "logits")
+    if x.dim() < 2:
+        raise RuntimeError(f"smaat_unet_b200: logits must be (B, K, ...), got shape {tuple(x.shape)}")
+    B, K = x.shape[0], x.shape[1]
+    P = x[0, 0].numel()
+    probs = torch.empty_like(x)
+    _call(f"smaat_softmax_channels_fwd[K{K}]", 8 * B * K * P, 0, _lib.load().smaat_softmax_channels_fwd, _ptr(x), _ptr(probs),
+          B, K, P, _stream())
+    return probs
 
 
 def argmax_channels(x):
