@@ -412,6 +412,30 @@ int smaat_conv3x3_fwd(const float* x0, int C0, int64_t x0_bstride, const float* 
                       double* stats, int B, int H, int W, int Cout, int relu, int mode, void* stream);
 int smaat_conv3x3_bwd_weight(const float* dz, const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1,
                              int64_t x1_bstride, float* dW, int B, int H, int W, int Cout, int mode, void* stream);
+/* The dense networks' last two modules in one kernel: the last 3x3 conv of up4's DoubleConv (+ eval BatchNorm2d + ReLU) followed
+ * by OutConv(Cout -> K) (models/unet_parts.py:16-21, 67-73), ending in the logits, the class map the reference's validation loop
+ * predicts (pred_class = torch.argmax(softmax(y_pred), dim=1), train_SmaAtUNet.py:76) or the softmax probabilities.  Conv
+ * arguments as smaat_conv3x3_fwd without y / y_bstride / stats; oc_w: (K, Cout), oc_b: (K) or NULL.
+ * smaat_conv3x3_classify_fwd: logits (B, K, H, W) or NULL, classes (B, H, W) int64 or NULL, not both NULL.
+ * smaat_conv3x3_probs_fwd: probs (B, K, H, W).
+ * Bitwise contract: the outputs equal, bit for bit, smaat_conv3x3_fwd -> smaat_outconv_fwd [-> smaat_argmax_channels_fwd /
+ *   smaat_softmax_channels_fwd] on the same inputs in the same mode: the epilogue forms the activation the conv writes, each
+ *   logit as the OutConv kernel sums it (the bias, then fmaf over the channels in order), the argmax with torch's rule (ties to
+ *   the first index, a NaN wins) and the probabilities with the softmax kernel's arithmetic.  Only the requested outputs reach
+ *   HBM; the Cout-channel activation never does.
+ * Eligibility (smaat_conv3x3_classify_eligible answers 1/0 for `mode`): that of smaat_conv3x3_tc_eligible, mode SMAAT_PW_TF32 or
+ *   SMAAT_PW_TF32X3, Cout <= 64 (one channel pass: a CTA holds all of a pixel's channels) and 1 <= K <= 32; no batch
+ *   statistics.  SMAAT_E_UNSUPPORTED otherwise (callers then run smaat_conv3x3_fwd, smaat_outconv_fwd and the argmax /
+ *   softmax kernel). */
+int smaat_conv3x3_classify_eligible(const float* x0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                                    const float* wp, int W, int Cout, int K, int mode);
+int smaat_conv3x3_classify_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                               const float* wp, const float* wp_lo, const float* scale, const float* shift, const float* oc_w,
+                               const float* oc_b, int K, float* logits, int64_t* classes, int B, int H, int W, int Cout, int relu,
+                               int mode, void* stream);
+int smaat_conv3x3_probs_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                            const float* wp, const float* wp_lo, const float* scale, const float* shift, const float* oc_w,
+                            const float* oc_b, int K, float* probs, int B, int H, int W, int Cout, int relu, int mode, void* stream);
 
 /* ---- optimizer step (reference models/regression_lightning.py:47-48, train_SmaAtUNet.py:25: torch.optim.Adam with its
  * defaults) over flat fp32 buffers of n floats (n % 4 == 0, 16-byte aligned; parameters, gradients, first and second moment

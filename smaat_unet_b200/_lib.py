@@ -83,6 +83,9 @@ SIGNATURES = {
     "smaat_conv3x3_pack_weight": [_p, _p, _i, _i, _i, _i, _p],
     "smaat_conv3x3_tc_eligible": [_p, _l, _p, _i, _l, _p, _i, _i],
     "smaat_conv3x3_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _p],
+    "smaat_conv3x3_classify_eligible": [_p, _l, _p, _i, _l, _p, _i, _i, _i, _i],
+    "smaat_conv3x3_classify_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _p],
+    "smaat_conv3x3_probs_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _i, _p, _i, _i, _i, _i, _i, _i, _p],
     "smaat_conv3x3_bwd_weight": [_p, _p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _p],
 }
 _SPECIAL = {

@@ -147,14 +147,41 @@ class UNet(nn.Module):
         x = self.up4(x, x1)
         return self.outc(x)
 
+    def forward_serving(self, x):
+        """``forward`` for ``engine.InferenceSession``, bit for bit ``forward``'s logits.  With ``ops.set_fused_dense_head(True)``
+        up4's last 3x3 conv applies the OutConv in its epilogue, so the 64-channel activation never reaches HBM; by default (the
+        faster route on an H100) and in train mode, under autograd, or where the epilogue does not take the shape ('fp32'
+        mode, W % 4 != 0, more than 32 classes), the plain calls."""
+        return self._serving(x)
+
     def forward_classes(self, x):
-        """The (B, H, W) int64 class map of ``forward``'s logits (train_SmaAtUNet.py:76): the forward, then the argmax kernel."""
-        return _classes_of(self, x)
+        """The (B, H, W) int64 class map of ``forward``'s logits (train_SmaAtUNet.py:76), bit for bit ``argmax_channels(forward(x))``:
+        with ``ops.set_fused_dense_head(True)`` up4's last conv applies the OutConv and the argmax in its epilogue, so neither its
+        activation nor the logits reach HBM.  Otherwise (see ``forward_serving``): the forward, then the argmax kernel."""
+        if self.training or _needs_grad(self, x):
+            return _classes_of(self, x)
+        return self._serving(x, classes=True)
 
     def forward_probs(self, x):
-        """The class probabilities of ``forward``'s logits (train_SmaAtUNet.py:76): the forward, then the softmax kernel.
-        Inference only, with no gradient."""
-        return _probs_of(self, x)
+        """The class probabilities of ``forward``'s logits (train_SmaAtUNet.py:76), bit for bit ``softmax_channels(forward(x))``:
+        with ``ops.set_fused_dense_head(True)`` up4's last conv applies the OutConv and the softmax in its epilogue.  Otherwise:
+        the forward, then the softmax kernel.  Inference only, with no gradient."""
+        if self.training or _needs_grad(self, x):
+            return _probs_of(self, x)
+        return self._serving(x, probs=True)
+
+    def _serving(self, x, classes=False, probs=False):
+        if self.training or _needs_grad(self, x):
+            return self.forward(x)
+        x1 = self.inc(x)
+        x2 = self.down1(x1)
+        x3 = self.down2(x2)
+        x4 = self.down3(x3)
+        x5 = self.down4(x4)
+        x = self.up1(x5, x4)
+        x = self.up2(x, x3)
+        x = self.up3(x, x2)
+        return self.up4(x, x1, outconv=self.outc, classes=classes, probs=probs)
 
 
 class UNetAttention(nn.Module):
@@ -199,11 +226,43 @@ class UNetAttention(nn.Module):
         x = self.up4(x, x1Att)
         return self.outc(x)
 
+    def forward_serving(self, x):
+        """``forward`` for ``engine.InferenceSession``, bit for bit ``forward``'s logits.  With ``ops.set_fused_dense_head(True)``
+        up4's last 3x3 conv applies the OutConv in its epilogue, so the 64-channel activation never reaches HBM; by default (the
+        faster route on an H100) and in train mode, under autograd, or where the epilogue does not take the shape ('fp32'
+        mode, W % 4 != 0, more than 32 classes), the plain calls."""
+        return self._serving(x)
+
     def forward_classes(self, x):
-        """The (B, H, W) int64 class map of ``forward``'s logits (train_SmaAtUNet.py:76): the forward, then the argmax kernel."""
-        return _classes_of(self, x)
+        """The (B, H, W) int64 class map of ``forward``'s logits (train_SmaAtUNet.py:76), bit for bit ``argmax_channels(forward(x))``:
+        with ``ops.set_fused_dense_head(True)`` up4's last conv applies the OutConv and the argmax in its epilogue, so neither its
+        activation nor the logits reach HBM.  Otherwise (see ``forward_serving``): the forward, then the argmax kernel."""
+        if self.training or _needs_grad(self, x):
+            return _classes_of(self, x)
+        return self._serving(x, classes=True)
 
     def forward_probs(self, x):
-        """The class probabilities of ``forward``'s logits (train_SmaAtUNet.py:76): the forward, then the softmax kernel.
-        Inference only, with no gradient."""
-        return _probs_of(self, x)
+        """The class probabilities of ``forward``'s logits (train_SmaAtUNet.py:76), bit for bit ``softmax_channels(forward(x))``:
+        with ``ops.set_fused_dense_head(True)`` up4's last conv applies the OutConv and the softmax in its epilogue.  Otherwise:
+        the forward, then the softmax kernel.  Inference only, with no gradient."""
+        if self.training or _needs_grad(self, x):
+            return _probs_of(self, x)
+        return self._serving(x, probs=True)
+
+    def _serving(self, x, classes=False, probs=False):
+        if self.training or _needs_grad(self, x):
+            return self.forward(x)
+        x1 = self.inc(x)
+        x1Att = self.cbam1(x1)
+        x2 = self.down1(x1)
+        x2Att = self.cbam2(x2)
+        x3 = self.down2(x2)
+        x3Att = self.cbam3(x3)
+        x4 = self.down3(x3)
+        x4Att = self.cbam4(x4)
+        x5 = self.down4(x4)
+        x5Att = self.cbam5(x5)
+        x = self.up1(x5Att, x4Att)
+        x = self.up2(x, x3Att)
+        x = self.up3(x, x2Att)
+        return self.up4(x, x1Att, outconv=self.outc, classes=classes, probs=probs)

@@ -453,11 +453,23 @@ class DoubleConv(_CachingModule):
             hit = self._fold[idx]
         return hit[1]
 
-    def run(self, x, x1=None):
+    def run(self, x, x1=None, outconv=None, classes=False, probs=False):
+        """``outconv`` (an OutConv module): return OutConv(block(x)), its logits.  ``classes=True``: the (B, H, W) int64 class map
+        of those logits instead; ``probs=True``: their (B, K, H, W) softmax probabilities (no gradient).  In eval mode without
+        autograd the last conv applies the OutConv and the argmax / softmax in its epilogue where it takes the shape
+        (``_run_head``): the block's output is then never written, and the result is bit for bit that of the separate calls."""
         ops._req(x, "input", 4)
         if x1 is not None:
             ops._req(x1, "input", 4)
         self._check()
+        if classes or probs or outconv is not None:
+            if outconv is None:
+                raise ValueError("DoubleConv.run(classes=True / probs=True) needs the OutConv that produces the logits")
+            out = self._run_head(x, x1, outconv, classes, probs)
+            if out is not None:
+                return out
+            head = outconv.probs if probs else (outconv.classes if classes else outconv)
+            return head(self.run(x, x1))
         if _needs_grad(self, x, x1):
             from .autograd import DoubleConvFn
             return DoubleConvFn.run(self, x, x1)
@@ -469,6 +481,32 @@ class DoubleConv(_CachingModule):
         y = self.conv(0, x, x1, scale=s0, shift=t0, relu=True)
         s1, t1 = self._folded(3)
         return self.conv(3, y, scale=s1, shift=t1, relu=True)
+
+    def _run_head(self, x, x1, outconv, classes, probs):
+        """The eval fast path of ``run`` with an OutConv: the first conv as usual, then the last conv with the K-class OutConv
+        and the argmax / softmax in its epilogue (smaat_conv3x3_classify_fwd / smaat_conv3x3_probs_fwd).  None where that
+        path does not apply (train mode, batch statistics, autograd, 'fp32', or a shape the epilogue does not take: Cout > 64,
+        K > 32, W % 4 != 0, ...), and unless ops.set_fused_dense_head(True): the caller then runs the separate calls."""
+        bns = (self.double_conv[1], self.double_conv[4])
+        if (not ops.fused_dense_head() or _needs_grad(self, x, x1) or _needs_grad(outconv, x) or self.training
+                or any(not bn.track_running_stats or bn.running_mean is None for bn in bns)):
+            return None
+        c3, oc = self.double_conv[3], outconv.conv
+        s0, t0 = self._folded(0)
+        y = self.conv(0, x, x1, scale=s0, shift=t0, relu=True)
+        s1, t1 = self._folded(3)
+        wp, hi, lo = self.packed(3, y.shape[1])
+        split = (hi, lo) if hi is not None else None
+        ob = oc.bias.detach() if oc.bias is not None else None
+        args = (y, wp, c3.out_channels, s1, t1, True, oc.weight.detach(), ob)
+        if probs:
+            out = ops.conv3x3_probs(*args, w_split=split)
+        else:
+            out = ops.conv3x3_classify(*args, w_split=split, want_logits=not classes, want_classes=classes)
+        if out is None:           # the last conv's shape is not taken: the same conv, OutConv and argmax / softmax apart
+            out = self.conv(3, y, scale=s1, shift=t1, relu=True)
+            out = outconv.probs(out) if probs else (outconv.classes(out) if classes else outconv(out))
+        return out
 
     def forward(self, x):
         return self.run(x)
@@ -511,17 +549,19 @@ class Up(_TransposedUp):
             self.conv = DoubleConv(in_channels, out_channels)
         self._packed = None
 
-    def forward(self, x1, x2):
+    def forward(self, x1, x2, outconv=None, classes=False, probs=False):
+        """``outconv``: return OutConv's logits of the block's output; with ``classes=True`` their class map, with ``probs=True``
+        their softmax probabilities (``DoubleConv.run``)."""
         ops._req(x1, "x1", 4)
         ops._req(x2, "x2", 4)
         if not self.bilinear:
-            return self.conv.run(x2, x1=self._up_transposed(x1, x2.shape[2], x2.shape[3]))
+            return self.conv.run(x2, x1=self._up_transposed(x1, x2.shape[2], x2.shape[3]), outconv=outconv, classes=classes, probs=probs)
         if torch.is_grad_enabled() and x1.requires_grad:
             from .autograd import Upsample2xPadFn
             up = Upsample2xPadFn.apply(x1, x2.shape[2], x2.shape[3])
         else:
             up = ops.upsample2x_pad(x1, x2.shape[2], x2.shape[3])
-        return self.conv.run(x2, x1=up)
+        return self.conv.run(x2, x1=up, outconv=outconv, classes=classes, probs=probs)
 
 
 class OutConv(nn.Module):

@@ -314,9 +314,9 @@ _fuse_classify = os.environ.get("SMAAT_FUSE_CLASSIFY", "1") != "0"
 
 
 def set_fused_classify(enabled: bool) -> None:
-    """Enable/disable the K-class OutConv + argmax or softmax in the last DS conv's epilogue (default on; off = that conv,
-    OutConv and the channel argmax / softmax kernel as separate launches).  For A/B measurements (tools/bench_classes.py,
-    tools/bench_probs.py)."""
+    """Enable/disable the K-class OutConv + argmax or softmax in the last DS conv's epilogue, and the OutConv epilogue of the
+    dense networks' last 3x3 conv (default on; off = that conv, OutConv and the channel argmax / softmax kernel as separate
+    launches).  For A/B measurements (tools/bench_classes.py, tools/bench_probs.py, tools/bench_dense_serving.py)."""
     global _fuse_classify
     _fuse_classify = bool(enabled)
 
@@ -494,6 +494,109 @@ def conv3x3(x, wp, Cout, scale, shift, relu, x1=None, mode=None, w_split=None, s
           _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(wp), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(y), Cout * H * W, _ptr(stats),
           B, H, W, Cout, int(bool(relu)), m, _stream())
     return y
+
+
+# Whether UNet / UNetAttention (DoubleConv.run with an OutConv) take the OutConv epilogue of their last 3x3 conv.  Off by
+# default: on an H100 the fused last conv is slower than the conv + OutConv (+ argmax / softmax) launches it replaces (README,
+# DESIGN section 6), and both routes give the same bits.
+_fuse_dense_head = os.environ.get("SMAAT_FUSE_DENSE_HEAD", "0") == "1"
+
+
+def set_fused_dense_head(enabled: bool) -> None:
+    """Let the dense networks' serving forward (``UNet`` / ``UNetAttention`` ``forward_serving`` / ``forward_classes`` /
+    ``forward_probs``, ``DoubleConv.run(outconv=...)``) run the OutConv and the argmax / softmax in the last 3x3 conv's
+    epilogue (``conv3x3_classify`` / ``conv3x3_probs``).  Default off (SMAAT_FUSE_DENSE_HEAD=1 presets it on): the outputs are
+    bit for bit the same, and the separate launches are faster on an H100.  set_fused_classify(False) turns it off too."""
+    global _fuse_dense_head
+    _fuse_dense_head = bool(enabled)
+
+
+def fused_dense_head() -> bool:
+    return _fuse_dense_head
+
+
+def conv3x3_classify_takes(x, x1, wp, Cout, n_classes, mode=None) -> bool:
+    """True when ``conv3x3_classify`` / ``conv3x3_probs`` run on these inputs: the tensor-core conv with a ``n_classes``-class
+    OutConv in its epilogue (smaat_conv3x3_classify_eligible: the tensor-core conv's shapes, Cout <= 64, 1 <= n_classes <= 32,
+    'tf32' / 'tf32x3'), and not set_fused_classify(False)."""
+    mode = mode or _pw_mode
+    if not _fuse_classify or PW_MODES[mode] == 0:
+        return False
+    x, bs0 = _nchw_bstride(x, "x")
+    C1, bs1 = 0, 0
+    if x1 is not None:
+        x1, bs1 = _nchw_bstride(x1, "x1")
+        C1 = x1.shape[1]
+    return bool(_lib.load().smaat_conv3x3_classify_eligible(_ptr(x), bs0, _ptr(x1), C1, bs1, _ptr(wp), x.shape[3], Cout, int(n_classes),
+                                                            PW_MODES[mode]))
+
+
+def _conv3x3_head_operands(x, x1, wp, Cout, oc_weight, oc_bias, mode, w_split):
+    """The checked operands of the dense OutConv epilogue (smaat_conv3x3_classify_fwd, smaat_conv3x3_probs_fwd):
+    (x, its batch stride, x1, C1, x1's batch stride, packed weight [tf32 hi], its tf32 lo or None, OutConv weight, bias or None)."""
+    x, bs0 = _nchw_bstride(x, "x")
+    B, C0, H, W = x.shape
+    C1, bs1 = 0, 0
+    if x1 is not None:
+        x1, bs1 = _nchw_bstride(x1, "x1")
+        assert x1.shape[0] == B and x1.shape[2:] == x.shape[2:], "concat inputs must agree in B, H, W"
+        C1 = x1.shape[1]
+    assert wp.shape == (Cout, 9 * (_pad32(C0) + _pad32(C1))), f"packed weight {tuple(wp.shape)} does not match Cin={C0}+{C1}"
+    ow = _dense(oc_weight, "outconv.weight")
+    K = ow.shape[0]
+    assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
+    ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
+    assert ob is None or ob.numel() == K, f"OutConv bias {tuple(oc_bias.shape)} does not match K={K}"
+    wlo = None
+    if PW_MODES[mode] == 2:
+        wp, wlo = w_split if w_split is not None else split_tf32(wp)
+    return x, bs0, x1, C1, bs1, wp, wlo, ow, ob
+
+
+def conv3x3_classify(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1=None, mode=None, w_split=None, want_logits=False,
+                     want_classes=True):
+    """``conv3x3`` followed by OutConv(Cout -> K) (and the channel argmax) in the tensor-core kernel's epilogue
+    (smaat_conv3x3_classify_fwd).  oc_weight (K, Cout[,1,1]), oc_bias (K) or None.  Returns the (B, H, W) int64 class map; with
+    ``want_logits`` also the (B, K, H, W) logits, as (classes, logits), or the logits alone with ``want_classes=False``.  Bit for
+    bit ``outconv(conv3x3(...))`` and ``argmax_channels`` of it.  Returns None where ``conv3x3_classify_takes`` is False (the
+    caller then runs the layers apart)."""
+    assert want_logits or want_classes, "conv3x3_classify: ask for the logits, the class map or both"
+    mode = mode or _pw_mode
+    K = _dense(oc_weight, "outconv.weight").shape[0]
+    if not conv3x3_classify_takes(x, x1, wp, Cout, K, mode):
+        return None
+    x, bs0, x1, C1, bs1, wp, wlo, ow, ob = _conv3x3_head_operands(x, x1, wp, Cout, oc_weight, oc_bias, mode, w_split)
+    B, C0, H, W = x.shape
+    classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64) if want_classes else None
+    logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
+    Cin = C0 + C1
+    _call(f"smaat_conv3x3_classify_fwd[C{Cin}_N{Cout}_K{K}_S{H}x{W}]",
+          4 * B * H * W * (Cin + (K if want_logits else 0) + (2 if want_classes else 0)) + 36 * Cin * Cout,
+          2 * B * H * W * Cout * (9 * Cin + K), _lib.load().smaat_conv3x3_classify_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(wp),
+          _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, _ptr(logits), _ptr(classes), B, H, W, Cout, int(bool(relu)),
+          PW_MODES[mode], _stream())
+    if not want_logits:
+        return classes
+    return (classes, logits) if want_classes else logits
+
+
+def conv3x3_probs(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1=None, mode=None, w_split=None):
+    """``conv3x3`` followed by OutConv(Cout -> K) and the softmax over the K classes in the tensor-core kernel's epilogue
+    (smaat_conv3x3_probs_fwd): the (B, K, H, W) fp32 probabilities, bit for bit ``softmax_channels(outconv(conv3x3(...)))``.
+    Inference only.  Returns None where ``conv3x3_classify_takes`` is False."""
+    mode = mode or _pw_mode
+    K = _dense(oc_weight, "outconv.weight").shape[0]
+    if not conv3x3_classify_takes(x, x1, wp, Cout, K, mode):
+        return None
+    x, bs0, x1, C1, bs1, wp, wlo, ow, ob = _conv3x3_head_operands(x, x1, wp, Cout, oc_weight, oc_bias, mode, w_split)
+    B, C0, H, W = x.shape
+    probs = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32)
+    Cin = C0 + C1
+    _call(f"smaat_conv3x3_probs_fwd[C{Cin}_N{Cout}_K{K}_S{H}x{W}]", 4 * B * H * W * (Cin + K) + 36 * Cin * Cout,
+          2 * B * H * W * Cout * (9 * Cin + K), _lib.load().smaat_conv3x3_probs_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(wp),
+          _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, _ptr(probs), B, H, W, Cout, int(bool(relu)), PW_MODES[mode],
+          _stream())
+    return probs
 
 
 def conv3x3_bwd_weight(dz, x, x1, dW, mode=None):
