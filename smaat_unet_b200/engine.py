@@ -92,14 +92,16 @@ class InferenceSession:
                     self.static_out = self._fwd(self.static_in)
             self.launches_per_forward = _lib.launch_count() - n0
             self.compute.synchronize()
-        # the graph has the addresses of the folded-BN / split-weight tensors baked in: keep them alive with the session.
-        # The session is a SNAPSHOT of the weights at construction; after training the model further call refresh().
-        from .modules import cached_tensors
-        self._keepalive = cached_tensors(self.model)
+        # the graph has the addresses of the weight caches, parameters and buffers baked in: the session holds them alive,
+        # whatever the model does with them afterwards (mode switches drop the caches, TrainSession re-points the parameters)
+        from .modules import graph_tensors
+        self._keepalive = graph_tensors(self.model)
 
     def refresh(self):
         """Re-derive the weight caches and re-capture the graph: call after the model's parameters / BatchNorm statistics
-        changed (e.g. more training) -- a session is a snapshot of the weights it was built from."""
+        changed (e.g. more training).  The session is not a snapshot: the folded BatchNorm, tf32 splits and packed weights
+        are derived at capture, but the other parameters (depthwise and tf32-mode pointwise weights, the CBAM MLP, OutConv,
+        biases) are read in place, so until refresh() the outputs mix old and new weights."""
         from . import ops
         ops.bump_weights_generation()
         self.model.eval()

@@ -16,6 +16,8 @@ There is no PyTorch / CPU fallback; unsupported requests raise.
 """
 from __future__ import annotations
 
+import weakref
+
 import torch
 from torch import nn
 
@@ -28,6 +30,13 @@ def _versions(*tensors):
     write through raw pointers, so the key also carries ``ops.weights_generation()`` -- bumped by every such write
     (ops.bn_finalize, TrainSession.step) and by every train()/eval() switch of a caching module."""
     return (ops.weights_generation(),) + tuple((t.data_ptr(), t._version) for t in tensors if t is not None)
+
+
+def _held(*tensors):
+    """Aliases of the tensors a cache entry was derived from, stored with the entry.  A ``_versions`` key names addresses:
+    while the entry holds their blocks, no tensor that replaces a source (``load_state_dict(..., assign=True)``,
+    ``p.data = ...``) can be allocated on a cached address at the cached version and hit the stale entry."""
+    return tuple(t.detach() for t in tensors if t is not None)
 
 
 class _CachingModule(nn.Module):
@@ -69,9 +78,10 @@ class DepthwiseSeparableConv(_CachingModule):
         self.kernels_per_layer = kernels_per_layer
         self._wsplit = None
         self._wsplit_key = None
+        self._wsplit_src = None
 
     def _drop_caches(self):
-        self._wsplit = self._wsplit_key = None
+        self._wsplit = self._wsplit_key = self._wsplit_src = None
 
     def _check(self):
         if self.depthwise.kernel_size != (3, 3) or self.depthwise.padding != (1, 1):
@@ -88,6 +98,7 @@ class DepthwiseSeparableConv(_CachingModule):
             with torch.no_grad():
                 self._wsplit = ops.split_tf32(w.detach().view(w.shape[0], -1))
             self._wsplit_key = None if in_train_capture else key
+            self._wsplit_src = _held(w)
         return self._wsplit
 
     def fused_takes(self, x, x1=None, stats=False) -> bool:
@@ -178,13 +189,14 @@ class DoubleConvDS(_CachingModule):
         """(scale, shift) of eval BatchNorm idx+1 folded with pointwise bias of DS conv idx; cached."""
         ds, bn = self.double_conv[idx], self.double_conv[idx + 1]
         pb = ds.pointwise.bias
-        key = _versions(bn.weight, bn.bias, bn.running_mean, bn.running_var, pb)
+        src = (bn.weight, bn.bias, bn.running_mean, bn.running_var, pb)
+        key = _versions(*src)
         hit = self._fold.get(idx)
         if hit is None or hit[0] != key:
             with torch.no_grad():
                 sc_sh = ops.bn_fold(bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var,
                                     pb.detach() if pb is not None else None, bn.eps)
-            self._fold[idx] = (key, sc_sh)
+            self._fold[idx] = (key, sc_sh, _held(*src))
             hit = self._fold[idx]
         return hit[1]
 
@@ -277,19 +289,25 @@ def _tensor_key(x):
 
 
 def _stash_maxpool(x, pooled):
+    """The entry names x by a weak reference (checked with ``is``) as well as by address and version: a tensor that is
+    allocated on x's block after x is freed has the same address and, fresh from a kernel, the same version 0."""
     global _maxpool_stash
-    _maxpool_stash = (_tensor_key(x), pooled)
+    _maxpool_stash = (weakref.ref(x), _tensor_key(x), pooled)
 
 
 def _take_stashed_maxpool(x):
+    """The stashed MaxPool2d(2)(x), or None.  Never under autograd: the stashed map was produced without a tape, so taking
+    it for an ``x`` that requires grad would cut the max-pool's gradient path to ``x``."""
     global _maxpool_stash
     hit = _maxpool_stash
     if hit is None or not isinstance(x, torch.Tensor) or not x.is_cuda:
         return None
-    if hit[0] != _tensor_key(x):
+    if torch.is_grad_enabled() and x.requires_grad:
+        return None
+    if hit[0]() is not x or hit[1] != _tensor_key(x):
         return None
     _maxpool_stash = None
-    return hit[1]
+    return hit[2]
 
 
 class DownDS(nn.Module):
@@ -332,7 +350,7 @@ class _TransposedUp(_CachingModule):
             with torch.no_grad():
                 wp = ops.convt2x2_pack_weight(w.detach())
                 split = ops.split_tf32(wp) if ops.get_pointwise_mode() == "tf32x3" else None
-            self._packed = (None if in_train_capture else key, wp, split)
+            self._packed = (None if in_train_capture else key, wp, split, _held(w))
         return self._packed[1], self._packed[2]
 
     def _up_transposed(self, x1, Ho, Wo):
@@ -428,7 +446,7 @@ class DoubleConv(_CachingModule):
             with torch.no_grad():
                 wp = ops.conv3x3_pack_weight(w.detach(), C0, C1, flip_transpose)
                 hi, lo = ops.split_tf32(wp) if mode == "tf32x3" else (None, None)
-            hit = (None if in_train_capture else key, (wp, hi, lo))
+            hit = (None if in_train_capture else key, (wp, hi, lo), _held(w))
             self._packed[slot] = hit
         return hit[1]
 
@@ -443,13 +461,14 @@ class DoubleConv(_CachingModule):
     def _folded(self, idx):
         """(scale, shift) of eval BatchNorm idx+1 folded with the bias of conv idx; cached."""
         conv, bn = self.double_conv[idx], self.double_conv[idx + 1]
-        key = _versions(bn.weight, bn.bias, bn.running_mean, bn.running_var, conv.bias)
+        src = (bn.weight, bn.bias, bn.running_mean, bn.running_var, conv.bias)
+        key = _versions(*src)
         hit = self._fold.get(idx)
         if hit is None or hit[0] != key:
             with torch.no_grad():
                 sc_sh = ops.bn_fold(bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var,
                                     conv.bias.detach() if conv.bias is not None else None, bn.eps)
-            self._fold[idx] = (key, sc_sh)
+            self._fold[idx] = (key, sc_sh, _held(*src))
             hit = self._fold[idx]
         return hit[1]
 
@@ -659,11 +678,12 @@ class SpatialAttention(_CachingModule):
             raise NotImplementedError("standalone SpatialAttention in train mode is not implemented (CBAM handles it); "
                                       "call .eval() or use CBAM")
         bn = self.bn
-        key = _versions(bn.weight, bn.bias, bn.running_mean, bn.running_var)
+        src = (bn.weight, bn.bias, bn.running_mean, bn.running_var)
+        key = _versions(*src)
         if self._fold is None or self._fold[0] != key:
             with torch.no_grad():
                 s, t = ops.bn_fold(bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var, None, bn.eps)
-                self._fold = (key, torch.cat([s, t]))
+                self._fold = (key, torch.cat([s, t]), _held(*src))
         return self._fold[1]
 
     def gate(self, x, sc):
@@ -723,20 +743,31 @@ class CBAM(nn.Module):
 
 
 def cached_tensors(model):
-    """Every tensor the eval fast path derived from ``model``'s parameters (folded BatchNorm affine, tf32 hi/lo splits).
-    A CUDA graph captured over the eval forward has their addresses baked in: whoever owns the graph must keep them alive."""
+    """Every tensor the eval fast path derived from ``model``'s parameters (folded BatchNorm affine, tf32 hi/lo splits,
+    packed 3x3 and transposed-conv weights).  A CUDA graph captured over the eval forward has their addresses baked in:
+    whoever owns the graph must keep them alive (``graph_tensors``)."""
     out = []
     for m in model.modules():
         if isinstance(m, DepthwiseSeparableConv) and m._wsplit is not None:
             out.extend(m._wsplit)
-        elif isinstance(m, DoubleConvDS):
-            for _, pair in m._fold.values():
-                out.extend(pair)
-        elif isinstance(m, DoubleConv):
-            for _, pair in m._fold.values():
-                out.extend(pair)
-            for _, trio in m._packed.values():
-                out.extend(t for t in trio if t is not None)
+        elif isinstance(m, (DoubleConvDS, DoubleConv)):
+            for entry in m._fold.values():
+                out.extend(entry[1])
+            if isinstance(m, DoubleConv):
+                for entry in m._packed.values():
+                    out.extend(t for t in entry[1] if t is not None)
         elif isinstance(m, SpatialAttention) and m._fold is not None:
             out.append(m._fold[1])
+        if isinstance(m, _TransposedUp) and m._packed is not None:
+            _, wp, split, _ = m._packed
+            out.append(wp)
+            out.extend(split or ())
     return out
+
+
+def graph_tensors(model):
+    """Everything a CUDA graph captured over ``model``'s eval forward reads by address, other than its own inputs and
+    activations: the caches (``cached_tensors``), and aliases of every parameter and buffer, which the kernels read in
+    place.  The aliases keep the storage alive after the model lets it go (``TrainSession`` re-points the parameters into
+    its flat buffer, ``load_state_dict(..., assign=True)`` replaces them, a mode switch drops the caches)."""
+    return cached_tensors(model) + [t.detach() for t in list(model.parameters()) + list(model.buffers())]

@@ -173,7 +173,9 @@ def pw1x1(x, weight, scale, shift, relu, mode=None, w_split=None, stats=None, ou
     mode = mode or _pw_mode
     m = PW_MODES[mode]
     wlo = None
-    if m != 0 and not tc_eligible(x, w2d):
+    # the tensor-core kernel stages an epilogue affine for at most 512 output channels (SmaAt_UNet(bilinear=False)'s
+    # 1024-channel bottleneck has more)
+    if m != 0 and (not tc_eligible(x, w2d) or (Cout > 512 and (scale is not None or shift is not None))):
         m = 0
     if m == 2:
         hi, wlo = w_split if w_split is not None else split_tf32(w2d)
@@ -741,15 +743,19 @@ def cbam_pool_maxpool(x):
 
 
 _cbam_counters = {}
+_retired_counters = []       # superseded buffers: a captured graph may still hand them to its kernels
 
 
 def _counters(device, n):
     """Zeroed int32 scratch (>= n entries) for the last-arriving-CTA hand-off of smaat_cbam_pool_mlp_fwd: the kernel returns
-    it at zero, so one buffer per device serves every call (stream-ordered; allocated outside any graph capture)."""
+    it at zero, so one buffer per device serves every call (stream-ordered; allocated outside any graph capture).  A larger
+    batch gets a larger buffer; the old one is kept, never freed, because graphs captured earlier have its address."""
     t = _cbam_counters.get(device)
     if t is None or t.numel() < n:
         if torch.cuda.is_current_stream_capturing():
             raise RuntimeError("smaat_unet_b200: run one eager forward before capturing a CUDA graph (CBAM scratch allocation)")
+        if t is not None:
+            _retired_counters.append(t)
         t = torch.zeros(max(n, 256), device=device, dtype=torch.int32)
         _cbam_counters[device] = t
     return t
