@@ -115,11 +115,16 @@ struct DsCfg {
                                                                            : 0;
   static constexpr int ST_BYTES = 2 * ST_BUFS * ST_BOX;
   static_assert(ST_BUFS > 0 || (FREE - 2 * ST_BOX) / IN_BYTES < 2, "staging falls back only where one buffer does not fit");
-  static constexpr int IS_FIT = (FREE - ST_BYTES) / IN_BYTES;
-  static constexpr int IS = IS_FIT > 8 ? 8 : IS_FIT;           // input ring: as deep as shared memory allows
-  // beside each input stage, the CBAM spatial gate's one-channel halo box (gated chunks only), in what the ring leaves over
+  // beside each input stage, the CBAM spatial gate's one-channel halo box (gated chunks only)
   static constexpr int SA_TX = BH * BW * 4;
   static constexpr int SA_BYTES = (SA_TX + 127) / 128 * 128;
+  // Input ring: as deep as shared memory allows, up to 8 stages, with a gate box per stage and, past the ring's end (rounded up
+  // to 1 KB: OFF_A), room for the class weights of a 21-class model (MAX_CLASSES, below).  The k <= 2 instances meet both
+  // with whole input boxes to spare; the 7 680 B boxes of k = 4 would not
+  static constexpr int CLS_MIN = 21 * (N_TILE + 1) * 4;
+  static constexpr int RING_CLS = (FREE - ST_BYTES + 3 * 1024 - CLS_MIN) / 1024 * 1024;
+  static constexpr int IS_FIT = (RING_CLS < FREE - ST_BYTES ? RING_CLS : FREE - ST_BYTES) / (IN_BYTES + SA_BYTES);
+  static constexpr int IS = IS_FIT > 8 ? 8 : IS_FIT;
   static_assert(IS * (IN_BYTES + SA_BYTES) + ST_BYTES <= FREE, "gate boxes fit beside the input ring");
   static constexpr int OFF_SA = IS * IN_BYTES;
   static constexpr int OFF_A = ((OFF_SA + IS * SA_BYTES + 1023) / 1024) * 1024;
@@ -189,12 +194,12 @@ __device__ __forceinline__ void quad_transpose(float (&v)[4], int q) {
   }
 }
 
+// The kernel body, shared by the k = 1 / 2 instances (dsconv_fused_kernel) and the k = 4 ones (dsconv_kpl4_kernel).  The tensor
+// maps are the kernels' __grid_constant__ parameters
 template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
-__global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1)
-    dsconv_fused_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
-                        const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
-                        const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_sa,
-                        const DsParams p) {
+__device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CUtensorMap& map_in1, const CUtensorMap& map_w,
+                                            const CUtensorMap& map_wlo, const CUtensorMap& map_y, const CUtensorMap& map_sa,
+                                            const DsParams& p) {
   using L = DsCfg<N_TILE, KPL, PW, X3, A_SMEM>;
   constexpr int PH = L::PH, BW = L::BW, BH = L::BH, CC = L::CC, IS = L::IS, AS = L::AS, BS = L::BS;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
@@ -668,6 +673,16 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
     const int g = (warp - L::PROD_WARP) >> 2;
     const int t = threadIdx.x - 32 * L::PROD_WARP - 128 * g;  // 0..127
     const int Cin = p.C0 + p.C1;
+    // A task is one (input channel, column quad[, row group]) of a chunk: NT = CC * 8 of them.  A thread computes KH of its KPL
+    // depthwise outputs: all of them at KPL = 1 / 2; at KPL = 4 (CC = 8: 64 tasks) two threads share each task, threads
+    // 64 h .. 64 h + 63 computing k-rows 4 ci + 2 h and 4 ci + 2 h + 1 (kr0 = 2 h), so that all 128 producer threads work and
+    // each holds the weight registers of KPL = 2
+    constexpr int KH = KPL == 4 ? 2 : KPL, NT = CC * 8;
+    const int kr0 = KH == KPL ? 0 : t / NT * KH;
+    // this thread's depthwise weights and biases start at k-row kr0 (offset in the pointers: in the per-chunk weight index,
+    // ptxas spilled the KPL = 4 producers)
+    const float* dw_w = p.dw_w + kr0 * 9;
+    const float* dw_b = p.dw_b ? p.dw_b + kr0 : nullptr;
     uint32_t gc = 0, iph = 0;       // iph: phase bit per input stage of this group's fill barriers
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const int b = tile / tiles_per_img;
@@ -677,18 +692,20 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
         // chunks of x0 under a CBAM gate: each staged value is read as (x * sc[b, c]) * sa[b, p], the two rounded products of
         // cbam_gate_scale_kernel in its order, so the stencil sees exactly the materialised CBAM output
         const bool gated = p.gate_sc && i * CC < p.C0;
+        // (thread t's task at KPL = 4: t % NT, both halves)
+        auto task_base = [&](int task) { return KH == KPL ? task : task & (NT - 1); };
         // depthwise weights of this thread's (first) task: issued before the ring waits so that their latency hides there
-        float wr[KPL][9], br[KPL], gsc = 0.f;
+        float wr[KH][9], br[KH], gsc = 0.f;
         auto task_channel = [&](int task) { return (PW == 32) ? (task >> 3) : (((task >> 4) << 1) | ((task >> 2) & 1)); };
         auto load_weights = [&](int task) {
-          const int gch = i * CC + task_channel(task);
+          const int gch = i * CC + task_channel(task_base(task));
           const bool chv = gch < Cin;
 #pragma unroll
-          for (int kk = 0; kk < KPL; ++kk) {
+          for (int kk = 0; kk < KH; ++kk) {
             const int gk = gch * KPL + kk;
 #pragma unroll
-            for (int w9 = 0; w9 < 9; ++w9) wr[kk][w9] = chv ? __ldg(p.dw_w + (int64_t)gk * 9 + w9) : 0.f;
-            br[kk] = (chv && p.dw_b) ? __ldg(p.dw_b + gk) : 0.f;
+            for (int w9 = 0; w9 < 9; ++w9) wr[kk][w9] = chv ? __ldg(dw_w + (int64_t)gk * 9 + w9) : 0.f;
+            br[kk] = (chv && dw_b) ? __ldg(dw_b + gk) : 0.f;
           }
           if (gated) gsc = gch < p.C0 ? __ldg(p.gate_sc + (int64_t)b * p.C0 + gch) : 0.f;
         };
@@ -704,21 +721,24 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
         auto stencil = [&](auto gate_c) {
           constexpr bool G = decltype(gate_c)::value;
 #pragma unroll 1
-          for (int task = t; task < CC * 8; task += 128) {
+          for (int task = t; task < NT * (KPL / KH); task += 128) {
             // task -> (input channel ci, column quad qc, row group rg).  A quarter-warp (8 lanes: one 128-bit shared-memory
             // wavefront) must touch 8 different 16-byte bank groups: PW = 32 -> the 8 quads of one channel row; PW = 16 ->
-            // the 4 quads of TWO channels (16 words apart in the input tile, and 2 k-rows apart = a different
+            // the 4 quads of TWO channels (16 words apart in the input tile, and KPL k-rows apart = a different
             // swizzle phase in the A operand).  Pairing the two row groups of one channel instead (rows 4 apart: 96 words in
             // the input tile, 4 KB in the A operand) put both halves on the same banks: every LDS.128 / STS.128 2-way.
+            // At KPL = 4 the two halves of a task are 64 threads apart (warps 0-1 and 2-3 of the group), so every warp maps its
+            // lanes as above: the halves read the same input window, and the A ring still takes 16 KB per chunk
+            const int tb = task_base(task);
             int ci, qc, rg;
             if (PW == 32) {
-              ci = task >> 3; qc = task & 7; rg = 0;
+              ci = tb >> 3; qc = tb & 7; rg = 0;
             } else {
-              qc = task & 3; ci = ((task >> 4) << 1) | ((task >> 2) & 1); rg = (task >> 3) & 1;
+              qc = tb & 3; ci = ((tb >> 4) << 1) | ((tb >> 2) & 1); rg = (tb >> 3) & 1;
             }
             constexpr int NQ = PW / 4;
             const int c0 = qc << 2, r0 = rg << 2;
-            if (task != t) load_weights(task);   // KPL = 1: a second task per chunk
+            if (task != t) load_weights(task);   // KPL = 1: a second task per chunk (every other KPL: one task per thread)
             // smem column of patch column c (dx = -1..1) is c + 4 + dx: the 4 outputs read cols c0+3 .. c0+8
             const float* trow = in_stage + (ci * BH + r0) * BW + c0 + 3;
             const float* srow = sa_stage + r0 * BW + c0 + 3;
@@ -755,7 +775,7 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
               const float* w2 = win[(rr + 2) % 3];
               const int m = (r0 + rr) * PW + c0;
 #pragma unroll
-              for (int kk = 0; kk < KPL; ++kk) {
+              for (int kk = 0; kk < KH; ++kk) {
                 float o4[4];
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
@@ -766,7 +786,7 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
                   o4[j] = a;
                 }
                 if (A_SMEM) {
-                  const int kr = ci * KPL + kk;
+                  const int kr = ci * KPL + kr0 + kk;
 #pragma unroll
                   for (int j = 0; j < 4; ++j) {
                     const uint32_t off = kmajor_offset(m + j, kr);
@@ -777,7 +797,7 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
                   continue;
                 }
                 // fp32 in both modes: the consumers split TF32X3's hi / lo parts after loading (one pass through shared memory)
-                *reinterpret_cast<float4*>(my_op + a_tile_offset(ci * KPL + kk, m)) = make_float4(o4[0], o4[1], o4[2], o4[3]);
+                *reinterpret_cast<float4*>(my_op + a_tile_offset(ci * KPL + kr0 + kk, m)) = make_float4(o4[0], o4[1], o4[2], o4[3]);
               }
             }
           }
@@ -792,10 +812,37 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1
 }
 
 template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
+__global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1)
+    dsconv_fused_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
+                        const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
+                        const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_sa,
+                        const DsParams p) {
+  dsconv_body<N_TILE, KPL, PW, X3, A_SMEM>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
+}
+
+// kernels_per_layer = 4: CC = 8 input channels per chunk (7 680 B input boxes at both patch widths), two producer threads per
+// task.  Register form only
+template <int N_TILE, int PW, bool X3>
+__global__ void __launch_bounds__(DsCfg<N_TILE, 4, PW, X3, false>::THREADS, 1)
+    dsconv_kpl4_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
+                       const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
+                       const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_sa,
+                       const DsParams p) {
+  dsconv_body<N_TILE, 4, PW, X3, false>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
+}
+
+template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
+static auto ds_kernel() {
+  static_assert(KPL == 1 || KPL == 2 || (KPL == 4 && !A_SMEM), "fused DS conv instances: k = 1, 2 (both A forms), 4 (register form)");
+  if constexpr (KPL == 4) return dsconv_kpl4_kernel<N_TILE, PW, X3>;
+  else return dsconv_fused_kernel<N_TILE, KPL, PW, X3, A_SMEM>;
+}
+
+template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
 static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl,
                      const CUtensorMap& my, const CUtensorMap& msa, DsParams p, int B, cudaStream_t st) {
   using L = DsCfg<N_TILE, KPL, PW, X3, A_SMEM>;
-  auto kern = dsconv_fused_kernel<N_TILE, KPL, PW, X3, A_SMEM>;
+  auto kern = ds_kernel<N_TILE, KPL, PW, X3, A_SMEM>();
   // the pools are read back from the staging buffers: instances with the direct-store epilogue do not take them
   if (p.pool_sum && !L::ST_BUFS) return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools need the staged epilogue");
   if (p.ncls > L::MAX_CLASSES)
@@ -841,10 +888,13 @@ static int pick_pw(int H, int W) {
 
 // y: the activation output, or null where it is not known yet (smaat_dsconv_eligible*) or not written (the fused OutConv).  The
 // epilogue stores it by TMA, which needs a 16-byte aligned base and 16-byte multiples as strides
+static int ds_impl();
+
 static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* pw_w,
                         const float* pw_w_lo, const float* y, int64_t y_bstride, int H, int W, int k, int Cout, bool stats,
                         bool outconv) {
-  if (k != 1 && k != 2) return false;
+  // k = 4 has register-form instances only (dsconv_kpl4_kernel): with the shared-memory A form selected it stays unfused
+  if (k != 1 && k != 2 && !(k == 4 && ds_impl() != 1)) return false;
   if (y && (!aligned16(y) || y_bstride % 4 != 0)) return false;
   // Cout > 128: whole passes of 128 channels; batch statistics and the fused OutConv need all channels in one pass
   if (Cout < 8 || Cout > 512 || (Cout > 128 && (Cout % 128 != 0 || stats || outconv))) return false;
@@ -856,31 +906,40 @@ static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, i
 }
 
 // Whether the instance dsconv_run dispatches to has the staged epilogue (ST_BUFS > 0), which the CBAM pools are read from
+// (k = 4: the register form, the only one it has)
 template <int N_TILE, int KPL, int PW>
 static bool ds_staged_t(bool x3, bool a_smem) {
-  return (x3 ? (a_smem ? DsCfg<N_TILE, KPL, PW, true, true>::ST_BUFS : DsCfg<N_TILE, KPL, PW, true, false>::ST_BUFS)
-             : (a_smem ? DsCfg<N_TILE, KPL, PW, false, true>::ST_BUFS : DsCfg<N_TILE, KPL, PW, false, false>::ST_BUFS)) > 0;
+  if constexpr (KPL == 4) return (x3 ? DsCfg<N_TILE, 4, PW, true, false>::ST_BUFS : DsCfg<N_TILE, 4, PW, false, false>::ST_BUFS) > 0;
+  else
+    return (x3 ? (a_smem ? DsCfg<N_TILE, KPL, PW, true, true>::ST_BUFS : DsCfg<N_TILE, KPL, PW, true, false>::ST_BUFS)
+               : (a_smem ? DsCfg<N_TILE, KPL, PW, false, true>::ST_BUFS : DsCfg<N_TILE, KPL, PW, false, false>::ST_BUFS)) > 0;
 }
 // The most classes whose OutConv weights the instance dsconv_run dispatches to keeps in shared memory (DsCfg::MAX_CLASSES)
 template <int N_TILE, int KPL, int PW>
 static int ds_max_classes_t(bool x3, bool a_smem) {
-  return x3 ? (a_smem ? DsCfg<N_TILE, KPL, PW, true, true>::MAX_CLASSES : DsCfg<N_TILE, KPL, PW, true, false>::MAX_CLASSES)
-            : (a_smem ? DsCfg<N_TILE, KPL, PW, false, true>::MAX_CLASSES : DsCfg<N_TILE, KPL, PW, false, false>::MAX_CLASSES);
+  if constexpr (KPL == 4) return x3 ? DsCfg<N_TILE, 4, PW, true, false>::MAX_CLASSES : DsCfg<N_TILE, 4, PW, false, false>::MAX_CLASSES;
+  else
+    return x3 ? (a_smem ? DsCfg<N_TILE, KPL, PW, true, true>::MAX_CLASSES : DsCfg<N_TILE, KPL, PW, true, false>::MAX_CLASSES)
+              : (a_smem ? DsCfg<N_TILE, KPL, PW, false, true>::MAX_CLASSES : DsCfg<N_TILE, KPL, PW, false, false>::MAX_CLASSES);
 }
 static int ds_max_classes(int n_tile, int k, int pw, bool x3, bool a_smem) {
   if (n_tile == 64) {
+    if (k == 4) return pw == 32 ? ds_max_classes_t<64, 4, 32>(x3, a_smem) : ds_max_classes_t<64, 4, 16>(x3, a_smem);
     if (k == 2) return pw == 32 ? ds_max_classes_t<64, 2, 32>(x3, a_smem) : ds_max_classes_t<64, 2, 16>(x3, a_smem);
     return pw == 32 ? ds_max_classes_t<64, 1, 32>(x3, a_smem) : ds_max_classes_t<64, 1, 16>(x3, a_smem);
   }
+  if (k == 4) return pw == 32 ? ds_max_classes_t<128, 4, 32>(x3, a_smem) : ds_max_classes_t<128, 4, 16>(x3, a_smem);
   if (k == 2) return pw == 32 ? ds_max_classes_t<128, 2, 32>(x3, a_smem) : ds_max_classes_t<128, 2, 16>(x3, a_smem);
   return pw == 32 ? ds_max_classes_t<128, 1, 32>(x3, a_smem) : ds_max_classes_t<128, 1, 16>(x3, a_smem);
 }
 
 static bool ds_staged(int n_tile, int k, int pw, bool x3, bool a_smem) {
   if (n_tile == 64) {
+    if (k == 4) return pw == 32 ? ds_staged_t<64, 4, 32>(x3, a_smem) : ds_staged_t<64, 4, 16>(x3, a_smem);
     if (k == 2) return pw == 32 ? ds_staged_t<64, 2, 32>(x3, a_smem) : ds_staged_t<64, 2, 16>(x3, a_smem);
     return pw == 32 ? ds_staged_t<64, 1, 32>(x3, a_smem) : ds_staged_t<64, 1, 16>(x3, a_smem);
   }
+  if (k == 4) return pw == 32 ? ds_staged_t<128, 4, 32>(x3, a_smem) : ds_staged_t<128, 4, 16>(x3, a_smem);
   if (k == 2) return pw == 32 ? ds_staged_t<128, 2, 32>(x3, a_smem) : ds_staged_t<128, 2, 16>(x3, a_smem);
   return pw == 32 ? ds_staged_t<128, 1, 32>(x3, a_smem) : ds_staged_t<128, 1, 16>(x3, a_smem);
 }
@@ -1027,13 +1086,20 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
                       : launch_ds<NT, KP, PWv, true, false>(m0, m1, mw, mwl, my, msa, p, B, st))                 \
             : (a_smem ? launch_ds<NT, KP, PWv, false, true>(m0, m1, mw, mwl, my, msa, p, B, st)                  \
                       : launch_ds<NT, KP, PWv, false, false>(m0, m1, mw, mwl, my, msa, p, B, st))
+// k = 4: the register form (ds_eligible)
+#define DS_DISPATCH4(NT, PWv)                                                                                  \
+  return x3 ? launch_ds<NT, 4, PWv, true, false>(m0, m1, mw, mwl, my, msa, p, B, st)                          \
+            : launch_ds<NT, 4, PWv, false, false>(m0, m1, mw, mwl, my, msa, p, B, st)
   if (n_tile == 64) {
-    if (k == 2) { if (pw == 32) { DS_DISPATCH(64, 2, 32); } else { DS_DISPATCH(64, 2, 16); } }
-    else        { if (pw == 32) { DS_DISPATCH(64, 1, 32); } else { DS_DISPATCH(64, 1, 16); } }
+    if (k == 4)      { if (pw == 32) { DS_DISPATCH4(64, 32); } else { DS_DISPATCH4(64, 16); } }
+    else if (k == 2) { if (pw == 32) { DS_DISPATCH(64, 2, 32); } else { DS_DISPATCH(64, 2, 16); } }
+    else             { if (pw == 32) { DS_DISPATCH(64, 1, 32); } else { DS_DISPATCH(64, 1, 16); } }
   } else {
-    if (k == 2) { if (pw == 32) { DS_DISPATCH(128, 2, 32); } else { DS_DISPATCH(128, 2, 16); } }
-    else        { if (pw == 32) { DS_DISPATCH(128, 1, 32); } else { DS_DISPATCH(128, 1, 16); } }
+    if (k == 4)      { if (pw == 32) { DS_DISPATCH4(128, 32); } else { DS_DISPATCH4(128, 16); } }
+    else if (k == 2) { if (pw == 32) { DS_DISPATCH(128, 2, 32); } else { DS_DISPATCH(128, 2, 16); } }
+    else             { if (pw == 32) { DS_DISPATCH(128, 1, 32); } else { DS_DISPATCH(128, 1, 16); } }
   }
+#undef DS_DISPATCH4
 #undef DS_DISPATCH
 }
 

@@ -333,5 +333,6 @@ extern "C" int smaat_dw3x3_fwd(const float* x0, int C0, int64_t x0_bstride, cons
 
   if (k == 1) return dispatch_dw<1>(m0, m1, p, rh, use_tma, pro, vec, threads, smem, grid, st);
   if (k == 2) return dispatch_dw<2>(m0, m1, p, rh, use_tma, pro, vec, threads, smem, grid, st);
+  if (k == 4) return dispatch_dw<4>(m0, m1, p, rh, use_tma, pro, vec, threads, smem, grid, st);
   return dispatch_dw<0>(m0, m1, p, rh, use_tma, pro, vec, threads, smem, grid, st);
 }

@@ -135,7 +135,7 @@ __global__ void __launch_bounds__(256) dw3x3_bwd_weight_tiled(const float* __res
 }
 
 // ---------------------------------------------------------------------------------------------
-// TMA variants (W % 4 == 0, k in {1,2}): same structure as the forward kernel (dw3x3.cu) -- the halo
+// TMA variants (W % 4 == 0, k in {1, 2, 4}): same structure as the forward kernel (dw3x3.cu) -- the halo
 // tile arrives by one bulk tensor copy per plane (out-of-bounds zero fill = padding), each thread walks
 // an RH-row strip of 4 columns with a 3-row register window, 128-bit global accesses.
 //   input : K gradient planes -> 1 dx plane, flipped taps.      bytes = 4*B*P*Cin*(k+1)
@@ -332,14 +332,20 @@ __global__ void __launch_bounds__(256) dw3x3_bwd_weight_tma(const __grid_constan
       if (lane == 0) red[kk * 10 + q][wp] = v;
     }
   __syncthreads();
-  if (tid < K * 10) {
+  auto flush = [&](int r) {   // sum r of the K * 10
     const int nw = (blockDim.x + 31) >> 5;
     float v = 0.f;
-    for (int i = 0; i < nw; ++i) v += red[tid][i];
-    const int kk = tid / 10, q = tid - kk * 10;
+    for (int i = 0; i < nw; ++i) v += red[r][i];
+    const int kk = r / 10, q = r - kk * 10;
     const int o = c * K + kk;
     if (q < 9) atomicAdd(p.dw + (int64_t)o * 9 + q, v);
     else if (p.db) atomicAdd(p.db + o, v);
+  };
+  // small planes launch a single warp: one sum per thread up to K = 3, a second pass at K = 4 (40 sums)
+  if constexpr (K * 10 <= 32) {
+    if (tid < K * 10) flush(tid);
+  } else {
+    for (int r = tid; r < K * 10; r += blockDim.x) flush(r);
   }
 }
 
@@ -394,7 +400,7 @@ static int dwb_input_try_tma(const float* dd, const float* w, float* dx0, int C0
   DwbParams p;
   memset(&p, 0, sizeof(p));
   int rh, threads;
-  if (!(k == 1 || k == 2) || !dwb_tma_geometry(H, W, &p, &rh, &threads)) return 1;
+  if (!(k == 1 || k == 2 || k == 4) || !dwb_tma_geometry(H, W, &p, &rh, &threads)) return 1;
   if (!aligned16(dd) || !aligned16(dx0) || bs0 % 4 != 0 || (C1 > 0 && (!aligned16(dx1) || bs1 % 4 != 0))) return 1;
   const int Cin = C0 + C1;
   p.g = dd; p.w = w; p.dx0 = dx0; p.dx1 = dx1; p.C0 = C0; p.C1 = C1; p.bs0 = bs0; p.bs1 = bs1;
@@ -407,7 +413,8 @@ static int dwb_input_try_tma(const float* dd, const float* w, float* dx0, int C0
   const int64_t grid = (int64_t)B * Cin * p.tiles_x * p.tiles_y;
   SMAAT_REQUIRE(grid < (1ll << 31), "dw3x3_bwd_input: grid too large");
   if (k == 1) return rh == 8 ? launch_dwb_input<1, 8>(mg, p, grid, threads, st) : launch_dwb_input<1, 4>(mg, p, grid, threads, st);
-  return rh == 8 ? launch_dwb_input<2, 8>(mg, p, grid, threads, st) : launch_dwb_input<2, 4>(mg, p, grid, threads, st);
+  if (k == 2) return rh == 8 ? launch_dwb_input<2, 8>(mg, p, grid, threads, st) : launch_dwb_input<2, 4>(mg, p, grid, threads, st);
+  return rh == 8 ? launch_dwb_input<4, 8>(mg, p, grid, threads, st) : launch_dwb_input<4, 4>(mg, p, grid, threads, st);
 }
 
 static int dwb_weight_try_tma(const float* dd, const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1,
@@ -416,7 +423,7 @@ static int dwb_weight_try_tma(const float* dd, const float* x0, int C0, int64_t 
   DwbParams p;
   memset(&p, 0, sizeof(p));
   int rh, threads;
-  if (!(k == 1 || k == 2) || !dwb_tma_geometry(H, W, &p, &rh, &threads)) return 1;
+  if (!(k == 1 || k == 2 || k == 4) || !dwb_tma_geometry(H, W, &p, &rh, &threads)) return 1;
   if (!aligned16(dd) || !aligned16(x0) || bs0 % 4 != 0 || (C1 > 0 && (!aligned16(x1) || bs1 % 4 != 0))) return 1;
   p.g = dd; p.C0 = C0; p.C1 = C1; p.bs0 = bs0; p.bs1 = bs1; p.in_scale = in_scale; p.in_shift = in_shift; p.dw = dw; p.db = db;
   CUtensorMap m0, m1;
@@ -450,7 +457,8 @@ static int dwb_weight_try_tma(const float* dd, const float* x0, int C0, int64_t 
 #define SMAAT_DWB_W(KK, RR) \
   (pro ? launch_dwb_weight<KK, RR, true>(m0, m1, mg, p, grid, threads, st) : launch_dwb_weight<KK, RR, false>(m0, m1, mg, p, grid, threads, st))
   if (k == 1) return rh == 8 ? SMAAT_DWB_W(1, 8) : SMAAT_DWB_W(1, 4);
-  return rh == 8 ? SMAAT_DWB_W(2, 8) : SMAAT_DWB_W(2, 4);
+  if (k == 2) return rh == 8 ? SMAAT_DWB_W(2, 8) : SMAAT_DWB_W(2, 4);
+  return rh == 8 ? SMAAT_DWB_W(4, 8) : SMAAT_DWB_W(4, 4);
 #undef SMAAT_DWB_W
 }
 

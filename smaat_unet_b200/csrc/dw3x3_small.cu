@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(32 * DWS_WARPS) dw3x3_small_kernel(const float
 // 1 = not applicable (caller uses the general kernel), else SMAAT_OK / error code
 int dw3x3_small_try(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* w, const float* bias,
                     const float* in_scale, const float* in_shift, float* y, int B, int H, int W, int k, cudaStream_t st) {
-  if (!(k == 1 || k == 2) || (int64_t)H * W > DWS_MAX_PIXELS || W > 62 || H > 62) return 1;
+  if (!(k == 1 || k == 2 || k == 4) || (int64_t)H * W > DWS_MAX_PIXELS || W > 62 || H > 62) return 1;
   const int64_t planes = (int64_t)B * (C0 + C1);
   const int64_t grid = ceil_div64(planes, DWS_WARPS);
   SMAAT_REQUIRE(grid < (1ll << 31), "dw3x3(small): grid too large");
@@ -81,9 +81,12 @@ int dw3x3_small_try(const float* x0, int C0, int64_t bs0, const float* x1, int C
   if (k == 1) {
     if (pro) dw3x3_small_kernel<1, true><<<g, thr, smem, st>>>(x0, C0, bs0, x1, C1, bs1, w, bias, in_scale, in_shift, y, planes, H, W);
     else dw3x3_small_kernel<1, false><<<g, thr, smem, st>>>(x0, C0, bs0, x1, C1, bs1, w, bias, in_scale, in_shift, y, planes, H, W);
-  } else {
+  } else if (k == 2) {
     if (pro) dw3x3_small_kernel<2, true><<<g, thr, smem, st>>>(x0, C0, bs0, x1, C1, bs1, w, bias, in_scale, in_shift, y, planes, H, W);
     else dw3x3_small_kernel<2, false><<<g, thr, smem, st>>>(x0, C0, bs0, x1, C1, bs1, w, bias, in_scale, in_shift, y, planes, H, W);
+  } else {
+    if (pro) dw3x3_small_kernel<4, true><<<g, thr, smem, st>>>(x0, C0, bs0, x1, C1, bs1, w, bias, in_scale, in_shift, y, planes, H, W);
+    else dw3x3_small_kernel<4, false><<<g, thr, smem, st>>>(x0, C0, bs0, x1, C1, bs1, w, bias, in_scale, in_shift, y, planes, H, W);
   }
   SMAAT_LAUNCH_CHECK("smaat_dw3x3_fwd");
   return SMAAT_OK;
