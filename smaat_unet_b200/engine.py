@@ -16,6 +16,7 @@ import collections
 import torch
 
 from . import _lib
+from .modules import apply_head
 
 
 class InferenceSession:
@@ -47,7 +48,7 @@ class InferenceSession:
         name = {"logits": "forward_serving", "classes": "forward_classes", "probs": "forward_probs"}[output]
         self._fwd = getattr(self.model, name, None) if serving_fusions else None
         if self._fwd is None:
-            self._fwd = {"logits": self.model, "classes": self._model_then_argmax, "probs": self._model_then_softmax}[output]
+            self._fwd = lambda x: apply_head(self.model, x, output)
         self._capture()
         self.out_shape = tuple(self.static_out.shape)
         # staging slots (device side) so H2D of step i+1 and D2H of step i-1 overlap compute of step i
@@ -61,14 +62,6 @@ class InferenceSession:
         self._d2h_done = [torch.cuda.Event() for _ in range(slots)]
         self._pending = collections.deque()
         self._step = 0
-
-    def _model_then_argmax(self, x):
-        from . import ops
-        return ops.argmax_channels(self.model(x))
-
-    def _model_then_softmax(self, x):
-        from . import ops
-        return ops.softmax_channels(self.model(x))
 
     def _capture(self):
         with torch.cuda.device(self.device), torch.no_grad():

@@ -203,11 +203,9 @@ def pw_bwd(dz, d, weight, dW, db, need_input=True):
 def dw_bwd(dd, dw_weight, x0, x1, in_scale, in_shift, k, dWdw, dbdw, need_input=True):
     """Depthwise 3x3 backward: accumulates weight/bias grads; returns (dx0, dx1) split over the virtual concat."""
     B, KC, H, W = dd.shape
-    C0 = x0.shape[1]
-    C1 = x1.shape[1] if x1 is not None else 0
+    x0c, bs0, x1c, C1, bs1 = ops._concat_operands(x0, x1)
+    C0 = x0c.shape[1]
     lib = _lib.load()
-    x0c, bs0 = ops._nchw_bstride(x0, "x0")
-    x1c, bs1 = (ops._nchw_bstride(x1, "x1") if x1 is not None else (None, 0))
     _call("smaat_dw3x3_bwd_weight", 4 * B * H * W * (KC + C0 + C1), 20 * B * H * W * KC, lib.smaat_dw3x3_bwd_weight, _ptr(dd), _ptr(x0c),
           C0, bs0, _ptr(x1c), C1, bs1, _ptr(in_scale), _ptr(in_shift), _ptr(dWdw), _ptr(dbdw), B, H, W, k, _stream())
     if not need_input:

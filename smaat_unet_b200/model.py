@@ -8,29 +8,50 @@ reference checkout is not importable (e.g. the GPU box).  With the reference on
 """
 from __future__ import annotations
 
-import torch
 from torch import nn
 
-from . import ops
-from .modules import CBAM, DoubleConv, DoubleConvDS, Down, DownDS, OutConv, Up, UpDS, _needs_grad
+from .modules import CBAM, DoubleConv, DoubleConvDS, Down, DownDS, OutConv, Up, UpDS, _needs_grad, apply_head
 
 _ENC = (64, 128, 256, 512)
 
 
-def _classes_of(model, x):
-    """The class map of ``model(x)``'s logits: the plain forward, then the channel argmax kernel (ops.argmax_channels)."""
-    with torch.no_grad():
-        return ops.argmax_channels(model(x))
+class _ServingForward(nn.Module):
+    """The serving forwards ``engine.InferenceSession`` captures, for the three networks.  Each network provides
+    ``_serving(x, head)``: its eval forward, ending in up4 with the OutConv and the head (modules.HEADS); its class docstring
+    says what that fuses.  In train mode or under autograd they run the plain forward, then ``modules.apply_head``."""
+
+    def forward_serving(self, x):
+        """``forward``'s logits, through the serving forward's fusions."""
+        return self._serve(x, "logits")
+
+    def forward_classes(self, x):
+        """The (B, H, W) int64 class map of the logits, argmax over their channels (the reference's
+        ``torch.argmax(softmax(y_pred), dim=1)``, train_SmaAtUNet.py:76).  Inference only."""
+        return self._serve(x, "classes")
+
+    def forward_probs(self, x):
+        """The (B, n_classes, H, W) fp32 class probabilities, softmax over the logits' channels (the reference's
+        ``softmax(y_pred)``, train_SmaAtUNet.py:76).  Inference only, with no gradient."""
+        return self._serve(x, "probs")
+
+    def _serve(self, x, head):
+        if self.training or _needs_grad(self, x):
+            return apply_head(self, x, head)
+        return self._serving(x, head)
 
 
-def _probs_of(model, x):
-    """The class probabilities of ``model(x)``'s logits: the plain forward, then the channel softmax kernel
-    (ops.softmax_channels), with no gradient."""
-    with torch.no_grad():
-        return ops.softmax_channels(model(x))
+class SmaAt_UNet(_ServingForward):
+    """The serving forward (``forward_serving`` / ``forward_classes`` / ``forward_probs``) has the fusions the plain-call API
+    cannot express:
+    * up4's last DS conv applies the OutConv in its epilogue (SmaAt_UNet.py:55-56), so the 64-channel activation never reaches
+      HBM: the 1-class OutConv for the logits, the n_classes-class OutConv and the argmax / softmax for class maps and
+      probabilities (n_classes <= 32; more classes take the unfused convs, OutConv and the argmax / softmax kernel).  Each
+      class's logit there is the one-class fused OutConv's arithmetic, which sums in another order than the unfused OutConv of
+      the logits route: pixels whose top two logits lie within rounding of each other may pick the other class;
+    * the three large CBAMs (levels 1-3) never write their output: they compute only their two gates, and the first DS
+      conv of up2 / up3 / up4 applies them as it loads the skip, with the products the CBAM's own kernel would have used
+      (bit for bit the same logits).  Levels 4-5 run the plain calls."""
 
-
-class SmaAt_UNet(nn.Module):
     def __init__(self, n_channels, n_classes, kernels_per_layer=2, bilinear=True, reduction_ratio=16):
         super().__init__()
         self.n_channels, self.n_classes, self.bilinear = n_channels, n_classes, bilinear
@@ -62,40 +83,7 @@ class SmaAt_UNet(nn.Module):
             y = getattr(self, f"up{i + 1}")(y, att[3 - i])          # attended maps are the skips
         return self.outc(y)
 
-    def forward_serving(self, x):
-        """Same graph with the fusions the plain-call API cannot express (``engine.InferenceSession``; inference only, the
-        plain calls under autograd / train mode):
-        * up4's last DS conv applies the 1-class OutConv in its epilogue (SmaAt_UNet.py:55-56), so the 64-channel activation
-          never reaches HBM;
-        * the three large CBAMs (levels 1-3) never write their output: they compute only their two gates, and the first DS
-          conv of up2 / up3 / up4 applies them as it loads the skip, with the products the CBAM's own kernel would have used
-          (bit for bit the same logits).  Levels 4-5 run the plain calls."""
-        return self._serving(x, classes=False)
-
-    def forward_classes(self, x):
-        """``forward_serving``'s graph ending in the (B, H, W) int64 class map the reference predicts from the logits
-        (``torch.argmax(softmax(y_pred), dim=1)``, train_SmaAtUNet.py:76): up4's last DS conv applies the n_classes-class
-        OutConv and the argmax in its epilogue (n_classes <= 32), so neither its 64-channel activation nor the logits reach
-        HBM.  Each class's logit there is the one-class fused OutConv's arithmetic, which sums in another order than the
-        unfused OutConv of the logits route: pixels whose top two logits lie within rounding of each other may pick the other
-        class.  Inference only; in train mode or under autograd the plain forward followed by the argmax kernel."""
-        if self.training or _needs_grad(self, x):
-            return _classes_of(self, x)
-        return self._serving(x, classes=True)
-
-    def forward_probs(self, x):
-        """``forward_serving``'s graph ending in the (B, n_classes, H, W) fp32 class probabilities, softmax over the logits'
-        channels (the reference's ``softmax(y_pred)``, train_SmaAtUNet.py:76): up4's last DS conv applies the n_classes-class
-        OutConv and the softmax in its epilogue (n_classes <= 32), so only the probabilities reach HBM; more classes take the
-        unfused convs, OutConv and the softmax kernel.  Inference only, with no gradient: in train mode or under autograd
-        the plain forward followed by the softmax kernel, under no_grad."""
-        if self.training or _needs_grad(self, x):
-            return _probs_of(self, x)
-        return self._serving(x, probs=True)
-
-    def _serving(self, x, classes=False, probs=False):
-        if self.training or _needs_grad(self, x):
-            return self.forward(x)
+    def _serving(self, x, head):
         skips, f = [], self.inc(x)
         for lvl in range(5):
             if lvl > 0:
@@ -113,12 +101,17 @@ class SmaAt_UNet(nn.Module):
             skip, gate = skips[3 - i]
             y = getattr(self, f"up{i + 1}")(y, skip, gate=gate)
         skip, gate = skips[0]
-        return self.up4(y, skip, outconv=self.outc, gate=gate, classes=classes, probs=probs)
+        return self.up4(y, skip, outconv=self.outc, gate=gate, head=head)
 
 
-class UNet(nn.Module):
+class UNet(_ServingForward):
     """The dense baseline of ``models/unet_precip_regression_lightning.py:7-38`` (the Lightning class without its training
-    plumbing): same attribute names (hence the reference's 128 state_dict keys with ``bilinear=True``) and forward order."""
+    plumbing): same attribute names (hence the reference's 128 state_dict keys with ``bilinear=True``) and forward order.
+
+    Its serving forward is bit for bit ``forward``'s logits and ``argmax_channels`` / ``softmax_channels`` of them.  With
+    ``ops.set_fused_dense_head(True)`` up4's last 3x3 conv applies the OutConv (and the argmax / softmax) in its epilogue, so
+    neither the 64-channel activation nor the logits reach HBM; by default (the faster route on an H100), and where the
+    epilogue does not take the shape ('fp32' mode, W % 4 != 0, more than 32 classes), the plain calls."""
 
     def __init__(self, n_channels, n_classes, bilinear=True):
         super().__init__()
@@ -135,58 +128,33 @@ class UNet(nn.Module):
         self.up4 = Up(128, 64, bilinear)
         self.outc = OutConv(64, n_classes)
 
+    def _to_up4(self, x):
+        """The encoder and up1-up3: up4's two inputs."""
+        x1 = self.inc(x)
+        x2 = self.down1(x1)
+        x3 = self.down2(x2)
+        x4 = self.down3(x3)
+        x5 = self.down4(x4)
+        x = self.up1(x5, x4)
+        x = self.up2(x, x3)
+        x = self.up3(x, x2)
+        return x, x1
+
     def forward(self, x):
-        x1 = self.inc(x)
-        x2 = self.down1(x1)
-        x3 = self.down2(x2)
-        x4 = self.down3(x3)
-        x5 = self.down4(x4)
-        x = self.up1(x5, x4)
-        x = self.up2(x, x3)
-        x = self.up3(x, x2)
-        x = self.up4(x, x1)
-        return self.outc(x)
+        return self.outc(self.up4(*self._to_up4(x)))
 
-    def forward_serving(self, x):
-        """``forward`` for ``engine.InferenceSession``, bit for bit ``forward``'s logits.  With ``ops.set_fused_dense_head(True)``
-        up4's last 3x3 conv applies the OutConv in its epilogue, so the 64-channel activation never reaches HBM; by default (the
-        faster route on an H100) and in train mode, under autograd, or where the epilogue does not take the shape ('fp32'
-        mode, W % 4 != 0, more than 32 classes), the plain calls."""
-        return self._serving(x)
-
-    def forward_classes(self, x):
-        """The (B, H, W) int64 class map of ``forward``'s logits (train_SmaAtUNet.py:76), bit for bit ``argmax_channels(forward(x))``:
-        with ``ops.set_fused_dense_head(True)`` up4's last conv applies the OutConv and the argmax in its epilogue, so neither its
-        activation nor the logits reach HBM.  Otherwise (see ``forward_serving``): the forward, then the argmax kernel."""
-        if self.training or _needs_grad(self, x):
-            return _classes_of(self, x)
-        return self._serving(x, classes=True)
-
-    def forward_probs(self, x):
-        """The class probabilities of ``forward``'s logits (train_SmaAtUNet.py:76), bit for bit ``softmax_channels(forward(x))``:
-        with ``ops.set_fused_dense_head(True)`` up4's last conv applies the OutConv and the softmax in its epilogue.  Otherwise:
-        the forward, then the softmax kernel.  Inference only, with no gradient."""
-        if self.training or _needs_grad(self, x):
-            return _probs_of(self, x)
-        return self._serving(x, probs=True)
-
-    def _serving(self, x, classes=False, probs=False):
-        if self.training or _needs_grad(self, x):
-            return self.forward(x)
-        x1 = self.inc(x)
-        x2 = self.down1(x1)
-        x3 = self.down2(x2)
-        x4 = self.down3(x3)
-        x5 = self.down4(x4)
-        x = self.up1(x5, x4)
-        x = self.up2(x, x3)
-        x = self.up3(x, x2)
-        return self.up4(x, x1, outconv=self.outc, classes=classes, probs=probs)
+    def _serving(self, x, head):
+        return self.up4(*self._to_up4(x), outconv=self.outc, head=head)
 
 
-class UNetAttention(nn.Module):
+class UNetAttention(_ServingForward):
     """``models/unet_precip_regression_lightning.py:41-83``: UNet with a CBAM on every skip (178 state_dict keys with
-    ``bilinear=True``).  ``downN`` runs on the un-attended map right after ``cbamN`` did, so the CBAM hands it its 2x2 max-pool."""
+    ``bilinear=True``).  ``downN`` runs on the un-attended map right after ``cbamN`` did, so the CBAM hands it its 2x2 max-pool.
+
+    Its serving forward is bit for bit ``forward``'s logits and ``argmax_channels`` / ``softmax_channels`` of them.  With
+    ``ops.set_fused_dense_head(True)`` up4's last 3x3 conv applies the OutConv (and the argmax / softmax) in its epilogue, so
+    neither the 64-channel activation nor the logits reach HBM; by default (the faster route on an H100), and where the
+    epilogue does not take the shape ('fp32' mode, W % 4 != 0, more than 32 classes), the plain calls."""
 
     def __init__(self, n_channels, n_classes, bilinear=True, reduction_ratio=16):
         super().__init__()
@@ -209,60 +177,25 @@ class UNetAttention(nn.Module):
         self.up4 = Up(128, 64, bilinear)
         self.outc = OutConv(64, n_classes)
 
+    def _to_up4(self, x):
+        """The encoder and up1-up3, in the reference's call order: up4's two inputs."""
+        x1 = self.inc(x)
+        x1Att = self.cbam1(x1)
+        x2 = self.down1(x1)
+        x2Att = self.cbam2(x2)
+        x3 = self.down2(x2)
+        x3Att = self.cbam3(x3)
+        x4 = self.down3(x3)
+        x4Att = self.cbam4(x4)
+        x5 = self.down4(x4)
+        x5Att = self.cbam5(x5)
+        x = self.up1(x5Att, x4Att)
+        x = self.up2(x, x3Att)
+        x = self.up3(x, x2Att)
+        return x, x1Att
+
     def forward(self, x):
-        x1 = self.inc(x)
-        x1Att = self.cbam1(x1)
-        x2 = self.down1(x1)
-        x2Att = self.cbam2(x2)
-        x3 = self.down2(x2)
-        x3Att = self.cbam3(x3)
-        x4 = self.down3(x3)
-        x4Att = self.cbam4(x4)
-        x5 = self.down4(x4)
-        x5Att = self.cbam5(x5)
-        x = self.up1(x5Att, x4Att)
-        x = self.up2(x, x3Att)
-        x = self.up3(x, x2Att)
-        x = self.up4(x, x1Att)
-        return self.outc(x)
+        return self.outc(self.up4(*self._to_up4(x)))
 
-    def forward_serving(self, x):
-        """``forward`` for ``engine.InferenceSession``, bit for bit ``forward``'s logits.  With ``ops.set_fused_dense_head(True)``
-        up4's last 3x3 conv applies the OutConv in its epilogue, so the 64-channel activation never reaches HBM; by default (the
-        faster route on an H100) and in train mode, under autograd, or where the epilogue does not take the shape ('fp32'
-        mode, W % 4 != 0, more than 32 classes), the plain calls."""
-        return self._serving(x)
-
-    def forward_classes(self, x):
-        """The (B, H, W) int64 class map of ``forward``'s logits (train_SmaAtUNet.py:76), bit for bit ``argmax_channels(forward(x))``:
-        with ``ops.set_fused_dense_head(True)`` up4's last conv applies the OutConv and the argmax in its epilogue, so neither its
-        activation nor the logits reach HBM.  Otherwise (see ``forward_serving``): the forward, then the argmax kernel."""
-        if self.training or _needs_grad(self, x):
-            return _classes_of(self, x)
-        return self._serving(x, classes=True)
-
-    def forward_probs(self, x):
-        """The class probabilities of ``forward``'s logits (train_SmaAtUNet.py:76), bit for bit ``softmax_channels(forward(x))``:
-        with ``ops.set_fused_dense_head(True)`` up4's last conv applies the OutConv and the softmax in its epilogue.  Otherwise:
-        the forward, then the softmax kernel.  Inference only, with no gradient."""
-        if self.training or _needs_grad(self, x):
-            return _probs_of(self, x)
-        return self._serving(x, probs=True)
-
-    def _serving(self, x, classes=False, probs=False):
-        if self.training or _needs_grad(self, x):
-            return self.forward(x)
-        x1 = self.inc(x)
-        x1Att = self.cbam1(x1)
-        x2 = self.down1(x1)
-        x2Att = self.cbam2(x2)
-        x3 = self.down2(x2)
-        x3Att = self.cbam3(x3)
-        x4 = self.down3(x3)
-        x4Att = self.cbam4(x4)
-        x5 = self.down4(x4)
-        x5Att = self.cbam5(x5)
-        x = self.up1(x5Att, x4Att)
-        x = self.up2(x, x3Att)
-        x = self.up3(x, x2Att)
-        return self.up4(x, x1Att, outconv=self.outc, classes=classes, probs=probs)
+    def _serving(self, x, head):
+        return self.up4(*self._to_up4(x), outconv=self.outc, head=head)

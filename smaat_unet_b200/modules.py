@@ -105,38 +105,39 @@ class DepthwiseSeparableConv(_CachingModule):
         """Whether the one-kernel depthwise->pointwise path takes this input (shape, alignment, arithmetic mode)."""
         return ops.dsconv_takes(x, x1, self.pointwise.weight.detach(), self.kernels_per_layer, stats=stats)
 
-    def run(self, x, x1=None, scale=None, shift=None, relu=False, in_scale=None, in_shift=None, stats=None, outconv=None):
-        """dw -> pw with the pw epilogue y = act(scale * acc + shift).  scale/shift None => (1, pointwise.bias)."""
+    def _operands(self, shift):
+        """What ``run``, ``run_head`` and ``run_cbam`` hand the kernels besides the input and the epilogue scale: the depthwise
+        bias, the epilogue shift (the pointwise bias where the caller gives none), the arithmetic mode and, in 'tf32x3', the
+        pointwise weight's cached tf32 split."""
         self._check()
         dw_b = self.depthwise.bias.detach() if self.depthwise.bias is not None else None
         if shift is None:
             shift = self.pointwise.bias.detach() if self.pointwise.bias is not None else None
         mode = ops.get_pointwise_mode()
-        split = self.pw_split() if mode == "tf32x3" else None
+        return dw_b, shift, mode, self.pw_split() if mode == "tf32x3" else None
+
+    def run(self, x, x1=None, scale=None, shift=None, relu=False, in_scale=None, in_shift=None, stats=None):
+        """dw -> pw with the pw epilogue y = act(scale * acc + shift).  scale/shift None => (1, pointwise.bias)."""
+        dw_b, shift, mode, split = self._operands(shift)
         if in_scale is None:
             # one kernel: the k*Cin-channel depthwise result never reaches HBM (where the shape allows)
             y = ops.dsconv(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(),
-                           scale, shift, relu, x1=x1, mode=mode, w_split=split, stats=stats, outconv=outconv)
+                           scale, shift, relu, x1=x1, mode=mode, w_split=split, stats=stats)
             if y is not None:
                 return y
-        if outconv is not None:
-            return None      # the caller runs this conv and the OutConv separately
         d = ops.dw3x3(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, x1=x1, in_scale=in_scale, in_shift=in_shift)
         return ops.pw1x1(d, self.pointwise.weight.detach(), scale, shift, relu, mode=mode, w_split=split, stats=stats)
 
-    def run_classify(self, x, scale, shift, relu, outconv, want_logits=False, probs=False):
-        """``run`` followed by OutConv(Cout -> K) and the channel argmax in the fused kernel's epilogue (``outconv=(weight (K, Cout[,1,1]),
-        bias or None)``): the (B, H, W) int64 class map [, the logits], or None where that kernel does not take the request.
-        ``probs=True``: the (B, K, H, W) softmax probabilities from that epilogue instead (``ops.dsconv_probs``)."""
-        self._check()
-        dw_b = self.depthwise.bias.detach() if self.depthwise.bias is not None else None
-        mode = ops.get_pointwise_mode()
-        split = self.pw_split() if mode == "tf32x3" else None
-        args = (x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(), scale, shift, relu,
-                outconv[0], outconv[1])
-        if probs:
-            return ops.dsconv_probs(*args, mode=mode, w_split=split)
-        return ops.dsconv_classify(*args, mode=mode, w_split=split, want_logits=want_logits)
+    def run_head(self, x, scale, shift, relu, outconv, head):
+        """``run`` followed by the OutConv ``outconv=(weight (K, Cout[,1,1]), bias or None)`` in the fused kernel's epilogue, ending
+        in ``head``: "logits" (one class: the (B, 1, H, W) logits, ``ops.dsconv``), "classes" (the (B, H, W) int64 class map of
+        the K-class logits, ``ops.dsconv_classify``) or "probs" (their (B, K, H, W) softmax probabilities, ``ops.dsconv_probs``).
+        None where that kernel does not take the request: the caller then runs this conv and the OutConv separately."""
+        dw_b, shift, mode, split = self._operands(shift)
+        args = (x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(), scale, shift, relu)
+        if head == "logits":
+            return ops.dsconv(*args, mode=mode, w_split=split, outconv=outconv)
+        return (ops.dsconv_probs if head == "probs" else ops.dsconv_classify)(*args, *outconv, mode=mode, w_split=split)
 
     def cbam_takes(self, x, x1=None, gate=False, pools=False) -> bool:
         """Whether ``run_cbam`` takes this input: the fused kernel with the serving forward's CBAM fusions."""
@@ -145,12 +146,7 @@ class DepthwiseSeparableConv(_CachingModule):
     def run_cbam(self, x, x1=None, scale=None, shift=None, relu=False, gate=None, pools=False):
         """``run`` in one fused kernel that reads x as the CBAM output (x * sc) * sa (``gate=(sc, sa)``) and / or also returns
         the channel gate's partial pools and the 2x2 max-pool of its output (``pools``): see ``ops.dsconv_cbam``."""
-        self._check()
-        dw_b = self.depthwise.bias.detach() if self.depthwise.bias is not None else None
-        if shift is None:
-            shift = self.pointwise.bias.detach() if self.pointwise.bias is not None else None
-        mode = ops.get_pointwise_mode()
-        split = self.pw_split() if mode == "tf32x3" else None
+        dw_b, shift, mode, split = self._operands(shift)
         return ops.dsconv_cbam(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(),
                                scale, shift, relu, x1=x1, mode=mode, w_split=split, gate=gate, pools=pools)
 
@@ -162,40 +158,54 @@ class DepthwiseSeparableConv(_CachingModule):
         return self.run(x)
 
 
-class DoubleConvDS(_CachingModule):
-    """models/unet_parts_depthwise_separable.py:10-39 -- (DS conv => BN => ReLU) * 2.
+# What a block call with an OutConv ends in: the OutConv's logits, their (B, H, W) int64 class map (the reference's
+# ``torch.argmax(softmax(y_pred), dim=1)``, train_SmaAtUNet.py:76) or their (B, K, H, W) softmax probabilities.
+HEADS = ("logits", "classes", "probs")
 
-    Eval mode runs 4 kernels: dw, pw(+folded BN +ReLU), dw, pw(+folded BN +ReLU).
-    """
 
-    def __init__(self, in_channels, out_channels, mid_channels=None, kernels_per_layer=1):
+def _check_head(head, outconv):
+    if head not in HEADS:
+        raise ValueError(f"smaat_unet_b200: head must be one of {HEADS}, got {head!r}")
+    if head != "logits" and outconv is None:
+        raise ValueError(f"smaat_unet_b200: head={head!r} needs the OutConv that produces the logits")
+
+
+def apply_head(module, x, head):
+    """``module(x)``'s logits (``head="logits"``), or their class map / probabilities from the channel argmax / softmax kernel,
+    with ``module`` run under no_grad: neither has a gradient.  The unfused end of every serving head (``OutConv.classes`` /
+    ``probs``, the blocks' and models' routes that do not fuse it, ``engine.InferenceSession`` for models without ``forward_*``)."""
+    if head == "logits":
+        return module(x)
+    with torch.no_grad():
+        logits = module(x)
+        return ops.argmax_channels(logits) if head == "classes" else ops.softmax_channels(logits)
+
+
+class _DoubleConvBase(_CachingModule):
+    """What DoubleConvDS and DoubleConv share: ``double_conv`` = (conv => BN => ReLU) * 2, its folded BatchNorm, and the routing
+    of a call to its eval fast path, to autograd / batch statistics, and to an OutConv head.  A subclass provides
+    ``_folded_conv`` (conv 0 or 3 with its folded BatchNorm and the ReLU), ``_unfolded`` (the block under autograd or batch
+    statistics) and ``_fused_last`` (the last conv with the OutConv and the head in its epilogue, or None)."""
+
+    def __init__(self, double_conv):
         super().__init__()
-        if not mid_channels:
-            mid_channels = out_channels
-        self.double_conv = nn.Sequential(
-            DepthwiseSeparableConv(in_channels, mid_channels, kernel_size=3, kernels_per_layer=kernels_per_layer, padding=1),
-            nn.BatchNorm2d(mid_channels),
-            nn.ReLU(inplace=True),
-            DepthwiseSeparableConv(mid_channels, out_channels, kernel_size=3, kernels_per_layer=kernels_per_layer, padding=1),
-            nn.BatchNorm2d(out_channels),
-            nn.ReLU(inplace=True),
-        )
-        self._fold = {}
+        self.double_conv = double_conv
+        self._drop_caches()
 
     def _drop_caches(self):
         self._fold = {}
 
     def _folded(self, idx):
-        """(scale, shift) of eval BatchNorm idx+1 folded with pointwise bias of DS conv idx; cached."""
-        ds, bn = self.double_conv[idx], self.double_conv[idx + 1]
-        pb = ds.pointwise.bias
-        src = (bn.weight, bn.bias, bn.running_mean, bn.running_var, pb)
+        """(scale, shift) of eval BatchNorm idx+1 folded with the bias of conv idx (a DS conv's pointwise bias); cached."""
+        conv, bn = self.double_conv[idx], self.double_conv[idx + 1]
+        cb = getattr(conv, "pointwise", conv).bias
+        src = (bn.weight, bn.bias, bn.running_mean, bn.running_var, cb)
         key = _versions(*src)
         hit = self._fold.get(idx)
         if hit is None or hit[0] != key:
             with torch.no_grad():
                 sc_sh = ops.bn_fold(bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var,
-                                    pb.detach() if pb is not None else None, bn.eps)
+                                    cb.detach() if cb is not None else None, bn.eps)
             self._fold[idx] = (key, sc_sh, _held(*src))
             hit = self._fold[idx]
         return hit[1]
@@ -206,75 +216,83 @@ class DoubleConvDS(_CachingModule):
         return not (_needs_grad(self, *inputs) or self.training
                     or any(not bn.track_running_stats or bn.running_mean is None for bn in bns))
 
-    def run(self, x, x1=None, outconv=None, gate=None, classes=False, probs=False):
-        """``outconv`` (an OutConv module with one class, inference only): fold it into the last kernel's epilogue and
-        return the logits -- the block's own output is then never materialised (models/SmaAt_UNet.py:55-56).
-        ``classes=True`` (with ``outconv`` of any class count): return the (B, H, W) int64 class map argmax_c OutConv(block(x))
-        instead, from the last kernel's epilogue where it takes the shape (``_run_classes``).  ``probs=True``: the same for the
-        (B, K, H, W) softmax probabilities of OutConv(block(x)) (no gradient).
-        ``gate=(sc, sa)``: x is the un-attended skip and the block's input is the CBAM output (x * sc) * sa, which the first
-        DS conv computes as it loads x (inference only; materialised first where that kernel does not take it)."""
-        ops._req(x, "input", 4)
-        if gate is not None and not (self._eval_folded(x, x1) and self.double_conv[0].cbam_takes(x, x1, gate=True)):
-            x, gate = ops.cbam_scale(x, gate[0], gate[1]), None
-        if classes or probs:
-            if outconv is None:
-                raise ValueError("DoubleConvDS.run(classes=True / probs=True) needs the OutConv that produces the logits")
-            return self._run_classes(x, x1, outconv, gate, probs=probs)
-        if outconv is not None:
-            y = self._run_with_outconv(x, x1, outconv, gate)
-            return y if y is not None else outconv(self.run(x, x1, gate=gate))
-        if _needs_grad(self, x, x1):
-            from .autograd import DoubleConvDSFn
-            return DoubleConvDSFn.run(self, x, x1)
-        bns = (self.double_conv[1], self.double_conv[4])
-        if self.training or any(not bn.track_running_stats or bn.running_mean is None for bn in bns):
-            from . import functional as Fn       # batch statistics (and running-stat update), no tape
-            return Fn.double_conv_fwd(self, x, x1)[0]
-        y = self._first_conv(x, x1, gate)
-        s1, t1 = self._folded(3)
-        return self.double_conv[3].run(y, scale=s1, shift=t1, relu=True)
+    def _plain(self, x, x1, gate=None):
+        """The block's own output."""
+        if self._eval_folded(x, x1):
+            return self._folded_conv(3, self._folded_conv(0, x, x1, gate))
+        return self._unfolded(x, x1)
 
-    def _first_conv(self, x, x1, gate):
-        s0, t0 = self._folded(0)
-        if gate is not None:
-            return self.double_conv[0].run_cbam(x, x1=x1, scale=s0, shift=t0, relu=True, gate=gate)
-        return self.double_conv[0].run(x, x1=x1, scale=s0, shift=t0, relu=True)
-
-    def _run_with_outconv(self, x, x1, outconv, gate=None):
-        bns = (self.double_conv[1], self.double_conv[4])
-        oc = outconv.conv
-        if (_needs_grad(self, x, x1) or _needs_grad(outconv, x) or self.training or oc.out_channels != 1
-                or any(not bn.track_running_stats or bn.running_mean is None for bn in bns)):
-            return None
-        y = self._first_conv(x, x1, gate)
-        s1, t1 = self._folded(3)
-        ob = oc.bias.detach() if oc.bias is not None else None
-        z = self.double_conv[3].run(y, scale=s1, shift=t1, relu=True, outconv=(oc.weight.detach(), ob))
-        if z is None:     # shape / mode not taken by the fused kernel: same two convs, OutConv as its own kernel
-            z = outconv(self.double_conv[3].run(y, scale=s1, shift=t1, relu=True))
-        return z
-
-    def _run_classes(self, x, x1, outconv, gate=None, probs=False):
-        """The class map of OutConv(block(x)), or with ``probs`` its softmax probabilities.  Eval fast path: the last DS conv
-        applies the K-class OutConv and the argmax / softmax in its epilogue (smaat_dsconv_classify_fwd / smaat_dsconv_probs_fwd),
-        so neither the block's output nor the logits reach HBM; where that kernel does not take the shape (K > 32, Cout > 128,
-        ...) the same two convs run, then OutConv and the channel argmax / softmax kernel.  Under autograd / batch statistics:
-        the plain block, OutConv and the argmax / softmax."""
-        head = outconv.probs if probs else outconv.classes
+    def _run_head(self, x, x1, outconv, head, gate=None):
+        """OutConv(block(x)) ending in ``head``.  Eval fast path: the first conv, then the last conv with the OutConv and the head
+        in its epilogue where ``_fused_last`` takes it, else the last conv and ``apply_head``.  Under autograd or batch
+        statistics: the plain block, then ``apply_head``."""
         if not (self._eval_folded(x, x1) and not _needs_grad(outconv, x)):
-            return head(self.run(x, x1, gate=gate))
-        y = self._first_conv(x, x1, gate)
-        s1, t1 = self._folded(3)
-        oc = outconv.conv
-        ob = oc.bias.detach() if oc.bias is not None else None
-        out = self.double_conv[3].run_classify(y, s1, t1, True, (oc.weight.detach(), ob), probs=probs)
-        if out is None:
-            out = head(self.double_conv[3].run(y, scale=s1, shift=t1, relu=True))
-        return out
+            return apply_head(outconv, self._plain(x, x1, gate), head)
+        y = self._folded_conv(0, x, x1, gate)
+        out = self._fused_last(y, outconv, head)
+        return out if out is not None else apply_head(outconv, self._folded_conv(3, y), head)
 
     def forward(self, x):
         return self.run(x)
+
+
+class DoubleConvDS(_DoubleConvBase):
+    """models/unet_parts_depthwise_separable.py:10-39 -- (DS conv => BN => ReLU) * 2.
+
+    Eval mode runs 4 kernels: dw, pw(+folded BN +ReLU), dw, pw(+folded BN +ReLU).
+    """
+
+    def __init__(self, in_channels, out_channels, mid_channels=None, kernels_per_layer=1):
+        if not mid_channels:
+            mid_channels = out_channels
+        super().__init__(nn.Sequential(
+            DepthwiseSeparableConv(in_channels, mid_channels, kernel_size=3, kernels_per_layer=kernels_per_layer, padding=1),
+            nn.BatchNorm2d(mid_channels),
+            nn.ReLU(inplace=True),
+            DepthwiseSeparableConv(mid_channels, out_channels, kernel_size=3, kernels_per_layer=kernels_per_layer, padding=1),
+            nn.BatchNorm2d(out_channels),
+            nn.ReLU(inplace=True),
+        ))
+
+    def run(self, x, x1=None, outconv=None, gate=None, head="logits"):
+        """``outconv`` (an OutConv module, inference only): return OutConv(block(x)) ending in ``head`` (``HEADS``) -- its logits,
+        their (B, H, W) int64 class map or their (B, K, H, W) softmax probabilities (no gradient).  In the eval fast path the
+        last kernel applies the OutConv and the head in its epilogue where it takes the shape (``_fused_last``), and the
+        block's own output is then never materialised (models/SmaAt_UNet.py:55-56).
+        ``gate=(sc, sa)``: x is the un-attended skip and the block's input is the CBAM output (x * sc) * sa, which the first
+        DS conv computes as it loads x (inference only; materialised first where that kernel does not take it)."""
+        _check_head(head, outconv)
+        ops._req(x, "input", 4)
+        if gate is not None and not (self._eval_folded(x, x1) and self.double_conv[0].cbam_takes(x, x1, gate=True)):
+            x, gate = ops.cbam_scale(x, gate[0], gate[1]), None
+        if outconv is not None:
+            return self._run_head(x, x1, outconv, head, gate)
+        return self._plain(x, x1, gate)
+
+    def _folded_conv(self, idx, x, x1=None, gate=None):
+        s, t = self._folded(idx)
+        if gate is not None:
+            return self.double_conv[idx].run_cbam(x, x1=x1, scale=s, shift=t, relu=True, gate=gate)
+        return self.double_conv[idx].run(x, x1=x1, scale=s, shift=t, relu=True)
+
+    def _unfolded(self, x, x1):
+        if _needs_grad(self, x, x1):
+            from .autograd import DoubleConvDSFn
+            return DoubleConvDSFn.run(self, x, x1)
+        from . import functional as Fn       # batch statistics (and running-stat update), no tape
+        return Fn.double_conv_fwd(self, x, x1)[0]
+
+    def _fused_last(self, y, outconv, head):
+        """The last DS conv with the OutConv and the head in its epilogue (smaat_dsconv_outconv_fwd, smaat_dsconv_classify_fwd,
+        smaat_dsconv_probs_fwd), or None where that kernel does not take the shape (K > 32, Cout > 128, ...).  Logits only for a
+        one-class OutConv: the K-class epilogue sums each logit in another order than the OutConv kernel, which would change
+        the logits ``InferenceSession`` serves (DESIGN section 9)."""
+        oc = outconv.conv
+        if head == "logits" and oc.out_channels != 1:
+            return None
+        s1, t1 = self._folded(3)
+        ob = oc.bias.detach() if oc.bias is not None else None
+        return self.double_conv[3].run_head(y, s1, t1, True, (oc.weight.detach(), ob), head)
 
 
 # The reference calls ``cbamN(x)`` and then ``downN(x)`` on the same un-attended map (models/SmaAt_UNet.py:42-50,
@@ -310,19 +328,13 @@ def _take_stashed_maxpool(x):
     return hit[2]
 
 
-class DownDS(nn.Module):
-    """models/unet_parts_depthwise_separable.py:42-53 -- MaxPool2d(2) then DoubleConvDS."""
-
-    def __init__(self, in_channels, out_channels, kernels_per_layer=1):
-        super().__init__()
-        self.maxpool_conv = nn.Sequential(
-            nn.MaxPool2d(2),
-            DoubleConvDS(in_channels, out_channels, kernels_per_layer=kernels_per_layer),
-        )
+class _Down(nn.Module):
+    """MaxPool2d(2) then the double conv ``maxpool_conv[1]``: DownDS and Down."""
 
     def forward(self, x, pooled=None):
         """``pooled``: MaxPool2d(2)(x) when the caller already has it.  Called plainly (``down(x)``, as the reference does)
-        it first looks for the 2x2 max-pool the preceding ``CBAM(x)`` call left behind (see ``CBAM.forward``)."""
+        it first looks for the 2x2 max-pool the preceding ``CBAM(x)`` call left behind (see ``CBAM.forward``): SmaAt-UNet's
+        ``cbamN(x)`` -> ``downN(x)`` (models/SmaAt_UNet.py:42-50), UNetAttention's (unet_precip_regression_lightning.py:68-77)."""
         if pooled is None:
             pooled = _take_stashed_maxpool(x)
         if pooled is None:
@@ -334,9 +346,30 @@ class DownDS(nn.Module):
         return self.maxpool_conv[1].run(pooled)
 
 
+class DownDS(_Down):
+    """models/unet_parts_depthwise_separable.py:42-53 -- MaxPool2d(2) then DoubleConvDS."""
+
+    def __init__(self, in_channels, out_channels, kernels_per_layer=1):
+        super().__init__()
+        self.maxpool_conv = nn.Sequential(
+            nn.MaxPool2d(2),
+            DoubleConvDS(in_channels, out_channels, kernels_per_layer=kernels_per_layer),
+        )
+
+
 class _TransposedUp(_CachingModule):
-    """ConvTranspose2d(Cin, Cin // 2, kernel_size=2, stride=2) + F.pad of Up / UpDS (``bilinear=False``): kernel = stride, so the
-    transposed conv is one wgmma pointwise GEMM to the 4 packed taps + a pixel shuffle (csrc/convt.cu)."""
+    """The upsample step of Up / UpDS: nn.Upsample(x2, bilinear, align_corners=True), or with ``bilinear=False``
+    ConvTranspose2d(Cin, Cin // 2, kernel_size=2, stride=2), then F.pad to the skip.  kernel = stride, so the transposed conv is
+    one wgmma pointwise GEMM to the 4 packed taps + a pixel shuffle (csrc/convt.cu)."""
+
+    def __init__(self, in_channels, bilinear):
+        super().__init__()
+        self.bilinear = bilinear
+        if bilinear:
+            self.up = nn.Upsample(scale_factor=2, mode="bilinear", align_corners=True)
+        else:
+            self.up = nn.ConvTranspose2d(in_channels, in_channels // 2, kernel_size=2, stride=2)
+        self._packed = None
 
     def _drop_caches(self):
         self._packed = None
@@ -365,6 +398,16 @@ class _TransposedUp(_CachingModule):
         t = ops.pw1x1(x1, wp, None, None, False, w_split=split)
         return ops.pixel_shuffle2_pad(t, up.bias.detach() if up.bias is not None else None, up.out_channels, Ho, Wo)
 
+    def _upsampled(self, x1, x2):
+        """x1 upsampled x2 and padded to x2's plane."""
+        Ho, Wo = x2.shape[2], x2.shape[3]
+        if not self.bilinear:
+            return self._up_transposed(x1, Ho, Wo)
+        if torch.is_grad_enabled() and x1.requires_grad:
+            from .autograd import Upsample2xPadFn
+            return Upsample2xPadFn.apply(x1, Ho, Wo)
+        return ops.upsample2x_pad(x1, Ho, Wo)
+
 
 class UpDS(_TransposedUp):
     """models/unet_parts_depthwise_separable.py:56-86 -- upsample x2, pad to the skip, concat, DoubleConvDS.
@@ -375,32 +418,18 @@ class UpDS(_TransposedUp):
     """
 
     def __init__(self, in_channels, out_channels, bilinear=True, kernels_per_layer=1):
-        super().__init__()
-        self.bilinear = bilinear
-        if bilinear:
-            self.up = nn.Upsample(scale_factor=2, mode="bilinear", align_corners=True)
-            self.conv = DoubleConvDS(in_channels, out_channels, in_channels // 2, kernels_per_layer=kernels_per_layer)
-        else:
-            self.up = nn.ConvTranspose2d(in_channels, in_channels // 2, kernel_size=2, stride=2)
-            self.conv = DoubleConvDS(in_channels, out_channels, kernels_per_layer=kernels_per_layer)
-        self._packed = None
+        super().__init__(in_channels, bilinear)
+        self.conv = DoubleConvDS(in_channels, out_channels, in_channels // 2 if bilinear else None, kernels_per_layer=kernels_per_layer)
 
-    def forward(self, x1, x2, outconv=None, gate=None, classes=False, probs=False):
+    def forward(self, x1, x2, outconv=None, gate=None, head="logits"):
         """``gate=(sc, sa)`` (serving forward, inference only): x2 is the un-attended skip, and the block reads the CBAM output
-        (x2 * sc) * sa as it loads it (DoubleConvDS.run).  ``classes=True`` with ``outconv``: the class map of the OutConv's logits;
-        ``probs=True``: their softmax probabilities."""
-        if not self.bilinear:
-            return self.conv.run(x2, x1=self._up_transposed(x1, x2.shape[2], x2.shape[3]), outconv=outconv, gate=gate, classes=classes,
-                                 probs=probs)
-        if torch.is_grad_enabled() and x1.requires_grad:
-            from .autograd import Upsample2xPadFn
-            up = Upsample2xPadFn.apply(x1, x2.shape[2], x2.shape[3])
-        else:
-            up = ops.upsample2x_pad(x1, x2.shape[2], x2.shape[3])
-        return self.conv.run(x2, x1=up, outconv=outconv, gate=gate, classes=classes, probs=probs)
+        (x2 * sc) * sa as it loads it (DoubleConvDS.run).  ``outconv``: the OutConv's logits of the block's output, or with
+        ``head="classes"`` / ``"probs"`` their class map / softmax probabilities."""
+        _check_head(head, outconv)
+        return self.conv.run(x2, x1=self._upsampled(x1, x2), outconv=outconv, gate=gate, head=head)
 
 
-class DoubleConv(_CachingModule):
+class DoubleConv(_DoubleConvBase):
     """models/unet_parts.py:8-25 -- (Conv2d 3x3 => BN => ReLU) * 2, the dense block of UNet / UNetAttention.
 
     Eval mode runs 2 kernels: conv3x3 (+folded BN +ReLU) twice (csrc/conv3x3_tc.cu; the exact CUDA-core kernel in 'fp32'
@@ -408,22 +437,19 @@ class DoubleConv(_CachingModule):
     """
 
     def __init__(self, in_channels, out_channels, mid_channels=None):
-        super().__init__()
         if not mid_channels:
             mid_channels = out_channels
-        self.double_conv = nn.Sequential(
+        super().__init__(nn.Sequential(
             nn.Conv2d(in_channels, mid_channels, kernel_size=3, padding=1),
             nn.BatchNorm2d(mid_channels),
             nn.ReLU(inplace=True),
             nn.Conv2d(mid_channels, out_channels, kernel_size=3, padding=1),
             nn.BatchNorm2d(out_channels),
             nn.ReLU(inplace=True),
-        )
-        self._fold = {}
-        self._packed = {}
+        ))
 
     def _drop_caches(self):
-        self._fold = {}
+        super()._drop_caches()
         self._packed = {}
 
     def _check(self):
@@ -458,98 +484,53 @@ class DoubleConv(_CachingModule):
         return ops.conv3x3(x, wp, self.double_conv[idx].out_channels, scale, shift, relu, x1=x1,
                            w_split=(hi, lo) if hi is not None else None, stats=stats)
 
-    def _folded(self, idx):
-        """(scale, shift) of eval BatchNorm idx+1 folded with the bias of conv idx; cached."""
-        conv, bn = self.double_conv[idx], self.double_conv[idx + 1]
-        src = (bn.weight, bn.bias, bn.running_mean, bn.running_var, conv.bias)
-        key = _versions(*src)
-        hit = self._fold.get(idx)
-        if hit is None or hit[0] != key:
-            with torch.no_grad():
-                sc_sh = ops.bn_fold(bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var,
-                                    conv.bias.detach() if conv.bias is not None else None, bn.eps)
-            self._fold[idx] = (key, sc_sh, _held(*src))
-            hit = self._fold[idx]
-        return hit[1]
-
-    def run(self, x, x1=None, outconv=None, classes=False, probs=False):
-        """``outconv`` (an OutConv module): return OutConv(block(x)), its logits.  ``classes=True``: the (B, H, W) int64 class map
-        of those logits instead; ``probs=True``: their (B, K, H, W) softmax probabilities (no gradient).  In eval mode without
-        autograd the last conv applies the OutConv and the argmax / softmax in its epilogue where it takes the shape
-        (``_run_head``): the block's output is then never written, and the result is bit for bit that of the separate calls."""
+    def run(self, x, x1=None, outconv=None, head="logits"):
+        """``outconv`` (an OutConv module): return OutConv(block(x)) ending in ``head`` (``HEADS``) -- its logits, their
+        (B, H, W) int64 class map or their (B, K, H, W) softmax probabilities (no gradient).  In eval mode without autograd the
+        last conv applies the OutConv and the argmax / softmax in its epilogue where it takes the shape (``_fused_last``): the
+        block's output is then never written, and the result is bit for bit that of the separate calls."""
+        _check_head(head, outconv)
         ops._req(x, "input", 4)
         if x1 is not None:
             ops._req(x1, "input", 4)
         self._check()
-        if classes or probs or outconv is not None:
-            if outconv is None:
-                raise ValueError("DoubleConv.run(classes=True / probs=True) needs the OutConv that produces the logits")
-            out = self._run_head(x, x1, outconv, classes, probs)
-            if out is not None:
-                return out
-            head = outconv.probs if probs else (outconv.classes if classes else outconv)
-            return head(self.run(x, x1))
+        if outconv is not None:
+            return self._run_head(x, x1, outconv, head)
+        return self._plain(x, x1)
+
+    def _folded_conv(self, idx, x, x1=None, gate=None):
+        s, t = self._folded(idx)
+        return self.conv(idx, x, x1, scale=s, shift=t, relu=True)
+
+    def _unfolded(self, x, x1):
         if _needs_grad(self, x, x1):
             from .autograd import DoubleConvFn
             return DoubleConvFn.run(self, x, x1)
-        bns = (self.double_conv[1], self.double_conv[4])
-        if self.training or any(not bn.track_running_stats or bn.running_mean is None for bn in bns):
-            from . import functional as Fn       # batch statistics (and running-stat update), no tape
-            return Fn.dense_double_conv_fwd(self, x, x1)[0]
-        s0, t0 = self._folded(0)
-        y = self.conv(0, x, x1, scale=s0, shift=t0, relu=True)
-        s1, t1 = self._folded(3)
-        return self.conv(3, y, scale=s1, shift=t1, relu=True)
+        from . import functional as Fn       # batch statistics (and running-stat update), no tape
+        return Fn.dense_double_conv_fwd(self, x, x1)[0]
 
-    def _run_head(self, x, x1, outconv, classes, probs):
-        """The eval fast path of ``run`` with an OutConv: the first conv as usual, then the last conv with the K-class OutConv
-        and the argmax / softmax in its epilogue (smaat_conv3x3_classify_fwd / smaat_conv3x3_probs_fwd).  None where that
-        path does not apply (train mode, batch statistics, autograd, 'fp32', or a shape the epilogue does not take: Cout > 64,
-        K > 32, W % 4 != 0, ...), and unless ops.set_fused_dense_head(True): the caller then runs the separate calls."""
-        bns = (self.double_conv[1], self.double_conv[4])
-        if (not ops.fused_dense_head() or _needs_grad(self, x, x1) or _needs_grad(outconv, x) or self.training
-                or any(not bn.track_running_stats or bn.running_mean is None for bn in bns)):
+    def _fused_last(self, y, outconv, head):
+        """The last conv with the OutConv and the head in its epilogue (smaat_conv3x3_classify_fwd / smaat_conv3x3_probs_fwd),
+        or None: unless ops.set_fused_dense_head(True), and where the epilogue does not take the shape ('fp32', Cout > 64,
+        K > 32, W % 4 != 0, ...)."""
+        if not ops.fused_dense_head():
             return None
-        c3, oc = self.double_conv[3], outconv.conv
-        s0, t0 = self._folded(0)
-        y = self.conv(0, x, x1, scale=s0, shift=t0, relu=True)
         s1, t1 = self._folded(3)
         wp, hi, lo = self.packed(3, y.shape[1])
+        oc = outconv.conv
+        args = (y, wp, self.double_conv[3].out_channels, s1, t1, True, oc.weight.detach(), oc.bias.detach() if oc.bias is not None else None)
         split = (hi, lo) if hi is not None else None
-        ob = oc.bias.detach() if oc.bias is not None else None
-        args = (y, wp, c3.out_channels, s1, t1, True, oc.weight.detach(), ob)
-        if probs:
-            out = ops.conv3x3_probs(*args, w_split=split)
-        else:
-            out = ops.conv3x3_classify(*args, w_split=split, want_logits=not classes, want_classes=classes)
-        if out is None:           # the last conv's shape is not taken: the same conv, OutConv and argmax / softmax apart
-            out = self.conv(3, y, scale=s1, shift=t1, relu=True)
-            out = outconv.probs(out) if probs else (outconv.classes(out) if classes else outconv(out))
-        return out
-
-    def forward(self, x):
-        return self.run(x)
+        if head == "probs":
+            return ops.conv3x3_probs(*args, w_split=split)
+        return ops.conv3x3_classify(*args, w_split=split, want_logits=head == "logits", want_classes=head == "classes")
 
 
-class Down(nn.Module):
+class Down(_Down):
     """models/unet_parts.py:28-36 -- MaxPool2d(2) then DoubleConv."""
 
     def __init__(self, in_channels, out_channels):
         super().__init__()
         self.maxpool_conv = nn.Sequential(nn.MaxPool2d(2), DoubleConv(in_channels, out_channels))
-
-    def forward(self, x, pooled=None):
-        """``pooled``: MaxPool2d(2)(x) when the caller already has it; a plain call takes the one a preceding ``CBAM(x)``
-        left behind (UNetAttention's ``cbamN(x)`` -> ``downN(x)``, unet_precip_regression_lightning.py:68-77), as DownDS does."""
-        if pooled is None:
-            pooled = _take_stashed_maxpool(x)
-        if pooled is None:
-            if _needs_grad(self, x):
-                from .autograd import MaxPool2Fn
-                pooled = MaxPool2Fn.apply(x) if x.requires_grad else ops.maxpool2(x)
-            else:
-                pooled = ops.maxpool2(ops._dense(x, "input"))
-        return self.maxpool_conv[1].run(pooled)
 
 
 class Up(_TransposedUp):
@@ -558,29 +539,16 @@ class Up(_TransposedUp):
     The concat is never materialised: the first 3x3 conv reads [skip, up] as a virtual concat."""
 
     def __init__(self, in_channels, out_channels, bilinear=True):
-        super().__init__()
-        self.bilinear = bilinear
-        if bilinear:
-            self.up = nn.Upsample(scale_factor=2, mode="bilinear", align_corners=True)
-            self.conv = DoubleConv(in_channels, out_channels, in_channels // 2)
-        else:
-            self.up = nn.ConvTranspose2d(in_channels, in_channels // 2, kernel_size=2, stride=2)
-            self.conv = DoubleConv(in_channels, out_channels)
-        self._packed = None
+        super().__init__(in_channels, bilinear)
+        self.conv = DoubleConv(in_channels, out_channels, in_channels // 2 if bilinear else None)
 
-    def forward(self, x1, x2, outconv=None, classes=False, probs=False):
-        """``outconv``: return OutConv's logits of the block's output; with ``classes=True`` their class map, with ``probs=True``
-        their softmax probabilities (``DoubleConv.run``)."""
+    def forward(self, x1, x2, outconv=None, head="logits"):
+        """``outconv``: return OutConv's logits of the block's output; with ``head="classes"`` / ``"probs"`` their class map /
+        softmax probabilities (``DoubleConv.run``)."""
+        _check_head(head, outconv)
         ops._req(x1, "x1", 4)
         ops._req(x2, "x2", 4)
-        if not self.bilinear:
-            return self.conv.run(x2, x1=self._up_transposed(x1, x2.shape[2], x2.shape[3]), outconv=outconv, classes=classes, probs=probs)
-        if torch.is_grad_enabled() and x1.requires_grad:
-            from .autograd import Upsample2xPadFn
-            up = Upsample2xPadFn.apply(x1, x2.shape[2], x2.shape[3])
-        else:
-            up = ops.upsample2x_pad(x1, x2.shape[2], x2.shape[3])
-        return self.conv.run(x2, x1=up, outconv=outconv, classes=classes, probs=probs)
+        return self.conv.run(x2, x1=self._upsampled(x1, x2), outconv=outconv, head=head)
 
 
 class OutConv(nn.Module):
@@ -599,14 +567,12 @@ class OutConv(nn.Module):
     def classes(self, x):
         """The (B, H, W) int64 class map argmax_c OutConv(x) (the reference's ``torch.argmax(softmax(y_pred), dim=1)``,
         train_SmaAtUNet.py:76): this module's logits, then the channel argmax kernel.  Inference only: a class map has no gradient."""
-        with torch.no_grad():
-            return ops.argmax_channels(self(x))
+        return apply_head(self, x, "classes")
 
     def probs(self, x):
         """The (B, K, H, W) class probabilities softmax_c OutConv(x) (the reference's ``softmax(y_pred)``, train_SmaAtUNet.py:76):
         this module's logits, then the channel softmax kernel.  Inference only: no gradient."""
-        with torch.no_grad():
-            return ops.softmax_channels(self(x))
+        return apply_head(self, x, "probs")
 
 
 class Flatten(nn.Module):

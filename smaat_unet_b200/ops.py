@@ -123,16 +123,45 @@ def _nchw_bstride(t, name):
     return t, Cc * H * W
 
 
+def _concat_operands(x, x1):
+    """The virtual concat [x, x1] as the C ABI reads it: (x, its batch stride, x1 or None, C1, x1's batch stride)."""
+    x, bs0 = _nchw_bstride(x, "x")
+    if x1 is None:
+        return x, bs0, None, 0, 0
+    x1, bs1 = _nchw_bstride(x1, "x1")
+    assert x1.shape[0] == x.shape[0] and x1.shape[2:] == x.shape[2:], "concat inputs must agree in B, H, W"
+    return x, bs0, x1, x1.shape[1], bs1
+
+
+def _pw_matrix(pw_weight, k=None, Cin=None):
+    """The pointwise weight (Cout, k Cin[, 1, 1]) as the GEMM's (Cout, k Cin) matrix, checked against k * Cin when given."""
+    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
+    assert k is None or w2d.shape[1] == k * Cin, f"pointwise weight {tuple(pw_weight.shape)} does not match k*Cin={k * Cin}"
+    return w2d
+
+
+def _tf32_split(w, m, w_split):
+    """(w, None), or in mode 2 ('tf32x3') w's tf32 (hi, lo): the caller's cached ``w_split``, else split now."""
+    if m != 2:
+        return w, None
+    return w_split if w_split is not None else split_tf32(w)
+
+
+def _outconv_operands(oc_weight, oc_bias, Cout):
+    """The K-class OutConv of a fused epilogue: (weight (K, Cout[,1,1]), bias (K) or None, K), checked against Cout."""
+    ow = _dense(oc_weight, "outconv.weight")
+    K = ow.shape[0]
+    assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
+    ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
+    assert ob is None or ob.numel() == K, f"OutConv bias {tuple(oc_bias.shape)} does not match K={K}"
+    return ow, ob, K
+
+
 # ---------------------------------------------------------------------------------------------
 def dw3x3(x, weight, bias, k, x1=None, in_scale=None, in_shift=None, loader=0):
     """Depthwise 3x3/pad 1 over the virtual concat [x, x1] (layers.py:38-44; parts_ds.py:85)."""
-    x, bs0 = _nchw_bstride(x, "x")
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        assert x1.shape[0] == B and x1.shape[2:] == x.shape[2:], "concat inputs must agree in B, H, W"
-        C1 = x1.shape[1]
     w = _dense(weight, "depthwise.weight")
     assert w.numel() == k * (C0 + C1) * 9, f"depthwise weight {tuple(w.shape)} does not match k*(C0+C1)={k * (C0 + C1)}"
     y = torch.empty((B, k * (C0 + C1), H, W), device=x.device, dtype=torch.float32)
@@ -161,7 +190,7 @@ def pw1x1(x, weight, scale, shift, relu, mode=None, w_split=None, stats=None, ou
     """
     x = _dense(x, "x")
     B, K, H, W = x.shape
-    w2d = _dense(weight, "pointwise.weight").view(weight.shape[0], -1)
+    w2d = _pw_matrix(weight)
     Cout = w2d.shape[0]
     assert w2d.shape[1] == K, f"pointwise weight {tuple(weight.shape)} does not match K={K}"
     P = H * W
@@ -172,14 +201,11 @@ def pw1x1(x, weight, scale, shift, relu, mode=None, w_split=None, stats=None, ou
         out, ybs = _nchw_bstride(out, "out")
     mode = mode or _pw_mode
     m = PW_MODES[mode]
-    wlo = None
     # the tensor-core kernel stages an epilogue affine for at most 512 output channels (SmaAt_UNet(bilinear=False)'s
     # 1024-channel bottleneck has more)
     if m != 0 and (not tc_eligible(x, w2d) or (Cout > 512 and (scale is not None or shift is not None))):
         m = 0
-    if m == 2:
-        hi, wlo = w_split if w_split is not None else split_tf32(w2d)
-        w2d = hi
+    w2d, wlo = _tf32_split(w2d, m, w_split)
     _call(f"smaat_pw1x1_fwd[K{K}_N{Cout}_P{P}]", 4 * B * P * (K + Cout) + 4 * K * Cout, 2 * B * P * K * Cout, _lib.load().smaat_pw1x1_fwd, _ptr(x), _ptr(w2d), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(out), ybs, _ptr(stats),
                                            B, K, Cout, P, int(bool(relu)), m, _stream())
     return out
@@ -205,12 +231,8 @@ def dsconv_takes(x, x1, pw_weight, k, mode=None, stats=False) -> bool:
     mode = mode or _pw_mode
     if not _fuse_ds or PW_MODES[mode] == 0:
         return False
-    x, bs0 = _nchw_bstride(x, "x")
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        C1 = x1.shape[1]
-    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
+    w2d = _pw_matrix(pw_weight)
     return bool(_lib.load().smaat_dsconv_eligible2(_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2], x.shape[3], k, w2d.shape[0], int(bool(stats))))
 
 
@@ -220,12 +242,8 @@ def dsconv_cbam_takes(x, x1, pw_weight, k, gate=False, pools=False, mode=None) -
     mode = mode or _pw_mode
     if not _fuse_ds or PW_MODES[mode] == 0:
         return False
-    x, bs0 = _nchw_bstride(x, "x")
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        C1 = x1.shape[1]
-    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
+    w2d = _pw_matrix(pw_weight)
     return bool(_lib.load().smaat_dsconv_cbam_eligible(_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2], x.shape[3], k,
                                                        w2d.shape[0], PW_MODES[mode], int(bool(gate)), int(bool(pools))))
 
@@ -237,19 +255,12 @@ def dsconv_cbam(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None
     mode = mode or _pw_mode
     if not dsconv_cbam_takes(x, x1, pw_weight, k, gate is not None, pools, mode):
         raise RuntimeError("smaat_unet_b200: dsconv_cbam called on a request the fused kernel does not take (check dsconv_cbam_takes)")
-    x, bs0 = _nchw_bstride(x, "x")
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        C1 = x1.shape[1]
-    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
+    Cin = C0 + C1
+    w2d, wlo = _tf32_split(_pw_matrix(pw_weight, k, Cin), PW_MODES[mode], w_split)
     Cout, K = w2d.shape
-    assert K == k * (C0 + C1), f"pointwise weight {tuple(pw_weight.shape)} does not match k*Cin={k * (C0 + C1)}"
     lib = _lib.load()
-    wlo = None
-    if PW_MODES[mode] == 2:
-        w2d, wlo = w_split if w_split is not None else split_tf32(w2d)
     sc = sa = None
     if gate is not None:
         sc, sa = _dense(gate[0], "gate sc"), _dense(gate[1], "gate sa")
@@ -261,7 +272,6 @@ def dsconv_cbam(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None
         pmax = torch.empty_like(psum)
         pooled = torch.empty((B, Cout, H // 2, W // 2), device=x.device, dtype=torch.float32)
     y = torch.empty((B, Cout, H, W), device=x.device, dtype=torch.float32)
-    Cin = C0 + C1
     extra = (4 * B * H * W * C0 if gate is not None else 0) + (4 * B * Cout * (H // 2) * (W // 2) + 8 * psum.numel() if pools else 0)
     _call(f"smaat_dsconv_fwd[C{Cin}_N{Cout}_S{H}]",
           4 * B * H * W * (Cin + Cout) + 4 * K * Cout + extra, 2 * B * H * W * K * (Cout + 9),
@@ -276,27 +286,17 @@ def dsconv(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, mod
     does not take this shape/mode (caller then runs dw3x3 + pw1x1).  ``outconv=(weight (1, Cout[,1,1]), bias or None)``
     appends the 1-class OutConv in the epilogue and returns the (B, 1, H, W) logits instead of the activation."""
     mode = mode or _pw_mode
-    if not _fuse_ds or PW_MODES[mode] == 0:
+    if not dsconv_takes(x, x1, pw_weight, k, mode, stats=stats is not None):
         return None
-    x, bs0 = _nchw_bstride(x, "x")
+    if outconv is not None and pw_weight.shape[0] > 128:     # the fused OutConv needs all channels in one pass (smaat_dsconv_outconv_fwd)
+        return None
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        C1 = x1.shape[1]
-    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
-    Cout, K = w2d.shape
-    assert K == k * (C0 + C1), f"pointwise weight {tuple(pw_weight.shape)} does not match k*Cin={k * (C0 + C1)}"
-    lib = _lib.load()
-    if not lib.smaat_dsconv_eligible2(_ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(w2d), H, W, k, Cout, int(stats is not None)):
-        return None
-    if outconv is not None and Cout > 128:     # the fused OutConv needs all channels in one pass (smaat_dsconv_outconv_fwd)
-        return None
-    wlo = None
-    if PW_MODES[mode] == 2:
-        w2d, wlo = w_split if w_split is not None else split_tf32(w2d)
-    dw_w = _dense(dw_weight, "depthwise.weight")
     Cin = C0 + C1
+    w2d, wlo = _tf32_split(_pw_matrix(pw_weight, k, Cin), PW_MODES[mode], w_split)
+    Cout, K = w2d.shape
+    lib = _lib.load()
+    dw_w = _dense(dw_weight, "depthwise.weight")
     if outconv is not None:
         ow, ob = outconv
         assert ow.numel() == Cout and stats is None, "fused OutConv: one class over the block's Cout channels, no batch statistics"
@@ -330,12 +330,8 @@ def dsconv_classify_takes(x, x1, pw_weight, k, n_classes, mode=None) -> bool:
     mode = mode or _pw_mode
     if not _fuse_ds or not _fuse_classify or PW_MODES[mode] == 0:
         return False
-    x, bs0 = _nchw_bstride(x, "x")
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        C1 = x1.shape[1]
-    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
+    w2d = _pw_matrix(pw_weight)
     return bool(_lib.load().smaat_dsconv_classify_eligible(_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2], x.shape[3],
                                                            k, w2d.shape[0], int(n_classes), PW_MODES[mode]))
 
@@ -346,45 +342,8 @@ def dsconv_classify(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_
     (smaat_dsconv_classify_fwd).  oc_weight (K, Cout[,1,1]), oc_bias (K) or None.  Returns the (B, H, W) int64 class map, or
     (classes, (B, K, H, W) logits) with ``want_logits``; class j's logits are bit for bit those of ``dsconv(..., outconv=(oc_weight[j],
     oc_bias[j]))``.  Returns None where ``dsconv_classify_takes`` is False (the caller then runs the layers apart)."""
-    mode = mode or _pw_mode
-    K = _dense(oc_weight, "outconv.weight").shape[0]
-    if not dsconv_classify_takes(x, x1, pw_weight, k, K, mode):
-        return None
-    x, bs0, x1, C1, bs1, w2d, wlo, ow, ob = _k_class_operands(x, x1, k, pw_weight, oc_weight, oc_bias, mode, w_split)
-    B, C0, H, W = x.shape
-    Cout, Kd = w2d.shape
-    classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64)
-    logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
-    Cin = C0 + C1
-    _call(f"smaat_dsconv_classify_fwd[C{Cin}_N{Cout}_K{K}_S{H}]",
-          4 * B * H * W * (Cin + (K if want_logits else 0) + 2) + 4 * Kd * Cout, 2 * B * H * W * (Kd * (Cout + 9) + K * Cout),
-          _lib.load().smaat_dsconv_classify_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(_dense(dw_weight, "depthwise.weight")),
-          _ptr(dw_bias), _ptr(w2d), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, _ptr(logits), _ptr(classes),
-          B, H, W, k, Cout, int(bool(relu)), PW_MODES[mode], _stream())
-    return (classes, logits) if want_logits else classes
-
-
-def _k_class_operands(x, x1, k, pw_weight, oc_weight, oc_bias, mode, w_split):
-    """The checked operands of the K-class epilogue entries (smaat_dsconv_classify_fwd, smaat_dsconv_probs_fwd):
-    (x, its batch stride, x1, C1, x1's batch stride, pointwise weight (Cout, k*Cin) [tf32 hi], its tf32 lo or None,
-    OutConv weight, OutConv bias or None)."""
-    x, bs0 = _nchw_bstride(x, "x")
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        C1 = x1.shape[1]
-    w2d = _dense(pw_weight, "pointwise.weight").view(pw_weight.shape[0], -1)
-    Cout, Kd = w2d.shape
-    assert Kd == k * (x.shape[1] + C1), f"pointwise weight {tuple(pw_weight.shape)} does not match k*Cin={k * (x.shape[1] + C1)}"
-    ow = _dense(oc_weight, "outconv.weight")
-    K = ow.shape[0]
-    assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
-    ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
-    assert ob is None or ob.numel() == K, f"OutConv bias {tuple(oc_bias.shape)} does not match K={K}"
-    wlo = None
-    if PW_MODES[mode] == 2:
-        w2d, wlo = w_split if w_split is not None else split_tf32(w2d)
-    return x, bs0, x1, C1, bs1, w2d, wlo, ow, ob
+    return _dsconv_head(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, False,
+                        want_logits)
 
 
 def dsconv_probs(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, x1=None, mode=None, w_split=None):
@@ -392,21 +351,38 @@ def dsconv_probs(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_wei
     (smaat_dsconv_probs_fwd): the (B, K, H, W) fp32 probabilities, bit for bit ``softmax_channels`` of the logits
     ``dsconv_classify(..., want_logits=True)`` returns.  Inference only.  Returns None where ``dsconv_classify_takes`` is
     False (the caller then runs the layers apart)."""
+    return _dsconv_head(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, True)
+
+
+def _dsconv_head(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, probs,
+                 want_logits=False):
+    """``dsconv_classify`` (smaat_dsconv_classify_fwd) or, with ``probs``, ``dsconv_probs`` (smaat_dsconv_probs_fwd)."""
     mode = mode or _pw_mode
     K = _dense(oc_weight, "outconv.weight").shape[0]
     if not dsconv_classify_takes(x, x1, pw_weight, k, K, mode):
         return None
-    x, bs0, x1, C1, bs1, w2d, wlo, ow, ob = _k_class_operands(x, x1, k, pw_weight, oc_weight, oc_bias, mode, w_split)
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
-    Cout, Kd = w2d.shape
-    probs = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32)
     Cin = C0 + C1
-    _call(f"smaat_dsconv_probs_fwd[C{Cin}_N{Cout}_K{K}_S{H}]",
-          4 * B * H * W * (Cin + K) + 4 * Kd * Cout, 2 * B * H * W * (Kd * (Cout + 9) + 2 * K * Cout),
-          _lib.load().smaat_dsconv_probs_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(_dense(dw_weight, "depthwise.weight")),
-          _ptr(dw_bias), _ptr(w2d), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, _ptr(probs),
-          B, H, W, k, Cout, int(bool(relu)), PW_MODES[mode], _stream())
-    return probs
+    w2d = _pw_matrix(pw_weight, k, Cin)
+    Cout, Kd = w2d.shape
+    ow, ob, K = _outconv_operands(oc_weight, oc_bias, Cout)
+    w2d, wlo = _tf32_split(w2d, PW_MODES[mode], w_split)
+    lib = _lib.load()
+    if probs:
+        out = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32)
+        name, fn, outs, written = "smaat_dsconv_probs_fwd", lib.smaat_dsconv_probs_fwd, (_ptr(out),), K
+    else:
+        classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64)
+        logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
+        out = (classes, logits) if want_logits else classes
+        name, fn, outs, written = ("smaat_dsconv_classify_fwd", lib.smaat_dsconv_classify_fwd, (_ptr(logits), _ptr(classes)),
+                                   (K if want_logits else 0) + 2)
+    _call(f"{name}[C{Cin}_N{Cout}_K{K}_S{H}]",
+          4 * B * H * W * (Cin + written) + 4 * Kd * Cout, 2 * B * H * W * (Kd * (Cout + 9) + (2 if probs else 1) * K * Cout),
+          fn, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(_dense(dw_weight, "depthwise.weight")), _ptr(dw_bias), _ptr(w2d), _ptr(wlo),
+          _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, *outs, B, H, W, k, Cout, int(bool(relu)), PW_MODES[mode], _stream())
+    return out
 
 
 def softmax_channels(x):
@@ -460,11 +436,7 @@ def conv3x3_takes(x, x1, wp, Cout, mode=None) -> bool:
     mode = mode or _pw_mode
     if PW_MODES[mode] == 0:
         return False
-    x, bs0 = _nchw_bstride(x, "x")
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        C1 = x1.shape[1]
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     return bool(_lib.load().smaat_conv3x3_tc_eligible(_ptr(x), bs0, _ptr(x1), C1, bs1, _ptr(wp), x.shape[3], Cout))
 
 
@@ -473,22 +445,15 @@ def conv3x3(x, wp, Cout, scale, shift, relu, x1=None, mode=None, w_split=None, s
 
     wp: ``conv3x3_pack_weight`` of the weight; w_split: its cached tf32 (hi, lo) for 'tf32x3'.  Shapes the tensor-core kernel
     does not take (W % 4 != 0, Cout < 8) run on the exact CUDA-core kernel."""
-    x, bs0 = _nchw_bstride(x, "x")
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        assert x1.shape[0] == B and x1.shape[2:] == x.shape[2:], "concat inputs must agree in B, H, W"
-        C1 = x1.shape[1]
     assert wp.shape == (Cout, 9 * (_pad32(C0) + _pad32(C1))), f"packed weight {tuple(wp.shape)} does not match Cin={C0}+{C1}"
     mode = mode or _pw_mode
     m = PW_MODES[mode]
     lib = _lib.load()
     if m != 0 and not lib.smaat_conv3x3_tc_eligible(_ptr(x), bs0, _ptr(x1), C1, bs1, _ptr(wp), W, Cout):
         m = 0
-    wlo = None
-    if m == 2:
-        wp, wlo = w_split if w_split is not None else split_tf32(wp)
+    wp, wlo = _tf32_split(wp, m, w_split)
     y = torch.empty((B, Cout, H, W), device=x.device, dtype=torch.float32)
     name = "smaat_conv3x3_fwd" if m else "smaat_conv3x3_fwd_simt"
     Cin = C0 + C1
@@ -524,35 +489,9 @@ def conv3x3_classify_takes(x, x1, wp, Cout, n_classes, mode=None) -> bool:
     mode = mode or _pw_mode
     if not _fuse_classify or PW_MODES[mode] == 0:
         return False
-    x, bs0 = _nchw_bstride(x, "x")
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        C1 = x1.shape[1]
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     return bool(_lib.load().smaat_conv3x3_classify_eligible(_ptr(x), bs0, _ptr(x1), C1, bs1, _ptr(wp), x.shape[3], Cout, int(n_classes),
                                                             PW_MODES[mode]))
-
-
-def _conv3x3_head_operands(x, x1, wp, Cout, oc_weight, oc_bias, mode, w_split):
-    """The checked operands of the dense OutConv epilogue (smaat_conv3x3_classify_fwd, smaat_conv3x3_probs_fwd):
-    (x, its batch stride, x1, C1, x1's batch stride, packed weight [tf32 hi], its tf32 lo or None, OutConv weight, bias or None)."""
-    x, bs0 = _nchw_bstride(x, "x")
-    B, C0, H, W = x.shape
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        assert x1.shape[0] == B and x1.shape[2:] == x.shape[2:], "concat inputs must agree in B, H, W"
-        C1 = x1.shape[1]
-    assert wp.shape == (Cout, 9 * (_pad32(C0) + _pad32(C1))), f"packed weight {tuple(wp.shape)} does not match Cin={C0}+{C1}"
-    ow = _dense(oc_weight, "outconv.weight")
-    K = ow.shape[0]
-    assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
-    ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
-    assert ob is None or ob.numel() == K, f"OutConv bias {tuple(oc_bias.shape)} does not match K={K}"
-    wlo = None
-    if PW_MODES[mode] == 2:
-        wp, wlo = w_split if w_split is not None else split_tf32(wp)
-    return x, bs0, x1, C1, bs1, wp, wlo, ow, ob
 
 
 def conv3x3_classify(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1=None, mode=None, w_split=None, want_logits=False,
@@ -563,54 +502,51 @@ def conv3x3_classify(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1=Non
     bit ``outconv(conv3x3(...))`` and ``argmax_channels`` of it.  Returns None where ``conv3x3_classify_takes`` is False (the
     caller then runs the layers apart)."""
     assert want_logits or want_classes, "conv3x3_classify: ask for the logits, the class map or both"
-    mode = mode or _pw_mode
-    K = _dense(oc_weight, "outconv.weight").shape[0]
-    if not conv3x3_classify_takes(x, x1, wp, Cout, K, mode):
-        return None
-    x, bs0, x1, C1, bs1, wp, wlo, ow, ob = _conv3x3_head_operands(x, x1, wp, Cout, oc_weight, oc_bias, mode, w_split)
-    B, C0, H, W = x.shape
-    classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64) if want_classes else None
-    logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
-    Cin = C0 + C1
-    _call(f"smaat_conv3x3_classify_fwd[C{Cin}_N{Cout}_K{K}_S{H}x{W}]",
-          4 * B * H * W * (Cin + (K if want_logits else 0) + (2 if want_classes else 0)) + 36 * Cin * Cout,
-          2 * B * H * W * Cout * (9 * Cin + K), _lib.load().smaat_conv3x3_classify_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(wp),
-          _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, _ptr(logits), _ptr(classes), B, H, W, Cout, int(bool(relu)),
-          PW_MODES[mode], _stream())
-    if not want_logits:
-        return classes
-    return (classes, logits) if want_classes else logits
+    return _conv3x3_head(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, False, want_logits, want_classes)
 
 
 def conv3x3_probs(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1=None, mode=None, w_split=None):
     """``conv3x3`` followed by OutConv(Cout -> K) and the softmax over the K classes in the tensor-core kernel's epilogue
     (smaat_conv3x3_probs_fwd): the (B, K, H, W) fp32 probabilities, bit for bit ``softmax_channels(outconv(conv3x3(...)))``.
     Inference only.  Returns None where ``conv3x3_classify_takes`` is False."""
+    return _conv3x3_head(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, True)
+
+
+def _conv3x3_head(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, probs, want_logits=False,
+                  want_classes=False):
+    """``conv3x3_classify`` (smaat_conv3x3_classify_fwd) or, with ``probs``, ``conv3x3_probs`` (smaat_conv3x3_probs_fwd)."""
     mode = mode or _pw_mode
     K = _dense(oc_weight, "outconv.weight").shape[0]
     if not conv3x3_classify_takes(x, x1, wp, Cout, K, mode):
         return None
-    x, bs0, x1, C1, bs1, wp, wlo, ow, ob = _conv3x3_head_operands(x, x1, wp, Cout, oc_weight, oc_bias, mode, w_split)
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
-    probs = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32)
     Cin = C0 + C1
-    _call(f"smaat_conv3x3_probs_fwd[C{Cin}_N{Cout}_K{K}_S{H}x{W}]", 4 * B * H * W * (Cin + K) + 36 * Cin * Cout,
-          2 * B * H * W * Cout * (9 * Cin + K), _lib.load().smaat_conv3x3_probs_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(wp),
-          _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, _ptr(probs), B, H, W, Cout, int(bool(relu)), PW_MODES[mode],
-          _stream())
-    return probs
+    assert wp.shape == (Cout, 9 * (_pad32(C0) + _pad32(C1))), f"packed weight {tuple(wp.shape)} does not match Cin={C0}+{C1}"
+    ow, ob, K = _outconv_operands(oc_weight, oc_bias, Cout)
+    wp, wlo = _tf32_split(wp, PW_MODES[mode], w_split)
+    lib = _lib.load()
+    if probs:
+        out = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32)
+        name, fn, outs, written = "smaat_conv3x3_probs_fwd", lib.smaat_conv3x3_probs_fwd, (_ptr(out),), K
+    else:
+        classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64) if want_classes else None
+        logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
+        out = ((classes, logits) if want_classes else logits) if want_logits else classes
+        name, fn, outs, written = ("smaat_conv3x3_classify_fwd", lib.smaat_conv3x3_classify_fwd, (_ptr(logits), _ptr(classes)),
+                                   (K if want_logits else 0) + (2 if want_classes else 0))
+    _call(f"{name}[C{Cin}_N{Cout}_K{K}_S{H}x{W}]", 4 * B * H * W * (Cin + written) + 36 * Cin * Cout,
+          2 * B * H * W * Cout * (9 * Cin + K), fn, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(wp), _ptr(wlo), _ptr(scale),
+          _ptr(shift), _ptr(ow), _ptr(ob), K, *outs, B, H, W, Cout, int(bool(relu)), PW_MODES[mode], _stream())
+    return out
 
 
 def conv3x3_bwd_weight(dz, x, x1, dW, mode=None):
     """dW (Cout, Cin, 3, 3) += the weight gradient of ``conv3x3`` over [x, x1] for output gradient dz (unet_parts.py:16,19).
     Tensor cores in 'tf32' / 'tf32x3' where the shape allows (W % 4 == 0, aligned), else the exact CUDA-core kernel."""
     dz = _dense(dz, "dz")
-    x, bs0 = _nchw_bstride(x, "x")
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
-    C1, bs1 = 0, 0
-    if x1 is not None:
-        x1, bs1 = _nchw_bstride(x1, "x1")
-        C1 = x1.shape[1]
     Cout = dz.shape[1]
     assert tuple(dW.shape) == (Cout, C0 + C1, 3, 3) and dW.is_contiguous()
     m = PW_MODES[mode or _pw_mode]

@@ -192,7 +192,7 @@ def test_fallbacks_give_todays_results(mode_guard):
         want = oc(dc.run(z))
         got, names = _launches(dc.run, z, None, oc)
         assert _bits_equal(got, want) and not any(k in names for k in FUSED)
-        got, names = _launches(lambda: dc.run(z, outconv=oc, classes=True))
+        got, names = _launches(lambda: dc.run(z, outconv=oc, head="classes"))
         assert torch.equal(got, ops.argmax_channels(want)) and not any(k in names for k in FUSED)
     # set_fused_classify(False): the separate launches, the same bits
     ops.set_fused_classify(False)
