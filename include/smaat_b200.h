@@ -29,7 +29,10 @@
 extern "C" {
 #endif
 
-#define SMAAT_ABI_VERSION 2   /* 2: the tensor-memory kernel's debug hooks and smaat_debug_dsconv_timing are gone */
+/* 2: the tensor-memory kernel's debug hooks and smaat_debug_dsconv_timing are gone
+ * 3: the DS conv's softmax epilogue and the dense 3x3 conv's OutConv / argmax / softmax epilogue are gone: each measured
+ *    slower than the separate launches it replaced */
+#define SMAAT_ABI_VERSION 3
 
 #define SMAAT_OK 0
 #define SMAAT_E_BADARG (-1)   /* shape / pointer / alignment rejected by host-side validation */
@@ -121,17 +124,6 @@ int smaat_dsconv_classify_fwd(const float* x0, int C0, int64_t x0_bstride, const
                               const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
                               const float* scale, const float* shift, const float* oc_w, const float* oc_b, int K,
                               float* logits, int64_t* classes, int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
-/* The same kernel ending in the per-pixel class probabilities, softmax(y_pred) over the K logits (train_SmaAtUNet.py:76
- * computes them before its argmax; an exceedance map such as P(rate > 1 mm/h) is a partial sum of them).  Arguments as
- * smaat_dsconv_classify_fwd with probs: (B, K, H, W) in place of logits / classes.  The epilogue computes each class's logit
- * twice: once for a running (max, sum of exp) per pixel, once more to write exp(l - max) / sum.  probs equals, bit for bit,
- * smaat_softmax_channels_fwd applied to the logits smaat_dsconv_classify_fwd writes for the same inputs.  Only the K
- * probability planes reach HBM.  Eligibility: smaat_dsconv_classify_eligible, unchanged (1 <= K <= 32, 22 for Cout > 64);
- * SMAAT_E_UNSUPPORTED otherwise (callers then run the two convs, smaat_outconv_fwd and smaat_softmax_channels_fwd). */
-int smaat_dsconv_probs_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
-                           const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
-                           const float* scale, const float* shift, const float* oc_w, const float* oc_b, int K,
-                           float* probs, int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
 
 /* The fused DS conv with the CBAM fusions of the serving forward (models/layers.py:90-141 around the DS blocks of
  * models/SmaAt_UNet.py:41-57); arguments as smaat_dsconv_fwd, without batch statistics.
@@ -347,7 +339,7 @@ int smaat_onehot_classes(const float* target, int64_t* classes, int B, int K, in
 /* smaat_argmax_channels_fwd: the class map of any (B, K, P) logits, classes[b, p] = argmax_c x[b, c, p] (int64), in one read:
  *   ties go to the first index and a NaN logit wins, as torch.argmax (and smaat_ce_fwd's confusion column).  1 <= K <= 1024
  *   (larger K: SMAAT_E_UNSUPPORTED).  128-bit loads when P % 4 == 0 and x / classes are 16-byte aligned, a scalar kernel
- *   otherwise.  Serves every model output smaat_dsconv_classify_fwd does not produce. */
+ *   otherwise.  Serves every class map smaat_dsconv_classify_fwd does not produce, the dense models' among them. */
 int smaat_argmax_channels_fwd(const float* x, int64_t* classes, int B, int K, int64_t P, void* stream);
 /* smaat_softmax_channels_fwd: the class probabilities of any (B, K, P) logits, probs[b, c, p] = softmax_c x[b, :, p], the
  *   softmax(y_pred) of train_SmaAtUNet.py:76 (torch.softmax(x, 1)).  One thread per pixel (4 with 128-bit loads when P % 4 == 0
@@ -355,7 +347,7 @@ int smaat_argmax_channels_fwd(const float* x, int64_t* classes, int B, int K, in
  *   from L2 (the grid is sized so that the lines it reads between its two sweeps fit in half of it), and writes
  *   exp(l - max) / sum.  Non-finite logits give torch's pattern: a NaN or +inf logit makes the pixel's K probabilities NaN, a
  *   pixel of -inf logits is NaN, a -inf logit among finite ones gets 0; K = 1 gives 1.  1 <= K <= 1024 (larger K:
- *   SMAAT_E_UNSUPPORTED).  Serves every model output smaat_dsconv_probs_fwd does not produce. */
+ *   SMAAT_E_UNSUPPORTED).  Serves the probabilities of every model: the softmax of the logits its serving forward returns. */
 int smaat_softmax_channels_fwd(const float* x, float* probs, int B, int K, int64_t P, void* stream);
 
 /* CBAM in three launches (reference models/layers.py:90-141).
@@ -412,30 +404,6 @@ int smaat_conv3x3_fwd(const float* x0, int C0, int64_t x0_bstride, const float* 
                       double* stats, int B, int H, int W, int Cout, int relu, int mode, void* stream);
 int smaat_conv3x3_bwd_weight(const float* dz, const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1,
                              int64_t x1_bstride, float* dW, int B, int H, int W, int Cout, int mode, void* stream);
-/* The dense networks' last two modules in one kernel: the last 3x3 conv of up4's DoubleConv (+ eval BatchNorm2d + ReLU) followed
- * by OutConv(Cout -> K) (models/unet_parts.py:16-21, 67-73), ending in the logits, the class map the reference's validation loop
- * predicts (pred_class = torch.argmax(softmax(y_pred), dim=1), train_SmaAtUNet.py:76) or the softmax probabilities.  Conv
- * arguments as smaat_conv3x3_fwd without y / y_bstride / stats; oc_w: (K, Cout), oc_b: (K) or NULL.
- * smaat_conv3x3_classify_fwd: logits (B, K, H, W) or NULL, classes (B, H, W) int64 or NULL, not both NULL.
- * smaat_conv3x3_probs_fwd: probs (B, K, H, W).
- * Bitwise contract: the outputs equal, bit for bit, smaat_conv3x3_fwd -> smaat_outconv_fwd [-> smaat_argmax_channels_fwd /
- *   smaat_softmax_channels_fwd] on the same inputs in the same mode: the epilogue forms the activation the conv writes, each
- *   logit as the OutConv kernel sums it (the bias, then fmaf over the channels in order), the argmax with torch's rule (ties to
- *   the first index, a NaN wins) and the probabilities with the softmax kernel's arithmetic.  Only the requested outputs reach
- *   HBM; the Cout-channel activation never does.
- * Eligibility (smaat_conv3x3_classify_eligible answers 1/0 for `mode`): that of smaat_conv3x3_tc_eligible, mode SMAAT_PW_TF32 or
- *   SMAAT_PW_TF32X3, Cout <= 64 (one channel pass: a CTA holds all of a pixel's channels) and 1 <= K <= 32; no batch
- *   statistics.  SMAAT_E_UNSUPPORTED otherwise (callers then run smaat_conv3x3_fwd, smaat_outconv_fwd and the argmax /
- *   softmax kernel). */
-int smaat_conv3x3_classify_eligible(const float* x0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
-                                    const float* wp, int W, int Cout, int K, int mode);
-int smaat_conv3x3_classify_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
-                               const float* wp, const float* wp_lo, const float* scale, const float* shift, const float* oc_w,
-                               const float* oc_b, int K, float* logits, int64_t* classes, int B, int H, int W, int Cout, int relu,
-                               int mode, void* stream);
-int smaat_conv3x3_probs_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
-                            const float* wp, const float* wp_lo, const float* scale, const float* shift, const float* oc_w,
-                            const float* oc_b, int K, float* probs, int B, int H, int W, int Cout, int relu, int mode, void* stream);
 
 /* ---- optimizer step (reference models/regression_lightning.py:47-48, train_SmaAtUNet.py:25: torch.optim.Adam with its
  * defaults) over flat fp32 buffers of n floats (n % 4 == 0, 16-byte aligned; parameters, gradients, first and second moment

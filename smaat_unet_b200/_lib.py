@@ -29,7 +29,6 @@ SIGNATURES = {
     "smaat_dsconv_outconv_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_classify_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _i],
     "smaat_dsconv_classify_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
-    "smaat_dsconv_probs_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_cbam_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _i, _i],
     "smaat_dsconv_pool_parts": [_i, _i],
     "smaat_dsconv_cbam_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _l, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
@@ -83,9 +82,6 @@ SIGNATURES = {
     "smaat_conv3x3_pack_weight": [_p, _p, _i, _i, _i, _i, _p],
     "smaat_conv3x3_tc_eligible": [_p, _l, _p, _i, _l, _p, _i, _i],
     "smaat_conv3x3_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _p],
-    "smaat_conv3x3_classify_eligible": [_p, _l, _p, _i, _l, _p, _i, _i, _i, _i],
-    "smaat_conv3x3_classify_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _p],
-    "smaat_conv3x3_probs_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _i, _p, _i, _i, _i, _i, _i, _i, _p],
     "smaat_conv3x3_bwd_weight": [_p, _p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _p],
 }
 _SPECIAL = {
@@ -116,7 +112,7 @@ def load():
         fn = getattr(lib, name)
         fn.argtypes = argtypes
         fn.restype = restype
-    if lib.smaat_abi_version() != 2:
+    if lib.smaat_abi_version() != 3:
         raise RuntimeError("smaat_unet_b200: ABI version mismatch between _lib.py and libsmaat_b200.so")
     _lib = lib
     return lib

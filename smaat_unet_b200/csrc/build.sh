@@ -15,7 +15,7 @@ pids=()
 for s in "${SRCS[@]}"; do
   o=../../build/${s%.cu}.o
   OBJS+=("$o")
-  if [[ ! -f "$o" || "$s" -nt "$o" || common.cuh -nt "$o" || tc_common.cuh -nt "$o" || softmax.cuh -nt "$o" || wgmma.cuh -nt "$o" || ../../include/smaat_b200.h -nt "$o" ]]; then
+  if [[ ! -f "$o" || "$s" -nt "$o" || common.cuh -nt "$o" || tc_common.cuh -nt "$o" || wgmma.cuh -nt "$o" || ../../include/smaat_b200.h -nt "$o" ]]; then
     ( "$NVCC" "${FLAGS[@]}" -c "$s" -o "$o" > "../../build/${s%.cu}.log" 2>&1 || { cat "../../build/${s%.cu}.log"; exit 1; } ) &
     pids+=($!)
   fi

@@ -16,7 +16,6 @@
 // non-zero bin, or for larger K straight to the global matrix; either way lanes holding the same (t, argmax) pair are
 // merged with __match_any_sync first, since neighbouring pixels of a segmentation map usually share both.
 #include "common.cuh"
-#include "softmax.cuh"
 
 namespace smaat {
 
@@ -445,8 +444,33 @@ __global__ void __launch_bounds__(CE_THREADS) argmax_channels_kernel(const float
   }
 }
 
+// Online (max m, sum s) over one pixel's logits, then p = exp(l - m) / s.  Each add() computes
+//   s = fmaf(s, exp(m_old - m_new), exp(l - m_new)),  m_new = fmaxf(m_old, l)
+// in two branches: a new maximum (l > m) evaluates that formula; otherwise m_new = m_old, exp(m - m) is exactly 1 wherever s is
+// still finite, and the fmaf is the single-rounding s + exp(l - m): one exp instead of two, the same bits.  The results match
+// torch.softmax on non-finite logits:
+//   a NaN logit: it is never a new maximum, exp(NaN - m) makes s NaN, and every class of the pixel is NaN;
+//   a +inf logit: exp(inf - inf) = NaN in s, every class NaN;
+//   all logits -inf: s stays 0 and exp(-inf + inf) / 0 is NaN for every class;
+//   a -inf logit among finite ones: exp(-inf - m) / s = 0 for that class;
+//   K = 1, finite: exp(0) / 1 = 1.
+// A -inf logit adds exp(-inf) = 0 and leaves the max alone, so add() skips it: fed through the formula as a pixel's first
+// logit it would give s = 0 * exp(-inf + inf) + exp(-inf + inf) = NaN and poison the finite classes after it.
+struct SoftmaxAcc {
+  float m = -INFINITY, s = 0.f;
+  __device__ __forceinline__ void add(float l) {
+    if (l > m) {
+      s = fmaf(s, expf(m - l), expf(l - l));   // l - l: NaN for l = +inf, as the formula
+      m = l;
+    } else if (l != -INFINITY) {
+      s += expf(l - m);
+    }
+  }
+  __device__ __forceinline__ float prob(float l) const { return expf(l - m) / s; }
+};
+
 // Channel softmax: the probabilities of (B, K, P) logits, NPX consecutive pixels of one image per thread, as
-// argmax_channels_kernel.  The first sweep feeds the classes in order to SoftmaxAcc (softmax.cuh); the second re-reads the
+// argmax_channels_kernel.  The first sweep feeds the classes in order to SoftmaxAcc; the second re-reads the
 // same lines, which the grid keeps in L2 (smaat_softmax_channels_fwd), and streams the probabilities out.
 template <int NPX>
 __global__ void __launch_bounds__(CE_THREADS) softmax_channels_kernel(const float* __restrict__ x, float* __restrict__ probs, int K,

@@ -18,10 +18,6 @@ bool conv3x3_tc_eligible(const float* x0, int64_t bs0, const float* x1, int C1, 
 int conv3x3_tc_launch(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* wp, const float* wp_lo,
                       const float* scale, const float* shift, float* y, int64_t y_bstride, double* stats, int B, int H, int W, int Cout,
                       int relu, bool x3, cudaStream_t st);
-bool conv3x3_head_eligible(const float* x0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* wp, int W, int Cout, int K);
-int conv3x3_head_launch(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* wp, const float* wp_lo,
-                        const float* scale, const float* shift, const float* oc_w, const float* oc_b, int K, float* logits,
-                        int64_t* classes, float* probs, int B, int H, int W, int Cout, int relu, bool x3, cudaStream_t st);
 int conv3x3_wgrad_tc_launch(const float* dz, const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, float* dW,
                             int B, int H, int W, int Cout, bool x3, cudaStream_t st);
 
@@ -256,54 +252,6 @@ extern "C" int smaat_conv3x3_fwd(const float* x0, int C0, int64_t x0_bstride, co
     default:
       return fail(SMAAT_E_BADARG, "conv3x3: unknown mode %d", mode);
   }
-}
-
-extern "C" int smaat_conv3x3_classify_eligible(const float* x0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
-                                               const float* wp, int W, int Cout, int K, int mode) {
-  if (mode != SMAAT_PW_TF32 && mode != SMAAT_PW_TF32X3) return 0;
-  return conv3x3_head_eligible(x0, x0_bstride, x1, C1, x1_bstride, wp, W, Cout, K) ? 1 : 0;
-}
-
-// Shared by the two head entry points: the checks of smaat_conv3x3_fwd, then the tensor-core kernel's OutConv epilogue.
-static int conv3x3_head(const char* what, const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
-                        const float* wp, const float* wp_lo, const float* scale, const float* shift, const float* oc_w, const float* oc_b,
-                        int K, float* logits, int64_t* classes, float* probs, int B, int H, int W, int Cout, int relu, int mode,
-                        void* stream) {
-  SMAAT_REQUIRE(x0 && wp && oc_w, "%s: null pointer", what);
-  SMAAT_REQUIRE(B > 0 && C0 > 0 && C1 >= 0 && H > 0 && W > 0 && Cout > 0 && K >= 1,
-                "%s: bad shape B=%d C0=%d C1=%d H=%d W=%d Cout=%d K=%d", what, B, C0, C1, H, W, Cout, K);
-  SMAAT_REQUIRE(C1 == 0 || x1, "%s: C1=%d but x1 is null", what, C1);
-  SMAAT_REQUIRE(x0_bstride >= (int64_t)C0 * H * W && (C1 == 0 || x1_bstride >= (int64_t)C1 * H * W), "%s: input batch stride too small",
-                what);
-  SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(oc_w) & 3u) == 0 && (reinterpret_cast<uintptr_t>(oc_b) & 3u) == 0 &&
-                    (reinterpret_cast<uintptr_t>(logits) & 3u) == 0 && (reinterpret_cast<uintptr_t>(probs) & 3u) == 0 &&
-                    (reinterpret_cast<uintptr_t>(classes) & 7u) == 0,
-                "%s: weights / logits / probs must be 4-byte and classes 8-byte aligned", what);
-  if (mode != SMAAT_PW_TF32 && mode != SMAAT_PW_TF32X3) {
-    SMAAT_REQUIRE(mode == SMAAT_PW_FP32_SIMT, "%s: unknown mode %d", what, mode);
-    return fail(SMAAT_E_UNSUPPORTED, "%s: SMAAT_PW_FP32_SIMT has no fused OutConv; use smaat_conv3x3_fwd + smaat_outconv_fwd", what);
-  }
-  return conv3x3_head_launch(x0, C0, x0_bstride, C1 ? x1 : nullptr, C1, x1_bstride, wp, mode == SMAAT_PW_TF32X3 ? wp_lo : nullptr,
-                             scale, shift, oc_w, oc_b, K, logits, classes, probs, B, H, W, Cout, relu, mode == SMAAT_PW_TF32X3,
-                             (cudaStream_t)stream);
-}
-
-extern "C" int smaat_conv3x3_classify_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
-                                          const float* wp, const float* wp_lo, const float* scale, const float* shift, const float* oc_w,
-                                          const float* oc_b, int K, float* logits, int64_t* classes, int B, int H, int W, int Cout,
-                                          int relu, int mode, void* stream) {
-  SMAAT_REQUIRE(logits || classes, "conv3x3+classify: needs a logits or a classes output");
-  return conv3x3_head("conv3x3+classify", x0, C0, x0_bstride, x1, C1, x1_bstride, wp, wp_lo, scale, shift, oc_w, oc_b, K, logits,
-                      classes, nullptr, B, H, W, Cout, relu, mode, stream);
-}
-
-extern "C" int smaat_conv3x3_probs_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
-                                       const float* wp, const float* wp_lo, const float* scale, const float* shift, const float* oc_w,
-                                       const float* oc_b, int K, float* probs, int B, int H, int W, int Cout, int relu, int mode,
-                                       void* stream) {
-  SMAAT_REQUIRE(probs, "conv3x3+probs: needs a probs output");
-  return conv3x3_head("conv3x3+probs", x0, C0, x0_bstride, x1, C1, x1_bstride, wp, wp_lo, scale, shift, oc_w, oc_b, K, nullptr, nullptr,
-                      probs, B, H, W, Cout, relu, mode, stream);
 }
 
 extern "C" int smaat_conv3x3_bwd_weight(const float* dz, const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1,

@@ -28,15 +28,6 @@
 // Warps 4-11 = two consumer warpgroups (64 pixels each).  Epilogue as pw1x1_tc.cu: affine/ReLU -> batch-strided NCHW stores,
 // BatchNorm sums from the raw accumulators in fp64 shared-memory partials (pixels outside the image masked), the affine
 // applied analytically at the flush.  Statistics work for every Cout (passes of N_TILE flush separately).
-//
-// HEAD instances (smaat_conv3x3_classify_fwd / smaat_conv3x3_probs_fwd) are the same kernel -- main loop, tile decode and tile
-// shapes unchanged -- with the K-class OutConv of UNet / UNetAttention (reference models/unet_parts.py:67-73) and the class map
-// or the softmax probabilities in the epilogue, for Cout <= N_TILE = 64 (one channel pass: the CTA holds every channel of its
-// pixels).  Each consumer warpgroup stages its 64-pixel x Cout activation in shared memory, [channel][pixel] at a padded pitch;
-// then one thread per pixel walks its channels in ascending order, fmaf(w[j][c], v[c], acc) from the bias, exactly as
-// outconv_kernel (glue.cu) does on the activation the plain launch writes, and ends in torch.argmax's rule
-// (smaat_argmax_channels_fwd) or SoftmaxAcc (softmax.cuh, as smaat_softmax_channels_fwd).  The activation never reaches HBM.
-#include "softmax.cuh"
 #include "tc_common.cuh"
 
 namespace smaat {
@@ -52,14 +43,6 @@ struct C3Params {
   int kc;         // channels per tap in the packed weight (c0p + c1p)
   int nch0, nch;  // chunks read from x0, chunks in total
   int tiles_x, tiles_y, tiles_n, total_tiles;
-  // HEAD instances only: OutConv weight (ncls, Cout) and bias (ncls) or null; outputs, each nullable: logits (B, ncls, H, W),
-  // class map (B, H, W) int64, probabilities (B, ncls, H, W)
-  const float* oc_w;
-  const float* oc_b;
-  int ncls;
-  float* oc_y;
-  int64_t* cls;
-  float* probs;
 };
 
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
@@ -69,9 +52,6 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-
-constexpr int C3_HEAD_MAX_COUT = 64;      // HEAD instances: one channel pass of N_TILE = 64
-constexpr int C3_HEAD_MAX_CLASSES = 32;
 
 template <int N_TILE, int PW, bool X3>
 struct C3Cfg {
@@ -99,105 +79,7 @@ struct C3Cfg {
   static constexpr int THREADS = 384;
 };
 
-// Shared memory of the HEAD instances: where the plain instances keep the statistics partials (a HEAD launch takes no
-// statistics), past the halo and weight rings, which the TMA warps refill for the next tile while the epilogue runs.
 template <int N_TILE, int PW, bool X3>
-struct C3HeadCfg : C3Cfg<N_TILE, PW, X3> {
-  using L = C3Cfg<N_TILE, PW, X3>;
-  static_assert(N_TILE == C3_HEAD_MAX_COUT, "the OutConv epilogue holds all of a pixel's channels: one channel pass of 64");
-  static constexpr int MAX_CLASSES = C3_HEAD_MAX_CLASSES;
-  // activation staging, per consumer warpgroup [N_TILE channels][ST_P]: ST_P = 4 mod 16 puts the fragment-layout writes
-  // (lane (g, t) at 2t * ST_P + g) on 32 different banks; the per-pixel reads are consecutive words
-  static constexpr int ST_P = 68;
-  static_assert(ST_P % 16 == 4 && ST_P >= 64, "staging pitch");
-  static constexpr int OFF_STG = L::OFF_SACC;
-  static constexpr int STG_BYTES = 2 * N_TILE * ST_P * 4;
-  static constexpr int OFF_CLS = OFF_STG + STG_BYTES;   // class weights [MAX_CLASSES][N_TILE], then MAX_CLASSES biases
-  static_assert(OFF_CLS % 16 == 0, "class weights are read as float4");
-  static constexpr int CLS_BYTES = (MAX_CLASSES * N_TILE + MAX_CLASSES) * 4;
-  static constexpr int TOTAL = OFF_CLS + CLS_BYTES + 1024;
-  static_assert(TOTAL <= 227 * 1024, "shared memory budget");
-};
-
-// The HEAD epilogue of one tile (Cout <= N_TILE, n0 = 0).  The warpgroup stages its activations fmaxf(fmaf(acc, sc, sh), act_lo)
-// -- the values the plain epilogue stores -- then its first two warps take one pixel per thread: the Cout activations into
-// registers, each class's logit as outconv_kernel forms it (bias or 0, then fmaf over c = 0 .. Cout - 1 in order), and the
-// requested outputs.  The warpgroup's named barrier brackets the staging buffer: written by all four warps, read by two, and
-// not overwritten by the next tile's epilogue before those reads are done.
-template <int N_TILE, int PW, bool X3>
-__device__ __forceinline__ void head_epilogue(const float (&acc)[N_TILE / 2], unsigned char* smem, const float* aff, float act_lo,
-                                              const C3Params& p, int b, int y0, int x0, int wg, int wq, int g, int t, int lane) {
-  using HC = C3HeadCfg<N_TILE, PW, X3>;
-  constexpr int ST_P = HC::ST_P, MAXK = HC::MAX_CLASSES;
-  float* stg = reinterpret_cast<float*>(smem + HC::OFF_STG) + wg * N_TILE * ST_P;
-  const float* cls_w = reinterpret_cast<const float*>(smem + HC::OFF_CLS);
-  const float* cls_b = cls_w + MAXK * N_TILE;
-  const int ml0 = 16 * wq + g, ml1 = ml0 + 8;   // the warpgroup's accumulator rows g / g + 8
-#pragma unroll
-  for (int j = 0; j < N_TILE / 8; ++j) {
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const int c = 8 * j + 2 * t + e;
-      const float sc = aff[c], sh = aff[HC::AFF_N + c];
-      stg[c * ST_P + ml0] = fmaxf(fmaf(acc[4 * j + e], sc, sh), act_lo);
-      stg[c * ST_P + ml1] = fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo);
-    }
-  }
-  asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-  const int ml = 32 * wq + lane, m = 64 * wg + ml;
-  const int py = y0 + m / PW, px = x0 + m % PW;
-  if (wq < 2 && py < p.H && px < p.W) {
-    float v[N_TILE];
-#pragma unroll
-    for (int c = 0; c < N_TILE; ++c) v[c] = stg[c * ST_P + ml];
-    float lg[MAXK];
-#pragma unroll
-    for (int cl = 0; cl < MAXK; ++cl) {
-      if (cl < p.ncls) {
-        const float* wr = cls_w + cl * N_TILE;   // the same address in every lane: broadcast loads
-        float a = cls_b[cl];
-#pragma unroll
-        for (int c = 0; c < N_TILE; c += 4) {
-          const float4 w = *reinterpret_cast<const float4*>(wr + c);
-          if (c < p.Cout) a = fmaf(w.x, v[c], a);
-          if (c + 1 < p.Cout) a = fmaf(w.y, v[c + 1], a);
-          if (c + 2 < p.Cout) a = fmaf(w.z, v[c + 2], a);
-          if (c + 3 < p.Cout) a = fmaf(w.w, v[c + 3], a);
-        }
-        lg[cl] = a;
-      }
-    }
-    const int64_t HW = (int64_t)p.H * p.W, o = (int64_t)py * p.W + px;
-    if (p.oc_y) {
-      float* yb = p.oc_y + (int64_t)b * p.ncls * HW + o;
-#pragma unroll
-      for (int cl = 0; cl < MAXK; ++cl)
-        if (cl < p.ncls) yb[cl * HW] = lg[cl];
-    }
-    if (p.cls) {
-      // torch.argmax: the first strictly larger logit wins, and a NaN wins and stays (argmax_channels_kernel's test)
-      float best = -INFINITY;
-      int arg = 0;
-#pragma unroll
-      for (int cl = 0; cl < MAXK; ++cl)
-        if (cl < p.ncls && best == best && (lg[cl] > best || lg[cl] != lg[cl])) { best = lg[cl]; arg = cl; }
-      p.cls[(int64_t)b * HW + o] = arg;
-    }
-    if (p.probs) {
-      SoftmaxAcc sm;
-#pragma unroll
-      for (int cl = 0; cl < MAXK; ++cl)
-        if (cl < p.ncls) sm.add(lg[cl]);
-      float* pb = p.probs + (int64_t)b * p.ncls * HW + o;
-#pragma unroll
-      for (int cl = 0; cl < MAXK; ++cl)
-        if (cl < p.ncls) pb[cl * HW] = sm.prob(lg[cl]);
-    }
-  }
-  asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-}
-
-template <int N_TILE, int PW, bool X3, bool HEAD>
 __global__ void __launch_bounds__(384, 1)
     conv3x3_tc_kernel(const __grid_constant__ CUtensorMap map_x0, const __grid_constant__ CUtensorMap map_x1,
                       const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo, const C3Params p) {
@@ -233,15 +115,6 @@ __global__ void __launch_bounds__(384, 1)
   for (int c = threadIdx.x; c < L::AFF_N; c += blockDim.x) {
     aff[c] = (c < p.Cout && p.scale) ? __ldg(p.scale + c) : 1.f;
     aff[L::AFF_N + c] = (c < p.Cout && p.shift) ? __ldg(p.shift + c) : 0.f;
-  }
-  if constexpr (HEAD) {
-    using HC = C3HeadCfg<N_TILE, PW, X3>;
-    float* cls_w = reinterpret_cast<float*>(smem + HC::OFF_CLS);
-    for (int i = threadIdx.x; i < p.ncls * N_TILE; i += blockDim.x) {
-      const int cl = i / N_TILE, c = i - cl * N_TILE;
-      cls_w[i] = c < p.Cout ? __ldg(p.oc_w + (int64_t)cl * p.Cout + c) : 0.f;
-    }
-    for (int cl = threadIdx.x; cl < p.ncls; cl += blockDim.x) cls_w[HC::MAX_CLASSES * N_TILE + cl] = p.oc_b ? __ldg(p.oc_b + cl) : 0.f;
   }
   __syncthreads();
 
@@ -384,10 +257,6 @@ __global__ void __launch_bounds__(384, 1)
       if (lane == 0) mbar_arrive(&in_empty[s]);
     }
 
-    if constexpr (HEAD) {
-      head_epilogue<N_TILE, PW, X3>(acc, smem, aff, act_lo, p, b, y0, x0, wg, wq, g, t, lane);
-      continue;
-    }
     // ----- epilogue: rows g / g + 8 are pixels (y0 + h0, x0 + w0) / (y0 + h1, x0 + w1), columns n0 + 8j + 2t + {0, 1}
     const int py0 = y0 + h0, px0 = x0 + w0, py1 = y0 + h1, px1 = x0 + w1;
     const bool v0 = py0 < p.H && px0 < p.W, v1 = py1 < p.H && px1 < p.W;
@@ -428,23 +297,15 @@ __global__ void __launch_bounds__(384, 1)
   if (p.stats && stat_n0 >= 0) flush_stats(stat_n0);
 }
 
-// Dynamic shared memory of an instance: the plain instances keep their own budget, only the HEAD ones request the staging
-template <int N_TILE, int PW, bool X3, bool HEAD>
-constexpr int c3_smem() {
-  if constexpr (HEAD) return C3HeadCfg<N_TILE, PW, X3>::TOTAL;
-  else return C3Cfg<N_TILE, PW, X3>::TOTAL;
-}
-
-template <int N_TILE, int PW, bool X3, bool HEAD = false>
+template <int N_TILE, int PW, bool X3>
 static int launch_c3(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl, C3Params p, int B,
                      cudaStream_t st) {
   using L = C3Cfg<N_TILE, PW, X3>;
-  constexpr int SMEM = c3_smem<N_TILE, PW, X3, HEAD>();
-  auto kern = conv3x3_tc_kernel<N_TILE, PW, X3, HEAD>;
+  auto kern = conv3x3_tc_kernel<N_TILE, PW, X3>;
   static std::atomic<uint64_t> attr_mask{0};
   if (first_use_on_device(attr_mask)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) return fail(SMAAT_E_CUDA, "conv3x3(tc): smem attribute (%d B): %s", SMEM, cudaGetErrorString(e));
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
+    if (e != cudaSuccess) return fail(SMAAT_E_CUDA, "conv3x3(tc): smem attribute (%d B): %s", L::TOTAL, cudaGetErrorString(e));
   }
   p.tiles_x = ceil_div(p.W, PW);
   p.tiles_y = ceil_div(p.H, L::PH);
@@ -453,8 +314,8 @@ static int launch_c3(const CUtensorMap& m0, const CUtensorMap& m1, const CUtenso
   SMAAT_REQUIRE(total < (1ll << 31), "conv3x3(tc): too many tiles");
   p.total_tiles = (int)total;
   const int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
-  kern<<<grid, L::THREADS, SMEM, st>>>(m0, m1, mw, mwl, p);
-  SMAAT_LAUNCH_CHECK(HEAD ? "smaat_conv3x3_classify_fwd / smaat_conv3x3_probs_fwd" : "smaat_conv3x3_fwd(tc)");
+  kern<<<grid, L::THREADS, L::TOTAL, st>>>(m0, m1, mw, mwl, p);
+  SMAAT_LAUNCH_CHECK("smaat_conv3x3_fwd(tc)");
   return SMAAT_OK;
 }
 
@@ -472,23 +333,21 @@ bool conv3x3_tc_eligible(const float* x0, int64_t bs0, const float* x1, int C1, 
   return aligned16(wp) && (wp_lo == nullptr || aligned16(wp_lo));
 }
 
-bool conv3x3_head_eligible(const float* x0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* wp, int W, int Cout, int K) {
-  return conv3x3_tc_eligible(x0, bs0, x1, C1, bs1, wp, nullptr, W, Cout) && Cout <= C3_HEAD_MAX_COUT && K >= 1 &&
-         K <= C3_HEAD_MAX_CLASSES;
-}
-
-// The tensor maps and parameters every launch of the kernel shares; the tile shape (pw, n_tile) depends on H, W and Cout alone.
-static int c3_prepare(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* wp, const float* wp_lo,
-                      const float* scale, const float* shift, int B, int H, int W, int Cout, int relu, bool x3, CUtensorMap& m0,
-                      CUtensorMap& m1, CUtensorMap& mw, CUtensorMap& mwl, C3Params& p, int& pw, int& n_tile) {
+int conv3x3_tc_launch(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* wp, const float* wp_lo,
+                      const float* scale, const float* shift, float* y, int64_t y_bstride, double* stats, int B, int H, int W, int Cout,
+                      int relu, bool x3, cudaStream_t st) {
+  if (!conv3x3_tc_eligible(x0, bs0, x1, C1, bs1, wp, wp_lo, W, Cout))
+    return fail(SMAAT_E_UNSUPPORTED, "conv3x3(tc): needs W %% 4 == 0, Cout >= 8, 16-byte aligned pointers and batch strides "
+                "(W=%d Cout=%d); use SMAAT_PW_FP32_SIMT", W, Cout);
   SMAAT_REQUIRE(!x3 || wp_lo, "conv3x3(tc): TF32X3 needs wp_lo (smaat_split_tf32 of the packed weight)");
   SMAAT_REQUIRE(Cout <= 1024 || (!scale && !shift), "conv3x3(tc): Cout=%d > 1024 with an epilogue affine", Cout);
-  pw = c3_pick_pw(H, W);
+  const int pw = c3_pick_pw(H, W);
   const int ph = TC_BM / pw;
-  n_tile = Cout > 64 ? 128 : 64;
+  const int n_tile = Cout > 64 ? 128 : 64;
   const int c0p = (C0 + TC_BK - 1) / TC_BK * TC_BK, c1p = (C1 + TC_BK - 1) / TC_BK * TC_BK;
   const int kc = c0p + c1p;
 
+  CUtensorMap m0, m1, mw, mwl;
   const uint32_t box[4] = {(uint32_t)(pw + 8), (uint32_t)(ph + 3), (uint32_t)TC_BK, 1u};
   {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)C0, (uint64_t)B};
@@ -515,26 +374,12 @@ static int c3_prepare(const float* x0, int C0, int64_t bs0, const float* x1, int
       if (r) return r;
     }
   }
-  p = C3Params{};
-  p.scale = scale; p.shift = shift;
+  C3Params p;
+  p.scale = scale; p.shift = shift; p.y = y; p.y_bstride = y_bstride; p.stats = stats;
   p.H = H; p.W = W; p.Cout = Cout; p.relu = relu;
   p.c0p = c0p; p.kc = kc;
   p.nch0 = c0p / TC_BK; p.nch = kc / TC_BK;
-  return SMAAT_OK;
-}
-
-int conv3x3_tc_launch(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* wp, const float* wp_lo,
-                      const float* scale, const float* shift, float* y, int64_t y_bstride, double* stats, int B, int H, int W, int Cout,
-                      int relu, bool x3, cudaStream_t st) {
-  if (!conv3x3_tc_eligible(x0, bs0, x1, C1, bs1, wp, wp_lo, W, Cout))
-    return fail(SMAAT_E_UNSUPPORTED, "conv3x3(tc): needs W %% 4 == 0, Cout >= 8, 16-byte aligned pointers and batch strides "
-                "(W=%d Cout=%d); use SMAAT_PW_FP32_SIMT", W, Cout);
-  CUtensorMap m0, m1, mw, mwl;
-  C3Params p;
-  int pw, n_tile;
-  int r = c3_prepare(x0, C0, bs0, x1, C1, bs1, wp, wp_lo, scale, shift, B, H, W, Cout, relu, x3, m0, m1, mw, mwl, p, pw, n_tile);
-  if (r) return r;
-  p.y = y; p.y_bstride = y_bstride; p.stats = stats;
+  p.tiles_x = p.tiles_y = p.tiles_n = p.total_tiles = 0;
 
   if (n_tile == 128) {
     if (pw == 32) return x3 ? launch_c3<128, 32, true>(m0, m1, mw, mwl, p, B, st) : launch_c3<128, 32, false>(m0, m1, mw, mwl, p, B, st);
@@ -542,23 +387,6 @@ int conv3x3_tc_launch(const float* x0, int C0, int64_t bs0, const float* x1, int
   }
   if (pw == 32) return x3 ? launch_c3<64, 32, true>(m0, m1, mw, mwl, p, B, st) : launch_c3<64, 32, false>(m0, m1, mw, mwl, p, B, st);
   return x3 ? launch_c3<64, 16, true>(m0, m1, mw, mwl, p, B, st) : launch_c3<64, 16, false>(m0, m1, mw, mwl, p, B, st);
-}
-
-int conv3x3_head_launch(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* wp, const float* wp_lo,
-                        const float* scale, const float* shift, const float* oc_w, const float* oc_b, int K, float* logits,
-                        int64_t* classes, float* probs, int B, int H, int W, int Cout, int relu, bool x3, cudaStream_t st) {
-  if (!conv3x3_head_eligible(x0, bs0, x1, C1, bs1, wp, W, Cout, K) || (wp_lo && !aligned16(wp_lo)))
-    return fail(SMAAT_E_UNSUPPORTED, "conv3x3+outconv: needs the tensor-core conv's shapes (W %% 4 == 0, 16-byte aligned pointers and "
-                "batch strides), 8 <= Cout <= %d and 1 <= K <= %d (W=%d Cout=%d K=%d); use smaat_conv3x3_fwd + smaat_outconv_fwd",
-                C3_HEAD_MAX_COUT, C3_HEAD_MAX_CLASSES, W, Cout, K);
-  CUtensorMap m0, m1, mw, mwl;
-  C3Params p;
-  int pw, n_tile;
-  int r = c3_prepare(x0, C0, bs0, x1, C1, bs1, wp, wp_lo, scale, shift, B, H, W, Cout, relu, x3, m0, m1, mw, mwl, p, pw, n_tile);
-  if (r) return r;
-  p.oc_w = oc_w; p.oc_b = oc_b; p.ncls = K; p.oc_y = logits; p.cls = classes; p.probs = probs;
-  if (pw == 32) return x3 ? launch_c3<64, 32, true, true>(m0, m1, mw, mwl, p, B, st) : launch_c3<64, 32, false, true>(m0, m1, mw, mwl, p, B, st);
-  return x3 ? launch_c3<64, 16, true, true>(m0, m1, mw, mwl, p, B, st) : launch_c3<64, 16, false, true>(m0, m1, mw, mwl, p, B, st);
 }
 
 }  // namespace smaat

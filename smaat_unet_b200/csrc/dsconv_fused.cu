@@ -40,7 +40,6 @@
 
 #include <type_traits>
 
-#include "softmax.cuh"
 #include "tc_common.cuh"
 
 namespace smaat {
@@ -65,11 +64,9 @@ struct DsParams {
   float* pooled;
   int npart;
   // K-class OutConv + argmax (smaat_dsconv_classify_fwd): ncls > 0 classes, oc_w (ncls, Cout), oc_b (ncls) or null, oc_y the
-  // (B, ncls, H, W) logits or null, cls the (B, H, W) class map or null.  probs (smaat_dsconv_probs_fwd): the (B, ncls, H, W)
-  // softmax probabilities instead of logits and class map
+  // (B, ncls, H, W) logits or null, cls the (B, H, W) class map or null
   int ncls;
   int64_t* cls;
-  float* probs;
   int C0, C1, H, W, Cout, relu, K;
   int tiles_x, tiles_y, npass, total_tiles, nchunks;
 };
@@ -453,7 +450,7 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
         }
       }
       if (p.ncls) {
-        // K-class OutConv + argmax (or softmax: p.probs).  The activations replace the accumulators in place (fmaxf(fmaf(acc, sc, sh), act_lo), as
+        // K-class OutConv + argmax.  The activations replace the accumulators in place (fmaxf(fmaf(acc, sc, sh), act_lo), as
         // below); then, one class at a time, the one-class dot product below in its order (fmaf over the thread's channels, the
         // two xor shuffles, + bias), so class j's logit is bit for bit what that epilogue writes with OutConv row j.  After the
         // butterfly all 4 lanes of a fragment group hold the same logits; each keeps the same running (max, first index) per
@@ -470,8 +467,10 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
             acc[4 * j + 2 + e] = fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo);
           }
         }
-        // class cl's logits at pixels m0 / m1
-        auto class_logits = [&](int cl, float& l0, float& l1) {
+        float best0 = -INFINITY, best1 = -INFINITY;
+        int arg0 = 0, arg1 = 0;
+#pragma unroll 1
+        for (int cl = 0; cl < p.ncls; ++cl) {
           const float* wr = cls_w + cl * N_TILE + 2 * t;   // zero past Cout, where the activation is 0 too
           float d0 = 0.f, d1 = 0.f;
 #pragma unroll
@@ -487,60 +486,18 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
           d1 += __shfl_xor_sync(0xffffffffu, d1, 1);
           d1 += __shfl_xor_sync(0xffffffffu, d1, 2);
           const float ob = cls_b[cl];
-          l0 = d0 + ob;
-          l1 = d1 + ob;
-        };
-        if (p.probs) {
-          // Softmax probabilities: pass 1 feeds the logits in class order to SoftmaxAcc (softmax.cuh), as
-          // smaat_softmax_channels_fwd does with the logits this epilogue writes; pass 2 recomputes each logit with the same
-          // code and stores its probability.  One more K-class dot-product loop, so that only two logits are held whatever K
-          // is.  In pass 2 lane t keeps the logits of class 4i + t of each group of 4 classes and normalises and stores them
-          // once the group is complete: one exp and one division per lane per 4 classes, stores rotating over the 4 lanes
-          SoftmaxAcc sm0, sm1;
-#pragma unroll 1
-          for (int cl = 0; cl < p.ncls; ++cl) {
-            float l0, l1;
-            class_logits(cl, l0, l1);
-            sm0.add(l0);
-            sm1.add(l1);
+          const float l0 = d0 + ob, l1 = d1 + ob;
+          if (best0 == best0 && (l0 > best0 || l0 != l0)) { best0 = l0; arg0 = cl; }
+          if (best1 == best1 && (l1 > best1 || l1 != l1)) { best1 = l1; arg1 = cl; }
+          if (p.oc_y && t == (cl & 3)) {
+            float* yk = p.oc_y + ((int64_t)b * p.ncls + cl) * P;
+            if (v0) yk[o0] = l0;
+            if (v1) yk[o1] = l1;
           }
-          float q0 = 0.f, q1 = 0.f;
-#pragma unroll 1
-          for (int cl = 0; cl < p.ncls; ++cl) {
-            float l0, l1;
-            class_logits(cl, l0, l1);
-            if (t == (cl & 3)) {
-              q0 = l0;
-              q1 = l1;
-            }
-            if ((cl & 3) == 3 || cl == p.ncls - 1) {
-              const int mine = (cl & ~3) + t;
-              if (mine <= cl) {
-                float* pk = p.probs + ((int64_t)b * p.ncls + mine) * P;
-                if (v0) pk[o0] = sm0.prob(q0);
-                if (v1) pk[o1] = sm1.prob(q1);
-              }
-            }
-          }
-        } else {
-          float best0 = -INFINITY, best1 = -INFINITY;
-          int arg0 = 0, arg1 = 0;
-#pragma unroll 1
-          for (int cl = 0; cl < p.ncls; ++cl) {
-            float l0, l1;
-            class_logits(cl, l0, l1);
-            if (best0 == best0 && (l0 > best0 || l0 != l0)) { best0 = l0; arg0 = cl; }
-            if (best1 == best1 && (l1 > best1 || l1 != l1)) { best1 = l1; arg1 = cl; }
-            if (p.oc_y && t == (cl & 3)) {
-              float* yk = p.oc_y + ((int64_t)b * p.ncls + cl) * P;
-              if (v0) yk[o0] = l0;
-              if (v1) yk[o1] = l1;
-            }
-          }
-          if (p.cls) {
-            if (v0 && t == 0) p.cls[(int64_t)b * P + o0] = arg0;
-            if (v1 && t == 1) p.cls[(int64_t)b * P + o1] = arg1;
-          }
+        }
+        if (p.cls) {
+          if (v0 && t == 0) p.cls[(int64_t)b * P + o0] = arg0;
+          if (v1 && t == 1) p.cls[(int64_t)b * P + o1] = arg1;
         }
       } else if (p.oc_y) {
         // fused OutConv: each pixel's dot product over all Cout <= N_TILE activations.  Channels past Cout have zero
@@ -999,11 +956,11 @@ extern "C" int smaat_dsconv_pool_parts(int H, int W) {
 static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride, const float* dw_w,
                       const float* dw_b, const float* pw_w, const float* pw_w_lo, const float* scale, const float* shift, float* y,
                       int64_t y_bstride, double* stats, const float* oc_w, const float* oc_b, float* oc_y, int ncls, int64_t* cls,
-                      float* probs, const float* gate_sc, const float* gate_sa, float* pool_sum, float* pool_max, float* pooled, int B,
-                      int H, int W, int k, int Cout, int relu, int mode, void* stream) {
-  // head: an OutConv in the epilogue (one class, or ncls classes with the argmax or the softmax) replaces the activation output
+                      const float* gate_sc, const float* gate_sa, float* pool_sum, float* pool_max, float* pooled, int B, int H, int W,
+                      int k, int Cout, int relu, int mode, void* stream) {
+  // head: an OutConv in the epilogue (one class, or ncls classes with the argmax) replaces the activation output
   const bool head = oc_y || ncls > 0;
-  SMAAT_REQUIRE(x0 && dw_w && pw_w && (y || oc_y || cls || probs), "dsconv: null pointer");
+  SMAAT_REQUIRE(x0 && dw_w && pw_w && (y || oc_y || cls), "dsconv: null pointer");
   SMAAT_REQUIRE(!gate_sc == !gate_sa, "dsconv: the CBAM gate needs both sc and sa");
   SMAAT_REQUIRE(!gate_sa || aligned16(gate_sa), "dsconv: the CBAM gate map must be 16-byte aligned");
   SMAAT_REQUIRE(!pool_sum || (pool_max && pooled && y && !oc_y && !stats), "dsconv: the CBAM pools need sum, max and max-pool outputs and y");
@@ -1076,7 +1033,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   }
   DsParams p;
   p.dw_w = dw_w; p.dw_b = dw_b; p.scale = scale; p.shift = shift; p.y = y; p.y_bstride = y_bstride; p.stats = stats;
-  p.oc_w = oc_w; p.oc_b = oc_b; p.oc_y = oc_y; p.ncls = ncls; p.cls = cls; p.probs = probs;
+  p.oc_w = oc_w; p.oc_b = oc_b; p.oc_y = oc_y; p.ncls = ncls; p.cls = cls;
   p.gate_sc = gate_sc; p.pool_sum = pool_sum; p.pool_max = pool_max; p.pooled = pooled; p.npart = 0;
   p.C0 = C0; p.C1 = C1; p.H = H; p.W = W; p.Cout = Cout; p.relu = relu; p.K = K;
   p.tiles_x = p.tiles_y = p.npass = p.total_tiles = p.nchunks = 0;
@@ -1109,8 +1066,7 @@ extern "C" int smaat_dsconv_fwd(const float* x0, int C0, int64_t x0_bstride, con
                                 int W, int k, int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(y, "dsconv: null output");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, stats, nullptr,
-                    nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode,
-                    stream);
+                    nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
 }
 
 /* The network's last two modules in one kernel: DS conv -> BN/ReLU -> OutConv(Cout -> 1) (reference models/SmaAt_UNet.py:55-56,
@@ -1122,7 +1078,7 @@ extern "C" int smaat_dsconv_outconv_fwd(const float* x0, int C0, int64_t x0_bstr
                                         float* logits, int B, int H, int W, int k, int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(oc_w && logits, "dsconv+outconv: null pointer");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
-                    logits, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
+                    logits, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
 }
 
 extern "C" int smaat_dsconv_classify_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
@@ -1151,26 +1107,7 @@ extern "C" int smaat_dsconv_classify_fwd(const float* x0, int C0, int64_t x0_bst
                     (reinterpret_cast<uintptr_t>(classes) & 7u) == 0,
                 "dsconv+classify: weights / logits must be 4-byte and classes 8-byte aligned");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
-                    logits, K, classes, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
-}
-
-/* The same epilogue ending in the K softmax probabilities of each pixel (the reference's softmax(y_pred) before its argmax,
- * train_SmaAtUNet.py:76).  The probabilities equal, bit for bit, smaat_softmax_channels_fwd applied to the logits
- * smaat_dsconv_classify_fwd writes: the same logits, fed to the same SoftmaxAcc (softmax.cuh) in the same class order.
- * Only the K probability planes reach HBM. */
-extern "C" int smaat_dsconv_probs_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
-                                      const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
-                                      const float* scale, const float* shift, const float* oc_w, const float* oc_b, int K,
-                                      float* probs, int B, int H, int W, int k, int Cout, int relu, int mode, void* stream) {
-  SMAAT_REQUIRE(oc_w && probs, "dsconv+probs: needs the OutConv weight and a probs output");
-  SMAAT_REQUIRE(K >= 1, "dsconv+probs: K=%d classes", K);
-  if (K > DS_MAX_CLASSES)
-    return fail(SMAAT_E_UNSUPPORTED, "dsconv+probs: K=%d classes, the fused epilogue takes at most %d; use smaat_dsconv_fwd + "
-                                     "smaat_outconv_fwd + smaat_softmax_channels_fwd", K, DS_MAX_CLASSES);
-  SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(oc_w) & 3u) == 0 && (reinterpret_cast<uintptr_t>(probs) & 3u) == 0,
-                "dsconv+probs: weights / probs must be 4-byte aligned");
-  return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
-                    nullptr, K, nullptr, probs, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
+                    logits, K, classes, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
 }
 
 /* The fused DS conv of the serving forward with the CBAM fusions around it (models/layers.py:90-141, SmaAt_UNet.py:41-57).
@@ -1185,6 +1122,5 @@ extern "C" int smaat_dsconv_cbam_fwd(const float* x0, int C0, int64_t x0_bstride
                                      int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(y, "dsconv_cbam: null output");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, nullptr, nullptr,
-                    nullptr, nullptr, 0, nullptr, nullptr, gate_sc, gate_sa, pool_sum, pool_max, pooled, B, H, W, k, Cout, relu, mode,
-                    stream);
+                    nullptr, nullptr, 0, nullptr, gate_sc, gate_sa, pool_sum, pool_max, pooled, B, H, W, k, Cout, relu, mode, stream);
 }

@@ -30,8 +30,8 @@ class _ServingForward(nn.Module):
         return self._serve(x, "classes")
 
     def forward_probs(self, x):
-        """The (B, n_classes, H, W) fp32 class probabilities, softmax over the logits' channels (the reference's
-        ``softmax(y_pred)``, train_SmaAtUNet.py:76).  Inference only, with no gradient."""
+        """The (B, n_classes, H, W) fp32 class probabilities, ``softmax_channels`` of ``forward_serving``'s logits (the
+        reference's ``softmax(y_pred)``, train_SmaAtUNet.py:76).  Inference only, with no gradient."""
         return self._serve(x, "probs")
 
     def _serve(self, x, head):
@@ -44,10 +44,11 @@ class SmaAt_UNet(_ServingForward):
     """The serving forward (``forward_serving`` / ``forward_classes`` / ``forward_probs``) has the fusions the plain-call API
     cannot express:
     * up4's last DS conv applies the OutConv in its epilogue (SmaAt_UNet.py:55-56), so the 64-channel activation never reaches
-      HBM: the 1-class OutConv for the logits, the n_classes-class OutConv and the argmax / softmax for class maps and
-      probabilities (n_classes <= 32; more classes take the unfused convs, OutConv and the argmax / softmax kernel).  Each
-      class's logit there is the one-class fused OutConv's arithmetic, which sums in another order than the unfused OutConv of
-      the logits route: pixels whose top two logits lie within rounding of each other may pick the other class;
+      HBM: the 1-class OutConv for the logits, the n_classes-class OutConv and the argmax for class maps (n_classes <= 32;
+      more classes take the unfused convs, OutConv and the argmax kernel).  Each class's logit there is the one-class fused
+      OutConv's arithmetic, which sums in another order than the unfused OutConv of the logits route: pixels whose top two
+      logits lie within rounding of each other may pick the other class.  The probabilities are the channel softmax of the
+      logits route's output;
     * the three large CBAMs (levels 1-3) never write their output: they compute only their two gates, and the first DS
       conv of up2 / up3 / up4 applies them as it loads the skip, with the products the CBAM's own kernel would have used
       (bit for bit the same logits).  Levels 4-5 run the plain calls."""
@@ -108,10 +109,8 @@ class UNet(_ServingForward):
     """The dense baseline of ``models/unet_precip_regression_lightning.py:7-38`` (the Lightning class without its training
     plumbing): same attribute names (hence the reference's 128 state_dict keys with ``bilinear=True``) and forward order.
 
-    Its serving forward is bit for bit ``forward``'s logits and ``argmax_channels`` / ``softmax_channels`` of them.  With
-    ``ops.set_fused_dense_head(True)`` up4's last 3x3 conv applies the OutConv (and the argmax / softmax) in its epilogue, so
-    neither the 64-channel activation nor the logits reach HBM; by default (the faster route on an H100), and where the
-    epilogue does not take the shape ('fp32' mode, W % 4 != 0, more than 32 classes), the plain calls."""
+    Its serving forward runs the plain calls: bit for bit ``forward``'s logits and ``argmax_channels`` / ``softmax_channels``
+    of them (an OutConv epilogue in up4's last 3x3 conv measured slower on an H100: DESIGN section 6)."""
 
     def __init__(self, n_channels, n_classes, bilinear=True):
         super().__init__()
@@ -151,10 +150,8 @@ class UNetAttention(_ServingForward):
     """``models/unet_precip_regression_lightning.py:41-83``: UNet with a CBAM on every skip (178 state_dict keys with
     ``bilinear=True``).  ``downN`` runs on the un-attended map right after ``cbamN`` did, so the CBAM hands it its 2x2 max-pool.
 
-    Its serving forward is bit for bit ``forward``'s logits and ``argmax_channels`` / ``softmax_channels`` of them.  With
-    ``ops.set_fused_dense_head(True)`` up4's last 3x3 conv applies the OutConv (and the argmax / softmax) in its epilogue, so
-    neither the 64-channel activation nor the logits reach HBM; by default (the faster route on an H100), and where the
-    epilogue does not take the shape ('fp32' mode, W % 4 != 0, more than 32 classes), the plain calls."""
+    Its serving forward runs the plain calls: bit for bit ``forward``'s logits and ``argmax_channels`` / ``softmax_channels``
+    of them (an OutConv epilogue in up4's last 3x3 conv measured slower on an H100: DESIGN section 6)."""
 
     def __init__(self, n_channels, n_classes, bilinear=True, reduction_ratio=16):
         super().__init__()

@@ -130,14 +130,16 @@ class DepthwiseSeparableConv(_CachingModule):
 
     def run_head(self, x, scale, shift, relu, outconv, head):
         """``run`` followed by the OutConv ``outconv=(weight (K, Cout[,1,1]), bias or None)`` in the fused kernel's epilogue, ending
-        in ``head``: "logits" (one class: the (B, 1, H, W) logits, ``ops.dsconv``), "classes" (the (B, H, W) int64 class map of
-        the K-class logits, ``ops.dsconv_classify``) or "probs" (their (B, K, H, W) softmax probabilities, ``ops.dsconv_probs``).
-        None where that kernel does not take the request: the caller then runs this conv and the OutConv separately."""
+        in ``head``: "logits" (one class: the (B, 1, H, W) logits, ``ops.dsconv``) or "classes" (the (B, H, W) int64 class map
+        of the K-class logits, ``ops.dsconv_classify``).  None where that kernel does not take the request: the caller then runs
+        this conv and the OutConv separately."""
+        if head not in ("logits", "classes"):
+            raise ValueError(f"run_head: head must be 'logits' or 'classes', got {head!r}")
         dw_b, shift, mode, split = self._operands(shift)
         args = (x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(), scale, shift, relu)
         if head == "logits":
             return ops.dsconv(*args, mode=mode, w_split=split, outconv=outconv)
-        return (ops.dsconv_probs if head == "probs" else ops.dsconv_classify)(*args, *outconv, mode=mode, w_split=split)
+        return ops.dsconv_classify(*args, *outconv, mode=mode, w_split=split)
 
     def cbam_takes(self, x, x1=None, gate=False, pools=False) -> bool:
         """Whether ``run_cbam`` takes this input: the fused kernel with the serving forward's CBAM fusions."""
@@ -184,8 +186,8 @@ def apply_head(module, x, head):
 class _DoubleConvBase(_CachingModule):
     """What DoubleConvDS and DoubleConv share: ``double_conv`` = (conv => BN => ReLU) * 2, its folded BatchNorm, and the routing
     of a call to its eval fast path, to autograd / batch statistics, and to an OutConv head.  A subclass provides
-    ``_folded_conv`` (conv 0 or 3 with its folded BatchNorm and the ReLU), ``_unfolded`` (the block under autograd or batch
-    statistics) and ``_fused_last`` (the last conv with the OutConv and the head in its epilogue, or None)."""
+    ``_folded_conv`` (conv 0 or 3 with its folded BatchNorm and the ReLU) and ``_unfolded`` (the block under autograd or batch
+    statistics), and may override ``_fused_last`` (the last conv with the OutConv and the head in its epilogue)."""
 
     def __init__(self, double_conv):
         super().__init__()
@@ -231,6 +233,10 @@ class _DoubleConvBase(_CachingModule):
         y = self._folded_conv(0, x, x1, gate)
         out = self._fused_last(y, outconv, head)
         return out if out is not None else apply_head(outconv, self._folded_conv(3, y), head)
+
+    def _fused_last(self, y, outconv, head):
+        """The last conv with the OutConv and the head in its epilogue, or None: then the last conv and ``apply_head`` run."""
+        return None
 
     def forward(self, x):
         return self.run(x)
@@ -283,12 +289,13 @@ class DoubleConvDS(_DoubleConvBase):
         return Fn.double_conv_fwd(self, x, x1)[0]
 
     def _fused_last(self, y, outconv, head):
-        """The last DS conv with the OutConv and the head in its epilogue (smaat_dsconv_outconv_fwd, smaat_dsconv_classify_fwd,
-        smaat_dsconv_probs_fwd), or None where that kernel does not take the shape (K > 32, Cout > 128, ...).  Logits only for a
-        one-class OutConv: the K-class epilogue sums each logit in another order than the OutConv kernel, which would change
-        the logits ``InferenceSession`` serves (DESIGN section 9)."""
+        """The last DS conv with the OutConv and the head in its epilogue (smaat_dsconv_outconv_fwd, smaat_dsconv_classify_fwd),
+        or None where that kernel does not take the shape (K > 32, Cout > 128, ...).  Logits only for a one-class OutConv: the
+        K-class epilogue sums each logit in another order than the OutConv kernel, which would change the logits
+        ``InferenceSession`` serves (DESIGN section 9).  Never probabilities: they are the channel softmax of the served logits,
+        and a softmax epilogue measured slower than that kernel (DESIGN section 6)."""
         oc = outconv.conv
-        if head == "logits" and oc.out_channels != 1:
+        if head == "probs" or (head == "logits" and oc.out_channels != 1):
             return None
         s1, t1 = self._folded(3)
         ob = oc.bias.detach() if oc.bias is not None else None
@@ -486,9 +493,8 @@ class DoubleConv(_DoubleConvBase):
 
     def run(self, x, x1=None, outconv=None, head="logits"):
         """``outconv`` (an OutConv module): return OutConv(block(x)) ending in ``head`` (``HEADS``) -- its logits, their
-        (B, H, W) int64 class map or their (B, K, H, W) softmax probabilities (no gradient).  In eval mode without autograd the
-        last conv applies the OutConv and the argmax / softmax in its epilogue where it takes the shape (``_fused_last``): the
-        block's output is then never written, and the result is bit for bit that of the separate calls."""
+        (B, H, W) int64 class map or their (B, K, H, W) softmax probabilities (no gradient): the block, the OutConv kernel and
+        the channel argmax / softmax kernel (``apply_head``)."""
         _check_head(head, outconv)
         ops._req(x, "input", 4)
         if x1 is not None:
@@ -508,21 +514,6 @@ class DoubleConv(_DoubleConvBase):
             return DoubleConvFn.run(self, x, x1)
         from . import functional as Fn       # batch statistics (and running-stat update), no tape
         return Fn.dense_double_conv_fwd(self, x, x1)[0]
-
-    def _fused_last(self, y, outconv, head):
-        """The last conv with the OutConv and the head in its epilogue (smaat_conv3x3_classify_fwd / smaat_conv3x3_probs_fwd),
-        or None: unless ops.set_fused_dense_head(True), and where the epilogue does not take the shape ('fp32', Cout > 64,
-        K > 32, W % 4 != 0, ...)."""
-        if not ops.fused_dense_head():
-            return None
-        s1, t1 = self._folded(3)
-        wp, hi, lo = self.packed(3, y.shape[1])
-        oc = outconv.conv
-        args = (y, wp, self.double_conv[3].out_channels, s1, t1, True, oc.weight.detach(), oc.bias.detach() if oc.bias is not None else None)
-        split = (hi, lo) if hi is not None else None
-        if head == "probs":
-            return ops.conv3x3_probs(*args, w_split=split)
-        return ops.conv3x3_classify(*args, w_split=split, want_logits=head == "logits", want_classes=head == "classes")
 
 
 class Down(_Down):

@@ -147,16 +147,6 @@ def _tf32_split(w, m, w_split):
     return w_split if w_split is not None else split_tf32(w)
 
 
-def _outconv_operands(oc_weight, oc_bias, Cout):
-    """The K-class OutConv of a fused epilogue: (weight (K, Cout[,1,1]), bias (K) or None, K), checked against Cout."""
-    ow = _dense(oc_weight, "outconv.weight")
-    K = ow.shape[0]
-    assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
-    ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
-    assert ob is None or ob.numel() == K, f"OutConv bias {tuple(oc_bias.shape)} does not match K={K}"
-    return ow, ob, K
-
-
 # ---------------------------------------------------------------------------------------------
 def dw3x3(x, weight, bias, k, x1=None, in_scale=None, in_shift=None, loader=0):
     """Depthwise 3x3/pad 1 over the virtual concat [x, x1] (layers.py:38-44; parts_ds.py:85)."""
@@ -316,9 +306,8 @@ _fuse_classify = os.environ.get("SMAAT_FUSE_CLASSIFY", "1") != "0"
 
 
 def set_fused_classify(enabled: bool) -> None:
-    """Enable/disable the K-class OutConv + argmax or softmax in the last DS conv's epilogue, and the OutConv epilogue of the
-    dense networks' last 3x3 conv (default on; off = that conv, OutConv and the channel argmax / softmax kernel as separate
-    launches).  For A/B measurements (tools/bench_classes.py, tools/bench_probs.py, tools/bench_dense_serving.py)."""
+    """Enable/disable the K-class OutConv + argmax in the last DS conv's epilogue (default on; off = that conv, OutConv and
+    the channel argmax kernel as separate launches).  For A/B measurements (tools/bench_classes.py, tools/bench_probs.py)."""
     global _fuse_classify
     _fuse_classify = bool(enabled)
 
@@ -342,23 +331,9 @@ def dsconv_classify(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_
     (smaat_dsconv_classify_fwd).  oc_weight (K, Cout[,1,1]), oc_bias (K) or None.  Returns the (B, H, W) int64 class map, or
     (classes, (B, K, H, W) logits) with ``want_logits``; class j's logits are bit for bit those of ``dsconv(..., outconv=(oc_weight[j],
     oc_bias[j]))``.  Returns None where ``dsconv_classify_takes`` is False (the caller then runs the layers apart)."""
-    return _dsconv_head(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, False,
-                        want_logits)
-
-
-def dsconv_probs(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, x1=None, mode=None, w_split=None):
-    """``dsconv`` followed by OutConv(Cout -> K) and the softmax over the K classes, all in the fused kernel's epilogue
-    (smaat_dsconv_probs_fwd): the (B, K, H, W) fp32 probabilities, bit for bit ``softmax_channels`` of the logits
-    ``dsconv_classify(..., want_logits=True)`` returns.  Inference only.  Returns None where ``dsconv_classify_takes`` is
-    False (the caller then runs the layers apart)."""
-    return _dsconv_head(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, True)
-
-
-def _dsconv_head(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, probs,
-                 want_logits=False):
-    """``dsconv_classify`` (smaat_dsconv_classify_fwd) or, with ``probs``, ``dsconv_probs`` (smaat_dsconv_probs_fwd)."""
     mode = mode or _pw_mode
-    K = _dense(oc_weight, "outconv.weight").shape[0]
+    ow = _dense(oc_weight, "outconv.weight")
+    K = ow.shape[0]
     if not dsconv_classify_takes(x, x1, pw_weight, k, K, mode):
         return None
     x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
@@ -366,23 +341,18 @@ def _dsconv_head(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_wei
     Cin = C0 + C1
     w2d = _pw_matrix(pw_weight, k, Cin)
     Cout, Kd = w2d.shape
-    ow, ob, K = _outconv_operands(oc_weight, oc_bias, Cout)
+    assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
+    ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
+    assert ob is None or ob.numel() == K, f"OutConv bias {tuple(oc_bias.shape)} does not match K={K}"
     w2d, wlo = _tf32_split(w2d, PW_MODES[mode], w_split)
-    lib = _lib.load()
-    if probs:
-        out = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32)
-        name, fn, outs, written = "smaat_dsconv_probs_fwd", lib.smaat_dsconv_probs_fwd, (_ptr(out),), K
-    else:
-        classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64)
-        logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
-        out = (classes, logits) if want_logits else classes
-        name, fn, outs, written = ("smaat_dsconv_classify_fwd", lib.smaat_dsconv_classify_fwd, (_ptr(logits), _ptr(classes)),
-                                   (K if want_logits else 0) + 2)
-    _call(f"{name}[C{Cin}_N{Cout}_K{K}_S{H}]",
-          4 * B * H * W * (Cin + written) + 4 * Kd * Cout, 2 * B * H * W * (Kd * (Cout + 9) + (2 if probs else 1) * K * Cout),
-          fn, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(_dense(dw_weight, "depthwise.weight")), _ptr(dw_bias), _ptr(w2d), _ptr(wlo),
-          _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, *outs, B, H, W, k, Cout, int(bool(relu)), PW_MODES[mode], _stream())
-    return out
+    classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64)
+    logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
+    _call(f"smaat_dsconv_classify_fwd[C{Cin}_N{Cout}_K{K}_S{H}]",
+          4 * B * H * W * (Cin + (K if want_logits else 0) + 2) + 4 * Kd * Cout, 2 * B * H * W * (Kd * (Cout + 9) + K * Cout),
+          _lib.load().smaat_dsconv_classify_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(_dense(dw_weight, "depthwise.weight")),
+          _ptr(dw_bias), _ptr(w2d), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob), K, _ptr(logits), _ptr(classes), B, H,
+          W, k, Cout, int(bool(relu)), PW_MODES[mode], _stream())
+    return (classes, logits) if want_logits else classes
 
 
 def softmax_channels(x):
@@ -461,84 +431,6 @@ def conv3x3(x, wp, Cout, scale, shift, relu, x1=None, mode=None, w_split=None, s
           _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(wp), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(y), Cout * H * W, _ptr(stats),
           B, H, W, Cout, int(bool(relu)), m, _stream())
     return y
-
-
-# Whether UNet / UNetAttention (DoubleConv.run with an OutConv) take the OutConv epilogue of their last 3x3 conv.  Off by
-# default: on an H100 the fused last conv is slower than the conv + OutConv (+ argmax / softmax) launches it replaces (README,
-# DESIGN section 6), and both routes give the same bits.
-_fuse_dense_head = os.environ.get("SMAAT_FUSE_DENSE_HEAD", "0") == "1"
-
-
-def set_fused_dense_head(enabled: bool) -> None:
-    """Let the dense networks' serving forward (``UNet`` / ``UNetAttention`` ``forward_serving`` / ``forward_classes`` /
-    ``forward_probs``, ``DoubleConv.run(outconv=...)``) run the OutConv and the argmax / softmax in the last 3x3 conv's
-    epilogue (``conv3x3_classify`` / ``conv3x3_probs``).  Default off (SMAAT_FUSE_DENSE_HEAD=1 presets it on): the outputs are
-    bit for bit the same, and the separate launches are faster on an H100.  set_fused_classify(False) turns it off too."""
-    global _fuse_dense_head
-    _fuse_dense_head = bool(enabled)
-
-
-def fused_dense_head() -> bool:
-    return _fuse_dense_head
-
-
-def conv3x3_classify_takes(x, x1, wp, Cout, n_classes, mode=None) -> bool:
-    """True when ``conv3x3_classify`` / ``conv3x3_probs`` run on these inputs: the tensor-core conv with a ``n_classes``-class
-    OutConv in its epilogue (smaat_conv3x3_classify_eligible: the tensor-core conv's shapes, Cout <= 64, 1 <= n_classes <= 32,
-    'tf32' / 'tf32x3'), and not set_fused_classify(False)."""
-    mode = mode or _pw_mode
-    if not _fuse_classify or PW_MODES[mode] == 0:
-        return False
-    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
-    return bool(_lib.load().smaat_conv3x3_classify_eligible(_ptr(x), bs0, _ptr(x1), C1, bs1, _ptr(wp), x.shape[3], Cout, int(n_classes),
-                                                            PW_MODES[mode]))
-
-
-def conv3x3_classify(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1=None, mode=None, w_split=None, want_logits=False,
-                     want_classes=True):
-    """``conv3x3`` followed by OutConv(Cout -> K) (and the channel argmax) in the tensor-core kernel's epilogue
-    (smaat_conv3x3_classify_fwd).  oc_weight (K, Cout[,1,1]), oc_bias (K) or None.  Returns the (B, H, W) int64 class map; with
-    ``want_logits`` also the (B, K, H, W) logits, as (classes, logits), or the logits alone with ``want_classes=False``.  Bit for
-    bit ``outconv(conv3x3(...))`` and ``argmax_channels`` of it.  Returns None where ``conv3x3_classify_takes`` is False (the
-    caller then runs the layers apart)."""
-    assert want_logits or want_classes, "conv3x3_classify: ask for the logits, the class map or both"
-    return _conv3x3_head(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, False, want_logits, want_classes)
-
-
-def conv3x3_probs(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1=None, mode=None, w_split=None):
-    """``conv3x3`` followed by OutConv(Cout -> K) and the softmax over the K classes in the tensor-core kernel's epilogue
-    (smaat_conv3x3_probs_fwd): the (B, K, H, W) fp32 probabilities, bit for bit ``softmax_channels(outconv(conv3x3(...)))``.
-    Inference only.  Returns None where ``conv3x3_classify_takes`` is False."""
-    return _conv3x3_head(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, True)
-
-
-def _conv3x3_head(x, wp, Cout, scale, shift, relu, oc_weight, oc_bias, x1, mode, w_split, probs, want_logits=False,
-                  want_classes=False):
-    """``conv3x3_classify`` (smaat_conv3x3_classify_fwd) or, with ``probs``, ``conv3x3_probs`` (smaat_conv3x3_probs_fwd)."""
-    mode = mode or _pw_mode
-    K = _dense(oc_weight, "outconv.weight").shape[0]
-    if not conv3x3_classify_takes(x, x1, wp, Cout, K, mode):
-        return None
-    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
-    B, C0, H, W = x.shape
-    Cin = C0 + C1
-    assert wp.shape == (Cout, 9 * (_pad32(C0) + _pad32(C1))), f"packed weight {tuple(wp.shape)} does not match Cin={C0}+{C1}"
-    ow, ob, K = _outconv_operands(oc_weight, oc_bias, Cout)
-    wp, wlo = _tf32_split(wp, PW_MODES[mode], w_split)
-    lib = _lib.load()
-    if probs:
-        out = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32)
-        name, fn, outs, written = "smaat_conv3x3_probs_fwd", lib.smaat_conv3x3_probs_fwd, (_ptr(out),), K
-    else:
-        classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64) if want_classes else None
-        logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
-        out = ((classes, logits) if want_classes else logits) if want_logits else classes
-        name, fn, outs, written = ("smaat_conv3x3_classify_fwd", lib.smaat_conv3x3_classify_fwd, (_ptr(logits), _ptr(classes)),
-                                   (K if want_logits else 0) + (2 if want_classes else 0))
-    _call(f"{name}[C{Cin}_N{Cout}_K{K}_S{H}x{W}]", 4 * B * H * W * (Cin + written) + 36 * Cin * Cout,
-          2 * B * H * W * Cout * (9 * Cin + K), fn, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(wp), _ptr(wlo), _ptr(scale),
-          _ptr(shift), _ptr(ow), _ptr(ob), K, *outs, B, H, W, Cout, int(bool(relu)), PW_MODES[mode], _stream())
-    return out
 
 
 def conv3x3_bwd_weight(dz, x, x1, dW, mode=None):

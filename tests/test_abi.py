@@ -34,7 +34,7 @@ def test_binding_table_matches_header():
 
 def test_abi_version_and_error_string():
     lib = S._lib.load()
-    assert lib.smaat_abi_version() == 2
+    assert lib.smaat_abi_version() == 3
     # argument validation happens on the host before any CUDA call: usable without a GPU
     rc = lib.smaat_maxpool2_fwd(None, None, 1, 4, 4, None)
     assert rc == -1 and b"maxpool2" in lib.smaat_last_error()

@@ -1,8 +1,7 @@
 """-m gpu: class probabilities from multi-class models.  smaat_softmax_channels_fwd against float64 softmax and torch.softmax,
-with torch's NaN / 0 / 1 pattern on non-finite logits; smaat_dsconv_probs_fwd (K-class OutConv + softmax in the last DS conv's
-epilogue) bit for bit against the softmax kernel applied to smaat_dsconv_classify_fwd's logits, at up4's last conv shapes and at
-partial tiles; SmaAt_UNet.forward_probs against float64 softmax of the float64 port's logits; InferenceSession(output="probs")
-end to end."""
+with torch's NaN / 0 / 1 pattern on non-finite logits; SmaAt_UNet.forward_probs bit for bit the softmax kernel applied to
+forward_serving's logits, and against float64 softmax of the float64 port's logits; InferenceSession(output="probs") end to
+end."""
 import numpy as np
 import pytest
 import torch
@@ -17,15 +16,7 @@ from tests._util import NET_TOL, load_np_state_dict
 
 pytestmark = pytest.mark.gpu
 
-C = 64                                    # up4's last conv: 64 -> 64 channels (UpDS(128, 64): DoubleConvDS(128, 64, 64))
 ABS_TOL, REL_TOL = 1e-6, 1e-5             # softmax rounding: absolute, and relative where the float64 probability > 1e-30
-
-
-@pytest.fixture(params=["smem", "regs"])
-def ds_impl(request):
-    ops.set_dsconv_impl(request.param)
-    yield request.param
-    ops.set_dsconv_impl("auto")
 
 
 def _mx(t):
@@ -123,103 +114,23 @@ def test_softmax_channels_nonfinite_is_torchs_pattern(vector):
     assert bool((ops.softmax_channels(x) == 1.0).all())
 
 
-# ---- the fused epilogue --------------------------------------------------------------------------------------------------------
-def _layer(B, H, W, k, seed, cout=C):
-    g = torch.Generator().manual_seed(seed)
-
-    def u(*shape, lo=-1.0, hi=1.0):
-        return (torch.rand(shape, generator=g) * (hi - lo) + lo).cuda()
-
-    return dict(x=u(B, C, H, W, lo=0.0), dw_w=u(k * C, 1, 3, 3, lo=-0.5, hi=0.5), dw_b=u(k * C, lo=-0.1, hi=0.1),
-                pw_w=u(cout, k * C, 1, 1, lo=-0.15, hi=0.15), scale=u(cout, lo=0.5, hi=1.5), shift=u(cout, lo=-0.2, hi=0.2), k=k, g=g,
-                cout=cout)
-
-
-def _oc(L, K):
-    g = L["g"]
-    # logits spread over several units, so the probabilities are far from uniform
-    return (torch.rand(K, L["cout"], generator=g) * 4.0 - 2.0).cuda(), (torch.rand(K, generator=g) * 2.0 - 1.0).cuda()
-
-
-def _args(L):
-    return (L["x"], L["dw_w"], L["dw_b"], L["k"], L["pw_w"], L["scale"], L["shift"], True)
-
-
-def _fused_equals_softmax_of_classify_logits(L, K, mode, bias=True):
-    ow, ob = _oc(L, K)
-    ob = ob if bias else None
-    p = ops.dsconv_probs(*_args(L), ow, ob, mode=mode)
-    assert p is not None, f"the fused probability epilogue refused the layer (K={K})"
-    _, lg = ops.dsconv_classify(*_args(L), ow, ob, mode=mode, want_logits=True)
-    want = ops.softmax_channels(lg)
-    B, _, H, W = L["x"].shape
-    assert p.dtype == torch.float32 and tuple(p.shape) == (B, K, H, W)
-    assert torch.equal(p, want), (f"K={K} bias={bias}: fused probabilities differ from softmax_channels(classify logits) at "
-                                  f"{int((p != want).sum())} of {p.numel()} values")
-    assert torch.equal(ops.dsconv_probs(*_args(L), ow, ob, mode=mode), p), f"K={K}: a second launch differs"
-    return p, lg
-
-
-@pytest.mark.parametrize("mode", ["tf32", "tf32x3"])
-@pytest.mark.parametrize("k", [1, 2])
-@pytest.mark.parametrize("shape", [(8, 224, 224), (2, 288, 288)])   # B, H, W
-def test_probs_are_the_softmax_of_the_classify_logits_bit_for_bit(shape, k, mode, ds_impl):
-    B, H, W = shape
-    L = _layer(B, H, W, k, seed=H + 10 * k)
-    for K in (2, 8, 21, 32):
-        for bias in (True, False) if K == 8 else (True,):
-            p, lg = _fused_equals_softmax_of_classify_logits(L, K, mode, bias)
-            if K == 21 and bias:
-                _check_softmax(p[:1, :, :64, :64], lg[:1, :, :64, :64].cpu(), f"fused K={K}")
-
-
-@pytest.mark.parametrize("mode", ["tf32", "tf32x3"])
-@pytest.mark.parametrize("k", [1, 2])
-def test_probs_at_cout_128_bit_for_bit(k, mode, ds_impl):
-    """Cout 128: the N_TILE 128 instances, which keep the weights of at most 22 classes beside their rings."""
-    L = _layer(2, 224, 224, k, seed=128 + k, cout=128)
-    _fused_equals_softmax_of_classify_logits(L, 22, mode)
-
-
-@pytest.mark.parametrize("mode", ["tf32", "tf32x3"])
-@pytest.mark.parametrize("k", [1, 2])
-@pytest.mark.parametrize("HW", [(99, 96), (70, 100)])   # PW 32 with an odd H; PW 16, partial tiles both ways
-def test_probs_at_partial_tiles_bit_for_bit(HW, k, mode, ds_impl):
-    H, W = HW
-    L = _layer(2, H, W, k, seed=H + W + k)
-    for K in (8, 21):
-        _fused_equals_softmax_of_classify_logits(L, K, mode)
-
-
-def test_probs_over_32_classes_take_the_unfused_route():
-    L = _layer(2, 64, 64, 2, seed=3)
-    ow, ob = _oc(L, 33)
-    assert ops.dsconv_probs(*_args(L), ow, ob) is None
-    torch.manual_seed(33)
-    m = S.SmaAt_UNet(3, 33).cuda().eval()
-    x = torch.rand(2, 3, 64, 64, device="cuda")
-    with ops.profile() as prof, torch.no_grad():
-        p = m.forward_probs(x)
-    names = prof.summary()
-    assert "smaat_dsconv_probs_fwd" not in names and "smaat_softmax_channels_fwd" in names and "smaat_outconv_fwd" in names
-    with torch.no_grad():
-        lg = m.forward_serving(x)            # the same convs and OutConv, ending in the logits
-    assert torch.equal(p, ops.softmax_channels(lg))
-    _check_softmax(p, lg.cpu(), "SmaAt_UNet(3, 33).forward_probs")
-
-
-def test_fused_classify_switch_turns_the_probability_fusion_off():
-    L = _layer(2, 64, 64, 2, seed=4)
-    ow, ob = _oc(L, 8)
-    ops.set_fused_classify(False)
-    try:
-        assert ops.dsconv_probs(*_args(L), ow, ob) is None
-    finally:
-        ops.set_fused_classify(True)
-    assert ops.dsconv_probs(*_args(L), ow, ob) is not None
-
-
 # ---- the network ---------------------------------------------------------------------------------------------------------------
+def test_forward_probs_is_the_softmax_of_the_serving_logits():
+    # K = 8 and 21 have a fused class-map epilogue, K = 33 does not: the probabilities take the logits route either way
+    for K in (8, 21, 33):
+        torch.manual_seed(K)
+        m = S.SmaAt_UNet(3, K).cuda().eval()
+        x = torch.rand(2, 3, 64, 64, device="cuda")
+        with ops.profile() as prof, torch.no_grad():
+            p = m.forward_probs(x)
+        names = prof.summary()
+        assert "smaat_softmax_channels_fwd" in names and "smaat_outconv_fwd" in names, f"K={K}"
+        with torch.no_grad():
+            lg = m.forward_serving(x)            # the same convs and OutConv, ending in the logits
+        assert torch.equal(p, ops.softmax_channels(lg)), f"K={K}"
+        _check_softmax(p, lg.cpu(), f"SmaAt_UNet(3, {K}).forward_probs")
+
+
 def _net(n_ch, K, seed):
     sd = cast_sd(fill_schema(smaat_unet_schema(n_ch, K, 2), seed), np.float32)
     m = load_np_state_dict(S.SmaAt_UNet(n_ch, K, kernels_per_layer=2), sd).cuda().eval()
@@ -242,7 +153,7 @@ def test_forward_probs_against_float64_port(cfg):
             names = prof.summary()
         finally:
             S.set_pointwise_mode("tf32x3")
-        assert "smaat_dsconv_probs_fwd" in names and "smaat_softmax_channels_fwd" not in names and "smaat_outconv_fwd" not in names
+        assert "smaat_outconv_fwd" in names and "smaat_softmax_channels_fwd" in names
         err = (p.double().cpu() - p64).abs()
         # the softmax Jacobian's infinity norm is at most 1/2: a logit error of e moves a probability by at most e / 2
         bound = 0.5 * NET_TOL[mode] * float(l64.abs().max()) + ABS_TOL + REL_TOL * p64

@@ -38,7 +38,6 @@ FAMILIES = {
     "unetatt_12_1": (lambda: S.UNetAttention(12, 1), 12, 1),
 }
 NAMES = list(FAMILIES)
-DENSE = {"unet_12_1", "unet_3_21_convt", "unetatt_12_1"}
 
 # one tensor per cache kind, where the family has it
 TARGETS = (
@@ -311,9 +310,7 @@ def _struct_cases():
         outputs = ("logits", "classes", "probs") if FAMILIES[name][2] > 1 else ("logits", "classes")
         for output in outputs:
             for fusions in (True, False):
-                out.append((name, output, fusions, False))
-                if fusions and name in DENSE:
-                    out.append((name, output, fusions, True))
+                out.append((name, output, fusions))
     return out
 
 
@@ -332,17 +329,12 @@ def disrupt(m, name):
     torch.cuda.synchronize()
 
 
-@pytest.mark.parametrize("name,output,fusions,dense_head", _struct_cases())
-def test_session_keeps_alive_every_address_its_graph_reads(name, output, fusions, dense_head, monkeypatch):
+@pytest.mark.parametrize("name,output,fusions", _struct_cases())
+def test_session_keeps_alive_every_address_its_graph_reads(name, output, fusions, monkeypatch):
     m = make(name)
-    was = ops.fused_dense_head()
     with monkeypatch.context() as mp:
         rec = PtrRecorder(mp)
-        ops.set_fused_dense_head(dense_head)
-        try:
-            sess = InferenceSession(m, B, (FAMILIES[name][1], HW, HW), output=output, serving_fusions=fusions)
-        finally:
-            ops.set_fused_dense_head(was)
+        sess = InferenceSession(m, B, (FAMILIES[name][1], HW, HW), output=output, serving_fusions=fusions)
     assert sess.graph is not None and rec.ptrs
     own = owners(m)
     pool = tuple(sess.graph.pool())
@@ -363,7 +355,7 @@ def test_session_keeps_alive_every_address_its_graph_reads(name, output, fusions
         blk = block_of(p, blks)
         if blk is None or blk[2] != "active_allocated" or any(a <= p < a + s for a, s in freed):
             stale.append(label(p, own))
-    assert not stale, (f"{name} output={output} fusions={fusions} dense_head={dense_head}: {len(stale)} of {len(rec.ptrs)} "
+    assert not stale, (f"{name} output={output} fusions={fusions}: {len(stale)} of {len(rec.ptrs)} "
                        f"addresses the graph reads were freed: {sorted(set(stale))[:12]}")
 
 

@@ -1,5 +1,5 @@
-"""CPU-side checks of the probability entry points (smaat_dsconv_probs_fwd, smaat_softmax_channels_fwd): bad arguments are
-rejected on the host, before any CUDA call, with SMAAT_E_BADARG or SMAAT_E_UNSUPPORTED; InferenceSession refuses an unknown
+"""CPU-side checks of the probability entry point (smaat_softmax_channels_fwd): bad arguments are rejected on the host,
+before any CUDA call, with SMAAT_E_BADARG or SMAAT_E_UNSUPPORTED; InferenceSession refuses an unknown
 output kind before it touches the device; every model offers probabilities."""
 import pytest
 import torch
@@ -9,27 +9,6 @@ import smaat_unet_b200 as S
 BADARG, UNSUPPORTED = -1, -3
 # fake, 16-byte aligned addresses: never dereferenced, validation fails first
 A = 1 << 20
-
-
-def _probs(lib, oc_w=A, K=8, probs=A, x0=A, Cout=64):
-    # up4's last conv at 64 x 64: x0 (B, 64, H, W), k = 2, Cout = 64, tf32x3
-    return lib.smaat_dsconv_probs_fwd(x0, 64, 64 * 64 * 64, None, 0, 0, A, None, A, A, None, None, oc_w, None, K, probs,
-                                      2, 64, 64, 2, Cout, 1, 2, None)
-
-
-def test_dsconv_probs_rejects_bad_arguments_before_launch():
-    lib = S._lib.load()
-    assert _probs(lib, oc_w=None) == BADARG and b"OutConv weight" in lib.smaat_last_error()
-    assert _probs(lib, probs=None) == BADARG and b"probs output" in lib.smaat_last_error()
-    assert _probs(lib, x0=None) == BADARG
-    assert _probs(lib, K=0) == BADARG and b"K=0" in lib.smaat_last_error()
-    assert _probs(lib, K=-3) == BADARG
-    assert _probs(lib, K=33) == UNSUPPORTED and b"at most 32" in lib.smaat_last_error()
-    assert _probs(lib, probs=A + 2) == BADARG and b"4-byte" in lib.smaat_last_error()
-    assert _probs(lib, oc_w=A + 1) == BADARG and b"4-byte" in lib.smaat_last_error()
-    # the fused kernel's TMA loads need a 16-byte aligned input; Cout > 128: the OutConv needs every channel in one pass
-    assert _probs(lib, x0=A + 4) == UNSUPPORTED
-    assert _probs(lib, Cout=256) == UNSUPPORTED
 
 
 def test_softmax_channels_rejects_bad_arguments_before_launch():

@@ -1,17 +1,15 @@
 """Probability serving timings: InferenceSession(output="logits") + torch.softmax against InferenceSession(output="probs"),
-unfused and fused, alternated rounds, medians and spread, with the card's name and power limit.
+alternated rounds, medians and spread, with the card's name and power limit.
 
     python tools/bench_probs.py [--rounds 7] [--iters 10]
 
 For SmaAt_UNet(3, 21) at B = 8, 3x224x224 (VOC) and SmaAt_UNet(12, 8) at B = 32, 12x288x288 (the rain-bucket classifier):
   dev_logits_softmax     sess.forward(x) on a device-resident batch, then torch.softmax(logits, 1) on the device
-  dev_probs_unfused      the "probs" session built with ops.set_fused_classify(False): the last conv, OutConv and
-                         smaat_softmax_channels_fwd as separate launches inside the graph
-  dev_probs              the "probs" session's forward: OutConv + softmax in the last DS conv's epilogue, inside the graph
-the last DS conv alone (up4's second conv: 64 -> 64 channels, k = 2): smaat_dsconv_classify_fwd (class map only) against
-smaat_dsconv_probs_fwd and against the unfused route (smaat_dsconv_fwd, smaat_outconv_fwd, smaat_softmax_channels_fwd), so the
-cost of the second class loop is visible; and smaat_softmax_channels_fwd alone on (B, K, H, W) logits against its HBM floor
-(8 K bytes per pixel: the logits read once, the probabilities written once), with torch.softmax beside it.
+  dev_probs              the "probs" session's forward: the last conv, OutConv and smaat_softmax_channels_fwd inside the graph
+the last DS conv alone (up4's second conv: 64 -> 64 channels, k = 2): smaat_dsconv_classify_fwd (class map only) against the
+probability route (smaat_dsconv_fwd, smaat_outconv_fwd, smaat_softmax_channels_fwd); and smaat_softmax_channels_fwd alone on
+(B, K, H, W) logits against its HBM floor (8 K bytes per pixel: the logits read once, the probabilities written once), with
+torch.softmax beside it.
 Each round runs every variant once, in turn, timed with CUDA events.  Writes nothing.
 """
 from __future__ import annotations
@@ -62,16 +60,10 @@ def variants_for(n_ch, K, B, HW):
     x = torch.rand(B, n_ch, HW, HW, device="cuda")
     sl = InferenceSession(m, B, (n_ch, HW, HW))
     sp = InferenceSession(m, B, (n_ch, HW, HW), output="probs")
-    ops.set_fused_classify(False)         # the same probabilities through the unfused last conv, OutConv and softmax kernel
-    su = InferenceSession(m, B, (n_ch, HW, HW), output="probs")
-    ops.set_fused_classify(True)
     sink = {}
 
     def dev_logits_softmax():
         sink["a"] = torch.softmax(sl.forward(x), 1)
-
-    def dev_probs_unfused():
-        sink["b"] = su.forward(x)
 
     def dev_probs():
         sink["c"] = sp.forward(x)
@@ -89,9 +81,6 @@ def variants_for(n_ch, K, B, HW):
     def conv_classify():
         sink["d"] = ops.dsconv_classify(*args, ow, ob, w_split=split)
 
-    def conv_probs():
-        sink["e"] = ops.dsconv_probs(*args, ow, ob, w_split=split)
-
     def conv_unfused_probs():
         a = ops.dsconv(*args, w_split=split)
         sink["f"] = ops.softmax_channels(ops.outconv(a, ow, ob))
@@ -105,18 +94,16 @@ def variants_for(n_ch, K, B, HW):
     def softmax_torch():
         sink["h"] = torch.softmax(lg, 1)
 
-    dev = {"dev_logits_softmax": dev_logits_softmax, "dev_probs_unfused": dev_probs_unfused, "dev_probs": dev_probs,
-           "last_conv_classify": conv_classify, "last_conv_probs": conv_probs, "last_conv_unfused_outconv_softmax": conv_unfused_probs,
-           "softmax_channels_kernel": softmax_kernel, "torch_softmax": softmax_torch}
+    dev = {"dev_logits_softmax": dev_logits_softmax, "dev_probs": dev_probs, "last_conv_classify": conv_classify,
+           "last_conv_unfused_outconv_softmax": conv_unfused_probs, "softmax_channels_kernel": softmax_kernel,
+           "torch_softmax": softmax_torch}
     extra = {"d2h_bytes_logits": sl.d2h_bytes_per_step, "d2h_bytes_probs": sp.d2h_bytes_per_step,
-             "launches_per_forward": {"logits": sl.launches_per_forward, "probs": sp.launches_per_forward,
-                                      "probs_unfused": su.launches_per_forward},
+             "launches_per_forward": {"logits": sl.launches_per_forward, "probs": sp.launches_per_forward},
              "softmax_hbm_bytes": 8 * K * B * HW * HW}
     with torch.no_grad():
         p = sp.forward(x).clone()
         pt = torch.softmax(sl.forward(x), 1)
-        extra["max_abs_diff_fused_vs_logits_torch_softmax"] = float((p - pt).abs().max())
-        extra["max_abs_diff_unfused_vs_logits_torch_softmax"] = float((su.forward(x) - pt).abs().max())
+        extra["max_abs_diff_probs_vs_logits_torch_softmax"] = float((p - pt).abs().max())
     return dev, extra
 
 
