@@ -39,10 +39,15 @@ extern "C" {
 #define SMAAT_E_CUDA (-2)     /* CUDA runtime or driver error at launch (see smaat_last_error) */
 #define SMAAT_E_UNSUPPORTED (-3) /* valid request this build has no kernel for */
 
-/* pointwise arithmetic modes (smaat_pw1x1_fwd) */
+/* GEMM arithmetic modes (the `mode` argument of smaat_pw1x1_fwd, smaat_dsconv_*, smaat_conv3x3_fwd) */
 #define SMAAT_PW_FP32_SIMT 0  /* CUDA-core FFMA, exact fp32 products                      */
 #define SMAAT_PW_TF32 1       /* wgmma tf32, fp32 accumulate (1 pass)                     */
 #define SMAAT_PW_TF32X3 2     /* wgmma 3xTF32 split (a_hi*b_hi + a_lo*b_hi + a_hi*b_lo)   */
+/* wgmma bf16: each GEMM operand rounded to bf16 (round to nearest even: fp32's exponent range, 8-bit significand), the products
+ * accumulated in fp32 registers, the epilogue unchanged.  Activations stay fp32 in memory (the kernels round them in
+ * registers); the weight argument is the smaat_pack_bf16 pack of the fp32 weight.  Forward GEMMs only: the weight-gradient
+ * entry points (smaat_pw1x1_bwd_weight_tc, smaat_conv3x3_bwd_weight) refuse it. */
+#define SMAAT_PW_BF16 3
 
 int smaat_abi_version(void);
 const char* smaat_last_error(void);
@@ -76,6 +81,7 @@ int smaat_dw3x3_fwd(const float* x0, int C0, int64_t x0_bstride,
  *   high parts, see smaat_split_tf32); NULL otherwise.
  * stats: NULL, or (2*Cout) fp64 zero-initialised accumulators receiving per-channel
  *   sum and sum of squares of the PRE-activation value scale*acc+shift (train-mode BN). */
+/* mode SMAAT_PW_BF16: w is the smaat_pack_bf16 pack of the (Cout, K) weight ((Cout, K rounded up to 32) bf16), w_lo NULL. */
 int smaat_pw1x1_fwd(const float* x, const float* w, const float* w_lo,
                     const float* scale, const float* shift,
                     float* y, int64_t y_bstride, double* stats,
@@ -87,7 +93,10 @@ int smaat_pw1x1_fwd(const float* x, const float* w, const float* w_lo,
  * the wgmma A operand tiles directly).  Arguments as smaat_dw3x3_fwd (input = virtual concat [x0, x1],
  * dw_w: (k*Cin,3,3), dw_b: (k*Cin) or NULL) and smaat_pw1x1_fwd (pw_w: (Cout, k*Cin) -- the tf32 hi
  * parts in TF32X3 mode, pw_w_lo the lo parts; scale/shift/stats/relu as there).
- * mode: SMAAT_PW_TF32 or SMAAT_PW_TF32X3.  Returns SMAAT_E_UNSUPPORTED for shapes the fused kernel
+ * mode: SMAAT_PW_TF32, SMAAT_PW_TF32X3 or SMAAT_PW_BF16 (pw_w the smaat_pack_bf16 pack of the (Cout, k*Cin) weight, pw_w_lo
+ * NULL; register A form only: with smaat_set_dsconv_impl(1) bf16 requests return SMAAT_E_UNSUPPORTED, as k = 4 does there).
+ * The same modes and weight forms apply to smaat_dsconv_outconv_fwd, smaat_dsconv_classify_fwd and smaat_dsconv_cbam_fwd.
+ * Returns SMAAT_E_UNSUPPORTED for shapes the fused kernel
  * does not take (k not in {1,2}; Cout < 8, or Cout > 128 unless a multiple of 128 up to 512 without batch
  * statistics or OutConv; W % 4; patch waste > 35 %): callers then run
  * smaat_dw3x3_fwd + smaat_pw1x1_fwd.  smaat_dsconv_eligible returns 1/0 for the same test. */
@@ -133,7 +142,8 @@ int smaat_dsconv_classify_fwd(const float* x0, int C0, int64_t x0_bstride, const
  *     partial sums / maxima of y (npart = smaat_dsconv_pool_parts(H, W); smaat_cbam_mlp_partials_fwd finishes the channel
  *     gate from them) and MaxPool2d(2)(y) (parts_ds.py:48; floor for odd H).  Fixed layout and order: no atomics.
  * smaat_dsconv_cbam_eligible: 1 if smaat_dsconv_cbam_fwd takes this request in `mode` (the pools need an instance with the
- *   staged epilogue), else 0. */
+ *   staged epilogue), else 0.  Answers for all three tensor-core modes (0 for SMAAT_PW_FP32_SIMT), as
+ *   smaat_dsconv_classify_eligible does. */
 int smaat_dsconv_cbam_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                                const float* pw_w, int H, int W, int k, int Cout, int mode, int with_gate, int with_pools);
 int smaat_dsconv_pool_parts(int H, int W);
@@ -155,6 +165,11 @@ int smaat_pw1x1_tc_eligible(const float* x, const float* w, int K, int Cout, int
 
 /* hi[i] = tf32_truncate(src[i]); lo[i] = src[i] - hi[i]   (weight preparation for TF32X3) */
 int smaat_split_tf32(const float* src, float* hi, float* lo, int64_t n, void* stream);
+/* Weight preparation for SMAAT_PW_BF16: w (rows, cols) fp32 -> out (rows, cols_out) bf16 (uint16 bit patterns), cols_out = cols
+ * rounded up to 32 (else SMAAT_E_BADARG), out 4-byte aligned.  out[r][16 q + l] = bf16_rn(w[r][16 q + (l & 8) | ((l & 1) << 2) |
+ * ((l >> 1) & 3)]), zero where that column is >= cols: round to nearest even (NaN stays NaN), and within each group of 16 the k
+ * order in which the kernels' bf16 register fragments present the activations, so the GEMM pairs every product as in fp32. */
+int smaat_pack_bf16(const float* w, uint16_t* out, int rows, int cols, int cols_out, void* stream);
 
 /* ---- eval-mode BatchNorm folded to the affine the pw epilogue applies -----------------
  * nn.BatchNorm2d.eval (parts_ds.py:25,34):  scale = gamma / sqrt(rv + eps),
@@ -390,7 +405,8 @@ int smaat_pixel_shuffle2_pad_bwd(const float* g, int64_t g_bstride, float* dt, i
  * smaat_conv3x3_fwd: y[b,o,p] = act(scale[o] * sum_{c,dy,dx} w[o,c,dy,dx] in[b,c,p+(dy-1,dx-1)] + shift[o]), zero outside the
  *   image; scale/shift/stats/relu/y_bstride as smaat_pw1x1_fwd (affine for Cout <= 1024).  mode: SMAAT_PW_FP32_SIMT (CUDA
  *   cores, any shape), SMAAT_PW_TF32 / SMAAT_PW_TF32X3 (wgmma implicit GEMM; wp_lo = the lo parts of smaat_split_tf32 of wp in
- *   TF32X3, wp the hi parts).  The tensor-core modes return SMAAT_E_UNSUPPORTED unless W % 4 == 0, Cout >= 8, x0 / x1 / wp
+ *   TF32X3, wp the hi parts) / SMAAT_PW_BF16 (wp the smaat_pack_bf16 pack of the packed weight, whose rows are already
+ *   multiples of 32 long).  The tensor-core modes return SMAAT_E_UNSUPPORTED unless W % 4 == 0, Cout >= 8, x0 / x1 / wp
  *   16-byte aligned and the batch strides multiples of 4; smaat_conv3x3_tc_eligible answers the same test (1/0).
  * smaat_conv3x3_bwd_weight: dW (Cout, C0 + C1, 3, 3) += sum_{b,p} dz[b,o,p] in[b,c,p+(dy-1,dx-1)], in the nn.Conv2d layout.
  *   dz: (B, Cout, H, W) dense.  mode: SMAAT_PW_FP32_SIMT (CUDA cores, any shape) or SMAAT_PW_TF32 / SMAAT_PW_TF32X3 (wgmma,

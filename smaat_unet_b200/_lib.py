@@ -33,6 +33,7 @@ SIGNATURES = {
     "smaat_dsconv_pool_parts": [_i, _i],
     "smaat_dsconv_cbam_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _l, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_split_tf32": [_p, _p, _p, _l, _p],
+    "smaat_pack_bf16": [_p, _p, _i, _i, _i, _p],
     "smaat_bn_fold": [_p, _p, _p, _p, _p, _f, _p, _p, _i, _p],
     "smaat_channel_stats": [_p, _p, _i, _i, _i, _p],
     "smaat_bn_finalize": [_p, C.c_double, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p, _p, _i, _p],

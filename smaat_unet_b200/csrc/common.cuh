@@ -46,6 +46,9 @@ PFN_encodeTiled get_encode_tiled();
 // Build a fp32 tiled tensor map.  dims/strides innermost first; strides in BYTES for dims 1..rank-1.
 int make_tmap_f32(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                   const uint32_t* box, CUtensorMapSwizzle swizzle, const char* who);
+// the same for any element type (the bf16 weight packs of SMAAT_PW_BF16: CU_TENSOR_MAP_DATA_TYPE_BFLOAT16)
+int make_tmap(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+              const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle, const char* who);
 
 int num_sms();
 

@@ -17,7 +17,7 @@ bool conv3x3_tc_eligible(const float* x0, int64_t bs0, const float* x1, int C1, 
                          int W, int Cout);
 int conv3x3_tc_launch(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* wp, const float* wp_lo,
                       const float* scale, const float* shift, float* y, int64_t y_bstride, double* stats, int B, int H, int W, int Cout,
-                      int relu, bool x3, cudaStream_t st);
+                      int relu, int mode, cudaStream_t st);
 int conv3x3_wgrad_tc_launch(const float* dz, const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, float* dW,
                             int B, int H, int W, int Cout, bool x3, cudaStream_t st);
 
@@ -244,11 +244,12 @@ extern "C" int smaat_conv3x3_fwd(const float* x0, int C0, int64_t x0_bstride, co
       return SMAAT_OK;
     }
     case SMAAT_PW_TF32:
+    case SMAAT_PW_BF16:
       return conv3x3_tc_launch(x0, C0, x0_bstride, x1, C1, x1_bstride, wp, nullptr, scale, shift, y, y_bstride, stats, B, H, W, Cout, relu,
-                               false, st);
+                               mode, st);
     case SMAAT_PW_TF32X3:
       return conv3x3_tc_launch(x0, C0, x0_bstride, x1, C1, x1_bstride, wp, wp_lo, scale, shift, y, y_bstride, stats, B, H, W, Cout, relu,
-                               true, st);
+                               mode, st);
     default:
       return fail(SMAAT_E_BADARG, "conv3x3: unknown mode %d", mode);
   }

@@ -23,6 +23,9 @@
 //      (hi, and lo in TF32X3 mode), through its own ring: one halo chunk feeds 9 weight stages.
 // TF32X3: the activations are split into tf32 hi/lo in registers, the weights arrive pre-split (smaat_split_tf32 of the
 // packed weight); three MMAs (hi*hi + lo*hi + hi*lo) per k-step.
+// BF16: the activations are rounded to bf16 in registers (two k8 fragments -> one k16 fragment, tc_common.cuh bf16_frag), the
+// weights arrive as smaat_pack_bf16 of the packed weight (every (chunk, tap) box starts on a multiple of 32 columns, so the
+// pack's k permutation lines up with the fragments); 64-byte swizzled boxes, one m64nNk16 MMA per 16 k.
 //
 // Persistent: one CTA per SM loops over tiles (channel pass fastest, so consecutive tiles re-read the same halo from L2).
 // Warps 4-11 = two consumer warpgroups (64 pixels each).  Epilogue as pw1x1_tc.cu: affine/ReLU -> batch-strided NCHW stores,
@@ -53,8 +56,9 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-template <int N_TILE, int PW, bool X3>
+template <int N_TILE, int PW, Prec P>
 struct C3Cfg {
+  static constexpr bool X3 = P == Prec::TF32X3;
   static constexpr int PH = TC_BM / PW;
   static constexpr int BW = PW + 8;
   static constexpr int BH = PH + 3;                 // one spare row: see the bank note in the header
@@ -63,9 +67,10 @@ struct C3Cfg {
   static constexpr int IS = 2;                      // halo ring depth
   static constexpr int IN_BYTES = TC_BK * CP * 4;
   static_assert((IS * IN_BYTES) % 1024 == 0, "weight ring must start 1 KB aligned");
-  static constexpr int WB_BYTES = N_TILE * TC_BK * 4;
+  static constexpr int WB_BYTES = N_TILE * TC_BK * (P == Prec::BF16 ? 2 : 4);
   static constexpr int WST_BYTES = (X3 ? 2 : 1) * WB_BYTES;
-  static constexpr int WS = (96 * 1024) / WST_BYTES;  // weight ring depth
+  // weight ring depth; BF16 keeps TF32's (its stages are half the size: the barrier block holds no more)
+  static constexpr int WS = (96 * 1024) / ((X3 ? 2 : 1) * N_TILE * TC_BK * 4);
   static constexpr int OFF_W = IS * IN_BYTES;
   static constexpr int OFF_BAR = OFF_W + WS * WST_BYTES;
   static constexpr int BAR_BYTES = 256;
@@ -79,11 +84,12 @@ struct C3Cfg {
   static constexpr int THREADS = 384;
 };
 
-template <int N_TILE, int PW, bool X3>
+template <int N_TILE, int PW, Prec P>
 __global__ void __launch_bounds__(384, 1)
     conv3x3_tc_kernel(const __grid_constant__ CUtensorMap map_x0, const __grid_constant__ CUtensorMap map_x1,
                       const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo, const C3Params p) {
-  using L = C3Cfg<N_TILE, PW, X3>;
+  using L = C3Cfg<N_TILE, PW, P>;
+  constexpr bool X3 = L::X3;
   constexpr int PH = L::PH, BW = L::BW, CP = L::CP, IS = L::IS, WS = L::WS;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
@@ -226,25 +232,41 @@ __global__ void __launch_bounds__(384, 1)
         const int ws = wc % WS;
         mbar_wait(&w_full[ws], (wc / WS) & 1u);
         const unsigned char* wst = smem + L::OFF_W + ws * L::WST_BYTES;
-        const uint64_t bd0 = make_kmajor_desc(smem_u32(wst));
+        const uint64_t bd0 = make_b_desc<P>(smem_u32(wst));
         const uint64_t bl0 = make_kmajor_desc(smem_u32(wst + L::WB_BYTES));
         const float* at = hb + (tap / 3) * BW + (tap % 3);
+        if constexpr (P == Prec::BF16) {
+          // both k16 fragments are written before the fence: registers an MMA reads may not change after it
+          uint32_t af[TC_BK / 16][4];
 #pragma unroll
-        for (int kk = 0; kk < TC_BK / 8; ++kk) {
-          const float* ak = at + 8 * kk * CP;
-          const float v[4] = {ak[base0], ak[base1], ak[base0 + 4 * CP], ak[base1 + 4 * CP]};
-          uint32_t ahi[4], alo[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float h = X3 ? tf32_hi(v[e]) : v[e];
-            ahi[e] = __float_as_uint(h);
-            alo[e] = __float_as_uint(v[e] - h);
+          for (int s2 = 0; s2 < TC_BK / 16; ++s2) {
+            const float* a0 = at + 16 * s2 * CP;
+            const float* a1 = a0 + 8 * CP;
+            const float v0[4] = {a0[base0], a0[base1], a0[base0 + 4 * CP], a0[base1 + 4 * CP]};
+            const float v1[4] = {a1[base0], a1[base1], a1[base0 + 4 * CP], a1[base1 + 4 * CP]};
+            bf16_frag(v0, v1, af[s2]);
           }
           wgmma_fence();
-          Wgmma<N_TILE>::rs(acc, ahi, bd0 + (uint64_t)(2 * kk), 1u);
-          if (X3) {
-            Wgmma<N_TILE>::rs(acc, alo, bd0 + (uint64_t)(2 * kk), 1u);
-            Wgmma<N_TILE>::rs(acc, ahi, bl0 + (uint64_t)(2 * kk), 1u);
+#pragma unroll
+          for (int s2 = 0; s2 < TC_BK / 16; ++s2) Wgmma<N_TILE>::rs_bf16(acc, af[s2], bd0 + (uint64_t)(2 * s2), 1u);
+        } else {
+#pragma unroll
+          for (int kk = 0; kk < TC_BK / 8; ++kk) {
+            const float* ak = at + 8 * kk * CP;
+            const float v[4] = {ak[base0], ak[base1], ak[base0 + 4 * CP], ak[base1 + 4 * CP]};
+            uint32_t ahi[4], alo[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float h = X3 ? tf32_hi(v[e]) : v[e];
+              ahi[e] = __float_as_uint(h);
+              alo[e] = __float_as_uint(v[e] - h);
+            }
+            wgmma_fence();
+            Wgmma<N_TILE>::rs(acc, ahi, bd0 + (uint64_t)(2 * kk), 1u);
+            if (X3) {
+              Wgmma<N_TILE>::rs(acc, alo, bd0 + (uint64_t)(2 * kk), 1u);
+              Wgmma<N_TILE>::rs(acc, ahi, bl0 + (uint64_t)(2 * kk), 1u);
+            }
           }
         }
         wgmma_commit();
@@ -297,11 +319,11 @@ __global__ void __launch_bounds__(384, 1)
   if (p.stats && stat_n0 >= 0) flush_stats(stat_n0);
 }
 
-template <int N_TILE, int PW, bool X3>
+template <int N_TILE, int PW, Prec P>
 static int launch_c3(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl, C3Params p, int B,
                      cudaStream_t st) {
-  using L = C3Cfg<N_TILE, PW, X3>;
-  auto kern = conv3x3_tc_kernel<N_TILE, PW, X3>;
+  using L = C3Cfg<N_TILE, PW, P>;
+  auto kern = conv3x3_tc_kernel<N_TILE, PW, P>;
   static std::atomic<uint64_t> attr_mask{0};
   if (first_use_on_device(attr_mask)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
@@ -335,7 +357,8 @@ bool conv3x3_tc_eligible(const float* x0, int64_t bs0, const float* x1, int C1, 
 
 int conv3x3_tc_launch(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* wp, const float* wp_lo,
                       const float* scale, const float* shift, float* y, int64_t y_bstride, double* stats, int B, int H, int W, int Cout,
-                      int relu, bool x3, cudaStream_t st) {
+                      int relu, int mode, cudaStream_t st) {
+  const bool x3 = mode == SMAAT_PW_TF32X3, bf16 = mode == SMAAT_PW_BF16;
   if (!conv3x3_tc_eligible(x0, bs0, x1, C1, bs1, wp, wp_lo, W, Cout))
     return fail(SMAAT_E_UNSUPPORTED, "conv3x3(tc): needs W %% 4 == 0, Cout >= 8, 16-byte aligned pointers and batch strides "
                 "(W=%d Cout=%d); use SMAAT_PW_FP32_SIMT", W, Cout);
@@ -363,10 +386,12 @@ int conv3x3_tc_launch(const float* x0, int C0, int64_t bs0, const float* x1, int
     if (r) return r;
   }
   {
+    // 9 kc is a multiple of 32: the bf16 pack of wp has wp's row length
     const uint64_t dims[2] = {(uint64_t)9 * kc, (uint64_t)Cout};
-    const uint64_t str[2] = {0, (uint64_t)9 * kc * 4};
+    const uint64_t str[2] = {0, (uint64_t)9 * kc * (bf16 ? 2 : 4)};
     const uint32_t wbox[2] = {(uint32_t)TC_BK, (uint32_t)n_tile};
-    int r = make_tmap_f32(&mw, wp, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "conv3x3(w)");
+    int r = bf16 ? make_tmap(&mw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, wp, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_64B, "conv3x3(w bf16)")
+                 : make_tmap_f32(&mw, wp, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "conv3x3(w)");
     if (r) return r;
     mwl = mw;
     if (x3) {
@@ -381,12 +406,17 @@ int conv3x3_tc_launch(const float* x0, int C0, int64_t bs0, const float* x1, int
   p.nch0 = c0p / TC_BK; p.nch = kc / TC_BK;
   p.tiles_x = p.tiles_y = p.tiles_n = p.total_tiles = 0;
 
+#define C3_DISPATCH(NT, PWv)                                                                     \
+  return x3 ? launch_c3<NT, PWv, Prec::TF32X3>(m0, m1, mw, mwl, p, B, st)                           \
+            : bf16 ? launch_c3<NT, PWv, Prec::BF16>(m0, m1, mw, mwl, p, B, st)                      \
+                   : launch_c3<NT, PWv, Prec::TF32>(m0, m1, mw, mwl, p, B, st)
   if (n_tile == 128) {
-    if (pw == 32) return x3 ? launch_c3<128, 32, true>(m0, m1, mw, mwl, p, B, st) : launch_c3<128, 32, false>(m0, m1, mw, mwl, p, B, st);
-    return x3 ? launch_c3<128, 16, true>(m0, m1, mw, mwl, p, B, st) : launch_c3<128, 16, false>(m0, m1, mw, mwl, p, B, st);
+    if (pw == 32) { C3_DISPATCH(128, 32); }
+    C3_DISPATCH(128, 16);
   }
-  if (pw == 32) return x3 ? launch_c3<64, 32, true>(m0, m1, mw, mwl, p, B, st) : launch_c3<64, 32, false>(m0, m1, mw, mwl, p, B, st);
-  return x3 ? launch_c3<64, 16, true>(m0, m1, mw, mwl, p, B, st) : launch_c3<64, 16, false>(m0, m1, mw, mwl, p, B, st);
+  if (pw == 32) { C3_DISPATCH(64, 32); }
+  C3_DISPATCH(64, 16);
+#undef C3_DISPATCH
 }
 
 }  // namespace smaat

@@ -15,7 +15,8 @@
 //               input may be the virtual concat [x0, x1] of UpDS (parts_ds.py:85).  An L2 prefetch of the next tile's boxes
 //               (cp.async.bulk.prefetch.tensor) made bench.py's B = 32 forward slower: 2 220 vs 2 346-2 369 frames/s (H100
 //               80GB HBM3 SXM, 700 W; two runs with, six without), so there is none
-//   warp 1      prefetches the weight chunks (K-major SW128, [hi rows | lo rows]) into their own ring
+//   warp 1      prefetches the weight chunks (K-major SW128, [hi rows | lo rows]; BF16: the smaat_pack_bf16 pack, K-major SW64)
+//               into their own ring
 //               (warpgroup 0 runs on 24 registers per thread: setmaxnreg hands the rest to the consumers)
 //   warps 4-11  two consumer warpgroups (64 pixels each): wgmma (TF32X3: A_hi B_hi + A_lo B_hi + A_hi B_lo per k-step) into
 //               register accumulators, with the A operand either read by the tensor core from the A ring (A_SMEM) or
@@ -36,6 +37,9 @@
 //                          once instead of hi and lo halves the A ring's shared-memory traffic in TF32X3 mode; the split
 //                          in the consumer is the same tf32_hi / v - hi on the same value, so results are unchanged
 // Which one runs is smaat_set_dsconv_impl's choice (csrc/dsconv_fused.cu, below).
+// BF16 (SMAAT_PW_BF16, dsconv_bf16_kernel): the register form only; the consumers round the fp32 A tiles to bf16 as they load
+// them (two k8 fragments make one k16 fragment, tc_common.cuh bf16_frag), so the producers, the A ring and its layout are
+// those of TF32, and the B stages are half as large.
 #include <stdlib.h>
 
 #include <type_traits>
@@ -73,14 +77,16 @@ struct DsParams {
 
 constexpr int DS_MAX_CLASSES = 32;   // classes of the fused K-class OutConv + argmax (smaat_dsconv_classify_fwd)
 
-template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM>
 struct DsCfg {
+  static constexpr bool X3 = P == Prec::TF32X3;
+  static_assert(P != Prec::BF16 || !A_SMEM, "BF16: register A form only");
   static constexpr int PH = TC_BM / PW;
   static constexpr int BW = PW + 8, BH = PH + 2;
   static constexpr int CC = TC_BK / KPL;                       // input channels per chunk
   static constexpr int IN_BYTES = CC * BH * BW * 4;            // multiple of 128 for PW in {16,32}
   static constexpr int A_BYTES = TC_BM * TC_BK * 4;            // 16 KB
-  static constexpr int B_BYTES = N_TILE * TC_BK * 4;
+  static constexpr int B_BYTES = N_TILE * TC_BK * (P == Prec::BF16 ? 2 : 4);   // 128-byte rows (bf16: 64-byte rows)
   // A ring stage: fp32 (register form: the consumers split hi / lo after loading), or hi [+ lo] (A_SMEM: the tensor core reads
   // the parts)
   static constexpr int AST_BYTES = (X3 && A_SMEM ? 2 : 1) * A_BYTES;
@@ -94,7 +100,9 @@ struct DsCfg {
   // A ring and weight ring (prefetched by its own warp).  The consumers hold two stages of each (chunk i in flight, chunk i - 1
   // retiring); the producers write NG more, the weight loader runs one ahead.  The input ring gets the rest (it must stay deep
   // enough to cover HBM latency).  TF32X3 in the A_SMEM form (32 KB A stages) keeps two-deep rings at N_TILE 128: deeper ones
-  // leave too little for the input ring
+  // leave too little for the input ring.  BF16 takes TF32's depths: its A stages are TF32's and the four B stages cover the
+  // same two in use, NG producing and one loading; the 16 / 32 KB its half-size B stages free go to the input ring and the
+  // staging buffers (the table in DESIGN §6)
   static constexpr int AS = X3 ? (A_SMEM ? (N_TILE > 64 ? 2 : 3) : 2 + NG) : 4;
   static constexpr int BS = X3 ? (A_SMEM && N_TILE > 64 ? 2 : 3) : 4;
   static constexpr int AFF_N = 512;                            // scale | shift | OutConv weights of up to 512 channels
@@ -193,11 +201,12 @@ __device__ __forceinline__ void quad_transpose(float (&v)[4], int q) {
 
 // The kernel body, shared by the k = 1 / 2 instances (dsconv_fused_kernel) and the k = 4 ones (dsconv_kpl4_kernel).  The tensor
 // maps are the kernels' __grid_constant__ parameters
-template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
+template <int N_TILE, int KPL, int PW, Prec PREC, bool A_SMEM>
 __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CUtensorMap& map_in1, const CUtensorMap& map_w,
                                             const CUtensorMap& map_wlo, const CUtensorMap& map_y, const CUtensorMap& map_sa,
                                             const DsParams& p) {
-  using L = DsCfg<N_TILE, KPL, PW, X3, A_SMEM>;
+  using L = DsCfg<N_TILE, KPL, PW, PREC, A_SMEM>;
+  constexpr bool X3 = L::X3;
   constexpr int PH = L::PH, BW = L::BW, BH = L::BH, CC = L::CC, IS = L::IS, AS = L::AS, BS = L::BS;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
@@ -363,7 +372,7 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
         mbar_wait(&a_full[sa], (gc / AS) & 1u);
         mbar_wait(&b_full[sb], (gc / BS) & 1u);
         ast = a_base + sa * L::AST_BYTES;
-        bd = make_kmajor_desc(smem_u32(b_base + sb * L::BST_BYTES));
+        bd = make_b_desc<PREC>(smem_u32(b_base + sb * L::BST_BYTES));
         bl = make_kmajor_desc(smem_u32(b_base + sb * L::BST_BYTES + L::OFF_BLO));
       };
       if (A_SMEM) {
@@ -396,17 +405,17 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
         constexpr int KS = L::KS, GPC = (TC_BK / 8) / KS;
         const unsigned char* ast = nullptr;
         uint64_t bd0 = 0, bl0 = 0;
-        auto group = [&](AFrags<X3, KS>& cur, AFrags<X3, KS>& prev, int q) {
+        auto group = [&](AFrags<PREC, KS>& cur, AFrags<PREC, KS>& prev, int q) {
           const int part = q % GPC;
           if (part == 0) wait_stages(ast, bd0, bl0);
-          load_a_frags<X3, KS>(ast, part * KS, t, m0, m1, cur);
-          mma_a_frags<N_TILE, X3, KS>(acc, cur, bd0, bl0, part * KS);
+          load_a_frags<PREC, KS>(ast, part * KS, t, m0, m1, cur);
+          mma_a_frags<N_TILE, PREC, KS>(acc, cur, bd0, bl0, part * KS);
           wgmma_wait<1>();
           wgmma_keep(prev);
           if (part == 0 && q > 0) release(gc - 1);
           if (part == GPC - 1) ++gc;
         };
-        AFrags<X3, KS> fa, fb;
+        AFrags<PREC, KS> fa, fb;
         const int ngrp = nch * GPC;
         int q = 0;
         for (; q + 1 < ngrp; q += 2) {
@@ -768,38 +777,52 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
   }
 }
 
+__host__ __device__ constexpr Prec tf32_prec(bool x3) { return x3 ? Prec::TF32X3 : Prec::TF32; }
+
 template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
-__global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, X3, A_SMEM>::THREADS, 1)
+__global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, tf32_prec(X3), A_SMEM>::THREADS, 1)
     dsconv_fused_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
                         const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
                         const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_sa,
                         const DsParams p) {
-  dsconv_body<N_TILE, KPL, PW, X3, A_SMEM>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
+  dsconv_body<N_TILE, KPL, PW, tf32_prec(X3), A_SMEM>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
 }
 
 // kernels_per_layer = 4: CC = 8 input channels per chunk (7 680 B input boxes at both patch widths), two producer threads per
 // task.  Register form only
 template <int N_TILE, int PW, bool X3>
-__global__ void __launch_bounds__(DsCfg<N_TILE, 4, PW, X3, false>::THREADS, 1)
+__global__ void __launch_bounds__(DsCfg<N_TILE, 4, PW, tf32_prec(X3), false>::THREADS, 1)
     dsconv_kpl4_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
                        const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
                        const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_sa,
                        const DsParams p) {
-  dsconv_body<N_TILE, 4, PW, X3, false>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
+  dsconv_body<N_TILE, 4, PW, tf32_prec(X3), false>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
 }
 
-template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
+// SMAAT_PW_BF16, k = 1, 2 and 4: the register form with bf16 operands.  A kernel of its own, so that the tf32 kernels above
+// keep their names and instance sets
+template <int N_TILE, int KPL, int PW>
+__global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, Prec::BF16, false>::THREADS, 1)
+    dsconv_bf16_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
+                       const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
+                       const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_sa,
+                       const DsParams p) {
+  dsconv_body<N_TILE, KPL, PW, Prec::BF16, false>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
+}
+
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM>
 static auto ds_kernel() {
   static_assert(KPL == 1 || KPL == 2 || (KPL == 4 && !A_SMEM), "fused DS conv instances: k = 1, 2 (both A forms), 4 (register form)");
-  if constexpr (KPL == 4) return dsconv_kpl4_kernel<N_TILE, PW, X3>;
-  else return dsconv_fused_kernel<N_TILE, KPL, PW, X3, A_SMEM>;
+  if constexpr (P == Prec::BF16) return dsconv_bf16_kernel<N_TILE, KPL, PW>;
+  else if constexpr (KPL == 4) return dsconv_kpl4_kernel<N_TILE, PW, P == Prec::TF32X3>;
+  else return dsconv_fused_kernel<N_TILE, KPL, PW, P == Prec::TF32X3, A_SMEM>;
 }
 
-template <int N_TILE, int KPL, int PW, bool X3, bool A_SMEM>
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM>
 static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl,
                      const CUtensorMap& my, const CUtensorMap& msa, DsParams p, int B, cudaStream_t st) {
-  using L = DsCfg<N_TILE, KPL, PW, X3, A_SMEM>;
-  auto kern = ds_kernel<N_TILE, KPL, PW, X3, A_SMEM>();
+  using L = DsCfg<N_TILE, KPL, PW, P, A_SMEM>;
+  auto kern = ds_kernel<N_TILE, KPL, PW, P, A_SMEM>();
   // the pools are read back from the staging buffers: instances with the direct-store epilogue do not take them
   if (p.pool_sum && !L::ST_BUFS) return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools need the staged epilogue");
   if (p.ncls > L::MAX_CLASSES)
@@ -849,9 +872,11 @@ static int ds_impl();
 
 static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* pw_w,
                         const float* pw_w_lo, const float* y, int64_t y_bstride, int H, int W, int k, int Cout, bool stats,
-                        bool outconv) {
-  // k = 4 has register-form instances only (dsconv_kpl4_kernel): with the shared-memory A form selected it stays unfused
+                        bool outconv, bool bf16 = false) {
+  // k = 4 and BF16 have register-form instances only (dsconv_kpl4_kernel, dsconv_bf16_kernel): with the shared-memory A form
+  // selected they stay unfused
   if (k != 1 && k != 2 && !(k == 4 && ds_impl() != 1)) return false;
+  if (bf16 && ds_impl() == 1) return false;
   if (y && (!aligned16(y) || y_bstride % 4 != 0)) return false;
   // Cout > 128: whole passes of 128 channels; batch statistics and the fused OutConv need all channels in one pass
   if (Cout < 8 || Cout > 512 || (Cout > 128 && (Cout % 128 != 0 || stats || outconv))) return false;
@@ -862,43 +887,36 @@ static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, i
   return pick_pw(H, W) != 0;
 }
 
-// Whether the instance dsconv_run dispatches to has the staged epilogue (ST_BUFS > 0), which the CBAM pools are read from
-// (k = 4: the register form, the only one it has)
-template <int N_TILE, int KPL, int PW>
-static bool ds_staged_t(bool x3, bool a_smem) {
-  if constexpr (KPL == 4) return (x3 ? DsCfg<N_TILE, 4, PW, true, false>::ST_BUFS : DsCfg<N_TILE, 4, PW, false, false>::ST_BUFS) > 0;
-  else
-    return (x3 ? (a_smem ? DsCfg<N_TILE, KPL, PW, true, true>::ST_BUFS : DsCfg<N_TILE, KPL, PW, true, false>::ST_BUFS)
-               : (a_smem ? DsCfg<N_TILE, KPL, PW, false, true>::ST_BUFS : DsCfg<N_TILE, KPL, PW, false, false>::ST_BUFS)) > 0;
-}
-// The most classes whose OutConv weights the instance dsconv_run dispatches to keeps in shared memory (DsCfg::MAX_CLASSES)
-template <int N_TILE, int KPL, int PW>
-static int ds_max_classes_t(bool x3, bool a_smem) {
-  if constexpr (KPL == 4) return x3 ? DsCfg<N_TILE, 4, PW, true, false>::MAX_CLASSES : DsCfg<N_TILE, 4, PW, false, false>::MAX_CLASSES;
-  else
-    return x3 ? (a_smem ? DsCfg<N_TILE, KPL, PW, true, true>::MAX_CLASSES : DsCfg<N_TILE, KPL, PW, true, false>::MAX_CLASSES)
-              : (a_smem ? DsCfg<N_TILE, KPL, PW, false, true>::MAX_CLASSES : DsCfg<N_TILE, KPL, PW, false, false>::MAX_CLASSES);
-}
-static int ds_max_classes(int n_tile, int k, int pw, bool x3, bool a_smem) {
-  if (n_tile == 64) {
-    if (k == 4) return pw == 32 ? ds_max_classes_t<64, 4, 32>(x3, a_smem) : ds_max_classes_t<64, 4, 16>(x3, a_smem);
-    if (k == 2) return pw == 32 ? ds_max_classes_t<64, 2, 32>(x3, a_smem) : ds_max_classes_t<64, 2, 16>(x3, a_smem);
-    return pw == 32 ? ds_max_classes_t<64, 1, 32>(x3, a_smem) : ds_max_classes_t<64, 1, 16>(x3, a_smem);
+// The configuration of the instance dsconv_run dispatches to, for a mode (SMAAT_PW_*) and A form (k = 4 and BF16: the register
+// form, the only one they have), handed to `f` as a DsCfg type
+template <int N_TILE, int KPL, int PW, typename F>
+static auto ds_cfg_t(int mode, bool a_smem, F f) {
+  if (mode == SMAAT_PW_BF16) return f(DsCfg<N_TILE, KPL, PW, Prec::BF16, false>{});
+  if constexpr (KPL == 4) {
+    return mode == SMAAT_PW_TF32X3 ? f(DsCfg<N_TILE, 4, PW, Prec::TF32X3, false>{}) : f(DsCfg<N_TILE, 4, PW, Prec::TF32, false>{});
+  } else {
+    if (mode == SMAAT_PW_TF32X3) return a_smem ? f(DsCfg<N_TILE, KPL, PW, Prec::TF32X3, true>{}) : f(DsCfg<N_TILE, KPL, PW, Prec::TF32X3, false>{});
+    return a_smem ? f(DsCfg<N_TILE, KPL, PW, Prec::TF32, true>{}) : f(DsCfg<N_TILE, KPL, PW, Prec::TF32, false>{});
   }
-  if (k == 4) return pw == 32 ? ds_max_classes_t<128, 4, 32>(x3, a_smem) : ds_max_classes_t<128, 4, 16>(x3, a_smem);
-  if (k == 2) return pw == 32 ? ds_max_classes_t<128, 2, 32>(x3, a_smem) : ds_max_classes_t<128, 2, 16>(x3, a_smem);
-  return pw == 32 ? ds_max_classes_t<128, 1, 32>(x3, a_smem) : ds_max_classes_t<128, 1, 16>(x3, a_smem);
 }
-
-static bool ds_staged(int n_tile, int k, int pw, bool x3, bool a_smem) {
+template <typename F>
+static int ds_cfg(int n_tile, int k, int pw, int mode, bool a_smem, F f) {
   if (n_tile == 64) {
-    if (k == 4) return pw == 32 ? ds_staged_t<64, 4, 32>(x3, a_smem) : ds_staged_t<64, 4, 16>(x3, a_smem);
-    if (k == 2) return pw == 32 ? ds_staged_t<64, 2, 32>(x3, a_smem) : ds_staged_t<64, 2, 16>(x3, a_smem);
-    return pw == 32 ? ds_staged_t<64, 1, 32>(x3, a_smem) : ds_staged_t<64, 1, 16>(x3, a_smem);
+    if (k == 4) return pw == 32 ? ds_cfg_t<64, 4, 32>(mode, a_smem, f) : ds_cfg_t<64, 4, 16>(mode, a_smem, f);
+    if (k == 2) return pw == 32 ? ds_cfg_t<64, 2, 32>(mode, a_smem, f) : ds_cfg_t<64, 2, 16>(mode, a_smem, f);
+    return pw == 32 ? ds_cfg_t<64, 1, 32>(mode, a_smem, f) : ds_cfg_t<64, 1, 16>(mode, a_smem, f);
   }
-  if (k == 4) return pw == 32 ? ds_staged_t<128, 4, 32>(x3, a_smem) : ds_staged_t<128, 4, 16>(x3, a_smem);
-  if (k == 2) return pw == 32 ? ds_staged_t<128, 2, 32>(x3, a_smem) : ds_staged_t<128, 2, 16>(x3, a_smem);
-  return pw == 32 ? ds_staged_t<128, 1, 32>(x3, a_smem) : ds_staged_t<128, 1, 16>(x3, a_smem);
+  if (k == 4) return pw == 32 ? ds_cfg_t<128, 4, 32>(mode, a_smem, f) : ds_cfg_t<128, 4, 16>(mode, a_smem, f);
+  if (k == 2) return pw == 32 ? ds_cfg_t<128, 2, 32>(mode, a_smem, f) : ds_cfg_t<128, 2, 16>(mode, a_smem, f);
+  return pw == 32 ? ds_cfg_t<128, 1, 32>(mode, a_smem, f) : ds_cfg_t<128, 1, 16>(mode, a_smem, f);
+}
+// Whether that instance has the staged epilogue (ST_BUFS > 0), which the CBAM pools are read from
+static bool ds_staged(int n_tile, int k, int pw, int mode, bool a_smem) {
+  return ds_cfg(n_tile, k, pw, mode, a_smem, [](auto c) { return (int)decltype(c)::ST_BUFS; }) > 0;
+}
+// The most classes whose OutConv weights that instance keeps in shared memory (DsCfg::MAX_CLASSES)
+static int ds_max_classes(int n_tile, int k, int pw, int mode, bool a_smem) {
+  return ds_cfg(n_tile, k, pw, mode, a_smem, [](auto c) { return (int)decltype(c)::MAX_CLASSES; });
 }
 
 // Where the A operand (the depthwise result) goes to the tensor core: 0 = auto (the register form), 1 = read by wgmma from
@@ -941,10 +959,12 @@ extern "C" int smaat_dsconv_eligible(const float* x0, int C0, int64_t x0_bstride
 
 extern "C" int smaat_dsconv_cbam_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                                           const float* pw_w, int H, int W, int k, int Cout, int mode, int with_gate, int with_pools) {
-  if (mode != SMAAT_PW_TF32 && mode != SMAAT_PW_TF32X3) return 0;
-  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, false, false)) return 0;
+  if (mode != SMAAT_PW_TF32 && mode != SMAAT_PW_TF32X3 && mode != SMAAT_PW_BF16) return 0;
+  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, false, false,
+                   mode == SMAAT_PW_BF16))
+    return 0;
   (void)with_gate;   // every fused instance takes the gate
-  if (with_pools && !ds_staged(Cout > 64 ? 128 : 64, k, pick_pw(H, W), mode == SMAAT_PW_TF32X3, ds_impl() == 1)) return 0;
+  if (with_pools && !ds_staged(Cout > 64 ? 128 : 64, k, pick_pw(H, W), mode, ds_impl() == 1)) return 0;
   return 1;
 }
 
@@ -967,12 +987,14 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   SMAAT_REQUIRE(!pooled || (reinterpret_cast<uintptr_t>(pooled) & 7u) == 0, "dsconv: the max-pool output must be 8-byte aligned");
   SMAAT_REQUIRE(B > 0 && C0 > 0 && C1 >= 0 && H > 0 && W > 0 && Cout > 0, "dsconv: bad shape");
   SMAAT_REQUIRE(C1 == 0 || x1, "dsconv: C1=%d but x1 is null", C1);
-  SMAAT_REQUIRE(mode == SMAAT_PW_TF32 || mode == SMAAT_PW_TF32X3, "dsconv: mode must be SMAAT_PW_TF32 or SMAAT_PW_TF32X3");
+  SMAAT_REQUIRE(mode == SMAAT_PW_TF32 || mode == SMAAT_PW_TF32X3 || mode == SMAAT_PW_BF16,
+                "dsconv: mode must be SMAAT_PW_TF32, SMAAT_PW_TF32X3 or SMAAT_PW_BF16");
   SMAAT_REQUIRE(mode != SMAAT_PW_TF32X3 || pw_w_lo, "dsconv: TF32X3 needs pw_w_lo (see smaat_split_tf32)");
   SMAAT_REQUIRE(head || y_bstride >= (int64_t)Cout * H * W, "dsconv: y batch stride too small");
   SMAAT_REQUIRE(!head || (oc_w && !stats),"dsconv+outconv: needs the OutConv weight and no batch statistics");
+  const bool bf16 = mode == SMAAT_PW_BF16;
   if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, pw_w_lo, head ? nullptr : y, y_bstride, H, W, k, Cout,
-                   stats != nullptr, head))
+                   stats != nullptr, head, bf16))
     return fail(SMAAT_E_UNSUPPORTED,
                 "dsconv: shape or output layout not taken by the fused kernel (k=%d Cout=%d H=%d W=%d, y 16-byte aligned with a "
                 "batch stride that is a multiple of 4); use dw3x3 + pw1x1",
@@ -1002,10 +1024,12 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
     if (r) return r;
   }
   {
-    const uint64_t dims[2] = {(uint64_t)K, (uint64_t)Cout};
-    const uint64_t str[2] = {0, (uint64_t)K * 4};
+    const uint64_t kw = bf16 ? (uint64_t)(K + TC_BK - 1) / TC_BK * TC_BK : (uint64_t)K;   // the bf16 pack's row length
+    const uint64_t dims[2] = {kw, (uint64_t)Cout};
+    const uint64_t str[2] = {0, kw * (bf16 ? 2 : 4)};
     const uint32_t wbox[2] = {(uint32_t)TC_BK, (uint32_t)n_tile};
-    int r = make_tmap_f32(&mw, pw_w, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "dsconv(w)");
+    int r = bf16 ? make_tmap(&mw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, pw_w, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_64B, "dsconv(w bf16)")
+                 : make_tmap_f32(&mw, pw_w, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "dsconv(w)");
     if (r) return r;
     mwl = mw;
     if (x3) {
@@ -1039,14 +1063,16 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   p.tiles_x = p.tiles_y = p.npass = p.total_tiles = p.nchunks = 0;
 
 #define DS_DISPATCH(NT, KP, PWv)                                                                           \
-  return x3 ? (a_smem ? launch_ds<NT, KP, PWv, true, true>(m0, m1, mw, mwl, my, msa, p, B, st)                   \
-                      : launch_ds<NT, KP, PWv, true, false>(m0, m1, mw, mwl, my, msa, p, B, st))                 \
-            : (a_smem ? launch_ds<NT, KP, PWv, false, true>(m0, m1, mw, mwl, my, msa, p, B, st)                  \
-                      : launch_ds<NT, KP, PWv, false, false>(m0, m1, mw, mwl, my, msa, p, B, st))
+  if (bf16) return launch_ds<NT, KP, PWv, Prec::BF16, false>(m0, m1, mw, mwl, my, msa, p, B, st);                    \
+  return x3 ? (a_smem ? launch_ds<NT, KP, PWv, Prec::TF32X3, true>(m0, m1, mw, mwl, my, msa, p, B, st)               \
+                      : launch_ds<NT, KP, PWv, Prec::TF32X3, false>(m0, m1, mw, mwl, my, msa, p, B, st))             \
+            : (a_smem ? launch_ds<NT, KP, PWv, Prec::TF32, true>(m0, m1, mw, mwl, my, msa, p, B, st)                 \
+                      : launch_ds<NT, KP, PWv, Prec::TF32, false>(m0, m1, mw, mwl, my, msa, p, B, st))
 // k = 4: the register form (ds_eligible)
 #define DS_DISPATCH4(NT, PWv)                                                                                  \
-  return x3 ? launch_ds<NT, 4, PWv, true, false>(m0, m1, mw, mwl, my, msa, p, B, st)                          \
-            : launch_ds<NT, 4, PWv, false, false>(m0, m1, mw, mwl, my, msa, p, B, st)
+  if (bf16) return launch_ds<NT, 4, PWv, Prec::BF16, false>(m0, m1, mw, mwl, my, msa, p, B, st);                  \
+  return x3 ? launch_ds<NT, 4, PWv, Prec::TF32X3, false>(m0, m1, mw, mwl, my, msa, p, B, st)                  \
+            : launch_ds<NT, 4, PWv, Prec::TF32, false>(m0, m1, mw, mwl, my, msa, p, B, st)
   if (n_tile == 64) {
     if (k == 4)      { if (pw == 32) { DS_DISPATCH4(64, 32); } else { DS_DISPATCH4(64, 16); } }
     else if (k == 2) { if (pw == 32) { DS_DISPATCH(64, 2, 32); } else { DS_DISPATCH(64, 2, 16); } }
@@ -1083,11 +1109,12 @@ extern "C" int smaat_dsconv_outconv_fwd(const float* x0, int C0, int64_t x0_bstr
 
 extern "C" int smaat_dsconv_classify_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                                               const float* pw_w, int H, int W, int k, int Cout, int K, int mode) {
-  if (mode != SMAAT_PW_TF32 && mode != SMAAT_PW_TF32X3) return 0;
+  if (mode != SMAAT_PW_TF32 && mode != SMAAT_PW_TF32X3 && mode != SMAAT_PW_BF16) return 0;
   if (K < 1 || K > DS_MAX_CLASSES) return 0;
-  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, false, true)) return 0;
+  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, false, true, mode == SMAAT_PW_BF16))
+    return 0;
   // the class weights must fit the shared memory the instance leaves free: 32 classes at Cout <= 64, 22 up to Cout = 128
-  return K <= ds_max_classes(Cout > 64 ? 128 : 64, k, pick_pw(H, W), mode == SMAAT_PW_TF32X3, ds_impl() == 1) ? 1 : 0;
+  return K <= ds_max_classes(Cout > 64 ? 128 : 64, k, pick_pw(H, W), mode, ds_impl() == 1) ? 1 : 0;
 }
 
 /* The network's last two modules for a K-class model, ending in the class map: DS conv -> BN/ReLU -> OutConv(Cout -> K) ->

@@ -1,5 +1,5 @@
 // glue.cu -- the memory-bound glue between the DS-conv blocks: BN folding, MaxPool2d(2),
-// OutConv, tf32 weight split (bilinear x2 + pad lives in upsample.cu).  All are streaming kernels
+// OutConv, tf32 weight split, bf16 weight pack (bilinear x2 + pad lives in upsample.cu).  All are streaming kernels
 // (no reuse beyond what L1/L2 give for free); coalesced 128-bit accesses where alignment allows.
 #include "common.cuh"
 
@@ -25,6 +25,26 @@ __global__ void split_tf32_kernel(const float* __restrict__ src, float* __restri
   const float h = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
   hi[i] = h;
   lo[i] = v - h;
+}
+
+// ---- bf16 weight pack (SMAAT_PW_BF16) --------------------------------------------------------------
+// out[r][c] = bf16_rn(w[r][src]), src = the physical k of logical k c in its group of 16 (tc_common.cuh bf16_frag), zero past
+// cols.  One thread per output pair: one bf16x2 store
+__global__ void pack_bf16_kernel(const float* __restrict__ w, uint32_t* __restrict__ out, int rows, int cols, int cols_out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;   // pair index
+  const int half = cols_out >> 1;
+  if (i >= (int64_t)rows * half) return;
+  const int r = (int)(i / half), c = 2 * (int)(i - (int64_t)r * half);
+  float v[2];
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const int l = (c + e) & 15;
+    const int src = ((c + e) & ~15) | (l & 8) | ((l & 1) << 2) | ((l >> 1) & 3);
+    v[e] = src < cols ? w[(int64_t)r * cols + src] : 0.f;
+  }
+  uint32_t p;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(p) : "f"(v[1]), "f"(v[0]));
+  out[i] = p;
 }
 
 // ---- MaxPool2d(2) ---------------------------------------------------------------------------------
@@ -130,6 +150,17 @@ extern "C" int smaat_split_tf32(const float* src, float* hi, float* lo, int64_t 
   SMAAT_REQUIRE(src && hi && lo && n > 0, "split_tf32: bad arguments");
   split_tf32_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, (cudaStream_t)stream>>>(src, hi, lo, n);
   SMAAT_LAUNCH_CHECK("smaat_split_tf32");
+  return SMAAT_OK;
+}
+
+extern "C" int smaat_pack_bf16(const float* w, uint16_t* out, int rows, int cols, int cols_out, void* stream) {
+  SMAAT_REQUIRE(w && out && rows > 0 && cols > 0, "pack_bf16: bad arguments rows=%d cols=%d", rows, cols);
+  SMAAT_REQUIRE(cols_out == (cols + 31) / 32 * 32, "pack_bf16: cols_out=%d must be cols=%d rounded up to 32", cols_out, cols);
+  SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3u) == 0, "pack_bf16: out must be 4-byte aligned");
+  const int64_t pairs = (int64_t)rows * (cols_out / 2);
+  pack_bf16_kernel<<<(unsigned)ceil_div64(pairs, 256), 256, 0, (cudaStream_t)stream>>>(w, reinterpret_cast<uint32_t*>(out), rows, cols,
+                                                                                        cols_out);
+  SMAAT_LAUNCH_CHECK("smaat_pack_bf16");
   return SMAAT_OK;
 }
 

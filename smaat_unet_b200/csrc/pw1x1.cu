@@ -6,7 +6,7 @@ namespace smaat {
 int pw1x1_simt_launch(const float* x, const float* w, const float* scale, const float* shift, float* y, int64_t y_bstride,
                       double* stats, int B, int K, int Cout, int P, int relu, cudaStream_t st);
 int pw1x1_tc_launch(const float* x, const float* w, const float* w_lo, const float* scale, const float* shift, float* y,
-                    int64_t y_bstride, double* stats, int B, int K, int Cout, int P, int relu, bool x3, cudaStream_t st);
+                    int64_t y_bstride, double* stats, int B, int K, int Cout, int P, int relu, int mode, cudaStream_t st);
 bool pw1x1_tc_eligible(const float* x, const float* w, const float* w_lo, int K, int Cout, int P);
 }  // namespace smaat
 
@@ -23,9 +23,11 @@ extern "C" int smaat_pw1x1_fwd(const float* x, const float* w, const float* w_lo
     case SMAAT_PW_FP32_SIMT:
       return pw1x1_simt_launch(x, w, scale, shift, y, y_bstride, stats, B, K, Cout, P, relu, st);
     case SMAAT_PW_TF32:
-      return pw1x1_tc_launch(x, w, nullptr, scale, shift, y, y_bstride, stats, B, K, Cout, P, relu, false, st);
+      return pw1x1_tc_launch(x, w, nullptr, scale, shift, y, y_bstride, stats, B, K, Cout, P, relu, mode, st);
     case SMAAT_PW_TF32X3:
-      return pw1x1_tc_launch(x, w, w_lo, scale, shift, y, y_bstride, stats, B, K, Cout, P, relu, true, st);
+      return pw1x1_tc_launch(x, w, w_lo, scale, shift, y, y_bstride, stats, B, K, Cout, P, relu, mode, st);
+    case SMAAT_PW_BF16:
+      return pw1x1_tc_launch(x, w, nullptr, scale, shift, y, y_bstride, stats, B, K, Cout, P, relu, mode, st);
     default:
       return fail(SMAAT_E_BADARG, "pw1x1: unknown mode %d", mode);
   }

@@ -13,6 +13,8 @@
 //   D in registers of two consumer warpgroups (64 pixels each).
 // TF32X3 mode (fp32-grade accuracy): the activations are split into a tf32 "hi" part and the "lo" remainder in registers,
 // the weights arrive pre-split; three MMAs (hi*hi + lo*hi + hi*lo) per k-step accumulate into the same registers.
+// BF16 mode: the activations are rounded to bf16 in registers, the weights arrive as a smaat_pack_bf16 pack ([Cout][K rounded
+// up to 32], K-major, 64-byte rows: TMA SWIZZLE_64B); one m64nNk16 MMA per 16 k.
 //
 // Persistent: one CTA per SM loops over output tiles (tile = blockIdx.x + i*gridDim.x; consecutive tiles share the activation
 // tile and differ in the channel tile, so the re-read hits L2).  Warp 0 = TMA producer, running ahead across tile boundaries
@@ -36,10 +38,11 @@ struct PwTcParams {
   int tiles_m, tiles_n, total_tiles;
 };
 
-template <int N_TILE, int STAGES, bool X3>
+template <int N_TILE, int STAGES, Prec P>
 struct PwTcCfg {
+  static constexpr bool X3 = P == Prec::TF32X3;
   static constexpr int A_BYTES = TC_BM * TC_BK * 4;   // 16 KB: 4 blocks x (32 k-rows x 128 B)
-  static constexpr int B_BYTES = N_TILE * TC_BK * 4;  // N_TILE rows x 128 B
+  static constexpr int B_BYTES = N_TILE * TC_BK * (P == Prec::BF16 ? 2 : 4);  // N_TILE rows x 128 B (bf16: 64 B)
   static constexpr int STAGE_BYTES = A_BYTES + (X3 ? 2 : 1) * B_BYTES;
   static constexpr int OFF_B = A_BYTES;
   static constexpr int OFF_BLO = A_BYTES + B_BYTES;  // X3 only
@@ -57,11 +60,12 @@ struct PwTcCfg {
   static_assert(TOTAL <= 227 * 1024, "shared memory budget");
 };
 
-template <int N_TILE, int STAGES, bool X3>
+template <int N_TILE, int STAGES, Prec P>
 __global__ void __launch_bounds__(384, 1)
     pw1x1_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
                     const __grid_constant__ CUtensorMap map_wlo, const PwTcParams p) {
-  using L = PwTcCfg<N_TILE, STAGES, X3>;
+  using L = PwTcCfg<N_TILE, STAGES, P>;
+  constexpr bool X3 = L::X3;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   // 1 KB alignment: 128-byte swizzle atoms.  Offset arithmetic on the __shared__ array (not a uintptr_t round trip) keeps the
   // accesses LDS/STS instead of generic LD/ST.
@@ -176,19 +180,19 @@ __global__ void __launch_bounds__(384, 1)
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[c % STAGES]);
     };
-    auto chunk = [&](AFrags<X3>& cur, AFrags<X3>& prev, int i) {
+    auto chunk = [&](AFrags<P>& cur, AFrags<P>& prev, int i) {
       const int s = it % STAGES;
       mbar_wait(&full_bar[s], (it / STAGES) & 1u);
       const unsigned char* st = smem + s * L::STAGE_BYTES;
-      load_a_frags<X3, TC_BK / 8>(st, 0, t, m0, m1, cur);
-      mma_a_frags<N_TILE, X3, TC_BK / 8>(acc, cur, make_kmajor_desc(smem_u32(st + L::OFF_B)),
-                                         make_kmajor_desc(smem_u32(st + L::OFF_BLO)), 0);
+      load_a_frags<P, TC_BK / 8>(st, 0, t, m0, m1, cur);
+      mma_a_frags<N_TILE, P, TC_BK / 8>(acc, cur, make_b_desc<P>(smem_u32(st + L::OFF_B)),
+                                        make_kmajor_desc(smem_u32(st + L::OFF_BLO)), 0);
       wgmma_wait<1>();
       wgmma_keep(prev);
       if (i > 0) release(it - 1);
       ++it;
     };
-    AFrags<X3> fa, fb;
+    AFrags<P> fa, fb;
     int i = 0;
     for (; i + 1 < nk; i += 2) {
       chunk(fa, fb, i);
@@ -242,10 +246,10 @@ __global__ void __launch_bounds__(384, 1)
   if (p.stats && stat_n0 >= 0) flush_stats(stat_n0);
 }
 
-template <int N_TILE, int STAGES, bool X3>
+template <int N_TILE, int STAGES, Prec P>
 static int launch_tc(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mwl, PwTcParams p, int B, cudaStream_t st) {
-  using L = PwTcCfg<N_TILE, STAGES, X3>;
-  auto kern = pw1x1_tc_kernel<N_TILE, STAGES, X3>;
+  using L = PwTcCfg<N_TILE, STAGES, P>;
+  auto kern = pw1x1_tc_kernel<N_TILE, STAGES, P>;
   static std::atomic<uint64_t> attr_mask{0};   // cudaFuncSetAttribute is per device
   if (first_use_on_device(attr_mask)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
@@ -268,8 +272,11 @@ bool pw1x1_tc_eligible(const float* x, const float* w, const float* w_lo, int K,
   return (P % 4 == 0) && (K % 4 == 0) && aligned16(x) && aligned16(w) && (w_lo == nullptr || aligned16(w_lo)) && Cout >= 8;
 }
 
+// mode: SMAAT_PW_TF32, SMAAT_PW_TF32X3 (w the tf32 hi parts, w_lo the lo parts) or SMAAT_PW_BF16 (w the smaat_pack_bf16 pack of
+// the (Cout, K) weight: (Cout, K rounded up to 32) bf16)
 int pw1x1_tc_launch(const float* x, const float* w, const float* w_lo, const float* scale, const float* shift, float* y,
-                    int64_t y_bstride, double* stats, int B, int K, int Cout, int P, int relu, bool x3, cudaStream_t st) {
+                    int64_t y_bstride, double* stats, int B, int K, int Cout, int P, int relu, int mode, cudaStream_t st) {
+  const bool x3 = mode == SMAAT_PW_TF32X3, bf16 = mode == SMAAT_PW_BF16;
   SMAAT_REQUIRE(pw1x1_tc_eligible(x, w, w_lo, K, Cout, P), "pw1x1(tc): needs P %% 4 == 0, K %% 4 == 0 and 16-byte aligned x/w");
   SMAAT_REQUIRE(!x3 || w_lo, "pw1x1(tc): TF32X3 needs w_lo (see smaat_split_tf32)");
   SMAAT_REQUIRE(Cout <= 512 || (!scale && !shift), "pw1x1(tc): Cout=%d > 512 with an epilogue affine (smem staging holds 512 channels)", Cout);
@@ -286,10 +293,12 @@ int pw1x1_tc_launch(const float* x, const float* w, const float* w_lo, const flo
     if (r) return r;
   }
   {
-    const uint64_t dims[2] = {(uint64_t)K, (uint64_t)Cout};
-    const uint64_t str[2] = {0, (uint64_t)K * 4};
+    const uint64_t kw = bf16 ? (uint64_t)(K + TC_BK - 1) / TC_BK * TC_BK : (uint64_t)K;   // the bf16 pack's row length
+    const uint64_t dims[2] = {kw, (uint64_t)Cout};
+    const uint64_t str[2] = {0, kw * (bf16 ? 2 : 4)};
     const uint32_t box[2] = {(uint32_t)TC_BK, (uint32_t)n_tile};
-    int r = make_tmap_f32(&mw, w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, "pw1x1(w)");
+    int r = bf16 ? make_tmap(&mw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B, "pw1x1(w bf16)")
+                 : make_tmap_f32(&mw, w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, "pw1x1(w)");
     if (r) return r;
     mwl = mw;
     if (x3) {
@@ -302,13 +311,18 @@ int pw1x1_tc_launch(const float* x, const float* w, const float* w_lo, const flo
   p.K = K; p.Cout = Cout; p.P = P; p.relu = relu;
   p.tiles_m = p.tiles_n = p.total_tiles = 0;
 
-  // one persistent CTA per SM: the smem ring takes ~150-200 KB of the 227 KB
+  // one persistent CTA per SM: the smem ring takes ~150-200 KB of the 227 KB.  BF16 keeps TF32's depths (its stages are
+  // smaller: 24 / 20 KB instead of 32 / 24 KB)
   if (x3) {
-    if (n_tile == 128) return launch_tc<128, 4, true>(mx, mw, mwl, p, B, st);
-    return launch_tc<64, 5, true>(mx, mw, mwl, p, B, st);
+    if (n_tile == 128) return launch_tc<128, 4, Prec::TF32X3>(mx, mw, mwl, p, B, st);
+    return launch_tc<64, 5, Prec::TF32X3>(mx, mw, mwl, p, B, st);
   }
-  if (n_tile == 128) return launch_tc<128, 5, false>(mx, mw, mwl, p, B, st);
-  return launch_tc<64, 6, false>(mx, mw, mwl, p, B, st);
+  if (bf16) {
+    if (n_tile == 128) return launch_tc<128, 5, Prec::BF16>(mx, mw, mwl, p, B, st);
+    return launch_tc<64, 6, Prec::BF16>(mx, mw, mwl, p, B, st);
+  }
+  if (n_tile == 128) return launch_tc<128, 5, Prec::TF32>(mx, mw, mwl, p, B, st);
+  return launch_tc<64, 6, Prec::TF32>(mx, mw, mwl, p, B, st);
 }
 
 }  // namespace smaat

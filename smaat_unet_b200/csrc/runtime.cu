@@ -36,6 +36,11 @@ PFN_encodeTiled get_encode_tiled() {
 
 int make_tmap_f32(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                   const uint32_t* box, CUtensorMapSwizzle swizzle, const char* who) {
+  return make_tmap(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rank, dims, strides_bytes, box, swizzle, who);
+}
+
+int make_tmap(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+              const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle, const char* who) {
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) return fail(SMAAT_E_CUDA, "%s: cuTensorMapEncodeTiled not available from the driver", who);
   cuuint64_t gdim[5];
@@ -48,7 +53,7 @@ int make_tmap_f32(CUtensorMap* map, const void* base, int rank, const uint64_t* 
     es[i] = 1;
     if (i > 0) gstr[i - 1] = strides_bytes[i];
   }
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
+  CUresult r = enc(map, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {

@@ -15,6 +15,11 @@ namespace smaat {
 constexpr int TC_BM = 128;  // pixels per tile: two consumer warpgroups x m64
 constexpr int TC_BK = 32;   // k per stage (one 128-byte swizzle row of fp32)
 
+// Operand precision of a tensor-core instance: one tf32 pass (SMAAT_PW_TF32), the 3xTF32 split (SMAAT_PW_TF32X3), or bf16
+// operands with fp32 accumulation (SMAAT_PW_BF16: A rounded to bf16 in registers, B a smaat_pack_bf16 pack, one
+// m64nNk16 MMA per 16 k)
+enum class Prec : int { TF32 = 0, TF32X3 = 1, BF16 = 2 };
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
@@ -72,6 +77,22 @@ __device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t saddr) {
   return d;
 }
 
+// The same for a K-major bf16 operand with 64-byte rows (32 bf16 of k) and the 64-byte swizzle (layout type 2): 8-row atoms
+// 512 B apart; one k16 step is 32 B along the row = +2 in the address field.  The tile base must be 512-byte aligned.
+__device__ __forceinline__ uint64_t make_kmajor_desc_sw64(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3fffu);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(512 >> 4) << 32;
+  d |= (uint64_t)2 << 62;
+  return d;
+}
+// B descriptor of a K-major weight tile in precision P: fp32 rows with the 128-byte swizzle, or bf16 rows with the 64-byte one
+template <Prec P>
+__device__ __forceinline__ uint64_t make_b_desc(uint32_t saddr) {
+  return P == Prec::BF16 ? make_kmajor_desc_sw64(saddr) : make_kmajor_desc(saddr);
+}
+
 // Byte offset of activation element (k-row kr, pixel m) inside one A tile stored as 4 blocks of [32 k-rows][32 px] with the
 // 128-byte swizzle (16-byte chunk index XOR k-row % 8) -- the layout TMA SWIZZLE_128B writes for a 32 px x 32 k box.
 __device__ __forceinline__ uint32_t a_tile_offset(int kr, int m) {
@@ -103,40 +124,74 @@ __device__ __forceinline__ void load_a_frag(const unsigned char* at, int kk, int
 
 __device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float(__float_as_uint(v) & 0xffffe000u); }
 
-// Register-A fragments of KS k-steps (one commit group; TC_BK / 8 = 4 k-steps make a k-chunk): f[0][kk] = the values (tf32)
-// or their tf32 hi parts (TF32X3), f[1][kk] = the lo remainders v - hi (TF32X3 only).  MMAs in flight read them until
-// their group retires.
-template <bool X3, int KS = TC_BK / 8>
-using AFrags = uint32_t[X3 ? 2 : 1][KS][4];
+// Two fp32 -> one bf16x2 register, round to nearest even: `lo` in the low half (the lower k), `hi` in the high half
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// The bf16 register-A fragment of one k16 step from the tf32 fragments v0 / v1 of k-steps 2s / 2s + 1 (load_a_frag's layout).
+// The MMA then sees logical k l of the 16 at physical k-row (l & 8) | ((l & 1) << 2) | ((l >> 1) & 3) of the step;
+// smaat_pack_bf16 gives B the same permutation, so the sum over k is the same sum
+__device__ __forceinline__ void bf16_frag(const float (&v0)[4], const float (&v1)[4], uint32_t (&a)[4]) {
+  a[0] = pack_bf16x2(v0[0], v0[2]);
+  a[1] = pack_bf16x2(v0[1], v0[3]);
+  a[2] = pack_bf16x2(v1[0], v1[2]);
+  a[3] = pack_bf16x2(v1[1], v1[3]);
+}
 
-// Loads k-steps kk0 .. kk0 + KS - 1 from an fp32 A tile at `at` and splits them in registers.
-template <bool X3, int KS>
-__device__ __forceinline__ void load_a_frags(const unsigned char* at, int kk0, int t, int m0, int m1, AFrags<X3, KS>& f) {
+// Register-A fragments of KS tf32 k-steps (one commit group; TC_BK / 8 = 4 k-steps make a k-chunk): f[0][kk] = the values
+// (tf32) or their tf32 hi parts (TF32X3), f[1][kk] = the lo remainders v - hi (TF32X3 only); in BF16 the KS / 2 k16
+// fragments.  MMAs in flight read them until their group retires.
+template <Prec P, int KS = TC_BK / 8>
+using AFrags = uint32_t[P == Prec::TF32X3 ? 2 : 1][P == Prec::BF16 ? KS / 2 : KS][4];
+
+// Loads k-steps kk0 .. kk0 + KS - 1 from an fp32 A tile at `at` and splits (TF32X3) or rounds (BF16) them in registers.
+template <Prec P, int KS>
+__device__ __forceinline__ void load_a_frags(const unsigned char* at, int kk0, int t, int m0, int m1, AFrags<P, KS>& f) {
+  constexpr bool X3 = P == Prec::TF32X3;
+  if constexpr (P == Prec::BF16) {
 #pragma unroll
-  for (int kk = 0; kk < KS; ++kk) {
-    float v[4];
-    load_a_frag(at, kk0 + kk, t, m0, m1, v);
+    for (int s = 0; s < KS / 2; ++s) {
+      float v0[4], v1[4];
+      load_a_frag(at, kk0 + 2 * s, t, m0, m1, v0);
+      load_a_frag(at, kk0 + 2 * s + 1, t, m0, m1, v1);
+      bf16_frag(v0, v1, f[0][s]);
+    }
+  } else {
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float h = X3 ? tf32_hi(v[e]) : v[e];
-      f[0][kk][e] = __float_as_uint(h);
-      if (X3) f[X3 ? 1 : 0][kk][e] = __float_as_uint(v[e] - h);
+    for (int kk = 0; kk < KS; ++kk) {
+      float v[4];
+      load_a_frag(at, kk0 + kk, t, m0, m1, v);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float h = X3 ? tf32_hi(v[e]) : v[e];
+        f[0][kk][e] = __float_as_uint(h);
+        if (X3) f[X3 ? 1 : 0][kk][e] = __float_as_uint(v[e] - h);
+      }
     }
   }
 }
 
-// One fence, the MMAs of k-steps kk0 .. kk0 + KS - 1 (TF32X3: A_hi B_hi + A_lo B_hi + A_hi B_lo per k-step) and one commit.
-// bd / bl: descriptors of the chunk's B hi / lo tiles.
-template <int N_TILE, bool X3, int KS>
-__device__ __forceinline__ void mma_a_frags(float (&acc)[N_TILE / 2], const AFrags<X3, KS>& f, uint64_t bd, uint64_t bl, int kk0) {
+// One fence, the MMAs of k-steps kk0 .. kk0 + KS - 1 (TF32X3: A_hi B_hi + A_lo B_hi + A_hi B_lo per k-step; BF16: one k16 MMA
+// per two k-steps) and one commit.  bd / bl: descriptors of the chunk's B (hi) / lo tiles.  A k8 step of fp32 B and a k16
+// step of bf16 B are both 32 B along the row: + 2 in the descriptor's address field
+template <int N_TILE, Prec P, int KS>
+__device__ __forceinline__ void mma_a_frags(float (&acc)[N_TILE / 2], const AFrags<P, KS>& f, uint64_t bd, uint64_t bl, int kk0) {
+  constexpr bool X3 = P == Prec::TF32X3;
   wgmma_fence();
+  if constexpr (P == Prec::BF16) {
 #pragma unroll
-  for (int kk = 0; kk < KS; ++kk) {
-    const uint64_t k2 = (uint64_t)(2 * (kk0 + kk));
-    Wgmma<N_TILE>::rs(acc, f[0][kk], bd + k2, 1u);
-    if (X3) {
-      Wgmma<N_TILE>::rs(acc, f[X3 ? 1 : 0][kk], bd + k2, 1u);
-      Wgmma<N_TILE>::rs(acc, f[0][kk], bl + k2, 1u);
+    for (int s = 0; s < KS / 2; ++s) Wgmma<N_TILE>::rs_bf16(acc, f[0][s], bd + (uint64_t)(2 * (kk0 / 2 + s)), 1u);
+  } else {
+#pragma unroll
+    for (int kk = 0; kk < KS; ++kk) {
+      const uint64_t k2 = (uint64_t)(2 * (kk0 + kk));
+      Wgmma<N_TILE>::rs(acc, f[0][kk], bd + k2, 1u);
+      if (X3) {
+        Wgmma<N_TILE>::rs(acc, f[X3 ? 1 : 0][kk], bd + k2, 1u);
+        Wgmma<N_TILE>::rs(acc, f[0][kk], bl + k2, 1u);
+      }
     }
   }
   wgmma_commit();

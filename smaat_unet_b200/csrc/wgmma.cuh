@@ -1,5 +1,5 @@
-// wgmma.cuh -- inline-PTX wrappers of the Hopper warpgroup MMA (wgmma.mma_async, kind tf32, fp32 accumulate) used by the
-// tensor-core kernels.  d[] is the m64nN accumulator fragment of one thread (N/2 floats): for n8 block j,
+// wgmma.cuh -- inline-PTX wrappers of the Hopper warpgroup MMA (wgmma.mma_async, kinds tf32 and bf16, fp32 accumulate) used
+// by the tensor-core kernels.  d[] is the m64nN accumulator fragment of one thread (N/2 floats): for n8 block j,
 // d[4j + 0/1] = (row g, columns 8j + 2t + 0/1), d[4j + 2/3] = (row g + 8, same columns), g = lane / 4, t = lane % 4,
 // rows relative to the warp's 16 rows (warp w % 4 of the warpgroup owns rows 16 (w % 4) ..).
 // RS form: A from registers, a[0..3] = (row g, k t), (row g + 8, k t), (row g, k t + 4), (row g + 8, k t + 4).
@@ -39,14 +39,33 @@ __device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t adesc, ui
       : "l"(adesc), "l"(bdesc), "r"(accum));
 }
 
+// bf16 RS form (SMAAT_PW_BF16): m64nNk16, A from registers as four bf16x2 (a[0..3] = (row g, k 2t, 2t + 1), (row g + 8, same k),
+// (row g, k 2t + 8, 2t + 9), (row g + 8, same k)), B a K-major bf16 tile through a descriptor (imm-trans-b 0), scales 1.
+__device__ __forceinline__ void wgmma_rs_n64_bf16(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accum));
+}
+__device__ __forceinline__ void wgmma_rs_n128_bf16(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accum));
+}
+
 template <int N> struct Wgmma;
 template <> struct Wgmma<64> {
   static __device__ __forceinline__ void rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t acc) { wgmma_rs_n64(d, a, b, acc); }
   static __device__ __forceinline__ void ss(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) { wgmma_ss_n64(d, a, b, acc); }
+  static __device__ __forceinline__ void rs_bf16(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t acc) { wgmma_rs_n64_bf16(d, a, b, acc); }
 };
 template <> struct Wgmma<128> {
   static __device__ __forceinline__ void rs(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t acc) { wgmma_rs_n128(d, a, b, acc); }
   static __device__ __forceinline__ void ss(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_ss_n128(d, a, b, acc); }
+  static __device__ __forceinline__ void rs_bf16(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t acc) { wgmma_rs_n128_bf16(d, a, b, acc); }
 };
 
 }  // namespace smaat

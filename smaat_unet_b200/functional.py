@@ -58,8 +58,7 @@ def ds_conv_fwd(ds, x, x1=None, in_scale=None, in_shift=None, stats=None):
     ds._check()
     d = ops.dw3x3(x, _p(ds.depthwise.weight), _p(ds.depthwise.bias), ds.kernels_per_layer, x1=x1, in_scale=in_scale, in_shift=in_shift)
     mode = ops.get_pointwise_mode()
-    split = ds.pw_split() if mode == "tf32x3" else None
-    z = ops.pw1x1(d, _p(ds.pointwise.weight), None, _p(ds.pointwise.bias), False, mode=mode, w_split=split, stats=stats)
+    z = ops.pw1x1(d, _p(ds.pointwise.weight), None, _p(ds.pointwise.bias), False, mode=mode, w_split=ds.pw_operands(), stats=stats)
     return d, z
 
 
@@ -185,7 +184,7 @@ def pw_bwd(dz, d, weight, dW, db, need_input=True):
     K = d.shape[1]
     P = H * W
     lib = _lib.load()
-    m = ops.PW_MODES[ops.get_pointwise_mode()]
+    m = ops.wgrad_mode(ops.PW_MODES[ops.get_pointwise_mode()])
     if m != 0 and P % 4 == 0 and K >= 8 and Cout >= 8:      # tensor cores: split-K over pixels, register accumulators, fp32 atomics to merge
         _call(f"smaat_pw1x1_bwd_weight_tc[K{K}_N{Cout}_P{P}]", 4 * B * P * (K + Cout), 2 * B * P * K * Cout, lib.smaat_pw1x1_bwd_weight_tc,
               _ptr(dz), _ptr(d), _ptr(dW), _ptr(db), B, K, Cout, P, m, _stream())
@@ -259,8 +258,8 @@ def conv3x3_bwd(mod, idx, dz, x0, x1, dW, need_input=True):
     if not need_input:
         return None, None
     C0, C1 = x0.shape[1], (x1.shape[1] if x1 is not None else 0)
-    wt, hi, lo = mod.packed(idx, C0, C1, flip_transpose=True)
-    dx = ops.conv3x3(dz, wt, C0 + C1, None, None, False, w_split=(hi, lo) if hi is not None else None)
+    wt, wops = mod.packed(idx, C0, C1, flip_transpose=True)
+    dx = ops.conv3x3(dz, wt, C0 + C1, None, None, False, w_split=wops)
     return (dx[:, :C0], dx[:, C0:]) if C1 else (dx, None)
 
 

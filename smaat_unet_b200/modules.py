@@ -88,15 +88,19 @@ class DepthwiseSeparableConv(_CachingModule):
             raise NotImplementedError("smaat_unet_b200 implements the depthwise conv the reference uses: 3x3, padding=1 "
                                       "(parts_ds.py:18-33)")
 
-    def pw_split(self):
-        """(hi, lo) tf32 split of the pointwise weight, cached on the parameter's version counter."""
+    def pw_operands(self):
+        """The pointwise weight's operands in the current mode (``ops.derived_operands``: the tf32 (hi, lo) split in 'tf32x3',
+        (bf16 pack, None) in 'bf16', None in the modes that take the weight as it is), cached on the parameter's version
+        counter and the mode."""
+        mode = ops.PW_MODES[ops.get_pointwise_mode()]
         w = self.pointwise.weight
-        key = _versions(w)
-        # while a training step is being captured into a CUDA graph the split must be part of the graph: replays see new weights
+        key = (_versions(w), mode)
+        # while a training step is being captured into a CUDA graph the operands must be part of the graph: replays see new
+        # weights
         in_train_capture = self.training and torch.cuda.is_current_stream_capturing()
         if in_train_capture or self._wsplit_key != key:
             with torch.no_grad():
-                self._wsplit = ops.split_tf32(w.detach().view(w.shape[0], -1))
+                self._wsplit = ops.derived_operands(w.detach().view(w.shape[0], -1), mode)
             self._wsplit_key = None if in_train_capture else key
             self._wsplit_src = _held(w)
         return self._wsplit
@@ -107,14 +111,14 @@ class DepthwiseSeparableConv(_CachingModule):
 
     def _operands(self, shift):
         """What ``run``, ``run_head`` and ``run_cbam`` hand the kernels besides the input and the epilogue scale: the depthwise
-        bias, the epilogue shift (the pointwise bias where the caller gives none), the arithmetic mode and, in 'tf32x3', the
-        pointwise weight's cached tf32 split."""
+        bias, the epilogue shift (the pointwise bias where the caller gives none), the arithmetic mode and the pointwise
+        weight's cached operands in that mode (``pw_operands``)."""
         self._check()
         dw_b = self.depthwise.bias.detach() if self.depthwise.bias is not None else None
         if shift is None:
             shift = self.pointwise.bias.detach() if self.pointwise.bias is not None else None
         mode = ops.get_pointwise_mode()
-        return dw_b, shift, mode, self.pw_split() if mode == "tf32x3" else None
+        return dw_b, shift, mode, self.pw_operands()
 
     def run(self, x, x1=None, scale=None, shift=None, relu=False, in_scale=None, in_shift=None, stats=None):
         """dw -> pw with the pw epilogue y = act(scale * acc + shift).  scale/shift None => (1, pointwise.bias)."""
@@ -382,14 +386,15 @@ class _TransposedUp(_CachingModule):
         self._packed = None
 
     def _packed_weight(self):
-        """((4 Cout, Cin) GEMM matrix of the transposed conv, its tf32 (hi, lo) split or None); cached on the weight's version."""
+        """((4 Cout, Cin) GEMM matrix of the transposed conv, its operands in the current mode (``ops.derived_operands``: None
+        where the mode takes it as it is)); cached on the weight's version and the mode."""
         w = self.up.weight
         key = (_versions(w), ops.get_pointwise_mode())
         in_train_capture = self.training and torch.cuda.is_current_stream_capturing()
         if in_train_capture or self._packed is None or self._packed[0] != key:
             with torch.no_grad():
                 wp = ops.convt2x2_pack_weight(w.detach())
-                split = ops.split_tf32(wp) if ops.get_pointwise_mode() == "tf32x3" else None
+                split = ops.derived_operands(wp, ops.PW_MODES[ops.get_pointwise_mode()])
             self._packed = (None if in_train_capture else key, wp, split, _held(w))
         return self._packed[1], self._packed[2]
 
@@ -467,8 +472,9 @@ class DoubleConv(_DoubleConvBase):
                                           "groups=1 (unet_parts.py:16,19)")
 
     def packed(self, idx, C0, C1=0, flip_transpose=False):
-        """(packed weight, tf32 hi, tf32 lo) of conv ``idx`` for inputs [C0 | C1] (hi/lo None unless 'tf32x3'); with
-        ``flip_transpose`` the input-gradient form.  Cached on the weight's version; re-derived inside a training capture."""
+        """(packed weight, its operands in the current mode (``ops.derived_operands``; None where the mode takes the packed
+        weight as it is)) of conv ``idx`` for inputs [C0 | C1]; with ``flip_transpose`` the input-gradient form.  Cached on the
+        weight's version and the mode; re-derived inside a training capture."""
         w = self.double_conv[idx].weight
         mode = ops.get_pointwise_mode()
         key = (_versions(w), mode)
@@ -478,8 +484,8 @@ class DoubleConv(_DoubleConvBase):
         if in_train_capture or hit is None or hit[0] != key:
             with torch.no_grad():
                 wp = ops.conv3x3_pack_weight(w.detach(), C0, C1, flip_transpose)
-                hi, lo = ops.split_tf32(wp) if mode == "tf32x3" else (None, None)
-            hit = (None if in_train_capture else key, (wp, hi, lo), _held(w))
+                wops = ops.derived_operands(wp, ops.PW_MODES[mode])
+            hit = (None if in_train_capture else key, (wp, wops), _held(w))
             self._packed[slot] = hit
         return hit[1]
 
@@ -487,9 +493,8 @@ class DoubleConv(_DoubleConvBase):
         """Conv ``idx`` (0 or 3) over [x, x1] with the epilogue y = act(scale * acc + shift)."""
         self._check()
         C0, C1 = x.shape[1], (x1.shape[1] if x1 is not None else 0)
-        wp, hi, lo = self.packed(idx, C0, C1)
-        return ops.conv3x3(x, wp, self.double_conv[idx].out_channels, scale, shift, relu, x1=x1,
-                           w_split=(hi, lo) if hi is not None else None, stats=stats)
+        wp, wops = self.packed(idx, C0, C1)
+        return ops.conv3x3(x, wp, self.double_conv[idx].out_channels, scale, shift, relu, x1=x1, w_split=wops, stats=stats)
 
     def run(self, x, x1=None, outconv=None, head="logits"):
         """``outconv`` (an OutConv module): return OutConv(block(x)) ending in ``head`` (``HEADS``) -- its logits, their
@@ -700,25 +705,27 @@ class CBAM(nn.Module):
 
 
 def cached_tensors(model):
-    """Every tensor the eval fast path derived from ``model``'s parameters (folded BatchNorm affine, tf32 hi/lo splits,
-    packed 3x3 and transposed-conv weights).  A CUDA graph captured over the eval forward has their addresses baked in:
+    """Every tensor the eval fast path derived from ``model``'s parameters (folded BatchNorm affine, tf32 hi/lo splits, bf16
+    packs, packed 3x3 and transposed-conv weights).  A CUDA graph captured over the eval forward has their addresses baked in:
     whoever owns the graph must keep them alive (``graph_tensors``)."""
     out = []
     for m in model.modules():
         if isinstance(m, DepthwiseSeparableConv) and m._wsplit is not None:
-            out.extend(m._wsplit)
+            out.extend(t for t in m._wsplit if t is not None)
         elif isinstance(m, (DoubleConvDS, DoubleConv)):
             for entry in m._fold.values():
                 out.extend(entry[1])
             if isinstance(m, DoubleConv):
                 for entry in m._packed.values():
-                    out.extend(t for t in entry[1] if t is not None)
+                    wp, wops = entry[1]
+                    out.append(wp)
+                    out.extend(t for t in wops or () if t is not None)
         elif isinstance(m, SpatialAttention) and m._fold is not None:
             out.append(m._fold[1])
         if isinstance(m, _TransposedUp) and m._packed is not None:
             _, wp, split, _ = m._packed
             out.append(wp)
-            out.extend(split or ())
+            out.extend(t for t in split or () if t is not None)
     return out
 
 

@@ -12,14 +12,17 @@ import torch
 
 from . import _lib
 
-PW_MODES = {"fp32": 0, "tf32": 1, "tf32x3": 2}
+PW_MODES = {"fp32": 0, "tf32": 1, "tf32x3": 2, "bf16": 3}
 _pw_mode = os.environ.get("SMAAT_PW_MODE", "tf32x3")
 assert _pw_mode in PW_MODES, f"SMAAT_PW_MODE must be one of {list(PW_MODES)}"
 
 
 def set_pointwise_mode(mode: str) -> None:
     """'tf32x3' (default; wgmma 3xTF32 split, fp32-grade), 'tf32' (wgmma single pass; what
-    cuDNN's allow_tf32=True default gives the reference on a GPU), 'fp32' (CUDA-core exact)."""
+    cuDNN's allow_tf32=True default gives the reference on a GPU), 'bf16' (wgmma on bf16-rounded operands, fp32
+    accumulation: what torch.set_float32_matmul_precision('medium') allows torch's matmuls), 'fp32' (CUDA-core exact).
+    The mode applies to the forward GEMMs (fused DS conv, pointwise, dense 3x3, and their input gradients); the weight
+    gradients run their tf32 kernels in 'bf16'."""
     global _pw_mode
     if mode not in PW_MODES:
         raise ValueError(f"pointwise mode must be one of {list(PW_MODES)}")
@@ -140,11 +143,29 @@ def _pw_matrix(pw_weight, k=None, Cin=None):
     return w2d
 
 
-def _tf32_split(w, m, w_split):
-    """(w, None), or in mode 2 ('tf32x3') w's tf32 (hi, lo): the caller's cached ``w_split``, else split now."""
-    if m != 2:
+_TAKES_W = (0, 1)        # mode codes whose kernels take the fp32 weight as it is ('fp32', 'tf32')
+
+
+def derived_operands(w, m):
+    """What the modules cache for the (rows, K) fp32 matrix w in mode code ``m``: w's tf32 (hi, lo) split in 'tf32x3', (its
+    bf16 pack, None) in 'bf16' (``pack_bf16``), None in the modes whose kernels take w as it is."""
+    if m in _TAKES_W:
+        return None
+    return split_tf32(w) if m == 2 else (pack_bf16(w), None)
+
+
+def weight_operands(w, m, cached=None):
+    """The weight operands a GEMM kernel takes in mode code ``m`` for the (rows, K) fp32 matrix w: (w, None) in 'fp32' /
+    'tf32', else ``derived_operands`` -- the caller's ``cached`` copy of them when given, derived now when None."""
+    if m in _TAKES_W:
         return w, None
-    return w_split if w_split is not None else split_tf32(w)
+    return cached if cached is not None else derived_operands(w, m)
+
+
+def wgrad_mode(m):
+    """The mode code the weight-gradient kernels run for forward mode code ``m``: 'bf16' runs their one-pass tf32 instance
+    (their operands reach shared memory as fp32, and operand width does not limit them)."""
+    return 1 if m == 3 else m
 
 
 # ---------------------------------------------------------------------------------------------
@@ -172,11 +193,24 @@ def split_tf32(w):
     return hi, lo
 
 
+def pack_bf16(w):
+    """The bf16 weight operand of 'bf16' mode: (rows, K) fp32 -> (rows, K rounded up to 32) bf16, each value rounded to
+    nearest even, k permuted within groups of 16 as the kernels' register fragments present the activations, zero padded
+    (smaat_pack_bf16)."""
+    w = _dense(w, "w")
+    rows, cols = w.shape[0], w[0].numel()
+    out = torch.empty((rows, _pad32(cols)), device=w.device, dtype=torch.bfloat16)
+    _call("smaat_pack_bf16", 4 * w.numel() + 2 * out.numel(), 0, _lib.load().smaat_pack_bf16, _ptr(w), _ptr(out), rows, cols,
+          out.shape[1], _stream())
+    return out
+
+
 def pw1x1(x, weight, scale, shift, relu, mode=None, w_split=None, stats=None, out=None):
     """Pointwise 1x1 + per-channel affine (+ReLU) (layers.py:45,49 + parts_ds.py:25-26).
 
-    weight: (Cout, K[,1,1]).  mode None = module-level default.  w_split = cached (hi, lo) for
-    'tf32x3'.  Falls to the exact CUDA-core kernel for shapes the tensor-core path does not take.
+    weight: (Cout, K[,1,1]).  mode None = module-level default.  w_split = cached weight operands of the mode
+    (``weight_operands``: the tf32 (hi, lo) for 'tf32x3', (bf16 pack, None) for 'bf16').  Falls to the exact CUDA-core kernel
+    for shapes the tensor-core path does not take.
     """
     x = _dense(x, "x")
     B, K, H, W = x.shape
@@ -195,7 +229,7 @@ def pw1x1(x, weight, scale, shift, relu, mode=None, w_split=None, stats=None, ou
     # 1024-channel bottleneck has more)
     if m != 0 and (not tc_eligible(x, w2d) or (Cout > 512 and (scale is not None or shift is not None))):
         m = 0
-    w2d, wlo = _tf32_split(w2d, m, w_split)
+    w2d, wlo = weight_operands(w2d, m, w_split)
     _call(f"smaat_pw1x1_fwd[K{K}_N{Cout}_P{P}]", 4 * B * P * (K + Cout) + 4 * K * Cout, 2 * B * P * K * Cout, _lib.load().smaat_pw1x1_fwd, _ptr(x), _ptr(w2d), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(out), ybs, _ptr(stats),
                                            B, K, Cout, P, int(bool(relu)), m, _stream())
     return out
@@ -223,7 +257,12 @@ def dsconv_takes(x, x1, pw_weight, k, mode=None, stats=False) -> bool:
         return False
     x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     w2d = _pw_matrix(pw_weight)
-    return bool(_lib.load().smaat_dsconv_eligible2(_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2], x.shape[3], k, w2d.shape[0], int(bool(stats))))
+    lib = _lib.load()
+    args = (_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2], x.shape[3], k, w2d.shape[0])
+    if not lib.smaat_dsconv_eligible2(*args, int(bool(stats))):
+        return False
+    # 'bf16' has register-A instances only: the mode-taking test also declines it under set_dsconv_impl('smem')
+    return PW_MODES[mode] != 3 or bool(lib.smaat_dsconv_cbam_eligible(*args, 3, 0, 0))
 
 
 def dsconv_cbam_takes(x, x1, pw_weight, k, gate=False, pools=False, mode=None) -> bool:
@@ -248,8 +287,9 @@ def dsconv_cbam(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None
     x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
     Cin = C0 + C1
-    w2d, wlo = _tf32_split(_pw_matrix(pw_weight, k, Cin), PW_MODES[mode], w_split)
+    w2d = _pw_matrix(pw_weight, k, Cin)
     Cout, K = w2d.shape
+    w2d, wlo = weight_operands(w2d, PW_MODES[mode], w_split)
     lib = _lib.load()
     sc = sa = None
     if gate is not None:
@@ -283,8 +323,9 @@ def dsconv(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, mod
     x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
     Cin = C0 + C1
-    w2d, wlo = _tf32_split(_pw_matrix(pw_weight, k, Cin), PW_MODES[mode], w_split)
+    w2d = _pw_matrix(pw_weight, k, Cin)
     Cout, K = w2d.shape
+    w2d, wlo = weight_operands(w2d, PW_MODES[mode], w_split)
     lib = _lib.load()
     dw_w = _dense(dw_weight, "depthwise.weight")
     if outconv is not None:
@@ -344,7 +385,7 @@ def dsconv_classify(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_
     assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
     ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
     assert ob is None or ob.numel() == K, f"OutConv bias {tuple(oc_bias.shape)} does not match K={K}"
-    w2d, wlo = _tf32_split(w2d, PW_MODES[mode], w_split)
+    w2d, wlo = weight_operands(w2d, PW_MODES[mode], w_split)
     classes = torch.empty((B, H, W), device=x.device, dtype=torch.int64)
     logits = torch.empty((B, K, H, W), device=x.device, dtype=torch.float32) if want_logits else None
     _call(f"smaat_dsconv_classify_fwd[C{Cin}_N{Cout}_K{K}_S{H}]",
@@ -413,7 +454,7 @@ def conv3x3_takes(x, x1, wp, Cout, mode=None) -> bool:
 def conv3x3(x, wp, Cout, scale, shift, relu, x1=None, mode=None, w_split=None, stats=None):
     """nn.Conv2d(Cin, Cout, 3, padding=1) over the virtual concat [x, x1] + per-channel affine (+ReLU) (unet_parts.py:16-21,63).
 
-    wp: ``conv3x3_pack_weight`` of the weight; w_split: its cached tf32 (hi, lo) for 'tf32x3'.  Shapes the tensor-core kernel
+    wp: ``conv3x3_pack_weight`` of the weight; w_split: its cached operands for the mode (``weight_operands``).  Shapes the tensor-core kernel
     does not take (W % 4 != 0, Cout < 8) run on the exact CUDA-core kernel."""
     x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
@@ -423,7 +464,7 @@ def conv3x3(x, wp, Cout, scale, shift, relu, x1=None, mode=None, w_split=None, s
     lib = _lib.load()
     if m != 0 and not lib.smaat_conv3x3_tc_eligible(_ptr(x), bs0, _ptr(x1), C1, bs1, _ptr(wp), W, Cout):
         m = 0
-    wp, wlo = _tf32_split(wp, m, w_split)
+    wp, wlo = weight_operands(wp, m, w_split)
     y = torch.empty((B, Cout, H, W), device=x.device, dtype=torch.float32)
     name = "smaat_conv3x3_fwd" if m else "smaat_conv3x3_fwd_simt"
     Cin = C0 + C1
@@ -435,13 +476,14 @@ def conv3x3(x, wp, Cout, scale, shift, relu, x1=None, mode=None, w_split=None, s
 
 def conv3x3_bwd_weight(dz, x, x1, dW, mode=None):
     """dW (Cout, Cin, 3, 3) += the weight gradient of ``conv3x3`` over [x, x1] for output gradient dz (unet_parts.py:16,19).
-    Tensor cores in 'tf32' / 'tf32x3' where the shape allows (W % 4 == 0, aligned), else the exact CUDA-core kernel."""
+    Tensor cores in 'tf32' / 'tf32x3' (and in 'bf16', which runs the tf32 kernel: ``wgrad_mode``) where the shape allows
+    (W % 4 == 0, aligned), else the exact CUDA-core kernel."""
     dz = _dense(dz, "dz")
     x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
     B, C0, H, W = x.shape
     Cout = dz.shape[1]
     assert tuple(dW.shape) == (Cout, C0 + C1, 3, 3) and dW.is_contiguous()
-    m = PW_MODES[mode or _pw_mode]
+    m = wgrad_mode(PW_MODES[mode or _pw_mode])
     tc_ok = W % 4 == 0 and bs0 % 4 == 0 and bs1 % 4 == 0 and all(t.data_ptr() % 16 == 0 for t in (dz, x) + ((x1,) if C1 else ()))
     if not tc_ok:
         m = 0
