@@ -6,6 +6,8 @@ batch stride larger than C*H*W is allowed where the C ABI takes a ``bstride``.
 """
 from __future__ import annotations
 
+import contextlib
+import gc
 import os
 
 import torch
@@ -610,6 +612,20 @@ def cbam_pool_maxpool(x):
     _call("smaat_cbam_pool_maxpool_fwd", 5 * B * Cc * H * W, 0, _lib.load().smaat_cbam_pool_maxpool_fwd, _ptr(x), _ptr(avg), _ptr(mx),
           _ptr(pooled), B * Cc, H, W, _stream())
     return avg, mx, pooled
+
+
+@contextlib.contextmanager
+def gc_paused():
+    """Keep Python's cyclic garbage collector out of a CUDA-graph capture.  A collection may free unreachable objects that
+    own CUDA resources (pinned host buffers, events, graphs of an earlier session); releasing them calls into the driver,
+    which invalidates the capture in progress.  They are collected after it instead."""
+    was = gc.isenabled()
+    gc.disable()
+    try:
+        yield
+    finally:
+        if was:
+            gc.enable()
 
 
 _cbam_counters = {}

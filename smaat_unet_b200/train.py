@@ -39,6 +39,14 @@ object afterwards does not change the session.  Targets are class indices: a flo
 with a weighted ``nn.CrossEntropyLoss``.
 
     sess = TrainSession(SmaAt_UNet(12, 8), 32, (12, 288, 288), loss=CrossEntropyLossWithOptions(weight=w, label_smoothing=0.1))
+
+Partial batches.  ``step`` takes 1 <= n <= batch rows and is one step on exactly those n samples: BatchNorm statistics,
+the loss's mean and the metric update run over n, on the leading rows of the static buffers.  ``batch_sizes`` names the
+sizes below ``batch`` that get captured graphs of their own (e.g. an epoch's tail, ``len(shard) % batch`` when it is not
+0); any other n runs the same step eagerly.  With several ranks every rank must step the same n (a partial step checks
+it).
+
+    sess = TrainSession(model, 32, (12, 288, 288), batch_sizes=(len(shard) % 32,))
 """
 from __future__ import annotations
 
@@ -59,7 +67,12 @@ _DEFAULT = object()  # metrics argument not given: the loss's own default metric
 
 class TrainSession:
     def __init__(self, model, batch, in_shape, lr=1e-3, device=None, use_graph=True, metrics=_DEFAULT, warmup=3,
-                 betas=(0.9, 0.999), eps=1e-8, overlap_allreduce=True, recompute_depthwise=False, loss="mse"):
+                 betas=(0.9, 0.999), eps=1e-8, overlap_allreduce=True, recompute_depthwise=False, loss="mse", batch_sizes=None):
+        batch = int(batch)
+        extra = [int(m) for m in (batch_sizes or ())]
+        if batch < 1 or any(not 1 <= m <= batch for m in extra):
+            raise ValueError(f"TrainSession: batch_sizes must lie in 1..batch={batch}, got {tuple(extra)}")
+        self.sizes = tuple(sorted(set(extra) | {batch}))     # sizes with captured graphs, ascending; the last is the capacity
         self._ce = None          # (ignore_index, reduction, weight, label_smoothing) of a loss instance
         if isinstance(loss, (CrossEntropyLoss, CrossEntropyLossWithOptions)):
             if loss.reduction not in ("mean", "sum"):
@@ -78,7 +91,8 @@ class TrainSession:
             w = None if ce_loss.weight is None else ce_loss.weight.detach().to(self.device, torch.float32).clone()
             self._ce = (int(ce_loss.ignore_index), ce_loss.reduction, w, float(ce_loss.label_smoothing))
         self.model = model.to(self.device).train()
-        self.batch, self.in_shape = int(batch), tuple(in_shape)
+        self.batch, self.in_shape = batch, tuple(in_shape)
+        self._rows = batch                # rows of the batch loaded in the static buffers
         self.world = dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1
         self.use_graph = bool(use_graph)
         self.recompute_depthwise = bool(recompute_depthwise)   # functional.set_recompute_depthwise for this session's forwards
@@ -112,7 +126,8 @@ class TrainSession:
         if self._split is not None:
             for m in self._split["boundary"]:
                 self._hooks.append(m.register_forward_hook(lambda mod, inp, out: self._bnd.append(out)))
-        self.graphs = None
+        self.graphs = None                  # the capacity size's (phase 1, phase 2, optimizer) graphs
+        self._size_graphs = {}              # size -> its (phase 1, phase 2) graphs; the optimizer graph serves every size
         self.launches_per_step = 0
         self.allreduce_events = None        # (start, end) pairs of the last step when record_comm_timing is on
         self.record_comm_timing = False
@@ -174,17 +189,18 @@ class TrainSession:
     # ---- the pieces of a step ----------------------------------------------------------------------------
     def _forward_loss(self):
         self._bnd.clear()
+        x, y = self.x[:self._rows], self.y[:self._rows]
         old = Fn.set_recompute_depthwise(self.recompute_depthwise)
         try:
-            pred = self.model(self.x)
+            pred = self.model(x)
         finally:
             Fn.set_recompute_depthwise(old)
         if self._ce is not None:
             ignore_index, reduction, weight, eps = self._ce
-            return ce_step(pred, self.y, self.metrics, ignore_index, reduction, weight=weight, label_smoothing=eps)
+            return ce_step(pred, y, self.metrics, ignore_index, reduction, weight=weight, label_smoothing=eps)
         if self.loss_kind == "cross_entropy":
-            return ce_step(pred, self.y, self.metrics)    # nn.CrossEntropyLoss + IoU.add in one pass (segmentation.py)
-        return step_loss(pred, self.y, self.metrics)      # loss_func + metrics.update in one pass (metrics.py)
+            return ce_step(pred, y, self.metrics)    # nn.CrossEntropyLoss + IoU.add in one pass (segmentation.py)
+        return step_loss(pred, y, self.metrics)      # loss_func + metrics.update in one pass (metrics.py)
 
     def _phase1(self):
         """Zero the bucket, forward, loss, backward down to the attention maps (all decoder gradients)."""
@@ -275,7 +291,7 @@ class TrainSession:
         if eager:
             self._phase2()
         else:
-            self.graphs[1].replay()
+            self._size_graphs[self._rows][1].replay()
         if two:
             self._reduce(0, tail, self.stream)
             self._ev_comm.record(self.comm)
@@ -292,25 +308,39 @@ class TrainSession:
         self.stream.wait_stream(cur)
         with torch.cuda.device(self.device), torch.cuda.stream(self.stream):
             self.allreduce_events = []
+            self._rows = self.batch
             self._verify_split()
-            for _ in range(max(1, warmup)):   # builds caches, sizes the allocator, warms NCCL
-                self._eager_step()
+            for m in reversed(self.sizes):    # every size before any capture: builds caches, sizes the allocator, warms NCCL
+                self._rows = m
+                for _ in range(max(1, warmup)):
+                    self._eager_step()
             self.stream.synchronize()
-            n0 = _lib.launch_count()
-            if self.use_graph:
-                g1, g2, g3 = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g1, stream=self.stream):
+            # Every size captures into the capacity's pool, as InferenceSession's sizes do (engine.py): one stream replays
+            # them, a step's graphs run back to back, and nothing in the pool outlives a step.
+            pool = None
+            for m in reversed(self.sizes):
+                self._rows = m
+                n0 = _lib.launch_count()
+                if self.use_graph:
+                    g1, g2 = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+                    with ops.gc_paused(), torch.cuda.graph(g1, stream=self.stream, pool=pool):
+                        self._phase1()
+                    pool = g1.pool() if pool is None else pool
+                    with ops.gc_paused(), torch.cuda.graph(g2, stream=self.stream, pool=pool):
+                        self._phase2()
+                    self._size_graphs[m] = (g1, g2)
+                    if m == self.batch:
+                        g3 = torch.cuda.CUDAGraph()
+                        with ops.gc_paused(), torch.cuda.graph(g3, stream=self.stream, pool=pool):
+                            self._optimise()
+                        self.graphs = (g1, g2, g3)
+                elif m == self.batch:
                     self._phase1()
-                with torch.cuda.graph(g2, stream=self.stream, pool=g1.pool()):
                     self._phase2()
-                with torch.cuda.graph(g3, stream=self.stream, pool=g1.pool()):
                     self._optimise()
-                self.graphs = (g1, g2, g3)
-            else:
-                self._phase1()
-                self._phase2()
-                self._optimise()
-            self.launches_per_step = int(_lib.launch_count() - n0)
+                if m == self.batch:
+                    self.launches_per_step = int(_lib.launch_count() - n0)
+            self._rows = self.batch
             self.stream.synchronize()
         self._restore(snap)
         cur.wait_stream(self.stream)
@@ -367,15 +397,16 @@ class TrainSession:
             self._n = 0
         i = self._n % 2
         self._n += 1
-        sx, sy = self._slots[i]
+        n = self._rows
+        sx, sy = self._slots[i][0][:n], self._slots[i][1][:n]
         with torch.cuda.stream(self.h2d):
             self.h2d.wait_event(self._slot_free[i])
             sx.copy_(x, non_blocking=True)
             sy.copy_(y.reshape(sy.shape), non_blocking=True)
             self._h2d_done[i].record(self.h2d)
         self.stream.wait_event(self._h2d_done[i])
-        self.x.copy_(sx, non_blocking=True)
-        self.y.copy_(sy, non_blocking=True)
+        self.x[:n].copy_(sx, non_blocking=True)
+        self.y[:n].copy_(sy, non_blocking=True)
         self._slot_free[i].record(self.stream)
 
     def last_h2d_event(self):
@@ -386,20 +417,39 @@ class TrainSession:
         return self._h2d_done[(self._n - 1) % 2]
 
     def load_batch(self, x, y):
-        """Copy a batch into the static input buffers (async).  Host tensors (pinned for true overlap) are staged on a
-        separate copy stream so the transfer of step i+1 hides behind the compute of step i."""
+        """Copy a batch of 1 <= n <= batch rows into the leading rows of the static input buffers (async).  Host tensors
+        (pinned for true overlap) are staged on a separate copy stream so the transfer of step i+1 hides behind the compute
+        of step i."""
         if self._ce is not None and y.is_floating_point():
             raise TypeError(f"TrainSession: this session's cross-entropy loss takes int64 class-index targets, got {y.dtype}; "
                             "probability targets go through the eager path (smaat_unet_b200.cross_entropy)")
+        n = int(x.shape[0]) if x.dim() == 1 + len(self.in_shape) else -1
+        if not 1 <= n <= self.batch or tuple(x.shape[1:]) != self.in_shape or y.numel() != n * self.y[0].numel():
+            raise ValueError(f"TrainSession: expected x (n, {', '.join(map(str, self.in_shape))}) and y with n * "
+                             f"{self.y[0].numel()} elements, 1 <= n <= {self.batch}; got x {tuple(x.shape)}, y {tuple(y.shape)}")
+        self._rows = n
         if x.device.type == "cpu":
             self._stage(x, y)
         else:
-            self.x.copy_(x, non_blocking=True)
-            self.y.copy_(y.reshape(self.y.shape), non_blocking=True)
+            self.x[:n].copy_(x, non_blocking=True)
+            self.y[:n].copy_(y.reshape(self.y[:n].shape), non_blocking=True)
+
+    def _check_rows_agree(self):
+        """Data-parallel ranks must step the same number of samples: a partial step all-gathers n and raises if a rank
+        differs.  Full steps are not checked, so that they stay free of host synchronisation; a full step on one rank
+        against a partial step on another therefore meets the all-gather with the gradient all-reduce and hangs."""
+        if self.world == 1 or self._rows == self.batch:
+            return
+        rows = [None] * self.world
+        dist.all_gather_object(rows, self._rows)
+        if len(set(rows)) != 1:
+            raise ValueError(f"TrainSession: the ranks step different batch sizes {rows}; every rank must step the same n "
+                             "(PinnedBatchLoader / shard_indices pad the shards to equal length)")
 
     def step(self, x=None, y=None):
-        """One training step on (x, y) (or on the batch already loaded).  Returns the loss (0-dim device tensor, valid in
-        stream order; it is overwritten by the next step)."""
+        """One training step on (x, y) of 1 <= n <= batch rows (or on the batch already loaded).  A size with captured
+        graphs replays them; any other runs the same step eagerly.  Returns the loss (0-dim device tensor, valid in stream
+        order; it is overwritten by the next step)."""
         cur = torch.cuda.current_stream(self.device)
         self.stream.wait_stream(cur)
         if self.record_comm_timing:
@@ -407,8 +457,10 @@ class TrainSession:
         with torch.cuda.stream(self.stream):
             if x is not None:
                 self.load_batch(x, y)
-            if self.use_graph:
-                self.graphs[0].replay()
+            self._check_rows_agree()
+            graphs = self._size_graphs.get(self._rows) if self.use_graph else None
+            if graphs is not None:
+                graphs[0].replay()
                 self._sync_grads_and_phase2(eager=False)
                 self.graphs[2].replay()
             else:
