@@ -429,6 +429,19 @@ int smaat_conv3x3_bwd_weight(const float* dz, const float* x0, int C0, int64_t x
 int smaat_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, const float* lr,
                     float* step, double beta1, double beta2, double eps, void* stream);
 
+/* ---- VOC training input: the per-sample random augmentations, ToTensor, Normalize and the target map of
+ * VOCSegmentation.__getitem__ / apply_augmentations (reference utils/dataset_VOC.py:139-168), after the deterministic
+ * Resize(256) + CenterCrop(224) (train_SmaAtUNet.py:149) has run offline, in one launch per batch.
+ * x_u8 (B, H, W, 3) uint8 RGB and y_u8 (B, H, W) uint8 mask indices, dense.  aug (B, 3) int8 device rows
+ * (flip, rot, bright), or NULL for none: flip != 0 -> TF.hflip of image and mask; then rot > 0 / < 0 -> TF.rotate(+10 / -10)
+ * of both (PIL NEAREST, expand=False, fill 0, bit for bit: the fixed-point or double coordinate walk PIL takes for H x W);
+ * then bright > 0 / < 0 -> TF.adjust_brightness(1.2 / 1.2 - 0.4) of the image.  x (B, 3, H, W) fp32 receives
+ * (v / 255 - mean[c]) / std[c] (IEEE fp32 operations, ToTensor + Normalize), y (B, H, W) int64 the mask with 255 -> 0;
+ * x_bstride >= 3 H W, y_bstride >= H W (elements).  mean, std: HOST float[3], read at the call (their values are baked into
+ * a captured launch).  Any H, W >= 1. */
+int smaat_voc_augment_fwd(const uint8_t* x_u8, const uint8_t* y_u8, const int8_t* aug, const float* mean, const float* std,
+                          float* x, int64_t x_bstride, int64_t* y, int64_t y_bstride, int B, int H, int W, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,8 +6,8 @@ reference's own classes (``patch_reference``), and the functional kernel wrapper
 All arithmetic runs in ``libsmaat_b200.so`` (C ABI: ``include/smaat_b200.h``).
 """
 from . import _lib, ops  # noqa: F401
-from .data import (PinnedBatchLoader, precipitation_maps_classification_shard, precipitation_maps_oversampled_shard,  # noqa: F401
-                   precipitation_maps_shard)
+from .data import (PinnedBatchLoader, convert_voc, precipitation_maps_classification_shard,  # noqa: F401
+                   precipitation_maps_oversampled_shard, precipitation_maps_shard, voc_segmentation_shard)
 from .metrics import PrecipitationMetrics, loss_func, step_loss  # noqa: F401
 from .segmentation import ConfusionMatrix, CrossEntropyLoss, CrossEntropyLossWithOptions, IoU, ce_step, cross_entropy  # noqa: F401
 from .model import SmaAt_UNet, UNet, UNetAttention  # noqa: F401

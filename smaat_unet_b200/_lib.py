@@ -84,6 +84,7 @@ SIGNATURES = {
     "smaat_conv3x3_tc_eligible": [_p, _l, _p, _i, _l, _p, _i, _i],
     "smaat_conv3x3_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _p],
     "smaat_conv3x3_bwd_weight": [_p, _p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _p],
+    "smaat_voc_augment_fwd": [_p, _p, _p, _p, _p, _p, _l, _p, _l, _i, _i, _i, _p],
 }
 _SPECIAL = {
     "smaat_abi_version": ([], _i),

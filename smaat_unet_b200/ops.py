@@ -7,6 +7,7 @@ batch stride larger than C*H*W is allowed where the C ABI takes a ``bstride``.
 from __future__ import annotations
 
 import contextlib
+import ctypes as C
 import gc
 import os
 
@@ -750,3 +751,66 @@ def outconv(x, weight, bias):
     y = torch.empty((B, ncls, H, W), device=x.device, dtype=torch.float32)
     _call("smaat_outconv_fwd", 4 * B * (Cin + ncls) * H * W, 2 * B * Cin * ncls * H * W, _lib.load().smaat_outconv_fwd, _ptr(x), _ptr(w), _ptr(bias), _ptr(y), B, Cin, ncls, H * W, _stream())
     return y
+
+
+# ---- VOC training input (reference utils/dataset_VOC.py:139-168) ----
+IMAGENET_MEAN = (0.485, 0.456, 0.406)
+IMAGENET_STD = (0.229, 0.224, 0.225)
+
+
+def _sample_bstride(t, name, dtype, shape):
+    """Batch stride of an output that must be written in place: ``dtype`` CUDA, ``shape``, dense within each sample."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dtype or tuple(t.shape) != tuple(shape):
+        raise ValueError(f"smaat_unet_b200: {name} must be a {dtype} CUDA tensor of shape {tuple(shape)}, got "
+                         f"{getattr(t, 'dtype', type(t).__name__)} {tuple(getattr(t, 'shape', ()))} on {getattr(t, 'device', None)}")
+    if not t[0].is_contiguous():
+        raise ValueError(f"smaat_unet_b200: {name} must be dense within each sample, got strides {t.stride()}")
+    return t.stride(0) if shape[0] > 1 else t[0].numel()
+
+
+def voc_augment(x_u8, y_u8, aug=None, mean=IMAGENET_MEAN, std=IMAGENET_STD, out_x=None, out_y=None):
+    """The VOC sample pipeline after Resize(256) + CenterCrop(224), on the device, bit for bit (smaat_voc_augment_fwd):
+    ``x_u8`` (B, H, W, 3) and ``y_u8`` (B, H, W) uint8 CUDA tensors (the shards of ``data.convert_voc``), ``aug`` (B, 3) int8
+    rows (flip, rot, bright) from ``voc_segmentation_shard.draw_augmentation`` or None for no augmentation (the reference's
+    validation set).  Returns ``(x, y)``: (B, 3, H, W) fp32 ``Normalize(mean, std)(ToTensor(img))`` and (B, H, W) int64 with
+    255 -> 0.  ``out_x`` / ``out_y`` receive the result in place (e.g. the leading rows of a session's static inputs); they
+    may have any batch stride."""
+    for t, name, nd in ((x_u8, "x_u8", 4), (y_u8, "y_u8", 3)):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8 or t.dim() != nd:
+            raise ValueError(f"smaat_unet_b200: {name} must be a {nd}-D uint8 CUDA tensor, got "
+                             f"{getattr(t, 'dtype', type(t).__name__)} {tuple(getattr(t, 'shape', ()))}")
+    B, H, W, C3 = x_u8.shape
+    if B < 1 or C3 != 3 or tuple(y_u8.shape) != (B, H, W):
+        raise ValueError(f"smaat_unet_b200: voc_augment needs x_u8 (B, H, W, 3) and y_u8 (B, H, W), got {tuple(x_u8.shape)} "
+                         f"and {tuple(y_u8.shape)}")
+    x_u8, y_u8 = x_u8.contiguous(), y_u8.contiguous()
+    if aug is not None:
+        if aug.dtype != torch.int8 or tuple(aug.shape) != (B, 3):
+            raise ValueError(f"smaat_unet_b200: aug must be (B, 3) = ({B}, 3) int8, got {aug.dtype} {tuple(aug.shape)}")
+        aug = aug.to(x_u8.device).contiguous()
+    if out_x is None:
+        out_x = torch.empty((B, 3, H, W), device=x_u8.device, dtype=torch.float32)
+    if out_y is None:
+        out_y = torch.empty((B, H, W), device=x_u8.device, dtype=torch.int64)
+    xbs = _sample_bstride(out_x, "out_x", torch.float32, (B, 3, H, W))
+    ybs = _sample_bstride(out_y, "out_y", torch.int64, (B, H, W))
+    m, s = (C.c_float * 3)(*[float(v) for v in mean]), (C.c_float * 3)(*[float(v) for v in std])
+    _call("smaat_voc_augment_fwd", 24 * B * H * W, 0, _lib.load().smaat_voc_augment_fwd, _ptr(x_u8), _ptr(y_u8), _ptr(aug), m, s,
+          _ptr(out_x), xbs, _ptr(out_y), ybs, B, H, W, _stream())
+    return out_x, out_y
+
+
+class VOCNormalize:
+    """The input transform of a ``TrainSession`` fed uint8 VOC batches: ``sess.step(x_u8, y_u8, aug=aug)`` runs
+    ``voc_augment`` straight into the session's static inputs.  ``mean`` / ``std``: the reference's Normalize arguments."""
+
+    def __init__(self, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+        self.mean, self.std = tuple(float(v) for v in mean), tuple(float(v) for v in std)
+        if len(self.mean) != 3 or len(self.std) != 3:
+            raise ValueError("VOCNormalize: mean and std need three values (RGB)")
+
+    def __call__(self, x_u8, y_u8, aug=None, out_x=None, out_y=None):
+        return voc_augment(x_u8, y_u8, aug, self.mean, self.std, out_x=out_x, out_y=out_y)
+
+    def __repr__(self):
+        return f"VOCNormalize(mean={self.mean}, std={self.std})"

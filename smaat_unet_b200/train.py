@@ -47,6 +47,17 @@ sizes below ``batch`` that get captured graphs of their own (e.g. an epoch's tai
 it).
 
     sess = TrainSession(model, 32, (12, 288, 288), batch_sizes=(len(shard) % 32,))
+
+uint8 input (VOC segmentation).  ``input_transform=ops.VOCNormalize(mean, std)`` makes ``step`` take the uint8 batches of
+``data.voc_segmentation_shard``: x (n, H, W, 3), y (n, H, W) and ``aug`` (n, 3) int8 (the loader's drawn choices, or None).
+Host batches are staged as uint8 (4x fewer bytes than fp32 for the image, 8x fewer than int64 for the target) and
+``ops.voc_augment`` writes the augmented, normalised fp32 image and int64 target straight into the static inputs on the compute
+stream; the captured graphs are the same.  Such a session takes uint8 batches only; ``in_shape`` is (3, H, W).
+
+    sess = TrainSession(SmaAt_UNet(3, 21), 8, (3, 224, 224), loss="cross_entropy", input_transform=ops.VOCNormalize())
+    for x, y, aug in loader:                  # PinnedBatchLoader(voc_segmentation_shard(prefix, augmentations=True), 8)
+        sess.step(x, y, aug=aug)
+        loader.guard(sess.last_h2d_event())
 """
 from __future__ import annotations
 
@@ -67,7 +78,8 @@ _DEFAULT = object()  # metrics argument not given: the loss's own default metric
 
 class TrainSession:
     def __init__(self, model, batch, in_shape, lr=1e-3, device=None, use_graph=True, metrics=_DEFAULT, warmup=3,
-                 betas=(0.9, 0.999), eps=1e-8, overlap_allreduce=True, recompute_depthwise=False, loss="mse", batch_sizes=None):
+                 betas=(0.9, 0.999), eps=1e-8, overlap_allreduce=True, recompute_depthwise=False, loss="mse", batch_sizes=None,
+                 input_transform=None):
         batch = int(batch)
         extra = [int(m) for m in (batch_sizes or ())]
         if batch < 1 or any(not 1 <= m <= batch for m in extra):
@@ -92,6 +104,10 @@ class TrainSession:
             self._ce = (int(ce_loss.ignore_index), ce_loss.reduction, w, float(ce_loss.label_smoothing))
         self.model = model.to(self.device).train()
         self.batch, self.in_shape = batch, tuple(in_shape)
+        self.input_transform = input_transform
+        if input_transform is not None and (loss != "cross_entropy" or len(self.in_shape) != 3 or self.in_shape[0] != 3):
+            raise ValueError(f"TrainSession: input_transform feeds RGB images and class-index targets: it needs in_shape "
+                             f"(3, H, W) and a cross-entropy loss, got in_shape {self.in_shape} and loss {loss!r}")
         self._rows = batch                # rows of the batch loaded in the static buffers
         self.world = dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1
         self.use_graph = bool(use_graph)
@@ -386,12 +402,18 @@ class TrainSession:
         dist.all_gather(out, t)
         return [o.tolist() for o in out]
 
-    def _stage(self, x, y):
+    def _stage(self, x, y, aug=None):
         """Host batch -> device staging slot on the copy stream (overlaps the previous step's compute), then a
-        device-to-device copy into the graph's static inputs on the compute stream."""
+        device-to-device copy (or the input transform) into the graph's static inputs on the compute stream."""
         if not hasattr(self, "_slots"):
             self.h2d = torch.cuda.Stream(self.device)
-            self._slots = [(torch.empty_like(self.x), torch.empty_like(self.y)) for _ in range(2)]
+            if self.input_transform is None:
+                self._slots = [(torch.empty_like(self.x), torch.empty_like(self.y), None) for _ in range(2)]
+            else:
+                B, (H, W) = self.batch, self.in_shape[1:]
+                u8 = dict(device=self.device, dtype=torch.uint8)
+                self._slots = [(torch.empty((B, H, W, 3), **u8), torch.empty((B, H, W), **u8),
+                                torch.empty((B, 3), device=self.device, dtype=torch.int8)) for _ in range(2)]
             self._h2d_done = [torch.cuda.Event() for _ in range(2)]
             self._slot_free = [torch.cuda.Event() for _ in range(2)]
             self._n = 0
@@ -399,14 +421,20 @@ class TrainSession:
         self._n += 1
         n = self._rows
         sx, sy = self._slots[i][0][:n], self._slots[i][1][:n]
+        sa = self._slots[i][2][:n] if aug is not None else None
         with torch.cuda.stream(self.h2d):
             self.h2d.wait_event(self._slot_free[i])
             sx.copy_(x, non_blocking=True)
             sy.copy_(y.reshape(sy.shape), non_blocking=True)
+            if sa is not None:
+                sa.copy_(aug, non_blocking=True)
             self._h2d_done[i].record(self.h2d)
         self.stream.wait_event(self._h2d_done[i])
-        self.x[:n].copy_(sx, non_blocking=True)
-        self.y[:n].copy_(sy, non_blocking=True)
+        if self.input_transform is None:
+            self.x[:n].copy_(sx, non_blocking=True)
+            self.y[:n].copy_(sy, non_blocking=True)
+        else:
+            self.input_transform(sx, sy, sa, out_x=self.x[:n], out_y=self.y[:n])
         self._slot_free[i].record(self.stream)
 
     def last_h2d_event(self):
@@ -416,10 +444,15 @@ class TrainSession:
             return None
         return self._h2d_done[(self._n - 1) % 2]
 
-    def load_batch(self, x, y):
+    def load_batch(self, x, y, aug=None):
         """Copy a batch of 1 <= n <= batch rows into the leading rows of the static input buffers (async).  Host tensors
         (pinned for true overlap) are staged on a separate copy stream so the transfer of step i+1 hides behind the compute
-        of step i."""
+        of step i.  With an ``input_transform``, x / y are uint8 (n, H, W, 3) / (n, H, W) and ``aug`` the (n, 3) int8
+        choices (or None), and the transform writes the static inputs."""
+        if self.input_transform is not None:
+            return self._load_u8(x, y, aug)
+        if x.dtype == torch.uint8 or aug is not None:
+            raise TypeError("TrainSession: uint8 batches and aug need a session built with input_transform=ops.VOCNormalize()")
         if self._ce is not None and y.is_floating_point():
             raise TypeError(f"TrainSession: this session's cross-entropy loss takes int64 class-index targets, got {y.dtype}; "
                             "probability targets go through the eager path (smaat_unet_b200.cross_entropy)")
@@ -434,6 +467,21 @@ class TrainSession:
             self.x[:n].copy_(x, non_blocking=True)
             self.y[:n].copy_(y.reshape(self.y[:n].shape), non_blocking=True)
 
+    def _load_u8(self, x, y, aug):
+        H, W = self.in_shape[1:]
+        n = int(x.shape[0]) if x.dim() == 4 else -1
+        if x.dtype != torch.uint8 or y.dtype != torch.uint8 or not 1 <= n <= self.batch or tuple(x.shape[1:]) != (H, W, 3) \
+                or y.numel() != n * H * W:
+            raise ValueError(f"TrainSession(input_transform=...): expected uint8 x (n, {H}, {W}, 3) and uint8 y with n * {H * W} "
+                             f"elements, 1 <= n <= {self.batch}; got x {x.dtype} {tuple(x.shape)}, y {y.dtype} {tuple(y.shape)}")
+        if aug is not None and (aug.dtype != torch.int8 or tuple(aug.shape) != (n, 3)):
+            raise ValueError(f"TrainSession: aug must be ({n}, 3) int8, got {aug.dtype} {tuple(aug.shape)}")
+        self._rows = n
+        if x.device.type == "cpu":
+            self._stage(x, y, aug)
+        else:
+            self.input_transform(x, y.reshape(n, H, W), aug, out_x=self.x[:n], out_y=self.y[:n])
+
     def _check_rows_agree(self):
         """Data-parallel ranks must step the same number of samples: a partial step all-gathers n and raises if a rank
         differs.  Full steps are not checked, so that they stay free of host synchronisation; a full step on one rank
@@ -446,17 +494,18 @@ class TrainSession:
             raise ValueError(f"TrainSession: the ranks step different batch sizes {rows}; every rank must step the same n "
                              "(PinnedBatchLoader / shard_indices pad the shards to equal length)")
 
-    def step(self, x=None, y=None):
+    def step(self, x=None, y=None, aug=None):
         """One training step on (x, y) of 1 <= n <= batch rows (or on the batch already loaded).  A size with captured
         graphs replays them; any other runs the same step eagerly.  Returns the loss (0-dim device tensor, valid in stream
-        order; it is overwritten by the next step)."""
+        order; it is overwritten by the next step).  ``aug``: the (n, 3) int8 augmentation choices of a uint8 batch on a
+        session with an ``input_transform``."""
         cur = torch.cuda.current_stream(self.device)
         self.stream.wait_stream(cur)
         if self.record_comm_timing:
             self.allreduce_events = []
         with torch.cuda.stream(self.stream):
             if x is not None:
-                self.load_batch(x, y)
+                self.load_batch(x, y, aug)
             self._check_rows_agree()
             graphs = self._size_graphs.get(self._rows) if self.use_graph else None
             if graphs is not None:
