@@ -442,6 +442,52 @@ int smaat_adam_step(float* params, const float* grads, float* exp_avg, float* ex
 int smaat_voc_augment_fwd(const uint8_t* x_u8, const uint8_t* y_u8, const int8_t* aug, const float* mean, const float* std,
                           float* x, int64_t x_bstride, int64_t* y, int64_t y_bstride, int B, int H, int W, void* stream);
 
+/* ---- bf16 activations: SmaAt-UNet's serving forward from bf16 input ------------------------------------------------------
+ * The serving forward's bf16 storage route keeps the input and the level 1-3 feature maps (and the logits / probabilities) as
+ * bf16 in HBM: raw uint16_t bits, round to nearest even, passed as void*.  Arithmetic stays fp32 (the GEMMs take bf16 operands
+ * with fp32 accumulation, as SMAAT_PW_BF16); every stored bf16 value is rounded once.  Weights, scales, gates, pools and the
+ * class map keep their fp32 / int64 forms.  Each entry point mirrors the fp32 one named beside it.
+ *
+ * smaat_dsconv_bf16_fwd (smaat_dsconv_fwd / smaat_dsconv_cbam_fwd): x0, x1 and y bf16, pw_w the smaat_pack_bf16 pack; gate_sc /
+ *   gate_sa (fp32, both or neither) read x0 as the CBAM output (x0 * sc) * sa, computed in fp32.  k = 1 or 2, the register A
+ *   form, W and the batch strides multiples of 8, 16-byte aligned tensors; no batch statistics, no CBAM pools.
+ * smaat_dsconv_outconv_bf16_fwd / smaat_dsconv_classify_bf16_fwd (the *_fwd of the same name): the 1-class OutConv, or the
+ *   K-class OutConv and the argmax, in the epilogue; logits (optional for classify) stored as bf16, the argmax taken on the fp32
+ *   logits in registers.
+ * smaat_dsconv_bf16_eligible: 1 if those take the request: ncls = 0 for smaat_dsconv_bf16_fwd, else the classes of the head.
+ * smaat_cbam_pool_mlp_bf16_fwd / smaat_cbam_pool_maxpool_bf16_fwd: the pools (+ MLP) and the 2x2 max-pool of a bf16 x; the max-pool
+ *   is written as bf16 (pooled_bf16 = 1) or fp32, the dtype of the level it feeds.  The max-pool is required (even H, W % 4 == 0).
+ * smaat_cbam_reduce_bf16_fwd: the per-pixel channel mean / max of x * sc from a bf16 x, fp32 out.
+ * smaat_upsample2x_pad_bf16_fwd: bilinear x2 + pad to a bf16 y, from an fp32 (x_bf16 = 0) or bf16 x; Wo % 4 == 0.
+ * smaat_outconv_bf16_fwd, smaat_argmax_channels_bf16_fwd, smaat_softmax_channels_bf16_fwd: the unfused heads from bf16
+ *   activations / logits; OutConv and the softmax write bf16. */
+int smaat_dsconv_bf16_eligible(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                               const void* pw_w, int H, int W, int k, int Cout, int ncls);
+int smaat_dsconv_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                          const float* dw_w, const float* dw_b, const uint16_t* pw_w, const float* scale, const float* shift,
+                          void* y, int64_t y_bstride, const float* gate_sc, const float* gate_sa, int B, int H, int W, int k,
+                          int Cout, int relu, void* stream);
+int smaat_dsconv_outconv_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                                  const float* dw_w, const float* dw_b, const uint16_t* pw_w, const float* scale,
+                                  const float* shift, const float* oc_w, const float* oc_b, void* logits, int B, int H, int W,
+                                  int k, int Cout, int relu, void* stream);
+int smaat_dsconv_classify_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                                   const float* dw_w, const float* dw_b, const uint16_t* pw_w, const float* scale,
+                                   const float* shift, const float* oc_w, const float* oc_b, int K, void* logits,
+                                   int64_t* classes, int B, int H, int W, int k, int Cout, int relu, void* stream);
+int smaat_cbam_pool_mlp_bf16_fwd(const void* x, float* avg, float* mx, void* pooled, int pooled_bf16, const float* w1,
+                                 const float* b1, const float* w2, const float* b2, float* sc, int* counters, int B, int C,
+                                 int H, int W, int hidden, void* stream);
+int smaat_cbam_pool_maxpool_bf16_fwd(const void* x, float* avg, float* mx, void* pooled, int pooled_bf16, int64_t N, int H,
+                                     int W, void* stream);
+int smaat_cbam_reduce_bf16_fwd(const void* x, const float* sc, float* pooled, int B, int C, int P, void* stream);
+int smaat_upsample2x_pad_bf16_fwd(const void* x, int x_bf16, void* y, int64_t y_bstride, int B, int C, int H, int W, int Ho,
+                                  int Wo, void* stream);
+int smaat_outconv_bf16_fwd(const void* x, const float* w, const float* bias, void* y, int B, int Cin, int ncls, int P,
+                           void* stream);
+int smaat_argmax_channels_bf16_fwd(const void* x, int64_t* classes, int B, int K, int64_t P, void* stream);
+int smaat_softmax_channels_bf16_fwd(const void* x, void* probs, int B, int K, int64_t P, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -85,6 +85,18 @@ SIGNATURES = {
     "smaat_conv3x3_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _p],
     "smaat_conv3x3_bwd_weight": [_p, _p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _p],
     "smaat_voc_augment_fwd": [_p, _p, _p, _p, _p, _p, _l, _p, _l, _i, _i, _i, _p],
+    # ---- bf16 activations (the serving forward's bf16 route)
+    "smaat_dsconv_bf16_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i],
+    "smaat_dsconv_bf16_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _l, _p, _p, _i, _i, _i, _i, _i, _i, _p],
+    "smaat_dsconv_outconv_bf16_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
+    "smaat_dsconv_classify_bf16_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _p],
+    "smaat_cbam_pool_mlp_bf16_fwd": [_p, _p, _p, _p, _i, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p],
+    "smaat_cbam_pool_maxpool_bf16_fwd": [_p, _p, _p, _p, _i, _l, _i, _i, _p],
+    "smaat_cbam_reduce_bf16_fwd": [_p, _p, _p, _i, _i, _i, _p],
+    "smaat_upsample2x_pad_bf16_fwd": [_p, _i, _p, _l, _i, _i, _i, _i, _i, _i, _p],
+    "smaat_outconv_bf16_fwd": [_p, _p, _p, _p, _i, _i, _i, _i, _p],
+    "smaat_argmax_channels_bf16_fwd": [_p, _p, _i, _i, _l, _p],
+    "smaat_softmax_channels_bf16_fwd": [_p, _p, _i, _i, _l, _p],
 }
 _SPECIAL = {
     "smaat_abi_version": ([], _i),

@@ -191,7 +191,9 @@ __global__ void __launch_bounds__(256) cbam_mlp_kernel(const float* __restrict__
 // ---- per-pixel channel mean / max of x*sc --------------------------------------------------------------
 // Large planes: a thread owns 4 pixels and walks every channel with 8 independent 128-bit loads in flight -- no
 // cross-thread reduction, no barrier; s_c of the image is staged in shared memory.
-__global__ void __launch_bounds__(256) cbam_reduce_v4_kernel(const float* __restrict__ x, const float* __restrict__ sc,
+// TI: the storage type of x (float, or uint16_t bf16 in the serving forward's bf16 route); pooled is fp32 either way
+template <typename TI>
+__global__ void __launch_bounds__(256) cbam_reduce_v4_kernel(const TI* __restrict__ x, const float* __restrict__ sc,
                                                              float* __restrict__ pooled, int C, int P4) {
   extern __shared__ float scs[];
   const int b = blockIdx.y;
@@ -199,14 +201,14 @@ __global__ void __launch_bounds__(256) cbam_reduce_v4_kernel(const float* __rest
   __syncthreads();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= P4) return;
-  const float4* x4 = reinterpret_cast<const float4*>(x) + (int64_t)b * C * P4 + i;
+  const TI* x4 = x + ((int64_t)b * C * P4 + i) * 4;
   float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
   float4 m = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
   int c = 0;
   for (; c + 8 <= C; c += 8) {
     float4 v[8];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) v[u] = __ldg(x4 + (int64_t)(c + u) * P4);
+    for (int u = 0; u < 8; ++u) v[u] = ld_act4(x4 + (int64_t)(c + u) * P4 * 4);
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
       const float g = scs[c + u];
@@ -216,7 +218,7 @@ __global__ void __launch_bounds__(256) cbam_reduce_v4_kernel(const float* __rest
     }
   }
   for (; c < C; ++c) {
-    const float4 v = __ldg(x4 + (int64_t)c * P4);
+    const float4 v = ld_act4(x4 + (int64_t)c * P4 * 4);
     const float g = scs[c];
     const float a0 = v.x * g, a1 = v.y * g, a2 = v.z * g, a3 = v.w * g;
     s.x += a0; s.y += a1; s.z += a2; s.w += a3;
@@ -229,15 +231,15 @@ __global__ void __launch_bounds__(256) cbam_reduce_v4_kernel(const float* __rest
 }
 
 // blockDim = (32 pixel-quads, 8 channel groups); smem tree over the 8 groups.
-template <bool VEC>
-__global__ void __launch_bounds__(256) cbam_reduce_kernel(const float* __restrict__ x, const float* __restrict__ sc,
+template <bool VEC, typename TI = float>
+__global__ void __launch_bounds__(256) cbam_reduce_kernel(const TI* __restrict__ x, const float* __restrict__ sc,
                                                           float* __restrict__ pooled, int C, int P) {
   __shared__ float4 rs[8][32];
   __shared__ float4 rm[8][32];
   const int tx = threadIdx.x, cg = threadIdx.y;
   const int b = blockIdx.y;
   const int pp = (blockIdx.x * 32 + tx) * 4;
-  const float* xb = x + (int64_t)b * C * P;
+  const TI* xb = x + (int64_t)b * C * P;
   const float* scb = sc + (int64_t)b * C;
   float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
   float4 m = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
@@ -246,14 +248,14 @@ __global__ void __launch_bounds__(256) cbam_reduce_kernel(const float* __restric
     for (int c = cg; c < C; c += 8) {
       const float g = __ldg(scb + c);
       float4 v;
-      const float* src = xb + (int64_t)c * P + pp;
+      const TI* src = xb + (int64_t)c * P + pp;
       if (VEC) {
-        v = __ldg(reinterpret_cast<const float4*>(src));
+        v = ld_act4(src);
       } else {
-        v.x = __ldg(src);
-        v.y = (pp + 1 < P) ? __ldg(src + 1) : 0.f;
-        v.z = (pp + 2 < P) ? __ldg(src + 2) : 0.f;
-        v.w = (pp + 3 < P) ? __ldg(src + 3) : 0.f;
+        v.x = ld_act(src);
+        v.y = (pp + 1 < P) ? ld_act(src + 1) : 0.f;
+        v.z = (pp + 2 < P) ? ld_act(src + 2) : 0.f;
+        v.w = (pp + 3 < P) ? ld_act(src + 3) : 0.f;
       }
       v.x *= g; v.y *= g; v.z *= g; v.w *= g;
       s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
@@ -398,9 +400,11 @@ __global__ void __launch_bounds__(256) cbam_scale_kernel(const float* __restrict
 // cbam_l (ChannelAttention pools, layers.py:107-108) and down_l (MaxPool2d(2), parts_ds.py:48) -- models/SmaAt_UNet.py:42-50.
 // A thread takes the same 4 columns of rows 2i and 2i+1 (two 128-bit loads), emits 2 pooled outputs (64-bit store) and
 // folds all 8 values into the plane's sum / max.  TPP threads per plane (256: one plane per CTA; 32: 8 planes per CTA).
-template <int TPP>
-__global__ void __launch_bounds__(256) cbam_pool_maxpool_kernel(const float* __restrict__ x, float* __restrict__ avg,
-                                                                float* __restrict__ mx, float* __restrict__ pooled, int64_t N,
+// TI / TO: the storage types of x and of pooled (float, or uint16_t bf16 in the serving forward's bf16 route; the max of bf16
+// values is a bf16 value, so a bf16 max-pool is exact in either type)
+template <int TPP, typename TI = float, typename TO = float>
+__global__ void __launch_bounds__(256) cbam_pool_maxpool_kernel(const TI* __restrict__ x, float* __restrict__ avg,
+                                                                float* __restrict__ mx, TO* __restrict__ pooled, int64_t N,
                                                                 int H, int W, const MlpTail tail) {
   constexpr int PPB = 256 / TPP;
   const int sub = threadIdx.x / TPP, lane = threadIdx.x % TPP;
@@ -409,14 +413,15 @@ __global__ void __launch_bounds__(256) cbam_pool_maxpool_kernel(const float* __r
   const int items = wq * hp;
   float s = 0.f, m = -INFINITY;
   if (n < N) {
-    const float4* src = reinterpret_cast<const float4*>(x + n * (int64_t)H * W);
-    float2* dst = reinterpret_cast<float2*>(pooled + n * (int64_t)hp * (W >> 1));
+    const TI* src = x + n * (int64_t)H * W;
+    TO* dst = pooled + n * (int64_t)hp * (W >> 1);
 #pragma unroll 2
     for (int i = lane; i < items; i += TPP) {
       const int rp = i / wq, q = i - rp * wq;
-      const float4 a = __ldg(src + (int64_t)(2 * rp) * wq + q), b = __ldg(src + (int64_t)(2 * rp + 1) * wq + q);
+      const float4 a = ld_act4(src + ((int64_t)(2 * rp) * wq + q) * 4), b = ld_act4(src + ((int64_t)(2 * rp + 1) * wq + q) * 4);
       const float m0 = fmaxf(fmaxf(a.x, a.y), fmaxf(b.x, b.y)), m1 = fmaxf(fmaxf(a.z, a.w), fmaxf(b.z, b.w));
-      dst[(int64_t)rp * wq + q] = make_float2(m0, m1);
+      if constexpr (sizeof(TO) == 4) reinterpret_cast<float2*>(dst)[(int64_t)rp * wq + q] = make_float2(m0, m1);
+      else reinterpret_cast<uint32_t*>(dst)[(int64_t)rp * wq + q] = f32x2_bf16x2(m0, m1);
       s += ((a.x + a.y) + (a.z + a.w)) + ((b.x + b.y) + (b.z + b.w));
       m = fmaxf(m, fmaxf(m0, m1));
     }
@@ -698,7 +703,7 @@ extern "C" int smaat_cbam_reduce_fwd(const float* x, const float* sc, float* poo
   SMAAT_REQUIRE(B <= 65535, "cbam_reduce: batch too large for grid.y");
   const bool vec = (P % 4 == 0) && aligned16(x) && aligned16(pooled);
   if (vec && P >= 8192 && (size_t)C * sizeof(float) <= 48 * 1024) {
-    cbam_reduce_v4_kernel<<<dim3(ceil_div(P / 4, 256), B), 256, (size_t)C * sizeof(float), (cudaStream_t)stream>>>(x, sc, pooled, C,
+    cbam_reduce_v4_kernel<float><<<dim3(ceil_div(P / 4, 256), B), 256, (size_t)C * sizeof(float), (cudaStream_t)stream>>>(x, sc, pooled, C,
                                                                                                               P / 4);
     SMAAT_LAUNCH_CHECK("smaat_cbam_reduce_fwd");
     return SMAAT_OK;
@@ -733,5 +738,80 @@ extern "C" int smaat_cbam_scale_fwd(const float* x, const float* sc, const float
   if (vec) cbam_scale_kernel<true><<<grid, threads, 0, (cudaStream_t)stream>>>(x, sc, sa, y, y_bstride, C, P);
   else cbam_scale_kernel<false><<<grid, threads, 0, (cudaStream_t)stream>>>(x, sc, sa, y, y_bstride, C, P);
   SMAAT_LAUNCH_CHECK("smaat_cbam_scale_fwd");
+  return SMAAT_OK;
+}
+
+/* ---- bf16 input: the serving forward's bf16 route ----------------------------------------------------------------------------
+ * x is bf16 (raw uint16_t bits); the pools, the MLP, the gates and the channel reduce run and are stored in fp32.  The 2x2 max-pool
+ * is written in the storage type of the level it feeds: bf16 (pooled_bf16 = 1) or fp32. */
+template <typename TO>
+static int cbam_pool_maxpool_bf16_launch(const uint16_t* x, float* avg, float* mx, void* pooled, int64_t N, int H, int W,
+                                         const MlpTail& t, cudaStream_t st) {
+  TO* po = static_cast<TO*>(pooled);
+  if ((int64_t)H * W >= 2048) {
+    SMAAT_REQUIRE(N < (1ll << 31), "cbam_pool_maxpool_bf16: too many planes");
+    cbam_pool_maxpool_kernel<256, uint16_t, TO><<<(unsigned)N, 256, 0, st>>>(x, avg, mx, po, N, H, W, t);
+  } else {
+    cbam_pool_maxpool_kernel<32, uint16_t, TO><<<(unsigned)ceil_div64(N, 8), 256, 0, st>>>(x, avg, mx, po, N, H, W, t);
+  }
+  return SMAAT_OK;
+}
+
+static int cbam_pool_maxpool_bf16_check(const void* x, void* pooled, int pooled_bf16, int H, int W) {
+  // 4 bf16 columns of a row are one 8-byte load; the two pooled values one 4-byte (bf16) or 8-byte (fp32) store
+  if (W % 4 != 0 || H % 2 != 0 || (reinterpret_cast<uintptr_t>(x) & 7u) ||
+      (reinterpret_cast<uintptr_t>(pooled) & (pooled_bf16 ? 3u : 7u)))
+    return fail(SMAAT_E_UNSUPPORTED, "cbam_pool_maxpool_bf16: needs W %% 4 == 0, even H and aligned pointers (H=%d W=%d)", H, W);
+  return SMAAT_OK;
+}
+
+extern "C" int smaat_cbam_pool_maxpool_bf16_fwd(const void* x, float* avg, float* mx, void* pooled, int pooled_bf16, int64_t N, int H,
+                                                int W, void* stream) {
+  SMAAT_REQUIRE(x && avg && mx && pooled && N > 0 && H > 0 && W > 0, "cbam_pool_maxpool_bf16: bad arguments");
+  if (int r = cbam_pool_maxpool_bf16_check(x, pooled, pooled_bf16, H, W)) return r;
+  const uint16_t* xb = static_cast<const uint16_t*>(x);
+  cudaStream_t st = (cudaStream_t)stream;
+  int r = pooled_bf16 ? cbam_pool_maxpool_bf16_launch<uint16_t>(xb, avg, mx, pooled, N, H, W, MlpTail{}, st)
+                      : cbam_pool_maxpool_bf16_launch<float>(xb, avg, mx, pooled, N, H, W, MlpTail{}, st);
+  if (r) return r;
+  SMAAT_LAUNCH_CHECK("smaat_cbam_pool_maxpool_bf16_fwd");
+  return SMAAT_OK;
+}
+
+/* smaat_cbam_pool_mlp_fwd with the max-pool (required here) from a bf16 x. */
+extern "C" int smaat_cbam_pool_mlp_bf16_fwd(const void* x, float* avg, float* mx, void* pooled, int pooled_bf16, const float* w1,
+                                            const float* b1, const float* w2, const float* b2, float* sc, int* counters, int B, int C,
+                                            int H, int W, int hidden, void* stream) {
+  SMAAT_REQUIRE(x && avg && mx && pooled && w1 && b1 && w2 && b2 && sc && counters && B > 0 && C > 0 && H > 0 && W > 0 && hidden > 0,
+                "cbam_pool_mlp_bf16: bad arguments");
+  if (C % 8 != 0 || C > 512 || hidden > 64)
+    return fail(SMAAT_E_UNSUPPORTED, "cbam_pool_mlp_bf16: needs C %% 8 == 0, C <= 512, hidden <= 64");
+  if (int r = cbam_pool_maxpool_bf16_check(x, pooled, pooled_bf16, H, W)) return r;
+  MlpTail t{w1, b1, w2, b2, sc, counters, C, hidden};
+  const uint16_t* xb = static_cast<const uint16_t*>(x);
+  const int64_t N = (int64_t)B * C;
+  cudaStream_t st = (cudaStream_t)stream;
+  int r = pooled_bf16 ? cbam_pool_maxpool_bf16_launch<uint16_t>(xb, avg, mx, pooled, N, H, W, t, st)
+                      : cbam_pool_maxpool_bf16_launch<float>(xb, avg, mx, pooled, N, H, W, t, st);
+  if (r) return r;
+  SMAAT_LAUNCH_CHECK("smaat_cbam_pool_mlp_bf16_fwd");
+  return SMAAT_OK;
+}
+
+/* smaat_cbam_reduce_fwd from a bf16 x: pooled (B, 2, H, W) fp32. */
+extern "C" int smaat_cbam_reduce_bf16_fwd(const void* x, const float* sc, float* pooled, int B, int C, int P, void* stream) {
+  SMAAT_REQUIRE(x && sc && pooled && B > 0 && C > 0 && P > 0, "cbam_reduce_bf16: bad arguments");
+  SMAAT_REQUIRE(B <= 65535, "cbam_reduce_bf16: batch too large for grid.y");
+  const uint16_t* xb = static_cast<const uint16_t*>(x);
+  const bool vec = (P % 4 == 0) && (reinterpret_cast<uintptr_t>(x) & 7u) == 0 && aligned16(pooled);
+  if (vec && P >= 8192 && (size_t)C * sizeof(float) <= 48 * 1024) {
+    cbam_reduce_v4_kernel<uint16_t><<<dim3(ceil_div(P / 4, 256), B), 256, (size_t)C * sizeof(float), (cudaStream_t)stream>>>(
+        xb, sc, pooled, C, P / 4);
+  } else {
+    dim3 grid(ceil_div(P, 128), B), block(32, 8);
+    if (vec) cbam_reduce_kernel<true, uint16_t><<<grid, block, 0, (cudaStream_t)stream>>>(xb, sc, pooled, C, P);
+    else cbam_reduce_kernel<false, uint16_t><<<grid, block, 0, (cudaStream_t)stream>>>(xb, sc, pooled, C, P);
+  }
+  SMAAT_LAUNCH_CHECK("smaat_cbam_reduce_bf16_fwd");
   return SMAAT_OK;
 }

@@ -444,6 +444,23 @@ __global__ void __launch_bounds__(CE_THREADS) argmax_channels_kernel(const float
   }
 }
 
+// bf16 logits (the serving forward's bf16 route): one pixel per thread, each logit widened exactly; the same rule
+__global__ void __launch_bounds__(CE_THREADS) argmax_channels_bf16_kernel(const uint16_t* __restrict__ x, int64_t* __restrict__ classes,
+                                                                          int K, int64_t P, int64_t n) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n; g += stride) {
+    const int64_t b = g / P, p = g - b * P;
+    const uint16_t* base = x + b * (int64_t)K * P + p;
+    float m = -INFINITY;
+    int am = 0;
+    for (int c = 0; c < K; ++c) {
+      const float v = ld_act(base + (int64_t)c * P);
+      if (m == m && (v > m || v != v)) { m = v; am = c; }
+    }
+    classes[g] = am;
+  }
+}
+
 // Online (max m, sum s) over one pixel's logits, then p = exp(l - m) / s.  Each add() computes
 //   s = fmaf(s, exp(m_old - m_new), exp(l - m_new)),  m_new = fmaxf(m_old, l)
 // in two branches: a new maximum (l > m) evaluates that formula; otherwise m_new = m_old, exp(m - m) is exactly 1 wherever s is
@@ -494,6 +511,20 @@ __global__ void __launch_bounds__(CE_THREADS) softmax_channels_kernel(const floa
       for (int j = 0; j < NPX; ++j) v[j] = acc[j].prob(v[j]);
       store_px<NPX>(probs + off + (int64_t)c * P, v);
     }
+  }
+}
+
+// bf16 logits to bf16 probabilities: softmax_channels_kernel's two sweeps (SoftmaxAcc) on the widened logits, one pixel
+// per thread, each probability rounded once
+__global__ void __launch_bounds__(CE_THREADS) softmax_channels_bf16_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ probs,
+                                                                           int K, int64_t P, int64_t n) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n; g += stride) {
+    const int64_t b = g / P;
+    const int64_t off = b * (int64_t)K * P + (g - b * P);
+    SoftmaxAcc acc;
+    for (int c = 0; c < K; ++c) acc.add(ld_act(x + off + (int64_t)c * P));
+    for (int c = 0; c < K; ++c) st_act(probs + off + (int64_t)c * P, acc.prob(ld_act(x + off + (int64_t)c * P)));
   }
 }
 
@@ -678,5 +709,41 @@ extern "C" int smaat_confusion_add(const int64_t* pred, const int64_t* target, i
   else
     confusion_add_kernel<false><<<(unsigned)blocks, CE_THREADS, 0, st>>>(pred, target, n, K, cf, iv);
   SMAAT_LAUNCH_CHECK("smaat_confusion_add");
+  return SMAAT_OK;
+}
+
+extern "C" int smaat_argmax_channels_bf16_fwd(const void* x, int64_t* classes, int B, int K, int64_t P, void* stream) {
+  SMAAT_REQUIRE(x && classes && B > 0 && P > 0, "argmax_channels_bf16: bad arguments (B=%d, P=%lld)", B, (long long)P);
+  SMAAT_REQUIRE(K >= 1, "argmax_channels_bf16: K=%d classes", K);
+  if (K > 1024) return fail(SMAAT_E_UNSUPPORTED, "argmax_channels_bf16: K=%d classes, this build supports at most 1024", K);
+  SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(x) & 1u) == 0 && (reinterpret_cast<uintptr_t>(classes) & 7u) == 0,
+                "argmax_channels_bf16: logits must be 2-byte and classes 8-byte aligned");
+  const int64_t n = (int64_t)B * P;
+  int64_t blocks = ceil_div64(n, CE_THREADS);
+  const int64_t cap = (int64_t)num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  argmax_channels_bf16_kernel<<<(unsigned)blocks, CE_THREADS, 0, (cudaStream_t)stream>>>(static_cast<const uint16_t*>(x), classes, K,
+                                                                                        P, n);
+  SMAAT_LAUNCH_CHECK("smaat_argmax_channels_bf16_fwd");
+  return SMAAT_OK;
+}
+
+extern "C" int smaat_softmax_channels_bf16_fwd(const void* x, void* probs, int B, int K, int64_t P, void* stream) {
+  SMAAT_REQUIRE(x && probs && B > 0 && P > 0, "softmax_channels_bf16: bad arguments (B=%d, P=%lld)", B, (long long)P);
+  SMAAT_REQUIRE(K >= 1, "softmax_channels_bf16: K=%d classes", K);
+  if (K > 1024) return fail(SMAAT_E_UNSUPPORTED, "softmax_channels_bf16: K=%d classes, this build supports at most 1024", K);
+  SMAAT_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(probs)) & 1u) == 0,
+                "softmax_channels_bf16: logits and probs must be 2-byte aligned");
+  const int64_t n = (int64_t)B * P;
+  // smaat_softmax_channels_fwd's grid rule: the lines the grid reads between its two sweeps fit in half of the L2
+  const int64_t per_cta = (int64_t)CE_THREADS * K * 2;
+  int64_t cap = l2_bytes() / 2 / per_cta;
+  if (cap < num_sms()) cap = num_sms();
+  if (cap > (int64_t)num_sms() * 8) cap = (int64_t)num_sms() * 8;
+  int64_t blocks = ceil_div64(n, CE_THREADS);
+  if (blocks > cap) blocks = cap;
+  softmax_channels_bf16_kernel<<<(unsigned)blocks, CE_THREADS, 0, (cudaStream_t)stream>>>(static_cast<const uint16_t*>(x),
+                                                                                         static_cast<uint16_t*>(probs), K, P, n);
+  SMAAT_LAUNCH_CHECK("smaat_softmax_channels_bf16_fwd");
   return SMAAT_OK;
 }

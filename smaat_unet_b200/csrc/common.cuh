@@ -111,6 +111,45 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
+// bf16 activations (the serving forward's bf16 storage route) are raw uint16_t bits: widened exactly, rounded to nearest even
+__device__ __forceinline__ float bf16_f32(uint16_t h) { return __uint_as_float((uint32_t)h << 16); }
+__device__ __forceinline__ uint16_t f32_bf16(float v) {
+  uint16_t r;
+  asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(r) : "f"(v));
+  return r;
+}
+__device__ __forceinline__ uint32_t f32x2_bf16x2(float lo, float hi) {   // lo at the lower address
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+__device__ __forceinline__ float4 bf16x4_f32(uint2 u) {
+  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                     __uint_as_float(u.y & 0xffff0000u));
+}
+// Activation loads and stores in the storage type T (float or uint16_t bf16), as fp32 values: one element, or four
+// consecutive ones (a 16-byte fp32 / 8-byte bf16 access, which must be aligned to its size)
+template <typename T>
+__device__ __forceinline__ float ld_act(const T* p) {
+  if constexpr (sizeof(T) == 4) return __ldg(p);
+  else return bf16_f32(__ldg(reinterpret_cast<const unsigned short*>(p)));
+}
+template <typename T>
+__device__ __forceinline__ float4 ld_act4(const T* p) {
+  if constexpr (sizeof(T) == 4) return __ldg(reinterpret_cast<const float4*>(p));
+  else return bf16x4_f32(__ldg(reinterpret_cast<const uint2*>(p)));
+}
+template <typename T>
+__device__ __forceinline__ void st_act(T* p, float v) {
+  if constexpr (sizeof(T) == 4) *p = v;
+  else *p = f32_bf16(v);
+}
+template <typename T>
+__device__ __forceinline__ void st_act4(T* p, float4 v) {
+  if constexpr (sizeof(T) == 4) *reinterpret_cast<float4*>(p) = v;
+  else *reinterpret_cast<uint2*>(p) = make_uint2(f32x2_bf16x2(v.x, v.y), f32x2_bf16x2(v.z, v.w));
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -11,7 +11,7 @@
 // channels (Cout <= 128: one pass, so the depthwise work is done exactly once; Cout in {256, 384, 512}: passes of 128).
 // K = k*Cin is walked in chunks of 32 depthwise channels (CC = 32/k input channels):
 //   warp 0      TMA: (PH+2) x (PW+8) x CC input halo box per chunk (OOB zero fill = padding=1; box
-//               starts at x0-4: the inner TMA coordinate must be 16-byte aligned) into an IS-deep ring;
+//               starts at x0-4, x0-8 for bf16 input: the inner TMA coordinate must be 16-byte aligned) into an IS-deep ring;
 //               input may be the virtual concat [x0, x1] of UpDS (parts_ds.py:85).  An L2 prefetch of the next tile's boxes
 //               (cp.async.bulk.prefetch.tensor) made bench.py's B = 32 forward slower: 2 220 vs 2 346-2 369 frames/s (H100
 //               80GB HBM3 SXM, 700 W; two runs with, six without), so there is none
@@ -77,14 +77,20 @@ struct DsParams {
 
 constexpr int DS_MAX_CLASSES = 32;   // classes of the fused K-class OutConv + argmax (smaat_dsconv_classify_fwd)
 
-template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM>
+// TA: the storage type of the input (x0, x1) and of the output (y or the logits): float, or uint16_t for the bf16 activations
+// of the serving forward's bf16 route (dsconv_bf16act_kernel)
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float>
 struct DsCfg {
   static constexpr bool X3 = P == Prec::TF32X3;
+  static constexpr int ESZ = (int)sizeof(TA);
+  static_assert(ESZ == 4 || (P == Prec::BF16 && KPL != 4), "bf16 activations: the bf16 register-form instances, k = 1, 2");
   static_assert(P != Prec::BF16 || !A_SMEM, "BF16: register A form only");
   static constexpr int PH = TC_BM / PW;
-  static constexpr int BW = PW + 8, BH = PH + 2;
+  // input boxes start XM columns left of the patch: 16 bytes, the alignment TMA takes for the inner coordinate (4 fp32, 8 bf16)
+  static constexpr int XM = 16 / ESZ;
+  static constexpr int BW = PW + 2 * XM, BH = PH + 2;
   static constexpr int CC = TC_BK / KPL;                       // input channels per chunk
-  static constexpr int IN_BYTES = CC * BH * BW * 4;            // multiple of 128 for PW in {16,32}
+  static constexpr int IN_BYTES = CC * BH * BW * ESZ;          // multiple of 128 for PW in {16,32}
   static constexpr int A_BYTES = TC_BM * TC_BK * 4;            // 16 KB
   static constexpr int B_BYTES = N_TILE * TC_BK * (P == Prec::BF16 ? 2 : 4);   // 128-byte rows (bf16: 64-byte rows)
   // A ring stage: fp32 (register form: the consumers split hi / lo after loading), or hi [+ lo] (A_SMEM: the tensor core reads
@@ -113,7 +119,7 @@ struct DsCfg {
   // 6 -> 4 at N_TILE 64 and 4 -> 2 at N_TILE 128 (one buffer there, with a 3-deep input ring, measured 1-6 % slower per
   // layer: DESIGN §6).  Where two would leave the input ring under 2 stages one is used, and where even one would (k = 1 at
   // N_TILE 128 in 3xTF32: 30 KB boxes), the instance keeps the direct-store epilogue (ST_BUFS = 0)
-  static constexpr int ST_BOX = 32 * 64 * 4;
+  static constexpr int ST_BOX = 32 * 64 * ESZ;
   static constexpr int ST_WANT = 2;
   static constexpr int ST_BUFS = (FREE - 2 * ST_WANT * ST_BOX) / IN_BYTES >= 2 ? ST_WANT
                                  : (FREE - 2 * ST_BOX) / IN_BYTES >= 2     ? 1
@@ -201,12 +207,13 @@ __device__ __forceinline__ void quad_transpose(float (&v)[4], int q) {
 
 // The kernel body, shared by the k = 1 / 2 instances (dsconv_fused_kernel) and the k = 4 ones (dsconv_kpl4_kernel).  The tensor
 // maps are the kernels' __grid_constant__ parameters
-template <int N_TILE, int KPL, int PW, Prec PREC, bool A_SMEM>
+template <int N_TILE, int KPL, int PW, Prec PREC, bool A_SMEM, typename TA = float>
 __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CUtensorMap& map_in1, const CUtensorMap& map_w,
                                             const CUtensorMap& map_wlo, const CUtensorMap& map_y, const CUtensorMap& map_sa,
                                             const DsParams& p) {
-  using L = DsCfg<N_TILE, KPL, PW, PREC, A_SMEM>;
+  using L = DsCfg<N_TILE, KPL, PW, PREC, A_SMEM, TA>;
   constexpr bool X3 = L::X3;
+  constexpr bool BA = L::ESZ == 2;   // bf16 activations
   constexpr int PH = L::PH, BW = L::BW, BH = L::BH, CC = L::CC, IS = L::IS, AS = L::AS, BS = L::BS;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
@@ -293,13 +300,13 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
           const bool gated = p.gate_sc && cb < p.C0;
           mbar_arrive_expect_tx(full, L::IN_BYTES + (gated ? L::SA_TX : 0));
           // the gate's halo box: same origin and extent as the input box, one channel; zero fill outside the image
-          if (gated) tma_load_3d(smem + L::OFF_SA + s * L::SA_BYTES, &map_sa, full, x0 - 4, y0 - 1, b);
+          if (gated) tma_load_3d(smem + L::OFF_SA + s * L::SA_BYTES, &map_sa, full, x0 - L::XM, y0 - 1, b);
           const CUtensorMap* m = (cb < p.C0) ? &map_in0 : &map_in1;
           const int cc = (cb < p.C0) ? cb : cb - p.C0;
           asm volatile(
               "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
                   "r"(smem_u32(smem + s * L::IN_BYTES)),
-              "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(full)), "r"(x0 - 4), "r"(y0 - 1), "r"(cc), "r"(b)
+              "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(full)), "r"(x0 - L::XM), "r"(y0 - 1), "r"(cc), "r"(b)
               : "memory");
         }
       }
@@ -346,8 +353,9 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
     const int quad = g & 3, slot = quad ^ (t & 2);
     const int st_ch = 2 * t + (slot & 1);           // channel of this lane's stores within an 8-channel fragment column
     const int st_px = ((slot & 2) ? m1 : m0) - quad - 64 * wg;   // first of its 4 pixels within the half-patch
-    const uint32_t st_a0 = (uint32_t)(st_ch * 256 + st_px * 4);
-    const uint32_t st_off = st_a0 ^ (((st_a0 >> 7) & SW_MASK) << 4);   // + 2 KB per fragment column: the swizzle phase repeats
+    // bf16 boxes (rows of 64 / 32 B) are staged and stored unswizzled: [channel][64 pixels] x 2 B, 8-byte stores
+    const uint32_t st_a0 = (uint32_t)(st_ch * 64 * L::ESZ + st_px * L::ESZ);
+    const uint32_t st_off = BA ? st_a0 : st_a0 ^ (((st_a0 >> 7) & SW_MASK) << 4);   // + 8 channels per fragment column
     const uint32_t st_base = smem_u32(smem + L::OFF_ST) + (uint32_t)(wg * L::ST_BUFS * L::ST_BOX);
     const bool st_leader = (threadIdx.x & 127) == 0;
     uint32_t st_n = 0;                              // this warpgroup's staged boxes so far (buffer st_n % ST_BUFS)
@@ -499,9 +507,9 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
           if (best0 == best0 && (l0 > best0 || l0 != l0)) { best0 = l0; arg0 = cl; }
           if (best1 == best1 && (l1 > best1 || l1 != l1)) { best1 = l1; arg1 = cl; }
           if (p.oc_y && t == (cl & 3)) {
-            float* yk = p.oc_y + ((int64_t)b * p.ncls + cl) * P;
-            if (v0) yk[o0] = l0;
-            if (v1) yk[o1] = l1;
+            TA* yk = reinterpret_cast<TA*>(p.oc_y) + ((int64_t)b * p.ncls + cl) * P;
+            if (v0) st_act(yk + o0, l0);
+            if (v1) st_act(yk + o1, l1);
           }
         }
         if (p.cls) {
@@ -528,8 +536,9 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
         d1 += __shfl_xor_sync(0xffffffffu, d1, 2);
         const float ob = p.oc_b ? __ldg(p.oc_b) : 0.f;
         if (t == 0) {
-          if (v0) p.oc_y[(int64_t)b * P + o0] = d0 + ob;
-          if (v1) p.oc_y[(int64_t)b * P + o1] = d1 + ob;
+          TA* oy = reinterpret_cast<TA*>(p.oc_y) + (int64_t)b * P;
+          if (v0) st_act(oy + o0, d0 + ob);
+          if (v1) st_act(oy + o1, d1 + ob);
         }
       } else if (L::ST_BUFS) {
         // One 32-channel slice at a time: wait until the buffer's previous store has been read out, stage the slice (the same
@@ -553,9 +562,15 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
             const float sc = aff[c], sh = aff[L::AFF_N + c];
             const float4 o = make_float4(fmaxf(fmaf(v[0], sc, sh), act_lo), fmaxf(fmaf(v[1], sc, sh), act_lo),
                                          fmaxf(fmaf(v[2], sc, sh), act_lo), fmaxf(fmaf(v[3], sc, sh), act_lo));
-            asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(buf + st_off + 2048u * jj), "f"(o.x), "f"(o.y),
-                         "f"(o.z), "f"(o.w)
-                         : "memory");
+            if constexpr (BA) {
+              asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(buf + st_off + 1024u * jj), "r"(f32x2_bf16x2(o.x, o.y)),
+                           "r"(f32x2_bf16x2(o.z, o.w))
+                           : "memory");
+            } else {
+              asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(buf + st_off + 2048u * jj), "f"(o.x), "f"(o.y),
+                           "f"(o.z), "f"(o.w)
+                           : "memory");
+            }
           }
           fence_proxy_async_smem();
           wg_sync(2 + wg);
@@ -563,7 +578,7 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
             tma_store_4d(&map_y, buf, tx * PW, y_half, n0 + 32 * s, b);
             bulk_commit();
           }
-          if (p.pool_sum) {
+          if (!BA && p.pool_sum) {
             // The CBAM channel gate's pools and the next level's MaxPool2d(2), read back from the staged slice (the stored values
             // bit for bit; the store reads the buffer too, and nothing writes it before the next wg_sync).  4 threads per
             // channel, 2 items each: an item is 4 columns of a row pair, i.e. two 2 x 2 windows (the half-patch origin is even
@@ -613,7 +628,7 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
           ++st_n;
         }
       } else {
-        float* yb = p.y + (int64_t)b * p.y_bstride;
+        TA* yb = reinterpret_cast<TA*>(p.y) + (int64_t)b * p.y_bstride;
 #pragma unroll
         for (int j = 0; j < N_TILE / 8; ++j) {
 #pragma unroll
@@ -621,9 +636,9 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
             const int c = n0 + 8 * j + 2 * t + e;
             if (c < p.Cout) {
               const float sc = aff[c], sh = aff[L::AFF_N + c];
-              float* yc = yb + (int64_t)c * P;
-              if (v0) yc[o0] = fmaxf(fmaf(acc[4 * j + e], sc, sh), act_lo);
-              if (v1) yc[o1] = fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo);
+              TA* yc = yb + (int64_t)c * P;
+              if (v0) st_act(yc + o0, fmaxf(fmaf(acc[4 * j + e], sc, sh), act_lo));
+              if (v1) st_act(yc + o1, fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo));
             }
           }
         }
@@ -681,7 +696,7 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
         const int sa = gc % AS;
         mbar_wait(&a_empty[sa], ((gc / AS) & 1u) ^ 1u);  // the MMAs that read this A stage AS chunks ago retired
         unsigned char* my_op = a_base + sa * L::AST_BYTES;
-        const float* in_stage = reinterpret_cast<const float*>(smem + s * L::IN_BYTES);
+        const TA* in_stage = reinterpret_cast<const TA*>(smem + s * L::IN_BYTES);
         const float* sa_stage = reinterpret_cast<const float*>(smem + L::OFF_SA + s * L::SA_BYTES);
         // the gated and the plain stencil are compiled apart, so that chunks without the gate run the plain loop unchanged
         auto stencil = [&](auto gate_c) {
@@ -705,9 +720,9 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
             constexpr int NQ = PW / 4;
             const int c0 = qc << 2, r0 = rg << 2;
             if (task != t) load_weights(task);   // KPL = 1: a second task per chunk (every other KPL: one task per thread)
-            // smem column of patch column c (dx = -1..1) is c + 4 + dx: the 4 outputs read cols c0+3 .. c0+8
-            const float* trow = in_stage + (ci * BH + r0) * BW + c0 + 3;
-            const float* srow = sa_stage + r0 * BW + c0 + 3;
+            // smem column of patch column c (dx = -1..1) is c + XM + dx: the 4 outputs read cols c0+XM-1 .. c0+XM+4
+            const TA* trow = in_stage + (ci * BH + r0) * BW + c0 + L::XM - 1;
+            const float* srow = sa_stage + r0 * BW + c0 + L::XM - 1;
             float win[3][6];
             // one LDS.128 per row; the two edge values come from the neighbouring quads' registers (lane -1 / +1 hold columns
             // c0-4..c0-1 / c0+4..c0+7 of the same channel row), only the first / last quad of a patch row reads the halo
@@ -715,7 +730,10 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
             const bool lb = (qc == 0), rb = (qc == NQ - 1);
             const int edge = lb ? 0 : 5;
             auto load_row = [&](float* wl, int r) {
-              float4 a = *reinterpret_cast<const float4*>(trow + r * BW + 1);
+              // bf16 stages: one LDS.64 per row (rows of 96 / 64 B, c0 + 8 a multiple of 4), widened to fp32 before the stencil
+              float4 a;
+              if constexpr (BA) a = bf16x4_f32(*reinterpret_cast<const uint2*>(trow + r * BW + 1));
+              else a = *reinterpret_cast<const float4*>(trow + r * BW + 1);
               if (G) {
                 const float4 ga = *reinterpret_cast<const float4*>(srow + r * BW + 1);
                 a.x = __fmul_rn(__fmul_rn(a.x, gsc), ga.x);
@@ -725,7 +743,9 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
               }
               float left = __shfl_up_sync(0xffffffffu, a.w, 1), right = __shfl_down_sync(0xffffffffu, a.x, 1);
               if (lb | rb) {
-                float e = trow[r * BW + edge];
+                float e;
+                if constexpr (BA) e = bf16_f32(trow[r * BW + edge]);
+                else e = trow[r * BW + edge];
                 if (G) e = __fmul_rn(__fmul_rn(e, gsc), srow[r * BW + edge]);
                 if (lb) left = e; else right = e;
               }
@@ -810,19 +830,31 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, Prec::BF16, false>::THR
   dsconv_body<N_TILE, KPL, PW, Prec::BF16, false>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
 }
 
-template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM>
+// The serving forward's bf16 route (smaat_dsconv_bf16_fwd and its head forms): bf16 input and output in HBM, bf16 operands.
+// k = 1, 2
+template <int N_TILE, int KPL, int PW>
+__global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, Prec::BF16, false, uint16_t>::THREADS, 1)
+    dsconv_bf16act_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
+                          const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
+                          const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_sa,
+                          const DsParams p) {
+  dsconv_body<N_TILE, KPL, PW, Prec::BF16, false, uint16_t>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
+}
+
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float>
 static auto ds_kernel() {
   static_assert(KPL == 1 || KPL == 2 || (KPL == 4 && !A_SMEM), "fused DS conv instances: k = 1, 2 (both A forms), 4 (register form)");
-  if constexpr (P == Prec::BF16) return dsconv_bf16_kernel<N_TILE, KPL, PW>;
+  if constexpr (sizeof(TA) == 2) return dsconv_bf16act_kernel<N_TILE, KPL, PW>;
+  else if constexpr (P == Prec::BF16) return dsconv_bf16_kernel<N_TILE, KPL, PW>;
   else if constexpr (KPL == 4) return dsconv_kpl4_kernel<N_TILE, PW, P == Prec::TF32X3>;
   else return dsconv_fused_kernel<N_TILE, KPL, PW, P == Prec::TF32X3, A_SMEM>;
 }
 
-template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM>
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float>
 static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl,
                      const CUtensorMap& my, const CUtensorMap& msa, DsParams p, int B, cudaStream_t st) {
-  using L = DsCfg<N_TILE, KPL, PW, P, A_SMEM>;
-  auto kern = ds_kernel<N_TILE, KPL, PW, P, A_SMEM>();
+  using L = DsCfg<N_TILE, KPL, PW, P, A_SMEM, TA>;
+  auto kern = ds_kernel<N_TILE, KPL, PW, P, A_SMEM, TA>();
   // the pools are read back from the staging buffers: instances with the direct-store epilogue do not take them
   if (p.pool_sum && !L::ST_BUFS) return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools need the staged epilogue");
   if (p.ncls > L::MAX_CLASSES)
@@ -872,25 +904,34 @@ static int ds_impl();
 
 static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* pw_w,
                         const float* pw_w_lo, const float* y, int64_t y_bstride, int H, int W, int k, int Cout, bool stats,
-                        bool outconv, bool bf16 = false) {
+                        bool outconv, bool bf16 = false, bool bact = false) {
   // k = 4 and BF16 have register-form instances only (dsconv_kpl4_kernel, dsconv_bf16_kernel): with the shared-memory A form
   // selected they stay unfused
   if (k != 1 && k != 2 && !(k == 4 && ds_impl() != 1)) return false;
   if (bf16 && ds_impl() == 1) return false;
+  // bf16 activations (dsconv_bf16act_kernel): bf16 operands, k = 1, 2, no batch statistics; TMA takes 16-byte row and plane
+  // strides, so W and the batch strides are multiples of 8 elements
+  if (bact && (!bf16 || k == 4 || stats || W % 8 != 0 || bs0 % 8 != 0 || (C1 > 0 && bs1 % 8 != 0) || (y && y_bstride % 8 != 0)))
+    return false;
   if (y && (!aligned16(y) || y_bstride % 4 != 0)) return false;
   // Cout > 128: whole passes of 128 channels; batch statistics and the fused OutConv need all channels in one pass
   if (Cout < 8 || Cout > 512 || (Cout > 128 && (Cout % 128 != 0 || stats || outconv))) return false;
   if (W % 4 != 0 || !aligned16(x0) || bs0 % 4 != 0) return false;
   if (C1 > 0 && (!aligned16(x1) || bs1 % 4 != 0 || C0 % (TC_BK / k) != 0)) return false;
   const int K = k * (C0 + C1);
-  if (K % 4 != 0 || !aligned16(pw_w) || (pw_w_lo && !aligned16(pw_w_lo))) return false;
+  // fp32 weight rows are K * 4 bytes, which TMA takes in multiples of 16; the bf16 pack's rows are padded to 32 k (bact only, so
+  // that the fp32 route keeps its choices)
+  if ((K % 4 != 0 && !bact) || !aligned16(pw_w) || (pw_w_lo && !aligned16(pw_w_lo))) return false;
   return pick_pw(H, W) != 0;
 }
 
 // The configuration of the instance dsconv_run dispatches to, for a mode (SMAAT_PW_*) and A form (k = 4 and BF16: the register
 // form, the only one they have), handed to `f` as a DsCfg type
 template <int N_TILE, int KPL, int PW, typename F>
-static auto ds_cfg_t(int mode, bool a_smem, F f) {
+static auto ds_cfg_t(int mode, bool a_smem, F f, bool bact) {
+  if constexpr (KPL != 4) {
+    if (bact) return f(DsCfg<N_TILE, KPL, PW, Prec::BF16, false, uint16_t>{});
+  }
   if (mode == SMAAT_PW_BF16) return f(DsCfg<N_TILE, KPL, PW, Prec::BF16, false>{});
   if constexpr (KPL == 4) {
     return mode == SMAAT_PW_TF32X3 ? f(DsCfg<N_TILE, 4, PW, Prec::TF32X3, false>{}) : f(DsCfg<N_TILE, 4, PW, Prec::TF32, false>{});
@@ -900,23 +941,23 @@ static auto ds_cfg_t(int mode, bool a_smem, F f) {
   }
 }
 template <typename F>
-static int ds_cfg(int n_tile, int k, int pw, int mode, bool a_smem, F f) {
+static int ds_cfg(int n_tile, int k, int pw, int mode, bool a_smem, F f, bool bact = false) {
   if (n_tile == 64) {
-    if (k == 4) return pw == 32 ? ds_cfg_t<64, 4, 32>(mode, a_smem, f) : ds_cfg_t<64, 4, 16>(mode, a_smem, f);
-    if (k == 2) return pw == 32 ? ds_cfg_t<64, 2, 32>(mode, a_smem, f) : ds_cfg_t<64, 2, 16>(mode, a_smem, f);
-    return pw == 32 ? ds_cfg_t<64, 1, 32>(mode, a_smem, f) : ds_cfg_t<64, 1, 16>(mode, a_smem, f);
+    if (k == 4) return pw == 32 ? ds_cfg_t<64, 4, 32>(mode, a_smem, f, bact) : ds_cfg_t<64, 4, 16>(mode, a_smem, f, bact);
+    if (k == 2) return pw == 32 ? ds_cfg_t<64, 2, 32>(mode, a_smem, f, bact) : ds_cfg_t<64, 2, 16>(mode, a_smem, f, bact);
+    return pw == 32 ? ds_cfg_t<64, 1, 32>(mode, a_smem, f, bact) : ds_cfg_t<64, 1, 16>(mode, a_smem, f, bact);
   }
-  if (k == 4) return pw == 32 ? ds_cfg_t<128, 4, 32>(mode, a_smem, f) : ds_cfg_t<128, 4, 16>(mode, a_smem, f);
-  if (k == 2) return pw == 32 ? ds_cfg_t<128, 2, 32>(mode, a_smem, f) : ds_cfg_t<128, 2, 16>(mode, a_smem, f);
-  return pw == 32 ? ds_cfg_t<128, 1, 32>(mode, a_smem, f) : ds_cfg_t<128, 1, 16>(mode, a_smem, f);
+  if (k == 4) return pw == 32 ? ds_cfg_t<128, 4, 32>(mode, a_smem, f, bact) : ds_cfg_t<128, 4, 16>(mode, a_smem, f, bact);
+  if (k == 2) return pw == 32 ? ds_cfg_t<128, 2, 32>(mode, a_smem, f, bact) : ds_cfg_t<128, 2, 16>(mode, a_smem, f, bact);
+  return pw == 32 ? ds_cfg_t<128, 1, 32>(mode, a_smem, f, bact) : ds_cfg_t<128, 1, 16>(mode, a_smem, f, bact);
 }
 // Whether that instance has the staged epilogue (ST_BUFS > 0), which the CBAM pools are read from
 static bool ds_staged(int n_tile, int k, int pw, int mode, bool a_smem) {
   return ds_cfg(n_tile, k, pw, mode, a_smem, [](auto c) { return (int)decltype(c)::ST_BUFS; }) > 0;
 }
 // The most classes whose OutConv weights that instance keeps in shared memory (DsCfg::MAX_CLASSES)
-static int ds_max_classes(int n_tile, int k, int pw, int mode, bool a_smem) {
-  return ds_cfg(n_tile, k, pw, mode, a_smem, [](auto c) { return (int)decltype(c)::MAX_CLASSES; });
+static int ds_max_classes(int n_tile, int k, int pw, int mode, bool a_smem, bool bact = false) {
+  return ds_cfg(n_tile, k, pw, mode, a_smem, [](auto c) { return (int)decltype(c)::MAX_CLASSES; }, bact);
 }
 
 // Where the A operand (the depthwise result) goes to the tensor core: 0 = auto (the register form), 1 = read by wgmma from
@@ -977,7 +1018,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
                       const float* dw_b, const float* pw_w, const float* pw_w_lo, const float* scale, const float* shift, float* y,
                       int64_t y_bstride, double* stats, const float* oc_w, const float* oc_b, float* oc_y, int ncls, int64_t* cls,
                       const float* gate_sc, const float* gate_sa, float* pool_sum, float* pool_max, float* pooled, int B, int H, int W,
-                      int k, int Cout, int relu, int mode, void* stream) {
+                      int k, int Cout, int relu, int mode, void* stream, bool bact = false) {
   // head: an OutConv in the epilogue (one class, or ncls classes with the argmax) replaces the activation output
   const bool head = oc_y || ncls > 0;
   SMAAT_REQUIRE(x0 && dw_w && pw_w && (y || oc_y || cls), "dsconv: null pointer");
@@ -993,12 +1034,19 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   SMAAT_REQUIRE(head || y_bstride >= (int64_t)Cout * H * W, "dsconv: y batch stride too small");
   SMAAT_REQUIRE(!head || (oc_w && !stats),"dsconv+outconv: needs the OutConv weight and no batch statistics");
   const bool bf16 = mode == SMAAT_PW_BF16;
+  SMAAT_REQUIRE(!bact || (bf16 && !stats && !pool_sum), "dsconv: bf16 activations take bf16 operands, no statistics and no pools");
   if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, pw_w_lo, head ? nullptr : y, y_bstride, H, W, k, Cout,
-                   stats != nullptr, head, bf16))
+                   stats != nullptr, head, bf16, bact)) {
+    if (bact)
+      return fail(SMAAT_E_UNSUPPORTED,
+                  "dsconv_bf16: not taken by the bf16-activation kernel (k=%d Cout=%d H=%d W=%d; needs k = 1 or 2, W and the batch "
+                  "strides multiples of 8, 16-byte aligned tensors, the register A form)",
+                  k, Cout, H, W);
     return fail(SMAAT_E_UNSUPPORTED,
                 "dsconv: shape or output layout not taken by the fused kernel (k=%d Cout=%d H=%d W=%d, y 16-byte aligned with a "
                 "batch stride that is a multiple of 4); use dw3x3 + pw1x1",
                 k, Cout, H, W);
+  }
   cudaStream_t st = (cudaStream_t)stream;
   const int pw = pick_pw(H, W);
   const int ph = TC_BM / pw;
@@ -1007,20 +1055,24 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   const bool x3 = mode == SMAAT_PW_TF32X3;
   const bool a_smem = ds_impl() == 1;
   const int K = k * (C0 + C1);
+  // activation maps: fp32, or bf16 (bact)
+  const CUtensorMapDataType adt = bact ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  const uint64_t esz = bact ? 2 : 4;
 
   CUtensorMap m0, m1, mw, mwl;
-  const uint32_t box[4] = {(uint32_t)(pw + 8), (uint32_t)(ph + 2), (uint32_t)cc, 1u};
+  const int xm = 16 / (int)esz;   // DsCfg::XM
+  const uint32_t box[4] = {(uint32_t)(pw + 2 * xm), (uint32_t)(ph + 2), (uint32_t)cc, 1u};
   {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)C0, (uint64_t)B};
-    const uint64_t str[4] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4, (uint64_t)x0_bstride * 4};
-    int r = make_tmap_f32(&m0, x0, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(x0)");
+    const uint64_t str[4] = {0, (uint64_t)W * esz, (uint64_t)H * W * esz, (uint64_t)x0_bstride * esz};
+    int r = make_tmap(&m0, adt, x0, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(x0)");
     if (r) return r;
     m1 = m0;
   }
   if (C1 > 0) {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)C1, (uint64_t)B};
-    const uint64_t str[4] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4, (uint64_t)x1_bstride * 4};
-    int r = make_tmap_f32(&m1, x1, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(x1)");
+    const uint64_t str[4] = {0, (uint64_t)W * esz, (uint64_t)H * W * esz, (uint64_t)x1_bstride * esz};
+    int r = make_tmap(&m1, adt, x1, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(x1)");
     if (r) return r;
   }
   {
@@ -1041,9 +1093,11 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   CUtensorMap my = m0;
   if (!head) {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)Cout, (uint64_t)B};
-    const uint64_t str[4] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4, (uint64_t)y_bstride * 4};
+    const uint64_t str[4] = {0, (uint64_t)W * esz, (uint64_t)H * W * esz, (uint64_t)y_bstride * esz};
     const uint32_t ybox[4] = {(uint32_t)pw, (uint32_t)(ph / 2), 32u, 1u};
-    int r = make_tmap_f32(&my, y, 4, dims, str, ybox, pw == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, "dsconv(y)");
+    // bf16 boxes are staged unswizzled (the epilogue's bf16 branch)
+    const CUtensorMapSwizzle ysw = bact ? CU_TENSOR_MAP_SWIZZLE_NONE : pw == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    int r = make_tmap(&my, adt, y, 4, dims, str, ybox, ysw, "dsconv(y)");
     if (r) return r;
   }
   // the CBAM spatial gate sa (B, 1, H, W): one-channel halo boxes at the input boxes' origin
@@ -1051,7 +1105,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   if (gate_sa) {
     const uint64_t dims[3] = {(uint64_t)W, (uint64_t)H, (uint64_t)B};
     const uint64_t str[3] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4};
-    const uint32_t sbox[3] = {(uint32_t)(pw + 8), (uint32_t)(ph + 2), 1u};
+    const uint32_t sbox[3] = {(uint32_t)(pw + 2 * xm), (uint32_t)(ph + 2), 1u};
     int r = make_tmap_f32(&msa, gate_sa, 3, dims, str, sbox, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(gate sa)");
     if (r) return r;
   }
@@ -1063,6 +1117,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   p.tiles_x = p.tiles_y = p.npass = p.total_tiles = p.nchunks = 0;
 
 #define DS_DISPATCH(NT, KP, PWv)                                                                           \
+  if (bact) return launch_ds<NT, KP, PWv, Prec::BF16, false, uint16_t>(m0, m1, mw, mwl, my, msa, p, B, st);         \
   if (bf16) return launch_ds<NT, KP, PWv, Prec::BF16, false>(m0, m1, mw, mwl, my, msa, p, B, st);                    \
   return x3 ? (a_smem ? launch_ds<NT, KP, PWv, Prec::TF32X3, true>(m0, m1, mw, mwl, my, msa, p, B, st)               \
                       : launch_ds<NT, KP, PWv, Prec::TF32X3, false>(m0, m1, mw, mwl, my, msa, p, B, st))             \
@@ -1150,4 +1205,62 @@ extern "C" int smaat_dsconv_cbam_fwd(const float* x0, int C0, int64_t x0_bstride
   SMAAT_REQUIRE(y, "dsconv_cbam: null output");
   return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, nullptr, nullptr,
                     nullptr, nullptr, 0, nullptr, gate_sc, gate_sa, pool_sum, pool_max, pooled, B, H, W, k, Cout, relu, mode, stream);
+}
+
+/* ---- bf16 activations: the serving forward's bf16 route -------------------------------------------------------------------
+ * x0 / x1 and the output (y or the logits) are bf16 (raw uint16_t bits) in HBM; the depthwise stencil, the accumulation and
+ * the epilogue run in fp32, the GEMM takes bf16 operands (pw_w: the smaat_pack_bf16 pack), and each stored value is rounded
+ * to bf16 once.  k = 1 or 2, the register A form, no batch statistics and no CBAM pools.  The CBAM gate (gate_sc, gate_sa:
+ * fp32, both or neither) is applied as in smaat_dsconv_cbam_fwd, (x0 * sc) * sa in fp32 from the widened x0. */
+extern "C" int smaat_dsconv_bf16_eligible(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                                          const void* pw_w, int H, int W, int k, int Cout, int ncls) {
+  if (ncls < 0 || ncls > DS_MAX_CLASSES) return 0;
+  if (!ds_eligible(static_cast<const float*>(x0), C0, x0_bstride, static_cast<const float*>(x1), C1, x1_bstride,
+                   static_cast<const float*>(pw_w), nullptr, nullptr, 0, H, W, k, Cout, false, ncls > 0, true, true))
+    return 0;
+  return ncls <= ds_max_classes(Cout > 64 ? 128 : 64, k, pick_pw(H, W), SMAAT_PW_BF16, false, true) ? 1 : 0;
+}
+
+extern "C" int smaat_dsconv_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                                     const float* dw_w, const float* dw_b, const uint16_t* pw_w, const float* scale,
+                                     const float* shift, void* y, int64_t y_bstride, const float* gate_sc, const float* gate_sa,
+                                     int B, int H, int W, int k, int Cout, int relu, void* stream) {
+  SMAAT_REQUIRE(y, "dsconv_bf16: null output");
+  return dsconv_run(static_cast<const float*>(x0), C0, x0_bstride, static_cast<const float*>(x1), C1, x1_bstride, dw_w, dw_b,
+                    reinterpret_cast<const float*>(pw_w), nullptr, scale, shift, static_cast<float*>(y), y_bstride, nullptr, nullptr,
+                    nullptr, nullptr, 0, nullptr, gate_sc, gate_sa, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, SMAAT_PW_BF16,
+                    stream, true);
+}
+
+/* smaat_dsconv_outconv_fwd from bf16 activations: the (B, 1, H, W) logits, accumulated in fp32 and stored as bf16. */
+extern "C" int smaat_dsconv_outconv_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                                             const float* dw_w, const float* dw_b, const uint16_t* pw_w, const float* scale,
+                                             const float* shift, const float* oc_w, const float* oc_b, void* logits, int B, int H,
+                                             int W, int k, int Cout, int relu, void* stream) {
+  SMAAT_REQUIRE(oc_w && logits, "dsconv+outconv bf16: null pointer");
+  SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(logits) & 1u) == 0, "dsconv+outconv bf16: logits must be 2-byte aligned");
+  return dsconv_run(static_cast<const float*>(x0), C0, x0_bstride, static_cast<const float*>(x1), C1, x1_bstride, dw_w, dw_b,
+                    reinterpret_cast<const float*>(pw_w), nullptr, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
+                    static_cast<float*>(logits), 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu,
+                    SMAAT_PW_BF16, stream, true);
+}
+
+/* smaat_dsconv_classify_fwd from bf16 activations: the argmax runs on the fp32 logits in registers; the logits, when asked
+ * for, are stored as bf16. */
+extern "C" int smaat_dsconv_classify_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                                              const float* dw_w, const float* dw_b, const uint16_t* pw_w, const float* scale,
+                                              const float* shift, const float* oc_w, const float* oc_b, int K, void* logits,
+                                              int64_t* classes, int B, int H, int W, int k, int Cout, int relu, void* stream) {
+  SMAAT_REQUIRE(oc_w && (logits || classes), "dsconv+classify bf16: needs the OutConv weight and a logits or a classes output");
+  SMAAT_REQUIRE(K >= 1, "dsconv+classify bf16: K=%d classes", K);
+  if (K > DS_MAX_CLASSES)
+    return fail(SMAAT_E_UNSUPPORTED, "dsconv+classify bf16: K=%d classes, the fused epilogue takes at most %d; use smaat_dsconv_bf16_fwd + "
+                                     "smaat_outconv_bf16_fwd + smaat_argmax_channels_bf16_fwd", K, DS_MAX_CLASSES);
+  SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(oc_w) & 3u) == 0 && (reinterpret_cast<uintptr_t>(logits) & 1u) == 0 &&
+                    (reinterpret_cast<uintptr_t>(classes) & 7u) == 0,
+                "dsconv+classify bf16: weights must be 4-byte, logits 2-byte and classes 8-byte aligned");
+  return dsconv_run(static_cast<const float*>(x0), C0, x0_bstride, static_cast<const float*>(x1), C1, x1_bstride, dw_w, dw_b,
+                    reinterpret_cast<const float*>(pw_w), nullptr, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
+                    static_cast<float*>(logits), K, classes, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu,
+                    SMAAT_PW_BF16, stream, true);
 }

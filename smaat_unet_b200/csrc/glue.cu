@@ -77,9 +77,11 @@ __global__ void __launch_bounds__(256) maxpool2_kernel(const float* __restrict__
 // ---- OutConv: 1x1, Cin -> ncls (small) -------------------------------------------------------------
 // HBM-bound on the Cin-channel read (SURVEY 8a row a12: 680 MB -> 10.6 MB).  One thread owns 4
 // consecutive pixels and NC classes; loops over Cin with coalesced float4 loads; weights in smem.
-template <int NC, bool VEC>
-__global__ void __launch_bounds__(256) outconv_kernel(const float* __restrict__ x, const float* __restrict__ w,
-                                                      const float* __restrict__ bias, float* __restrict__ y, int Cin, int ncls,
+// TA: the storage type of x and y (float, or uint16_t bf16 in the serving forward's bf16 route: fp32 accumulation, each logit
+// rounded once)
+template <int NC, bool VEC, typename TA = float>
+__global__ void __launch_bounds__(256) outconv_kernel(const TA* __restrict__ x, const float* __restrict__ w,
+                                                      const float* __restrict__ bias, TA* __restrict__ y, int Cin, int ncls,
                                                       int P) {
   extern __shared__ float wsm[];  // [NC][Cin]
   const int cls0 = blockIdx.y * NC;
@@ -98,18 +100,18 @@ __global__ void __launch_bounds__(256) outconv_kernel(const float* __restrict__ 
 #pragma unroll
     for (int q = 0; q < 4; ++q) acc[j][q] = bj;
   }
-  const float* xb = x + (int64_t)b * Cin * P + pp;
+  const TA* xb = x + (int64_t)b * Cin * P + pp;
 #pragma unroll 4
   for (int c = 0; c < Cin; ++c) {
     float4 v;
     if (VEC) {
-      v = __ldg(reinterpret_cast<const float4*>(xb + (int64_t)c * P));
+      v = ld_act4(xb + (int64_t)c * P);
     } else {
-      const float* s = xb + (int64_t)c * P;
-      v.x = __ldg(s);
-      v.y = (pp + 1 < P) ? __ldg(s + 1) : 0.f;
-      v.z = (pp + 2 < P) ? __ldg(s + 2) : 0.f;
-      v.w = (pp + 3 < P) ? __ldg(s + 3) : 0.f;
+      const TA* s = xb + (int64_t)c * P;
+      v.x = ld_act(s);
+      v.y = (pp + 1 < P) ? ld_act(s + 1) : 0.f;
+      v.z = (pp + 2 < P) ? ld_act(s + 2) : 0.f;
+      v.w = (pp + 3 < P) ? ld_act(s + 3) : 0.f;
     }
 #pragma unroll
     for (int j = 0; j < NC; ++j) {
@@ -123,13 +125,13 @@ __global__ void __launch_bounds__(256) outconv_kernel(const float* __restrict__ 
 #pragma unroll
   for (int j = 0; j < NC; ++j) {
     if (cls0 + j >= ncls) break;
-    float* dst = y + ((int64_t)b * ncls + cls0 + j) * P + pp;
+    TA* dst = y + ((int64_t)b * ncls + cls0 + j) * P + pp;
     if (VEC) {
-      *reinterpret_cast<float4*>(dst) = make_float4(acc[j][0], acc[j][1], acc[j][2], acc[j][3]);
+      st_act4(dst, make_float4(acc[j][0], acc[j][1], acc[j][2], acc[j][3]));
     } else {
 #pragma unroll
       for (int q = 0; q < 4; ++q)
-        if (pp + q < P) dst[q] = acc[j][q];
+        if (pp + q < P) st_act(dst + q, acc[j][q]);
     }
   }
 }
@@ -202,5 +204,36 @@ extern "C" int smaat_outconv_fwd(const float* x, const float* w, const float* bi
     else outconv_kernel<NC, false><<<grid, threads, smem, st>>>(x, w, bias, y, Cin, ncls, P);
   }
   SMAAT_LAUNCH_CHECK("smaat_outconv_fwd");
+  return SMAAT_OK;
+}
+
+/* smaat_outconv_fwd from bf16 activations to bf16 logits (the serving forward's bf16 route): the same fp32 accumulation, each
+ * logit rounded to bf16 once. */
+extern "C" int smaat_outconv_bf16_fwd(const void* x, const float* w, const float* bias, void* y, int B, int Cin, int ncls, int P,
+                                      void* stream) {
+  SMAAT_REQUIRE(x && w && y && B > 0 && Cin > 0 && ncls > 0 && P > 0, "outconv_bf16: bad arguments");
+  SMAAT_REQUIRE(B <= 65535, "outconv_bf16: batch too large for grid.z");
+  SMAAT_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 1u) == 0, "outconv_bf16: x and y must be 2-byte aligned");
+  const uint16_t* xb = static_cast<const uint16_t*>(x);
+  uint16_t* yb = static_cast<uint16_t*>(y);
+  const bool vec = (P % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 7u) == 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int threads = 128;
+  const unsigned gx = (unsigned)ceil_div(ceil_div(P, 4), threads);
+  if (ncls <= 2) {
+    constexpr int NC = 2;
+    dim3 grid(gx, ceil_div(ncls, NC), B);
+    const size_t smem = (size_t)NC * Cin * sizeof(float);
+    if (vec) outconv_kernel<NC, true, uint16_t><<<grid, threads, smem, st>>>(xb, w, bias, yb, Cin, ncls, P);
+    else outconv_kernel<NC, false, uint16_t><<<grid, threads, smem, st>>>(xb, w, bias, yb, Cin, ncls, P);
+  } else {
+    constexpr int NC = 8;
+    dim3 grid(gx, ceil_div(ncls, NC), B);
+    const size_t smem = (size_t)NC * Cin * sizeof(float);
+    SMAAT_REQUIRE(smem <= 48 * 1024, "outconv_bf16: Cin=%d too large", Cin);
+    if (vec) outconv_kernel<NC, true, uint16_t><<<grid, threads, smem, st>>>(xb, w, bias, yb, Cin, ncls, P);
+    else outconv_kernel<NC, false, uint16_t><<<grid, threads, smem, st>>>(xb, w, bias, yb, Cin, ncls, P);
+  }
+  SMAAT_LAUNCH_CHECK("smaat_outconv_bf16_fwd");
   return SMAAT_OK;
 }

@@ -99,8 +99,11 @@ __global__ void __launch_bounds__(UP_THREADS) upsample2x_pad_kernel(const float*
 // h[j] = w_x0[j] * v[x0[j]] + w_x1[j] * v[x0[j] + 1] is kept in registers for source rows y0 and y0 + 1 and recomputed only when
 // the walk crosses into the next source row (every ~2 output rows): ~2.5 scalar loads (L1 / L2 hits: the source is 4x smaller
 // than the output and every value is read by ~4 neighbouring threads), 16 flops and one 128-bit store per 4 outputs.
+// TI / TO: the storage types of x and y (float, or uint16_t bf16 in the serving forward's bf16 route: the blend runs in fp32 and
+// each output is rounded to bf16 once)
 constexpr int UPS_ROWS = 8;
-__global__ void __launch_bounds__(256) upsample2x_pad_stream_kernel(const float* __restrict__ x, float* __restrict__ y, int64_t y_bstride,
+template <typename TI = float, typename TO = float>
+__global__ void __launch_bounds__(256) upsample2x_pad_stream_kernel(const TI* __restrict__ x, TO* __restrict__ y, int64_t y_bstride,
                                                                     int C, int H, int W, int Ho, int Wo, int pad_t, int pad_l, float ry,
                                                                     float rx, int quads, int row_groups, int64_t planes) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -125,13 +128,13 @@ __global__ void __launch_bounds__(256) upsample2x_pad_stream_kernel(const float*
     wx0[j] = in ? 1.f - lx : 0.f;
     wx1[j] = in ? lx : 0.f;
   }
-  const float* plane = x + ((int64_t)b * C + c) * H * W;
+  const TI* plane = x + ((int64_t)b * C + c) * H * W;
   auto hrow = [&](int yy, float (&h)[4]) {
-    const float* r = plane + (int64_t)yy * W;
+    const TI* r = plane + (int64_t)yy * W;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) h[j] = wx0[j] * __ldg(r + xi[j]) + wx1[j] * __ldg(r + min(xi[j] + 1, W - 1));
+    for (int j = 0; j < 4; ++j) h[j] = wx0[j] * ld_act(r + xi[j]) + wx1[j] * ld_act(r + min(xi[j] + 1, W - 1));
   };
-  float* dst = y + (int64_t)b * y_bstride + (int64_t)c * Ho * Wo + ox;
+  TO* dst = y + (int64_t)b * y_bstride + (int64_t)c * Ho * Wo + ox;
   float h0[4], h1[4];
   int cur = -1;                                        // source row held in h0 (h1 = row min(cur + 1, H - 1))
   const int oy0 = rg * UPS_ROWS;
@@ -155,8 +158,8 @@ __global__ void __launch_bounds__(256) upsample2x_pad_stream_kernel(const float*
       hrow(min(y0 + 1, H - 1), h1);
       cur = y0;
     }
-    *reinterpret_cast<float4*>(dst + (int64_t)oy * Wo) =
-        make_float4(w0 * h0[0] + w1 * h1[0], w0 * h0[1] + w1 * h1[1], w0 * h0[2] + w1 * h1[2], w0 * h0[3] + w1 * h1[3]);
+    st_act4(dst + (int64_t)oy * Wo,
+            make_float4(w0 * h0[0] + w1 * h1[0], w0 * h0[1] + w1 * h1[1], w0 * h0[2] + w1 * h1[2], w0 * h0[3] + w1 * h1[3]));
   }
 }
 
@@ -179,7 +182,7 @@ extern "C" int smaat_upsample2x_pad_fwd(const float* x, float* y, int64_t y_bstr
     const int quads = Wo / 4, row_groups = ceil_div(Ho, UPS_ROWS);
     const int64_t threads = (int64_t)quads * row_groups * C * B;
     SMAAT_REQUIRE(ceil_div64(threads, 256) < (1ll << 31), "upsample2x: grid too large");
-    upsample2x_pad_stream_kernel<<<(unsigned)ceil_div64(threads, 256), 256, 0, (cudaStream_t)stream>>>(
+    upsample2x_pad_stream_kernel<float, float><<<(unsigned)ceil_div64(threads, 256), 256, 0, (cudaStream_t)stream>>>(
         x, y, y_bstride, C, H, W, Ho, Wo, pad_t, pad_l, ry, rx, quads, row_groups, (int64_t)B * C);
     SMAAT_LAUNCH_CHECK("smaat_upsample2x_pad_fwd");
     return SMAAT_OK;
@@ -193,5 +196,35 @@ extern "C" int smaat_upsample2x_pad_fwd(const float* x, float* y, int64_t y_bstr
     upsample2x_pad_kernel<false><<<grid, UP_THREADS, 0, (cudaStream_t)stream>>>(x, y, y_bstride, C, H, W, Ho, Wo, pad_t, pad_l, ry, rx,
                                                                                tiles_x);
   SMAAT_LAUNCH_CHECK("smaat_upsample2x_pad_fwd");
+  return SMAAT_OK;
+}
+
+/* smaat_upsample2x_pad_fwd with a bf16 output (the serving forward's bf16 route), from an fp32 (x_bf16 = 0: the 36 x 36 level
+ * into up2) or a bf16 x.  Needs Wo % 4 == 0, an 8-byte aligned y and y_bstride % 4 == 0 (every thread stores 4 outputs at once):
+ * SMAAT_E_UNSUPPORTED otherwise. */
+extern "C" int smaat_upsample2x_pad_bf16_fwd(const void* x, int x_bf16, void* y, int64_t y_bstride, int B, int C, int H, int W, int Ho,
+                                             int Wo, void* stream) {
+  SMAAT_REQUIRE(x && y && B > 0 && C > 0 && H > 0 && W > 0, "upsample2x_bf16: bad arguments");
+  SMAAT_REQUIRE(Ho >= 2 * H && Wo >= 2 * W, "upsample2x_bf16: target %dx%d smaller than 2x source %dx%d (negative pad = crop unsupported)",
+                Ho, Wo, H, W);
+  SMAAT_REQUIRE(y_bstride >= (int64_t)C * Ho * Wo, "upsample2x_bf16: y batch stride too small");
+  if (Wo % 4 != 0 || (reinterpret_cast<uintptr_t>(y) & 7u) || y_bstride % 4 != 0)
+    return fail(SMAAT_E_UNSUPPORTED, "upsample2x_bf16: needs Wo %% 4 == 0, an 8-byte aligned output and a batch stride that is a "
+                                     "multiple of 4 (Wo=%d)", Wo);
+  const int pad_t = (Ho - 2 * H) / 2, pad_l = (Wo - 2 * W) / 2;
+  const float ry = (2 * H > 1) ? (float)(H - 1) / (float)(2 * H - 1) : 0.f;
+  const float rx = (2 * W > 1) ? (float)(W - 1) / (float)(2 * W - 1) : 0.f;
+  const int quads = Wo / 4, row_groups = ceil_div(Ho, UPS_ROWS);
+  const int64_t threads = (int64_t)quads * row_groups * C * B;
+  SMAAT_REQUIRE(ceil_div64(threads, 256) < (1ll << 31), "upsample2x_bf16: grid too large");
+  const unsigned grid = (unsigned)ceil_div64(threads, 256);
+  uint16_t* yb = static_cast<uint16_t*>(y);
+  if (x_bf16)
+    upsample2x_pad_stream_kernel<uint16_t, uint16_t><<<grid, 256, 0, (cudaStream_t)stream>>>(
+        static_cast<const uint16_t*>(x), yb, y_bstride, C, H, W, Ho, Wo, pad_t, pad_l, ry, rx, quads, row_groups, (int64_t)B * C);
+  else
+    upsample2x_pad_stream_kernel<float, uint16_t><<<grid, 256, 0, (cudaStream_t)stream>>>(
+        static_cast<const float*>(x), yb, y_bstride, C, H, W, Ho, Wo, pad_t, pad_l, ry, rx, quads, row_groups, (int64_t)B * C);
+  SMAAT_LAUNCH_CHECK("smaat_upsample2x_pad_bf16_fwd");
   return SMAAT_OK;
 }

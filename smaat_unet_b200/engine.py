@@ -24,7 +24,7 @@ from .modules import apply_head
 
 class InferenceSession:
     def __init__(self, model, batch, in_shape, device=None, use_graph=True, slots=2, serving_fusions=True, output="logits",
-                 batch_sizes=None):
+                 batch_sizes=None, dtype=torch.float32):
         """``output="logits"`` (default): the model's fp32 output.  ``output="classes"``: the (batch, H, W) int64 class map
         argmax over its channels (the reference's ``torch.argmax(softmax(y_pred), dim=1)``, train_SmaAtUNet.py:76), computed
         inside the captured graph: ``model.forward_classes`` where the model has it (SmaAt_UNet: OutConv and argmax in the last
@@ -37,7 +37,13 @@ class InferenceSession:
         ``batch`` is the capacity: the largest request and the size captured in any case.  ``batch_sizes``: further sizes in
         ``1..batch``, each captured in a graph of its own over the leading rows of the one input buffer.  ``forward`` /
         ``submit`` take any 1 <= n <= batch rows and run the smallest captured size m >= n; rows n..m are padding (eval
-        samples are independent, so they change no real row) and only the n real rows are returned."""
+        samples are independent, so they change no real row) and only the n real rows are returned.
+
+        ``dtype=torch.bfloat16`` captures SmaAt_UNet's bf16 storage route (``SmaAt_UNet._serve_bf16``): the input and its
+        staging buffers are bf16, and so are the logits and probabilities (class maps stay int64); requests must be bf16.
+        Models and settings without that route raise ``ValueError`` here."""
+        if dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"InferenceSession: dtype must be torch.float32 or torch.bfloat16, got {dtype}")
         if output not in ("logits", "classes", "probs"):
             raise ValueError(f"InferenceSession: output must be one of 'probs', 'logits' or 'classes', got {output!r}")
         batch = int(batch)
@@ -53,7 +59,8 @@ class InferenceSession:
         self.compute = torch.cuda.Stream(self.device)
         self.h2d = torch.cuda.Stream(self.device)
         self.d2h = torch.cuda.Stream(self.device)
-        self.static_in = torch.zeros((batch,) + self.in_shape, device=self.device, dtype=torch.float32)
+        self.dtype = dtype
+        self.static_in = torch.zeros((batch,) + self.in_shape, device=self.device, dtype=dtype)
         self.launches_per_forward = 0
         self.graph = None            # the capacity size's graph
         self._graphs = {}            # size -> captured graph
@@ -143,6 +150,8 @@ class InferenceSession:
         return next(m for m in self.sizes if m >= n)
 
     def _rows(self, x):
+        if self.dtype == torch.bfloat16 and x.dtype != torch.bfloat16:
+            raise ValueError(f"InferenceSession(dtype=torch.bfloat16): requests must be bfloat16, got {x.dtype}")
         if x.dim() != 1 + len(self.in_shape) or tuple(x.shape[1:]) != self.in_shape:
             raise ValueError(f"InferenceSession: expected (n, {', '.join(map(str, self.in_shape))}) with 1 <= n <= {self.batch}, "
                              f"got {tuple(x.shape)}")

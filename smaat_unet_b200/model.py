@@ -8,11 +8,21 @@ reference checkout is not importable (e.g. the GPU box).  With the reference on
 """
 from __future__ import annotations
 
+import torch
 from torch import nn
 
-from .modules import CBAM, DoubleConv, DoubleConvDS, Down, DownDS, OutConv, Up, UpDS, _needs_grad, apply_head
+from .modules import (CBAM, Bf16Declined, DoubleConv, DoubleConvDS, Down, DownDS, OutConv, Up, UpDS, _needs_grad,
+                      apply_head)
 
 _ENC = (64, 128, 256, 512)
+
+BF16_ROUTE = ("bf16 input is taken by SmaAt_UNet's serving forward only: forward_serving / forward_classes / forward_probs in "
+              "eval mode under torch.no_grad(), or InferenceSession(model, ..., dtype=torch.bfloat16)")
+
+
+def _refuse_bf16(x, why):
+    if isinstance(x, torch.Tensor) and x.dtype == torch.bfloat16:
+        raise ValueError(f"{BF16_ROUTE}; {why}")
 
 
 class _ServingForward(nn.Module):
@@ -35,9 +45,14 @@ class _ServingForward(nn.Module):
         return self._serve(x, "probs")
 
     def _serve(self, x, head):
+        if isinstance(x, torch.Tensor) and x.dtype == torch.bfloat16:
+            return self._serve_bf16(x, head)
         if self.training or _needs_grad(self, x):
             return apply_head(self, x, head)
         return self._serving(x, head)
+
+    def _serve_bf16(self, x, head):
+        _refuse_bf16(x, f"{type(self).__name__} has no bf16 route")
 
 
 class SmaAt_UNet(_ServingForward):
@@ -74,6 +89,7 @@ class SmaAt_UNet(_ServingForward):
         """The reference's graph, block for block and in its call order (models/SmaAt_UNet.py:41-57): plain calls only --
         exactly what a ``patch_reference()`` user of the unchanged reference class executes.  The max-pool fusion still
         happens: ``cbamN(f)`` leaves MaxPool2d(2)(f) behind for the ``downN(f)`` that follows (modules.CBAM.forward)."""
+        _refuse_bf16(x, "model(x) runs the fp32 plain-call graph")
         f = self.inc(x)
         att = [self.cbam1(f)]
         for lvl in range(1, 5):
@@ -84,6 +100,25 @@ class SmaAt_UNet(_ServingForward):
             y = getattr(self, f"up{i + 1}")(y, att[3 - i])          # attended maps are the skips
         return self.outc(y)
 
+    def _serve_bf16(self, x, head):
+        """The bf16 storage route (opt-in by the input's dtype): the input and the level 1-3 maps are bf16 in HBM, levels 4-5
+        fp32 with the fp32 route's kernels; the level 1-3 GEMMs take bf16 operands whatever ``set_pointwise_mode`` says.  Every
+        request it does not take raises ``ValueError`` before any launch; a level 1-3 conv its kernel declines raises naming
+        the layer."""
+        if self.training or _needs_grad(self, x):
+            _refuse_bf16(x, "train mode and autograd have no bf16 route")
+        if self.inc.double_conv[0].kernels_per_layer not in (1, 2):
+            _refuse_bf16(x, f"kernels_per_layer={self.inc.double_conv[0].kernels_per_layer} has no bf16 kernel (1 or 2 only)")
+        if not self.bilinear:
+            _refuse_bf16(x, "bilinear=False (the transposed-conv upsample) has no bf16 route")
+        if x.dim() != 4 or x.shape[2] % 32 or x.shape[3] % 32:
+            _refuse_bf16(x, f"H and W must be multiples of 32 (16-byte bf16 rows at levels 1-3), got shape {tuple(x.shape)}")
+        try:
+            return self._serving(x, head)
+        except Bf16Declined as e:
+            name = next((n for n, m in self.named_modules() if m is e.module), type(e.module).__name__)
+            raise ValueError(f"SmaAt_UNet bf16 serving forward: {name}: {e}") from None
+
     def _serving(self, x, head):
         skips, f = [], self.inc(x)
         for lvl in range(5):
@@ -92,7 +127,8 @@ class SmaAt_UNet(_ServingForward):
             cbam = getattr(self, f"cbam{lvl + 1}")
             bn = cbam.spatial_att.bn
             if lvl < 3 and not bn.training and bn.track_running_stats:
-                sc, sa, pooled = cbam.serving_gates(f)
+                # the bf16 route's max-pool is bf16 into levels 2-3, fp32 into level 4
+                sc, sa, pooled = cbam.serving_gates(f, pooled_dtype=torch.float32 if lvl == 2 else f.dtype)
                 skips.append((f, (sc, sa)))
             else:
                 skips.append((cbam(f), None))       # a plain call leaves its max-pool for the DownDS that follows
@@ -140,6 +176,7 @@ class UNet(_ServingForward):
         return x, x1
 
     def forward(self, x):
+        _refuse_bf16(x, "UNet has no bf16 route")
         return self.outc(self.up4(*self._to_up4(x)))
 
     def _serving(self, x, head):
@@ -192,6 +229,7 @@ class UNetAttention(_ServingForward):
         return x, x1Att
 
     def forward(self, x):
+        _refuse_bf16(x, "UNetAttention has no bf16 route")
         return self.outc(self.up4(*self._to_up4(x)))
 
     def _serving(self, x, head):

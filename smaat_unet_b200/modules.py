@@ -60,6 +60,15 @@ def _needs_grad(mod, *inputs):
     return any(p.requires_grad for p in mod.parameters())
 
 
+class Bf16Declined(RuntimeError):
+    """A bf16 request the bf16 route's fused kernel does not take, raised by the module (``module``) that declined it: the bf16
+    route has no unfused fallback.  SmaAt_UNet names the layer (model.py)."""
+
+    def __init__(self, module, msg):
+        super().__init__(msg)
+        self.module = module
+
+
 def _no_autograd(mod, *inputs):
     if _needs_grad(mod, *inputs):
         raise NotImplementedError(
@@ -88,11 +97,11 @@ class DepthwiseSeparableConv(_CachingModule):
             raise NotImplementedError("smaat_unet_b200 implements the depthwise conv the reference uses: 3x3, padding=1 "
                                       "(parts_ds.py:18-33)")
 
-    def pw_operands(self):
-        """The pointwise weight's operands in the current mode (``ops.derived_operands``: the tf32 (hi, lo) split in 'tf32x3',
-        (bf16 pack, None) in 'bf16', None in the modes that take the weight as it is), cached on the parameter's version
-        counter and the mode."""
-        mode = ops.PW_MODES[ops.get_pointwise_mode()]
+    def pw_operands(self, mode=None):
+        """The pointwise weight's operands in the current mode (or ``mode``: the bf16 route always takes 'bf16') --
+        ``ops.derived_operands``: the tf32 (hi, lo) split in 'tf32x3', (bf16 pack, None) in 'bf16', None in the modes that take
+        the weight as it is -- cached on the parameter's version counter and the mode."""
+        mode = ops.PW_MODES[mode or ops.get_pointwise_mode()]
         w = self.pointwise.weight
         key = (_versions(w), mode)
         # while a training step is being captured into a CUDA graph the operands must be part of the graph: replays see new
@@ -120,8 +129,26 @@ class DepthwiseSeparableConv(_CachingModule):
         mode = ops.get_pointwise_mode()
         return dw_b, shift, mode, self.pw_operands()
 
+    def _bf16(self, x, x1, scale, shift, relu, gate=None):
+        """The bf16 route (bf16 x [, x1] -> bf16 y, bf16 GEMM operands whatever the pointwise mode): the fused kernel or
+        ``Bf16Declined``."""
+        self._check()
+        if not ops.dsconv_bf16_takes(x, x1, self.pointwise.weight.detach(), self.kernels_per_layer):
+            raise Bf16Declined(self, f"the bf16 DS conv does not take input {tuple(x.shape)}"
+                                     f"{'' if x1 is None else f' + {tuple(x1.shape)}'}, kernels_per_layer={self.kernels_per_layer} "
+                                     "(needs k = 1 or 2, W a multiple of 8, set_dsconv_impl other than 'smem' and "
+                                     "set_fused_dsconv(True))")
+        dw_b = self.depthwise.bias.detach() if self.depthwise.bias is not None else None
+        if shift is None:
+            shift = self.pointwise.bias.detach() if self.pointwise.bias is not None else None
+        return ops.dsconv_bf16(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(), scale,
+                               shift, relu, x1=x1, w_split=self.pw_operands("bf16"), gate=gate)
+
     def run(self, x, x1=None, scale=None, shift=None, relu=False, in_scale=None, in_shift=None, stats=None):
-        """dw -> pw with the pw epilogue y = act(scale * acc + shift).  scale/shift None => (1, pointwise.bias)."""
+        """dw -> pw with the pw epilogue y = act(scale * acc + shift).  scale/shift None => (1, pointwise.bias).  A bf16 x is the
+        bf16 route: bf16 output from the fused kernel (no input affine, no statistics)."""
+        if ops.is_bf16(x) and in_scale is None and stats is None:
+            return self._bf16(x, x1, scale, shift, relu)
         dw_b, shift, mode, split = self._operands(shift)
         if in_scale is None:
             # one kernel: the k*Cin-channel depthwise result never reaches HBM (where the shape allows)
@@ -139,6 +166,14 @@ class DepthwiseSeparableConv(_CachingModule):
         this conv and the OutConv separately."""
         if head not in ("logits", "classes"):
             raise ValueError(f"run_head: head must be 'logits' or 'classes', got {head!r}")
+        if ops.is_bf16(x):          # the bf16 route: bf16 logits / the class map from bf16 activations
+            self._check()
+            dw_b = self.depthwise.bias.detach() if self.depthwise.bias is not None else None
+            if shift is None:
+                shift = self.pointwise.bias.detach() if self.pointwise.bias is not None else None
+            return ops.dsconv_head_bf16(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer,
+                                        self.pointwise.weight.detach(), scale, shift, relu, *outconv, head,
+                                        w_split=self.pw_operands("bf16"))
         dw_b, shift, mode, split = self._operands(shift)
         args = (x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(), scale, shift, relu)
         if head == "logits":
@@ -146,12 +181,18 @@ class DepthwiseSeparableConv(_CachingModule):
         return ops.dsconv_classify(*args, *outconv, mode=mode, w_split=split)
 
     def cbam_takes(self, x, x1=None, gate=False, pools=False) -> bool:
-        """Whether ``run_cbam`` takes this input: the fused kernel with the serving forward's CBAM fusions."""
+        """Whether ``run_cbam`` takes this input: the fused kernel with the serving forward's CBAM fusions.  For a bf16 x (the bf16
+        route, gate only) always: that kernel is its only form, and ``run_cbam`` raises ``Bf16Declined`` where it declines."""
+        if ops.is_bf16(x) and not pools:
+            return True
         return ops.dsconv_cbam_takes(x, x1, self.pointwise.weight.detach(), self.kernels_per_layer, gate=gate, pools=pools)
 
     def run_cbam(self, x, x1=None, scale=None, shift=None, relu=False, gate=None, pools=False):
         """``run`` in one fused kernel that reads x as the CBAM output (x * sc) * sa (``gate=(sc, sa)``) and / or also returns
-        the channel gate's partial pools and the 2x2 max-pool of its output (``pools``): see ``ops.dsconv_cbam``."""
+        the channel gate's partial pools and the 2x2 max-pool of its output (``pools``): see ``ops.dsconv_cbam``.  A bf16 x: the
+        bf16 route, gate only."""
+        if ops.is_bf16(x) and not pools:
+            return self._bf16(x, x1, scale, shift, relu, gate=gate)
         dw_b, shift, mode, split = self._operands(shift)
         return ops.dsconv_cbam(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(),
                                scale, shift, relu, x1=x1, mode=mode, w_split=split, gate=gate, pools=pools)
@@ -272,7 +313,7 @@ class DoubleConvDS(_DoubleConvBase):
         ``gate=(sc, sa)``: x is the un-attended skip and the block's input is the CBAM output (x * sc) * sa, which the first
         DS conv computes as it loads x (inference only; materialised first where that kernel does not take it)."""
         _check_head(head, outconv)
-        ops._req(x, "input", 4)
+        ops._req(x, "input", 4, bf16=True)
         if gate is not None and not (self._eval_folded(x, x1) and self.double_conv[0].cbam_takes(x, x1, gate=True)):
             x, gate = ops.cbam_scale(x, gate[0], gate[1]), None
         if outconv is not None:
@@ -418,7 +459,8 @@ class _TransposedUp(_CachingModule):
         if torch.is_grad_enabled() and x1.requires_grad:
             from .autograd import Upsample2xPadFn
             return Upsample2xPadFn.apply(x1, Ho, Wo)
-        return ops.upsample2x_pad(x1, Ho, Wo)
+        # the bf16 route: the upsampled map joins a bf16 skip, so it is written in bf16 (from fp32 level 4 into up2)
+        return ops.upsample2x_pad(x1, Ho, Wo, out_dtype=torch.bfloat16 if ops.is_bf16(x2) else torch.float32)
 
 
 class UpDS(_TransposedUp):
@@ -593,19 +635,19 @@ class ChannelAttention(nn.Module):
             nn.Linear(input_channels // reduction_ratio, input_channels),
         )
 
-    def gate(self, x, with_maxpool=False):
+    def gate(self, x, with_maxpool=False, pooled_dtype=torch.float32):
         """sigmoid(MLP(avg) + MLP(max)) as a (B, C) tensor.  ``with_maxpool``: also return MaxPool2d(2)(x) (or None), computed
-        in the same read of x as the global pools."""
+        in the same read of x as the global pools; a bf16 x (the bf16 route) writes it in ``pooled_dtype``."""
         l1, l2 = self.MLP[1], self.MLP[3]
         # 512 channels: the MLP runs as a second launch instead of in the last-arriving pooling CTA of each image, whose
         # serial 512-channel MLP sits on the critical path of these small planes
         one = None if x.shape[1] >= 512 else ops.cbam_pool_mlp(x, l1.weight.detach(), l1.bias.detach(), l2.weight.detach(), l2.bias.detach(),
-                                                               with_maxpool=with_maxpool)
+                                                               with_maxpool=with_maxpool, pooled_dtype=pooled_dtype)
         if one is not None:          # pools + MLP + sigmoid (+ the 2x2 max-pool) in one launch
             sc, _, _, pooled = one
             return (sc, pooled) if with_maxpool else sc
         pooled = None
-        fused = ops.cbam_pool_maxpool(x) if with_maxpool else None
+        fused = ops.cbam_pool_maxpool(x, pooled_dtype=pooled_dtype) if with_maxpool else None
         if fused is not None:
             avg, mx, pooled = fused
         else:
@@ -695,11 +737,12 @@ class CBAM(nn.Module):
             y = ops.cbam_scale(x, sc, sa, out=out)
         return (y, pooled) if with_maxpool else y
 
-    def serving_gates(self, x):
+    def serving_gates(self, x, pooled_dtype=torch.float32):
         """Serving forward, inference only: CBAM(x)'s two gates (sc (B, C), sa (B, 1, H, W)) and MaxPool2d(2)(x) (or None),
         without writing CBAM(x): pools + MLP (+ max-pool), channel reduce, k x k gate -- the same launches and values as
-        ``forward``.  The consumer applies (x * sc) * sa as it loads x (``UpDS.forward(..., gate=(sc, sa))``)."""
-        sc, pooled = self.channel_att.gate(x, with_maxpool=True)
+        ``forward``.  The consumer applies (x * sc) * sa as it loads x (``UpDS.forward(..., gate=(sc, sa))``).  A bf16 x (the
+        bf16 route): the gates stay fp32, the max-pool is written in ``pooled_dtype``."""
+        sc, pooled = self.channel_att.gate(x, with_maxpool=True, pooled_dtype=pooled_dtype)
         red = ops.cbam_reduce(x, sc)
         return sc, ops.cbam_gate(red, self.spatial_att.conv.weight.detach(), self.spatial_att.bn_affine()), pooled
 

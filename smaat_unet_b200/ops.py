@@ -2,7 +2,9 @@
 
 PyTorch is plumbing here (device memory, streams); every byte of arithmetic happens in
 libsmaat_b200.so.  Tensors must be fp32 CUDA tensors, NCHW, dense in (C?, H, W) -- a
-batch stride larger than C*H*W is allowed where the C ABI takes a ``bstride``.
+batch stride larger than C*H*W is allowed where the C ABI takes a ``bstride``.  The ops of
+SmaAt-UNet's serving forward also take bf16 activations (its bf16 storage route: the
+``*_bf16`` entry points of include/smaat_b200.h); each says so.
 """
 from __future__ import annotations
 
@@ -103,9 +105,11 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
-def _req(t, name, ndim=None):
-    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32:
-        raise RuntimeError(f"smaat_unet_b200: {name} must be a float32 CUDA tensor "
+def _req(t, name, ndim=None, bf16=False):
+    """``bf16``: a bfloat16 tensor is accepted too (the bf16 route's activations)."""
+    ok = (torch.float32, torch.bfloat16) if bf16 else (torch.float32,)
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype not in ok:
+        raise RuntimeError(f"smaat_unet_b200: {name} must be a float32{' or bfloat16' if bf16 else ''} CUDA tensor "
                            f"(got {type(t).__name__} {getattr(t, 'dtype', None)} {getattr(t, 'device', None)}); "
                            "there is no CPU fallback")
     if ndim is not None and t.dim() != ndim:
@@ -113,14 +117,14 @@ def _req(t, name, ndim=None):
     return t
 
 
-def _dense(t, name):
-    _req(t, name)
+def _dense(t, name, bf16=False):
+    _req(t, name, bf16=bf16)
     return t if t.is_contiguous() else t.contiguous()
 
 
-def _nchw_bstride(t, name):
+def _nchw_bstride(t, name, bf16=False):
     """Accept NCHW tensors that are dense in (C,H,W); return (tensor, batch stride in elements)."""
-    _req(t, name, 4)
+    _req(t, name, 4, bf16=bf16)
     B, Cc, H, W = t.shape
     st = t.stride()
     if (st[3] == 1 or W == 1) and (st[2] == W or H == 1) and (st[1] == H * W or Cc == 1) and (B == 1 or st[0] >= Cc * H * W):
@@ -129,12 +133,17 @@ def _nchw_bstride(t, name):
     return t, Cc * H * W
 
 
-def _concat_operands(x, x1):
-    """The virtual concat [x, x1] as the C ABI reads it: (x, its batch stride, x1 or None, C1, x1's batch stride)."""
-    x, bs0 = _nchw_bstride(x, "x")
+def _concat_operands(x, x1, bf16=False):
+    """The virtual concat [x, x1] as the C ABI reads it: (x, its batch stride, x1 or None, C1, x1's batch stride).  ``bf16``:
+    both bfloat16 (the bf16 route)."""
+    x, bs0 = _nchw_bstride(x, "x", bf16=bf16)
+    if bf16 and x.dtype != torch.bfloat16:
+        raise RuntimeError("smaat_unet_b200: the bf16 route's x must be bfloat16")
     if x1 is None:
         return x, bs0, None, 0, 0
-    x1, bs1 = _nchw_bstride(x1, "x1")
+    x1, bs1 = _nchw_bstride(x1, "x1", bf16=bf16)
+    if x1.dtype != x.dtype:
+        raise RuntimeError(f"smaat_unet_b200: concat inputs must have one dtype, got {x.dtype} and {x1.dtype}")
     assert x1.shape[0] == x.shape[0] and x1.shape[2:] == x.shape[2:], "concat inputs must agree in B, H, W"
     return x, bs0, x1, x1.shape[1], bs1
 
@@ -399,16 +408,90 @@ def dsconv_classify(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_
     return (classes, logits) if want_logits else classes
 
 
+def is_bf16(t) -> bool:
+    return isinstance(t, torch.Tensor) and t.dtype == torch.bfloat16
+
+
+def dsconv_bf16_takes(x, x1, pw_weight, k, ncls=0) -> bool:
+    """True when the bf16-activation DS conv (smaat_dsconv_bf16_eligible) takes bf16 x [, x1]: ``ncls`` = 0 for ``dsconv_bf16``,
+    else the classes of ``dsconv_head_bf16``'s OutConv.  set_fused_dsconv(False) declines it too: it has no unfused form."""
+    if not _fuse_ds:
+        return False
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1, bf16=True)
+    w2d = _pw_matrix(pw_weight)
+    return bool(_lib.load().smaat_dsconv_bf16_eligible(_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2], x.shape[3], k,
+                                                       w2d.shape[0], int(ncls)))
+
+
+def _ds_bf16_args(x, x1, dw_weight, k, pw_weight, w_split):
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1, bf16=True)
+    B, C0, H, W = x.shape
+    Cin = C0 + C1
+    w2d = _pw_matrix(pw_weight, k, Cin)
+    pack, _ = weight_operands(w2d, PW_MODES["bf16"], w_split)
+    return x, bs0, x1, C1, bs1, B, C0, H, W, Cin, w2d.shape[0], pack, _dense(dw_weight, "depthwise.weight")
+
+
+def dsconv_bf16(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, w_split=None, gate=None):
+    """``dsconv`` / ``dsconv_cbam`` (gate only) on bf16 activations (smaat_dsconv_bf16_fwd): bf16 x [, x1] -> bf16 y, bf16 GEMM
+    operands whatever the pointwise mode (``w_split``: the cached 'bf16' operands), fp32 arithmetic, each output rounded once.
+    Raises where ``dsconv_bf16_takes`` is False: the bf16 route has no unfused DS conv."""
+    if not dsconv_bf16_takes(x, x1, pw_weight, k):
+        raise RuntimeError("smaat_unet_b200: the bf16 DS conv does not take this request (k = 1 or 2, W a multiple of 8, the "
+                           "register A form, set_fused_dsconv(True))")
+    x, bs0, x1, C1, bs1, B, C0, H, W, Cin, Cout, pack, dw_w = _ds_bf16_args(x, x1, dw_weight, k, pw_weight, w_split)
+    sc = sa = None
+    if gate is not None:
+        sc, sa = _dense(gate[0], "gate sc"), _dense(gate[1], "gate sa")
+        assert sc.numel() == B * C0 and sa.numel() == B * H * W, "CBAM gate: sc (B, C0), sa (B, 1, H, W)"
+    y = torch.empty((B, Cout, H, W), device=x.device, dtype=torch.bfloat16)
+    _call(f"smaat_dsconv_bf16_fwd[C{Cin}_N{Cout}_S{H}]", 2 * B * H * W * (Cin + Cout) + 2 * k * Cin * Cout + (4 * B * H * W if gate else 0),
+          2 * B * H * W * k * Cin * (Cout + 9), _lib.load().smaat_dsconv_bf16_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(dw_w),
+          _ptr(dw_bias), _ptr(pack), _ptr(scale), _ptr(shift), _ptr(y), Cout * H * W, _ptr(sc), _ptr(sa), B, H, W, k, Cout,
+          int(bool(relu)), _stream())
+    return y
+
+
+def dsconv_head_bf16(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, head, w_split=None):
+    """The last DS conv of the bf16 route with the OutConv in its epilogue: ``head="logits"`` (one class: the (B, 1, H, W) bf16
+    logits, smaat_dsconv_outconv_bf16_fwd) or ``"classes"`` (the (B, H, W) int64 class map, smaat_dsconv_classify_bf16_fwd).
+    None where the kernel does not take it (the caller runs the conv and the OutConv apart)."""
+    ow = _dense(oc_weight, "outconv.weight")
+    K = ow.shape[0]
+    if (head == "logits" and K != 1) or not dsconv_bf16_takes(x, None, pw_weight, k, ncls=K):
+        return None
+    x, bs0, _, _, _, B, C0, H, W, Cin, Cout, pack, dw_w = _ds_bf16_args(x, None, dw_weight, k, pw_weight, w_split)
+    assert ow.numel() == K * Cout, f"OutConv weight {tuple(oc_weight.shape)} does not match (K, Cout={Cout})"
+    ob = _dense(oc_bias, "outconv.bias") if oc_bias is not None else None
+    lib = _lib.load()
+    flops = 2 * B * H * W * (k * Cin * (Cout + 9) + K * Cout)
+    if head == "logits":
+        out = torch.empty((B, 1, H, W), device=x.device, dtype=torch.bfloat16)
+        _call(f"smaat_dsconv_outconv_bf16_fwd[C{Cin}_N{Cout}_S{H}]", 2 * B * H * W * (Cin + 1), flops, lib.smaat_dsconv_outconv_bf16_fwd,
+              _ptr(x), C0, bs0, None, 0, 0, _ptr(dw_w), _ptr(dw_bias), _ptr(pack), _ptr(scale), _ptr(shift), _ptr(ow), _ptr(ob),
+              _ptr(out), B, H, W, k, Cout, int(bool(relu)), _stream())
+        return out
+    out = torch.empty((B, H, W), device=x.device, dtype=torch.int64)
+    _call(f"smaat_dsconv_classify_bf16_fwd[C{Cin}_N{Cout}_K{K}_S{H}]", 2 * B * H * W * Cin + 8 * B * H * W, flops,
+          lib.smaat_dsconv_classify_bf16_fwd, _ptr(x), C0, bs0, None, 0, 0, _ptr(dw_w), _ptr(dw_bias), _ptr(pack), _ptr(scale),
+          _ptr(shift), _ptr(ow), _ptr(ob), K, None, _ptr(out), B, H, W, k, Cout, int(bool(relu)), _stream())
+    return out
+
+
 def softmax_channels(x):
     """The class probabilities of (B, K, ...) logits: fp32 of the same shape, torch.softmax(x, 1) within fp32 rounding, with
     torch's NaN / 0 / 1 pattern on non-finite logits (smaat_softmax_channels_fwd, 1 <= K <= 1024).  Inference only: no
     gradient."""
-    x = _dense(x, "logits")
+    x = _dense(x, "logits", bf16=True)
     if x.dim() < 2:
         raise RuntimeError(f"smaat_unet_b200: logits must be (B, K, ...), got shape {tuple(x.shape)}")
     B, K = x.shape[0], x.shape[1]
     P = x[0, 0].numel()
     probs = torch.empty_like(x)
+    if is_bf16(x):      # bf16 logits -> bf16 probabilities (the bf16 route)
+        _call(f"smaat_softmax_channels_bf16_fwd[K{K}]", 4 * B * K * P, 0, _lib.load().smaat_softmax_channels_bf16_fwd, _ptr(x),
+              _ptr(probs), B, K, P, _stream())
+        return probs
     _call(f"smaat_softmax_channels_fwd[K{K}]", 8 * B * K * P, 0, _lib.load().smaat_softmax_channels_fwd, _ptr(x), _ptr(probs),
           B, K, P, _stream())
     return probs
@@ -417,12 +500,16 @@ def softmax_channels(x):
 def argmax_channels(x):
     """The class map of (B, K, H, W) logits: int64 (B, H, W), torch.argmax(x, 1) exactly -- ties to the first index, a NaN
     wins (smaat_argmax_channels_fwd, 1 <= K <= 1024)."""
-    x = _dense(x, "logits")
+    x = _dense(x, "logits", bf16=True)
     if x.dim() < 2:
         raise RuntimeError(f"smaat_unet_b200: logits must be (B, K, ...), got shape {tuple(x.shape)}")
     B, K = x.shape[0], x.shape[1]
     P = x[0, 0].numel()
     classes = torch.empty((B,) + tuple(x.shape[2:]), device=x.device, dtype=torch.int64)
+    if is_bf16(x):
+        _call(f"smaat_argmax_channels_bf16_fwd[K{K}]", 2 * B * K * P + 8 * B * P, 0, _lib.load().smaat_argmax_channels_bf16_fwd,
+              _ptr(x), _ptr(classes), B, K, P, _stream())
+        return classes
     _call(f"smaat_argmax_channels_fwd[K{K}]", 4 * B * K * P + 8 * B * P, 0, _lib.load().smaat_argmax_channels_fwd, _ptr(x), _ptr(classes),
           B, K, P, _stream())
     return classes
@@ -563,8 +650,16 @@ def maxpool2(x):
     return y
 
 
-def upsample2x_pad(x, Ho, Wo):
-    """nn.Upsample(x2, bilinear, align_corners=True) + F.pad to (Ho, Wo) (parts_ds.py:64,78-81)."""
+def upsample2x_pad(x, Ho, Wo, out_dtype=torch.float32):
+    """nn.Upsample(x2, bilinear, align_corners=True) + F.pad to (Ho, Wo) (parts_ds.py:64,78-81).  ``out_dtype=torch.bfloat16``
+    (the bf16 route): a bf16 output from an fp32 or bf16 x."""
+    if out_dtype == torch.bfloat16:
+        x = _dense(x, "x", bf16=True)
+        B, Cc, H, W = x.shape
+        y = torch.empty((B, Cc, Ho, Wo), device=x.device, dtype=torch.bfloat16)
+        _call(f"smaat_upsample2x_pad_bf16_fwd[C{Cc}_S{H}]", B * Cc * (x.element_size() * H * W + 2 * Ho * Wo), 0,
+              _lib.load().smaat_upsample2x_pad_bf16_fwd, _ptr(x), int(is_bf16(x)), _ptr(y), Cc * Ho * Wo, B, Cc, H, W, Ho, Wo, _stream())
+        return y
     x = _dense(x, "x")
     B, Cc, H, W = x.shape
     y = torch.empty((B, Cc, Ho, Wo), device=x.device, dtype=torch.float32)
@@ -601,10 +696,30 @@ def cbam_pool(x):
     return avg, mx
 
 
-def cbam_pool_maxpool(x):
-    """(avg, mx, maxpool2(x)) from one read of x, or None when the shape is not taken (odd H, W % 4 != 0)."""
-    x = _dense(x, "x")
+def _pool_bf16(x, pooled_dtype):
+    """bf16 x: (its batch of planes, the (B, C, H / 2, W / 2) max-pool buffer in ``pooled_dtype``), or None where the bf16 kernel
+    does not take the shape."""
     B, Cc, H, W = x.shape
+    if W % 4 != 0 or H % 2 != 0:
+        return None
+    return torch.empty((B, Cc, H // 2, W // 2), device=x.device, dtype=pooled_dtype)
+
+
+def cbam_pool_maxpool(x, pooled_dtype=torch.float32):
+    """(avg, mx, maxpool2(x)) from one read of x, or None when the shape is not taken (odd H, W % 4 != 0).  A bf16 x (the bf16
+    route) writes its max-pool in ``pooled_dtype`` (bf16 or fp32: the dtype of the level it feeds)."""
+    x = _dense(x, "x", bf16=True)
+    B, Cc, H, W = x.shape
+    if is_bf16(x):
+        pooled = _pool_bf16(x, pooled_dtype)
+        if pooled is None:
+            return None
+        avg = torch.empty((B, Cc), device=x.device, dtype=torch.float32)
+        mx = torch.empty_like(avg)
+        _call("smaat_cbam_pool_maxpool_bf16_fwd", 2 * B * Cc * H * W + pooled.numel() * pooled.element_size(), 0,
+              _lib.load().smaat_cbam_pool_maxpool_bf16_fwd, _ptr(x), _ptr(avg), _ptr(mx), _ptr(pooled), int(is_bf16(pooled)), B * Cc,
+              H, W, _stream())
+        return avg, mx, pooled
     if W % 4 != 0 or H % 2 != 0:
         return None
     avg = torch.empty((B, Cc), device=x.device, dtype=torch.float32)
@@ -648,14 +763,27 @@ def _counters(device, n):
     return t
 
 
-def cbam_pool_mlp(x, w1, b1, w2, b2, with_maxpool=False):
+def cbam_pool_mlp(x, w1, b1, w2, b2, with_maxpool=False, pooled_dtype=torch.float32):
     """ChannelAttention gate in ONE launch: (sc, avg, mx, pooled or None); None when the shape is not taken
-    (C % 8, C > 512, hidden > 64) -- callers then use cbam_pool / cbam_pool_maxpool + cbam_mlp."""
-    x = _dense(x, "x")
+    (C % 8, C > 512, hidden > 64) -- callers then use cbam_pool / cbam_pool_maxpool + cbam_mlp.  A bf16 x (the bf16 route) is
+    taken with the max-pool only, written in ``pooled_dtype``."""
+    x = _dense(x, "x", bf16=True)
     B, Cc, H, W = x.shape
     hidden = w1.shape[0]
     if Cc % 8 != 0 or Cc > 512 or hidden > 64:
         return None
+    if is_bf16(x):
+        pooled = _pool_bf16(x, pooled_dtype) if with_maxpool else None
+        if pooled is None:
+            return None
+        avg = torch.empty((B, Cc), device=x.device, dtype=torch.float32)
+        mx = torch.empty_like(avg)
+        sc = torch.empty_like(avg)
+        cnt = _counters(x.device, B)
+        _call(f"smaat_cbam_pool_mlp_bf16_fwd[C{Cc}_S{H}]", 2 * B * Cc * H * W + pooled.numel() * pooled.element_size(), 0,
+              _lib.load().smaat_cbam_pool_mlp_bf16_fwd, _ptr(x), _ptr(avg), _ptr(mx), _ptr(pooled), int(is_bf16(pooled)),
+              _ptr(_dense(w1, "w1")), _ptr(b1), _ptr(_dense(w2, "w2")), _ptr(b2), _ptr(sc), _ptr(cnt), B, Cc, H, W, hidden, _stream())
+        return sc, avg, mx, pooled
     want_pool = with_maxpool and W % 4 == 0 and H % 2 == 0
     avg = torch.empty((B, Cc), device=x.device, dtype=torch.float32)
     mx = torch.empty_like(avg)
@@ -713,9 +841,14 @@ def cbam_mlp(avg, mx, w1, b1, w2, b2):
 
 
 def cbam_reduce(x, sc):
-    x = _dense(x, "x")
+    """Per-pixel channel mean / max of x * sc: (B, 2, H, W) fp32, from an fp32 or (the bf16 route) a bf16 x."""
+    x = _dense(x, "x", bf16=True)
     B, Cc, H, W = x.shape
     pooled = torch.empty((B, 2, H, W), device=x.device, dtype=torch.float32)
+    if is_bf16(x):
+        _call(f"smaat_cbam_reduce_bf16_fwd[C{Cc}_S{H}]", 2 * B * Cc * H * W + 8 * B * H * W, 0, _lib.load().smaat_cbam_reduce_bf16_fwd,
+              _ptr(x), _ptr(sc), _ptr(pooled), B, Cc, H * W, _stream())
+        return pooled
     _call(f"smaat_cbam_reduce_fwd[C{Cc}_S{H}]", 4 * B * (Cc + 2) * H * W, 0, _lib.load().smaat_cbam_reduce_fwd, _ptr(x), _ptr(sc), _ptr(pooled), B, Cc, H * W, _stream())
     return pooled
 
@@ -743,11 +876,16 @@ def cbam_scale(x, sc, sa, out=None):
 
 
 def outconv(x, weight, bias):
-    """OutConv 1x1 (unet_parts.py:70)."""
-    x = _dense(x, "x")
+    """OutConv 1x1 (unet_parts.py:70).  A bf16 x (the bf16 route) gives bf16 logits, accumulated in fp32."""
+    x = _dense(x, "x", bf16=True)
     B, Cin, H, W = x.shape
     w = _dense(weight, "weight")
     ncls = w.shape[0]
+    if is_bf16(x):
+        y = torch.empty((B, ncls, H, W), device=x.device, dtype=torch.bfloat16)
+        _call("smaat_outconv_bf16_fwd", 2 * B * (Cin + ncls) * H * W, 2 * B * Cin * ncls * H * W, _lib.load().smaat_outconv_bf16_fwd,
+              _ptr(x), _ptr(w), _ptr(bias), _ptr(y), B, Cin, ncls, H * W, _stream())
+        return y
     y = torch.empty((B, ncls, H, W), device=x.device, dtype=torch.float32)
     _call("smaat_outconv_fwd", 4 * B * (Cin + ncls) * H * W, 2 * B * Cin * ncls * H * W, _lib.load().smaat_outconv_fwd, _ptr(x), _ptr(w), _ptr(bias), _ptr(y), B, Cin, ncls, H * W, _stream())
     return y
