@@ -25,6 +25,19 @@ def _refuse_bf16(x, why):
         raise ValueError(f"{BF16_ROUTE}; {why}")
 
 
+def bf16_shape_refusal(shape):
+    """Why SmaAt_UNet's bf16 route does not take an input of this shape, or None.  Levels 1-3 are H x W, H / 2 x W / 2 and
+    H / 4 x W / 4; the bf16 DS conv needs rows of a multiple of 8 bf16 (16 bytes, for TMA) at each, and tiles a map in patches
+    16 or 32 pixels wide: an 8-wide level-3 map (W = 32) wastes half of either patch and is declined."""
+    shape = tuple(shape)
+    if len(shape) != 4 or shape[2] % 32 or shape[3] % 32:
+        return f"H and W must be multiples of 32 (16-byte bf16 rows at levels 1-3), got shape {shape}"
+    if shape[3] < 64:
+        return (f"W must be at least 64: at W = {shape[3]} the level-3 maps are {shape[3] // 4} wide, which the fused bf16 DS conv "
+                f"does not tile, got shape {shape}")
+    return None
+
+
 class _ServingForward(nn.Module):
     """The serving forwards ``engine.InferenceSession`` captures, for the three networks.  Each network provides
     ``_serving(x, head)``: its eval forward, ending in up4 with the OutConv and the head (modules.HEADS); its class docstring
@@ -111,8 +124,9 @@ class SmaAt_UNet(_ServingForward):
             _refuse_bf16(x, f"kernels_per_layer={self.inc.double_conv[0].kernels_per_layer} has no bf16 kernel (1 or 2 only)")
         if not self.bilinear:
             _refuse_bf16(x, "bilinear=False (the transposed-conv upsample) has no bf16 route")
-        if x.dim() != 4 or x.shape[2] % 32 or x.shape[3] % 32:
-            _refuse_bf16(x, f"H and W must be multiples of 32 (16-byte bf16 rows at levels 1-3), got shape {tuple(x.shape)}")
+        why = bf16_shape_refusal(x.shape)
+        if why:
+            _refuse_bf16(x, why)
         try:
             return self._serving(x, head)
         except Bf16Declined as e:

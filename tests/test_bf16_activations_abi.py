@@ -92,6 +92,58 @@ def test_cbam_upsample_and_head_entry_points_validate_their_arguments():
     assert lib.smaat_argmax_channels_bf16_fwd(A, A + 4, 2, 4, 64, None) == BADARG
 
 
+def _model_ds_convs(n_ch, n_cls, H, W):
+    """(name, C0, C1, Cout, H, W, ncls) of SmaAt_UNet(n_ch, n_cls)'s level 1-3 DS convs on an H x W input (C1: the upsampled
+    half of the decoder's virtual concat; ncls: the classes of the OutConv up4's last conv carries for class maps, else 0)."""
+    convs = []
+    for blk, s, cin, mid, cout, cat in (("inc", 1, n_ch, 64, 64, False), ("down1", 2, 64, 128, 128, False),
+                                        ("down2", 4, 128, 256, 256, False), ("up2", 4, 512, 256, 128, True),
+                                        ("up3", 2, 256, 128, 64, True), ("up4", 1, 128, 64, 64, True)):
+        C0, C1 = (cin // 2, cin // 2) if cat else (cin, 0)
+        convs.append((f"{blk}.0", C0, C1, mid, H // s, W // s, 0))
+        convs.append((f"{blk}.1", mid, 0, cout, H // s, W // s, 0))
+    if n_cls <= 32:
+        convs.append(("up4.1+outc", 64, 0, 64, H, W, n_cls))
+    return convs
+
+
+def test_the_bf16_shape_check_admits_only_what_every_level_1_3_conv_takes():
+    """For H, W multiples of 32 up to 640: an input shape SmaAt_UNet's bf16 route admits has every level 1-3 DS conv (and the
+    class-map head) taken by the bf16 kernel, so a request it admits never stops half-way on a declined layer.  W = 32 is
+    refused: its 8-wide level-3 maps waste half of a 16- or 32-pixel patch."""
+    from smaat_unet_b200.model import bf16_shape_refusal
+    lib = S._lib.load()
+    sizes = range(32, 641, 32)
+    for k in (1, 2):
+        for n_ch, n_cls in ((12, 1), (3, 21), (1, 2)):
+            for H in sizes:
+                for W in sizes:
+                    admitted = bf16_shape_refusal((2, n_ch, H, W)) is None
+                    assert admitted == (W >= 64), (H, W)
+                    if not admitted:
+                        continue
+                    for name, C0, C1, Cout, h, w, ncls in _model_ds_convs(n_ch, n_cls, H, W):
+                        if k == 1 and C1 and C0 % 32:
+                            continue     # no concat conv of the model has C0 < 32
+                        got = lib.smaat_dsconv_bf16_eligible(A, C0, C0 * h * w, A if C1 else None, C1, C1 * h * w, A, h, w, k, Cout,
+                                                             ncls)
+                        assert got == 1, (k, n_ch, n_cls, H, W, name)
+    # the check and the kernel agree on why: at W = 32, level 3 (8 wide) is what the kernel declines
+    assert _elig(lib, 128, 0, 8, 256, W=8) == 0 and _elig(lib, 256, 256, 8, 256, W=8) == 0
+    assert _elig(lib, 128, 0, 16, 256, W=16) == 1
+
+
+def test_w32_is_refused_before_any_device_work():
+    model = S.SmaAt_UNet(12, 1).eval()
+    with torch.no_grad():
+        for call in (model.forward_serving, model.forward_classes, model.forward_probs):
+            with pytest.raises(ValueError, match="level-3 maps are 8 wide"):
+                call(_x((2, 12, 64, 32)))
+        # a 32-row, 64-column image is admitted: it fails later, at the first kernel, because x is on the CPU
+        with pytest.raises(RuntimeError, match="CUDA"):
+            model.forward_serving(_x((1, 12, 32, 64)))
+
+
 def _x(shape=(2, 12, 64, 64)):
     return torch.zeros(shape, dtype=BF)
 
