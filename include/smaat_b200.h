@@ -152,6 +152,18 @@ int smaat_dsconv_cbam_fwd(const float* x0, int C0, int64_t x0_bstride, const flo
                           const float* scale, const float* shift, float* y, int64_t y_bstride,
                           const float* gate_sc, const float* gate_sa, float* pool_sum, float* pool_max, float* pooled,
                           int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
+/* The fused DS conv that also writes pooled = MaxPool2d(2)(y) (parts_ds.py:48) for the DownDS that reads y next, as the CBAM
+ * pools' epilogue does but without the partial sums (no atomics either way): UNetDS's encoder, which has no CBAM to hand the
+ * max-pool over (unet_precip_regression_lightning.py:107-112).  pooled (B, Cout, H / 2, W / 2), 8-byte aligned, bit for bit the
+ * max-pool of the stored y; floor for odd H.  Arguments otherwise as smaat_dsconv_fwd, without batch statistics.
+ * smaat_dsconv_maxpool_eligible: 1 if smaat_dsconv_maxpool_fwd takes the request in `mode` (an instance with the staged
+ * epilogue: smaat_dsconv_cbam_eligible with with_pools), else 0. */
+int smaat_dsconv_maxpool_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                                  const float* pw_w, int H, int W, int k, int Cout, int mode);
+int smaat_dsconv_maxpool_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                             const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
+                             const float* scale, const float* shift, float* y, int64_t y_bstride, float* pooled,
+                             int B, int H, int W, int k, int Cout, int relu, int mode, void* stream);
 
 /* How the fused DS conv (smaat_dsconv_fwd / smaat_dsconv_outconv_fwd, same reference lines, models/layers.py:47-50) hands the
  * depthwise result to the tensor core: 0 = auto (default; 2, the faster of the two on an H100), 1 = K-major tiles in shared memory that wgmma reads
@@ -455,6 +467,9 @@ int smaat_voc_augment_fwd(const uint8_t* x_u8, const uint8_t* y_u8, const int8_t
  *   K-class OutConv and the argmax, in the epilogue; logits (optional for classify) stored as bf16, the argmax taken on the fp32
  *   logits in registers.
  * smaat_dsconv_bf16_eligible: 1 if those take the request: ncls = 0 for smaat_dsconv_bf16_fwd, else the classes of the head.
+ * smaat_dsconv_maxpool_bf16_fwd (smaat_dsconv_maxpool_fwd): bf16 y and its max-pool, written as bf16 (pooled_bf16 = 1, 4-byte
+ *   aligned) or fp32 (8-byte aligned), the dtype of the level it feeds; bit for bit the max-pool of the stored y.
+ *   smaat_dsconv_maxpool_bf16_eligible: 1 if it takes the request (smaat_dsconv_bf16_eligible and the staged epilogue).
  * smaat_cbam_pool_mlp_bf16_fwd / smaat_cbam_pool_maxpool_bf16_fwd: the pools (+ MLP) and the 2x2 max-pool of a bf16 x; the max-pool
  *   is written as bf16 (pooled_bf16 = 1) or fp32, the dtype of the level it feeds.  The max-pool is required (even H, W % 4 == 0).
  * smaat_cbam_reduce_bf16_fwd: the per-pixel channel mean / max of x * sc from a bf16 x, fp32 out.
@@ -475,6 +490,12 @@ int smaat_dsconv_classify_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, c
                                    const float* dw_w, const float* dw_b, const uint16_t* pw_w, const float* scale,
                                    const float* shift, const float* oc_w, const float* oc_b, int K, void* logits,
                                    int64_t* classes, int B, int H, int W, int k, int Cout, int relu, void* stream);
+int smaat_dsconv_maxpool_bf16_eligible(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                                       const void* pw_w, int H, int W, int k, int Cout);
+int smaat_dsconv_maxpool_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                                  const float* dw_w, const float* dw_b, const uint16_t* pw_w, const float* scale,
+                                  const float* shift, void* y, int64_t y_bstride, void* pooled, int pooled_bf16, int B, int H,
+                                  int W, int k, int Cout, int relu, void* stream);
 int smaat_cbam_pool_mlp_bf16_fwd(const void* x, float* avg, float* mx, void* pooled, int pooled_bf16, const float* w1,
                                  const float* b1, const float* w2, const float* b2, float* sc, int* counters, int B, int C,
                                  int H, int W, int hidden, void* stream);

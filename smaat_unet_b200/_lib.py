@@ -31,6 +31,8 @@ SIGNATURES = {
     "smaat_dsconv_classify_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_cbam_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _i, _i],
     "smaat_dsconv_pool_parts": [_i, _i],
+    "smaat_dsconv_maxpool_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i],
+    "smaat_dsconv_maxpool_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_cbam_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _l, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_split_tf32": [_p, _p, _p, _l, _p],
     "smaat_pack_bf16": [_p, _p, _i, _i, _i, _p],
@@ -90,6 +92,8 @@ SIGNATURES = {
     "smaat_dsconv_bf16_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _l, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_outconv_bf16_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_classify_bf16_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _p],
+    "smaat_dsconv_maxpool_bf16_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i],
+    "smaat_dsconv_maxpool_bf16_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_cbam_pool_mlp_bf16_fwd": [_p, _p, _p, _p, _i, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p],
     "smaat_cbam_pool_maxpool_bf16_fwd": [_p, _p, _p, _p, _i, _l, _i, _i, _p],
     "smaat_cbam_reduce_bf16_fwd": [_p, _p, _p, _i, _i, _i, _p],

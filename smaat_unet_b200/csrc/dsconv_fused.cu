@@ -61,11 +61,13 @@ struct DsParams {
   float* oc_y;
   // CBAM fusions of the serving forward (smaat_dsconv_cbam_fwd).  gate_sc (B, C0): x0 is read as the CBAM output
   // (x0 * gate_sc[b, c]) * gate_sa[b, p], gate_sa coming in by its own TMA map.  pool_sum / pool_max (B, npart, Cout): per
-  // half-patch partial sums / maxima of the output for the channel gate's pools; pooled (B, Cout, H / 2, W / 2): its 2x2 max-pool
+  // half-patch partial sums / maxima of the output for the channel gate's pools; pooled (B, Cout, H / 2, W / 2): its 2x2 max-pool,
+  // also without the pools (smaat_dsconv_maxpool_fwd), and from bf16 maps as bf16 (pooled_bf16) or fp32
   const float* gate_sc;
   float* pool_sum;
   float* pool_max;
   float* pooled;
+  int pooled_bf16;
   int npart;
   // K-class OutConv + argmax (smaat_dsconv_classify_fwd): ncls > 0 classes, oc_w (ncls, Cout), oc_b (ncls) or null, oc_y the
   // (B, ncls, H, W) logits or null, cls the (B, H, W) class map or null
@@ -578,12 +580,14 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
             tma_store_4d(&map_y, buf, tx * PW, y_half, n0 + 32 * s, b);
             bulk_commit();
           }
-          if (!BA && p.pool_sum) {
-            // The CBAM channel gate's pools and the next level's MaxPool2d(2), read back from the staged slice (the stored values
-            // bit for bit; the store reads the buffer too, and nothing writes it before the next wg_sync).  4 threads per
+          if (p.pooled) {
+            // The next level's MaxPool2d(2) [and the CBAM channel gate's pools: pool_sum, fp32 maps only], read back from the
+            // staged slice (the stored values bit for bit -- bf16 boxes hold the rounded values, and the max of bf16 values is
+            // one of them; the store reads the buffer too, and nothing writes it before the next wg_sync).  4 threads per
             // channel, 2 items each: an item is 4 columns of a row pair, i.e. two 2 x 2 windows (the half-patch origin is even
             // and PH / 2 is even, so no window straddles it).  Pixels outside H or W are masked; an odd last row goes into the
             // pools but not the max-pool (floor, as MaxPool2d)
+            const bool parts = !BA && p.pool_sum;
             const int pt = threadIdx.x & 127, pch = pt >> 2, pq = pt & 3;
             const int c = n0 + 32 * s + pch;
             float psum = 0.f, pmax = -INFINITY;
@@ -592,37 +596,54 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
               constexpr int NQ = PW / 4;
               const int item = pq + 4 * it, rp = item / NQ, qd = item % NQ;   // lanes pq = 0..3: 4 adjacent items, 32 B of max-pool
               const int px = 2 * rp * PW + 4 * qd;
-              const uint32_t a0 = (uint32_t)(pch * 256 + px * 4), a1 = a0 + (uint32_t)(PW * 4);
               float4 u, v;
-              asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(u.x), "=f"(u.y), "=f"(u.z), "=f"(u.w)
-                           : "r"(buf + (a0 ^ (((a0 >> 7) & SW_MASK) << 4))));
-              asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-                           : "r"(buf + (a1 ^ (((a1 >> 7) & SW_MASK) << 4))));
+              if constexpr (BA) {
+                // unswizzled [channel][64 pixels] x 2 B: 4 pixels are one 8-byte load
+                const uint32_t a0 = (uint32_t)(pch * 128 + px * 2), a1 = a0 + (uint32_t)(PW * 2);
+                uint2 hu, hv;
+                asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(hu.x), "=r"(hu.y) : "r"(buf + a0));
+                asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(hv.x), "=r"(hv.y) : "r"(buf + a1));
+                u = bf16x4_f32(hu);
+                v = bf16x4_f32(hv);
+              } else {
+                const uint32_t a0 = (uint32_t)(pch * 256 + px * 4), a1 = a0 + (uint32_t)(PW * 4);
+                asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(u.x), "=f"(u.y), "=f"(u.z), "=f"(u.w)
+                             : "r"(buf + (a0 ^ (((a0 >> 7) & SW_MASK) << 4))));
+                asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+                             : "r"(buf + (a1 ^ (((a1 >> 7) & SW_MASK) << 4))));
+              }
               const int gy = y_half + 2 * rp, gx = tx * PW + 4 * qd;      // W % 4 == 0: a quad is all in or all out
               const bool in0 = gx < p.W && gy < p.H, in1 = gx < p.W && gy + 1 < p.H;
-              if (in0) {
+              if (parts && in0) {
                 psum += (u.x + u.y) + (u.z + u.w);
                 pmax = fmaxf(pmax, fmaxf(fmaxf(u.x, u.y), fmaxf(u.z, u.w)));
               }
               if (in1) {
-                psum += (v.x + v.y) + (v.z + v.w);
-                pmax = fmaxf(pmax, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
+                if (parts) {
+                  psum += (v.x + v.y) + (v.z + v.w);
+                  pmax = fmaxf(pmax, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
+                }
                 if (c < p.Cout) {
                   const int hw = p.W >> 1;
+                  const int64_t o = ((int64_t)b * p.Cout + c) * (int64_t)(p.H >> 1) * hw + (int64_t)(gy >> 1) * hw + (gx >> 1);
                   const float2 m2 = make_float2(fmaxf(fmaxf(u.x, u.y), fmaxf(v.x, v.y)), fmaxf(fmaxf(u.z, u.w), fmaxf(v.z, v.w)));
-                  *reinterpret_cast<float2*>(p.pooled + ((int64_t)b * p.Cout + c) * (int64_t)(p.H >> 1) * hw +
-                                             (int64_t)(gy >> 1) * hw + (gx >> 1)) = m2;
+                  if (BA && p.pooled_bf16)   // exact: both maxima are bf16 values
+                    *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.pooled) + o) = f32x2_bf16x2(m2.x, m2.y);
+                  else
+                    *reinterpret_cast<float2*>(p.pooled + o) = m2;
                 }
               }
             }
-            psum += __shfl_xor_sync(0xffffffffu, psum, 1);
-            psum += __shfl_xor_sync(0xffffffffu, psum, 2);
-            pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 1));
-            pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 2));
-            if (pq == 0 && c < p.Cout) {
-              const int64_t o = ((int64_t)b * p.npart + 2 * (ty * p.tiles_x + tx) + wg) * p.Cout + c;
-              p.pool_sum[o] = psum;
-              p.pool_max[o] = pmax;
+            if (parts) {   // uniform over the CTA
+              psum += __shfl_xor_sync(0xffffffffu, psum, 1);
+              psum += __shfl_xor_sync(0xffffffffu, psum, 2);
+              pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 1));
+              pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 2));
+              if (pq == 0 && c < p.Cout) {
+                const int64_t o = ((int64_t)b * p.npart + 2 * (ty * p.tiles_x + tx) + wg) * p.Cout + c;
+                p.pool_sum[o] = psum;
+                p.pool_max[o] = pmax;
+              }
             }
           }
           ++st_n;
@@ -855,8 +876,8 @@ static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtenso
                      const CUtensorMap& my, const CUtensorMap& msa, DsParams p, int B, cudaStream_t st) {
   using L = DsCfg<N_TILE, KPL, PW, P, A_SMEM, TA>;
   auto kern = ds_kernel<N_TILE, KPL, PW, P, A_SMEM, TA>();
-  // the pools are read back from the staging buffers: instances with the direct-store epilogue do not take them
-  if (p.pool_sum && !L::ST_BUFS) return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools need the staged epilogue");
+  // the pools and the max-pool are read back from the staging buffers: instances with the direct-store epilogue do not take them
+  if (p.pooled && !L::ST_BUFS) return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools and the max-pool need the staged epilogue");
   if (p.ncls > L::MAX_CLASSES)
     return fail(SMAAT_E_UNSUPPORTED, "dsconv+classify: %d classes, this instance keeps the weights of at most %d", p.ncls, L::MAX_CLASSES);
   static std::atomic<uint64_t> attr_mask{0};   // cudaFuncSetAttribute is per device
@@ -951,9 +972,9 @@ static int ds_cfg(int n_tile, int k, int pw, int mode, bool a_smem, F f, bool ba
   if (k == 2) return pw == 32 ? ds_cfg_t<128, 2, 32>(mode, a_smem, f, bact) : ds_cfg_t<128, 2, 16>(mode, a_smem, f, bact);
   return pw == 32 ? ds_cfg_t<128, 1, 32>(mode, a_smem, f, bact) : ds_cfg_t<128, 1, 16>(mode, a_smem, f, bact);
 }
-// Whether that instance has the staged epilogue (ST_BUFS > 0), which the CBAM pools are read from
-static bool ds_staged(int n_tile, int k, int pw, int mode, bool a_smem) {
-  return ds_cfg(n_tile, k, pw, mode, a_smem, [](auto c) { return (int)decltype(c)::ST_BUFS; }) > 0;
+// Whether that instance has the staged epilogue (ST_BUFS > 0), which the CBAM pools and the max-pool are read from
+static bool ds_staged(int n_tile, int k, int pw, int mode, bool a_smem, bool bact = false) {
+  return ds_cfg(n_tile, k, pw, mode, a_smem, [](auto c) { return (int)decltype(c)::ST_BUFS; }, bact) > 0;
 }
 // The most classes whose OutConv weights that instance keeps in shared memory (DsCfg::MAX_CLASSES)
 static int ds_max_classes(int n_tile, int k, int pw, int mode, bool a_smem, bool bact = false) {
@@ -1018,14 +1039,17 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
                       const float* dw_b, const float* pw_w, const float* pw_w_lo, const float* scale, const float* shift, float* y,
                       int64_t y_bstride, double* stats, const float* oc_w, const float* oc_b, float* oc_y, int ncls, int64_t* cls,
                       const float* gate_sc, const float* gate_sa, float* pool_sum, float* pool_max, float* pooled, int B, int H, int W,
-                      int k, int Cout, int relu, int mode, void* stream, bool bact = false) {
+                      int k, int Cout, int relu, int mode, void* stream, bool bact = false, int pooled_bf16 = 0) {
   // head: an OutConv in the epilogue (one class, or ncls classes with the argmax) replaces the activation output
   const bool head = oc_y || ncls > 0;
   SMAAT_REQUIRE(x0 && dw_w && pw_w && (y || oc_y || cls), "dsconv: null pointer");
   SMAAT_REQUIRE(!gate_sc == !gate_sa, "dsconv: the CBAM gate needs both sc and sa");
   SMAAT_REQUIRE(!gate_sa || aligned16(gate_sa), "dsconv: the CBAM gate map must be 16-byte aligned");
   SMAAT_REQUIRE(!pool_sum || (pool_max && pooled && y && !oc_y && !stats), "dsconv: the CBAM pools need sum, max and max-pool outputs and y");
-  SMAAT_REQUIRE(!pooled || (reinterpret_cast<uintptr_t>(pooled) & 7u) == 0, "dsconv: the max-pool output must be 8-byte aligned");
+  SMAAT_REQUIRE(!pooled || (y && !head && !stats), "dsconv: the max-pool needs y, and no OutConv or batch statistics");
+  SMAAT_REQUIRE(!pooled_bf16 || bact, "dsconv: a bf16 max-pool needs bf16 activations");
+  SMAAT_REQUIRE(!pooled || (reinterpret_cast<uintptr_t>(pooled) & (pooled_bf16 ? 3u : 7u)) == 0,
+                "dsconv: the max-pool output must be %d-byte aligned", pooled_bf16 ? 4 : 8);
   SMAAT_REQUIRE(B > 0 && C0 > 0 && C1 >= 0 && H > 0 && W > 0 && Cout > 0, "dsconv: bad shape");
   SMAAT_REQUIRE(C1 == 0 || x1, "dsconv: C1=%d but x1 is null", C1);
   SMAAT_REQUIRE(mode == SMAAT_PW_TF32 || mode == SMAAT_PW_TF32X3 || mode == SMAAT_PW_BF16,
@@ -1112,7 +1136,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   DsParams p;
   p.dw_w = dw_w; p.dw_b = dw_b; p.scale = scale; p.shift = shift; p.y = y; p.y_bstride = y_bstride; p.stats = stats;
   p.oc_w = oc_w; p.oc_b = oc_b; p.oc_y = oc_y; p.ncls = ncls; p.cls = cls;
-  p.gate_sc = gate_sc; p.pool_sum = pool_sum; p.pool_max = pool_max; p.pooled = pooled; p.npart = 0;
+  p.gate_sc = gate_sc; p.pool_sum = pool_sum; p.pool_max = pool_max; p.pooled = pooled; p.pooled_bf16 = pooled_bf16; p.npart = 0;
   p.C0 = C0; p.C1 = C1; p.H = H; p.W = W; p.Cout = Cout; p.relu = relu; p.K = K;
   p.tiles_x = p.tiles_y = p.npass = p.total_tiles = p.nchunks = 0;
 
@@ -1207,6 +1231,24 @@ extern "C" int smaat_dsconv_cbam_fwd(const float* x0, int C0, int64_t x0_bstride
                     nullptr, nullptr, 0, nullptr, gate_sc, gate_sa, pool_sum, pool_max, pooled, B, H, W, k, Cout, relu, mode, stream);
 }
 
+/* The fused DS conv that also writes MaxPool2d(2) of its output, for the DownDS that reads it next (UNetDS's encoder, which has
+ * no CBAM to hand the max-pool over): the staged epilogue reads each stored slice back, so pooled is the max-pool of y bit for
+ * bit, without a second read of y.  No partial sums, no atomics.  pooled (B, Cout, H / 2, W / 2), 8-byte aligned; floor for
+ * odd H.  Eligibility: smaat_dsconv_cbam_eligible with pools. */
+extern "C" int smaat_dsconv_maxpool_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                                             const float* pw_w, int H, int W, int k, int Cout, int mode) {
+  return smaat_dsconv_cbam_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout, mode, 0, 1);
+}
+
+extern "C" int smaat_dsconv_maxpool_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
+                                        const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
+                                        const float* scale, const float* shift, float* y, int64_t y_bstride, float* pooled, int B,
+                                        int H, int W, int k, int Cout, int relu, int mode, void* stream) {
+  SMAAT_REQUIRE(y && pooled, "dsconv_maxpool: null output");
+  return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, nullptr, nullptr,
+                    nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, pooled, B, H, W, k, Cout, relu, mode, stream);
+}
+
 /* ---- bf16 activations: the serving forward's bf16 route -------------------------------------------------------------------
  * x0 / x1 and the output (y or the logits) are bf16 (raw uint16_t bits) in HBM; the depthwise stencil, the accumulation and
  * the epilogue run in fp32, the GEMM takes bf16 operands (pw_w: the smaat_pack_bf16 pack), and each stored value is rounded
@@ -1263,4 +1305,24 @@ extern "C" int smaat_dsconv_classify_bf16_fwd(const void* x0, int C0, int64_t x0
                     reinterpret_cast<const float*>(pw_w), nullptr, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
                     static_cast<float*>(logits), K, classes, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu,
                     SMAAT_PW_BF16, stream, true);
+}
+
+/* smaat_dsconv_maxpool_fwd from bf16 activations: y bf16, the max-pool written as bf16 (pooled_bf16 = 1, 4-byte aligned) or
+ * fp32 (8-byte aligned), the dtype of the level it feeds; either way bit for bit MaxPool2d(2) of the stored y. */
+extern "C" int smaat_dsconv_maxpool_bf16_eligible(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1,
+                                                  int64_t x1_bstride, const void* pw_w, int H, int W, int k, int Cout) {
+  if (!smaat_dsconv_bf16_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout, 0)) return 0;
+  return ds_staged(Cout > 64 ? 128 : 64, k, pick_pw(H, W), SMAAT_PW_BF16, false, true) ? 1 : 0;
+}
+
+extern "C" int smaat_dsconv_maxpool_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
+                                             const float* dw_w, const float* dw_b, const uint16_t* pw_w, const float* scale,
+                                             const float* shift, void* y, int64_t y_bstride, void* pooled, int pooled_bf16, int B,
+                                             int H, int W, int k, int Cout, int relu, void* stream) {
+  SMAAT_REQUIRE(y && pooled, "dsconv_maxpool_bf16: null output");
+  SMAAT_REQUIRE(pooled_bf16 == 0 || pooled_bf16 == 1, "dsconv_maxpool_bf16: pooled_bf16 must be 0 or 1");
+  return dsconv_run(static_cast<const float*>(x0), C0, x0_bstride, static_cast<const float*>(x1), C1, x1_bstride, dw_w, dw_b,
+                    reinterpret_cast<const float*>(pw_w), nullptr, scale, shift, static_cast<float*>(y), y_bstride, nullptr, nullptr,
+                    nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, static_cast<float*>(pooled), B, H, W, k, Cout,
+                    relu, SMAAT_PW_BF16, stream, true, pooled_bf16);
 }

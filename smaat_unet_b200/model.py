@@ -1,8 +1,9 @@
-"""SmaAt-UNet and the paper's dense baselines (UNet, UNetAttention) assembled from the H100 drop-in blocks.
+"""SmaAt-UNet, its ablations (UNetDS, UNetDSAttention4CBAMs) and the paper's dense baselines (UNet, UNetAttention) assembled
+from the H100 drop-in blocks.
 
 Same constructor, attribute names (hence state_dict keys) and forward graph as the
-reference's ``models/SmaAt_UNet.py:7-57``; provided so the full model can be built where the
-reference checkout is not importable (e.g. the GPU box).  With the reference on
+reference's ``models/SmaAt_UNet.py:7-57`` and the Lightning classes of ``models/unet_precip_regression_lightning.py``; provided so
+the full models can be built where the reference checkout is not importable (e.g. the GPU box).  With the reference on
 ``sys.path`` prefer ``smaat_unet_b200.patch_reference()`` and use its own ``SmaAt_UNet``
 (and the Lightning wrappers) unchanged.
 """
@@ -16,8 +17,9 @@ from .modules import (CBAM, Bf16Declined, DoubleConv, DoubleConvDS, Down, DownDS
 
 _ENC = (64, 128, 256, 512)
 
-BF16_ROUTE = ("bf16 input is taken by SmaAt_UNet's serving forward only: forward_serving / forward_classes / forward_probs in "
-              "eval mode under torch.no_grad(), or InferenceSession(model, ..., dtype=torch.bfloat16)")
+BF16_ROUTE = ("bf16 input is taken by the serving forward of SmaAt_UNet, UNetDSAttention4CBAMs and UNetDS only: forward_serving / "
+              "forward_classes / forward_probs in eval mode under torch.no_grad(), or InferenceSession(model, ..., "
+              "dtype=torch.bfloat16)")
 
 
 def _refuse_bf16(x, why):
@@ -26,9 +28,10 @@ def _refuse_bf16(x, why):
 
 
 def bf16_shape_refusal(shape):
-    """Why SmaAt_UNet's bf16 route does not take an input of this shape, or None.  Levels 1-3 are H x W, H / 2 x W / 2 and
-    H / 4 x W / 4; the bf16 DS conv needs rows of a multiple of 8 bf16 (16 bytes, for TMA) at each, and tiles a map in patches
-    16 or 32 pixels wide: an 8-wide level-3 map (W = 32) wastes half of either patch and is declined."""
+    """Why the bf16 route of SmaAt_UNet, UNetDSAttention4CBAMs and UNetDS does not take an input of this shape, or None.
+    Levels 1-3 are H x W, H / 2 x W / 2 and H / 4 x W / 4; the bf16 DS conv (and its max-pool epilogue) needs rows of a multiple
+    of 8 bf16 (16 bytes, for TMA) at each, and tiles a map in patches 16 or 32 pixels wide: an 8-wide level-3 map (W = 32)
+    wastes half of either patch and is declined."""
     shape = tuple(shape)
     if len(shape) != 4 or shape[2] % 32 or shape[3] % 32:
         return f"H and W must be multiples of 32 (16-byte bf16 rows at levels 1-3), got shape {shape}"
@@ -39,7 +42,7 @@ def bf16_shape_refusal(shape):
 
 
 class _ServingForward(nn.Module):
-    """The serving forwards ``engine.InferenceSession`` captures, for the three networks.  Each network provides
+    """The serving forwards ``engine.InferenceSession`` captures, for the five networks.  Each network provides
     ``_serving(x, head)``: its eval forward, ending in up4 with the OutConv and the head (modules.HEADS); its class docstring
     says what that fuses.  In train mode or under autograd they run the plain forward, then ``modules.apply_head``."""
 
@@ -68,18 +71,27 @@ class _ServingForward(nn.Module):
         _refuse_bf16(x, f"{type(self).__name__} has no bf16 route")
 
 
-class SmaAt_UNet(_ServingForward):
-    """The serving forward (``forward_serving`` / ``forward_classes`` / ``forward_probs``) has the fusions the plain-call API
-    cannot express:
+class _DSUNet(_ServingForward):
+    """The depthwise-separable networks of the paper: SmaAt_UNet, UNetDSAttention4CBAMs and UNetDS, one body parameterised by
+    ``CBAM_LEVELS``, the levels (1-5) whose encoder map carries a CBAM.  Attribute names and parameter registration order are
+    the reference's (models/SmaAt_UNet.py:22-38, unet_precip_regression_lightning.py:87-104 and :173-190): inc, [cbam1], down1,
+    [cbam2], ..., down4, [cbam5], up1-up4, outc.
+
+    Serving forward (``forward_serving`` / ``forward_classes`` / ``forward_probs``):
     * up4's last DS conv applies the OutConv in its epilogue (SmaAt_UNet.py:55-56), so the 64-channel activation never reaches
       HBM: the 1-class OutConv for the logits, the n_classes-class OutConv and the argmax for class maps (n_classes <= 32;
       more classes take the unfused convs, OutConv and the argmax kernel).  Each class's logit there is the one-class fused
       OutConv's arithmetic, which sums in another order than the unfused OutConv of the logits route: pixels whose top two
       logits lie within rounding of each other may pick the other class.  The probabilities are the channel softmax of the
       logits route's output;
-    * the three large CBAMs (levels 1-3) never write their output: they compute only their two gates, and the first DS
-      conv of up2 / up3 / up4 applies them as it loads the skip, with the products the CBAM's own kernel would have used
-      (bit for bit the same logits).  Levels 4-5 run the plain calls."""
+    * a CBAM at level 1-3 never writes its output: it computes only its two gates, and the first DS conv of up2 / up3 / up4
+      applies them as it loads the skip, with the products the CBAM's own kernel would have used (bit for bit the same
+      logits).  A CBAM at level 4-5 runs the plain call, which hands its max-pool to the DownDS that follows;
+    * a level 1-4 map without a CBAM (UNetDS) gets its 2x2 max-pool from the epilogue of the DS conv that produced it, bit for
+      bit the max-pool of the stored map, so the next DownDS does not read the map again (``smaat_maxpool2_fwd`` where that
+      kernel declines the shape)."""
+
+    CBAM_LEVELS = ()
 
     def __init__(self, n_channels, n_classes, kernels_per_layer=2, bilinear=True, reduction_ratio=16):
         super().__init__()
@@ -88,29 +100,36 @@ class SmaAt_UNet(_ServingForward):
         factor = 2 if bilinear else 1
         widths = list(_ENC) + [1024 // factor]            # channels of x1..x5
         self.inc = DoubleConvDS(n_channels, widths[0], kernels_per_layer=k)
-        for lvl in range(5):                                # [down_l,] cbam_{l+1} -- registration order = reference's
+        for lvl in range(5):                                # [down_l,] [cbam_{l+1}] -- registration order = reference's
             if lvl > 0:
                 setattr(self, f"down{lvl}", DownDS(widths[lvl - 1], widths[lvl], kernels_per_layer=k))
-            setattr(self, f"cbam{lvl + 1}", CBAM(widths[lvl], reduction_ratio=r))
+            if lvl + 1 in self.CBAM_LEVELS:
+                setattr(self, f"cbam{lvl + 1}", CBAM(widths[lvl], reduction_ratio=r))
         dec_in = (1024, 512, 256, 128)
         dec_out = (512 // factor, 256 // factor, 128 // factor, 64)
         for i in range(4):                                  # up1..up4
             setattr(self, f"up{i + 1}", UpDS(dec_in[i], dec_out[i], bilinear, kernels_per_layer=k))
         self.outc = OutConv(64, n_classes)
 
+    def _cbam(self, lvl):
+        return getattr(self, f"cbam{lvl + 1}", None)
+
     def forward(self, x):
-        """The reference's graph, block for block and in its call order (models/SmaAt_UNet.py:41-57): plain calls only --
-        exactly what a ``patch_reference()`` user of the unchanged reference class executes.  The max-pool fusion still
-        happens: ``cbamN(f)`` leaves MaxPool2d(2)(f) behind for the ``downN(f)`` that follows (modules.CBAM.forward)."""
+        """The reference's graph, block for block and in its call order (models/SmaAt_UNet.py:41-57,
+        unet_precip_regression_lightning.py:107-118 and :193-208): plain calls only -- exactly what a ``patch_reference()`` user
+        of the unchanged reference class executes.  Where a CBAM precedes a DownDS the max-pool fusion still happens:
+        ``cbamN(f)`` leaves MaxPool2d(2)(f) behind for the ``downN(f)`` that follows (modules.CBAM.forward)."""
         _refuse_bf16(x, "model(x) runs the fp32 plain-call graph")
         f = self.inc(x)
-        att = [self.cbam1(f)]
-        for lvl in range(1, 5):
-            f = getattr(self, f"down{lvl}")(f)
-            att.append(getattr(self, f"cbam{lvl + 1}")(f))
-        y = att[4]                                                  # x5Att is the decoder input
+        att = []
+        for lvl in range(5):
+            if lvl > 0:
+                f = getattr(self, f"down{lvl}")(f)
+            cbam = self._cbam(lvl)
+            att.append(cbam(f) if cbam is not None else f)
+        y = att[4]                                                  # x5 (x5Att) is the decoder input
         for i in range(4):
-            y = getattr(self, f"up{i + 1}")(y, att[3 - i])          # attended maps are the skips
+            y = getattr(self, f"up{i + 1}")(y, att[3 - i])          # attended maps, where there is a CBAM, are the skips
         return self.outc(y)
 
     def _serve_bf16(self, x, head):
@@ -131,17 +150,24 @@ class SmaAt_UNet(_ServingForward):
             return self._serving(x, head)
         except Bf16Declined as e:
             name = next((n for n, m in self.named_modules() if m is e.module), type(e.module).__name__)
-            raise ValueError(f"SmaAt_UNet bf16 serving forward: {name}: {e}") from None
+            raise ValueError(f"{type(self).__name__} bf16 serving forward: {name}: {e}") from None
 
     def _serving(self, x, head):
-        skips, f = [], self.inc(x)
+        skips, pooled = [], None
         for lvl in range(5):
-            if lvl > 0:
-                f = getattr(self, f"down{lvl}")(f, pooled=pooled)
-            cbam = getattr(self, f"cbam{lvl + 1}")
+            cbam = self._cbam(lvl)
+            # no CBAM to hand the max-pool over: the conv that makes the map writes it for the next DownDS.  The bf16 route's
+            # max-pool is bf16 into levels 2-3, fp32 into level 4
+            kw = {} if cbam is not None or lvl == 4 else {
+                "with_maxpool": True, "pooled_dtype": torch.float32 if lvl >= 2 else x.dtype}
+            f = self.inc.run(x, **kw) if lvl == 0 else getattr(self, f"down{lvl}")(f, pooled=pooled, **kw)
+            if kw:
+                f, pooled = f
+            if cbam is None:
+                skips.append((f, None))
+                continue
             bn = cbam.spatial_att.bn
             if lvl < 3 and not bn.training and bn.track_running_stats:
-                # the bf16 route's max-pool is bf16 into levels 2-3, fp32 into level 4
                 sc, sa, pooled = cbam.serving_gates(f, pooled_dtype=torch.float32 if lvl == 2 else f.dtype)
                 skips.append((f, (sc, sa)))
             else:
@@ -153,6 +179,32 @@ class SmaAt_UNet(_ServingForward):
             y = getattr(self, f"up{i + 1}")(y, skip, gate=gate)
         skip, gate = skips[0]
         return self.up4(y, skip, outconv=self.outc, gate=gate, head=head)
+
+
+class SmaAt_UNet(_DSUNet):
+    """models/SmaAt_UNet.py:7-57: a CBAM on every level.  Serving forward: ``_DSUNet``'s, with the three large CBAMs (levels
+    1-3) as gates applied on load and levels 4-5 as plain calls."""
+
+    CBAM_LEVELS = (1, 2, 3, 4, 5)
+
+
+class UNetDSAttention4CBAMs(_DSUNet):
+    """``models/unet_precip_regression_lightning.py:173-208`` (the Lightning class without its training plumbing): SmaAt-UNet
+    without the bottleneck's CBAM, so x5 goes to up1 un-attended.  Serving forward: ``_DSUNet``'s -- levels 1-3 gated on load,
+    level 4 a plain ``cbam4`` call that hands its max-pool to ``down4``."""
+
+    CBAM_LEVELS = (1, 2, 3, 4)
+
+
+class UNetDS(_DSUNet):
+    """``models/unet_precip_regression_lightning.py:86-118``: SmaAt-UNet without attention, the DS convs' ablation.  Serving
+    forward: ``_DSUNet``'s -- the un-attended maps are the skips, and the max-pools feeding down1-down4 come from the epilogues
+    of the convs that produced the maps."""
+
+    CBAM_LEVELS = ()
+
+    def __init__(self, n_channels, n_classes, kernels_per_layer=2, bilinear=True):
+        super().__init__(n_channels, n_classes, kernels_per_layer=kernels_per_layer, bilinear=bilinear)
 
 
 class UNet(_ServingForward):

@@ -180,6 +180,26 @@ class DepthwiseSeparableConv(_CachingModule):
             return ops.dsconv(*args, mode=mode, w_split=split, outconv=outconv)
         return ops.dsconv_classify(*args, *outconv, mode=mode, w_split=split)
 
+    def run_maxpool(self, x, scale, shift, relu, pooled_dtype=torch.float32):
+        """``run`` that also returns MaxPool2d(2) of its output, written by the fused kernel's epilogue: (y, pooled), pooled None
+        where that kernel does not take the shape (the caller then runs ``ops.maxpool2``).  A bf16 x: the bf16 route, pooled in
+        ``pooled_dtype`` (bf16 or fp32), or ``Bf16Declined``."""
+        if ops.is_bf16(x):
+            self._check()
+            if not ops.dsconv_maxpool_bf16_takes(x, None, self.pointwise.weight.detach(), self.kernels_per_layer):
+                raise Bf16Declined(self, f"the bf16 DS conv with the max-pool epilogue does not take input {tuple(x.shape)}, "
+                                         f"kernels_per_layer={self.kernels_per_layer} (needs k = 1 or 2, W a multiple of 8, "
+                                         "set_dsconv_impl other than 'smem' and set_fused_dsconv(True))")
+            dw_b = self.depthwise.bias.detach() if self.depthwise.bias is not None else None
+            if shift is None:
+                shift = self.pointwise.bias.detach() if self.pointwise.bias is not None else None
+            return ops.dsconv_maxpool_bf16(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(),
+                                           scale, shift, relu, w_split=self.pw_operands("bf16"), pooled_dtype=pooled_dtype)
+        dw_b, shift, mode, split = self._operands(shift)
+        out = ops.dsconv_maxpool(x, self.depthwise.weight.detach(), dw_b, self.kernels_per_layer, self.pointwise.weight.detach(),
+                                 scale, shift, relu, mode=mode, w_split=split)
+        return out if out is not None else (self.run(x, scale=scale, shift=shift, relu=relu), None)
+
     def cbam_takes(self, x, x1=None, gate=False, pools=False) -> bool:
         """Whether ``run_cbam`` takes this input: the fused kernel with the serving forward's CBAM fusions.  For a bf16 x (the bf16
         route, gate only) always: that kernel is its only form, and ``run_cbam`` raises ``Bf16Declined`` where it declines."""
@@ -305,19 +325,27 @@ class DoubleConvDS(_DoubleConvBase):
             nn.ReLU(inplace=True),
         ))
 
-    def run(self, x, x1=None, outconv=None, gate=None, head="logits"):
+    def run(self, x, x1=None, outconv=None, gate=None, head="logits", with_maxpool=False, pooled_dtype=torch.float32):
         """``outconv`` (an OutConv module, inference only): return OutConv(block(x)) ending in ``head`` (``HEADS``) -- its logits,
         their (B, H, W) int64 class map or their (B, K, H, W) softmax probabilities (no gradient).  In the eval fast path the
         last kernel applies the OutConv and the head in its epilogue where it takes the shape (``_fused_last``), and the
         block's own output is then never materialised (models/SmaAt_UNet.py:55-56).
         ``gate=(sc, sa)``: x is the un-attended skip and the block's input is the CBAM output (x * sc) * sa, which the first
-        DS conv computes as it loads x (inference only; materialised first where that kernel does not take it)."""
+        DS conv computes as it loads x (inference only; materialised first where that kernel does not take it).
+        ``with_maxpool`` (no ``outconv``): return (block(x), MaxPool2d(2) of it or None).  In the eval fast path the last DS conv
+        writes the max-pool in its epilogue where it takes the shape (``DepthwiseSeparableConv.run_maxpool``; a bf16 x writes it in
+        ``pooled_dtype``); elsewhere it is None and the DownDS that reads the block's output pools it itself."""
         _check_head(head, outconv)
         ops._req(x, "input", 4, bf16=True)
         if gate is not None and not (self._eval_folded(x, x1) and self.double_conv[0].cbam_takes(x, x1, gate=True)):
             x, gate = ops.cbam_scale(x, gate[0], gate[1]), None
         if outconv is not None:
             return self._run_head(x, x1, outconv, head, gate)
+        if with_maxpool:
+            if not self._eval_folded(x, x1):
+                return self._plain(x, x1, gate), None
+            s1, t1 = self._folded(3)
+            return self.double_conv[3].run_maxpool(self._folded_conv(0, x, x1, gate), s1, t1, True, pooled_dtype=pooled_dtype)
         return self._plain(x, x1, gate)
 
     def _folded_conv(self, idx, x, x1=None, gate=None):
@@ -383,10 +411,11 @@ def _take_stashed_maxpool(x):
 class _Down(nn.Module):
     """MaxPool2d(2) then the double conv ``maxpool_conv[1]``: DownDS and Down."""
 
-    def forward(self, x, pooled=None):
+    def forward(self, x, pooled=None, **run_kw):
         """``pooled``: MaxPool2d(2)(x) when the caller already has it.  Called plainly (``down(x)``, as the reference does)
         it first looks for the 2x2 max-pool the preceding ``CBAM(x)`` call left behind (see ``CBAM.forward``): SmaAt-UNet's
-        ``cbamN(x)`` -> ``downN(x)`` (models/SmaAt_UNet.py:42-50), UNetAttention's (unet_precip_regression_lightning.py:68-77)."""
+        ``cbamN(x)`` -> ``downN(x)`` (models/SmaAt_UNet.py:42-50), UNetAttention's (unet_precip_regression_lightning.py:68-77).
+        ``run_kw`` goes to the double conv's ``run`` (DownDS: ``with_maxpool`` / ``pooled_dtype``, DoubleConvDS.run)."""
         if pooled is None:
             pooled = _take_stashed_maxpool(x)
         if pooled is None:
@@ -395,7 +424,7 @@ class _Down(nn.Module):
                 pooled = MaxPool2Fn.apply(x) if x.requires_grad else ops.maxpool2(x)
             else:
                 pooled = ops.maxpool2(x)
-        return self.maxpool_conv[1].run(pooled)
+        return self.maxpool_conv[1].run(pooled, **run_kw)
 
 
 class DownDS(_Down):

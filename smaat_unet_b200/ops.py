@@ -323,6 +323,40 @@ def dsconv_cbam(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None
     return (y, psum, pmax, pooled) if pools else y
 
 
+def dsconv_maxpool_takes(x, x1, pw_weight, k, mode=None) -> bool:
+    """True when ``dsconv_maxpool`` runs on these inputs: a fused instance with the staged epilogue
+    (smaat_dsconv_maxpool_eligible) in the arithmetic mode, and set_fused_dsconv(True)."""
+    mode = mode or _pw_mode
+    if not _fuse_ds or PW_MODES[mode] == 0:
+        return False
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
+    w2d = _pw_matrix(pw_weight)
+    return bool(_lib.load().smaat_dsconv_maxpool_eligible(_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2],
+                                                          x.shape[3], k, w2d.shape[0], PW_MODES[mode]))
+
+
+def dsconv_maxpool(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, mode=None, w_split=None):
+    """``dsconv`` that also returns MaxPool2d(2) of its output from the epilogue (smaat_dsconv_maxpool_fwd): (y, pooled), pooled
+    bit for bit the max-pool of y, without a second read of y.  None where ``dsconv_maxpool_takes`` is False (the caller then
+    runs ``dsconv`` and ``maxpool2``)."""
+    mode = mode or _pw_mode
+    if not dsconv_maxpool_takes(x, x1, pw_weight, k, mode):
+        return None
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1)
+    B, C0, H, W = x.shape
+    Cin = C0 + C1
+    w2d = _pw_matrix(pw_weight, k, Cin)
+    Cout, K = w2d.shape
+    w2d, wlo = weight_operands(w2d, PW_MODES[mode], w_split)
+    y = torch.empty((B, Cout, H, W), device=x.device, dtype=torch.float32)
+    pooled = torch.empty((B, Cout, H // 2, W // 2), device=x.device, dtype=torch.float32)
+    _call(f"smaat_dsconv_maxpool_fwd[C{Cin}_N{Cout}_S{H}]", 4 * B * H * W * (Cin + Cout) + 4 * K * Cout + 4 * pooled.numel(),
+          2 * B * H * W * K * (Cout + 9), _lib.load().smaat_dsconv_maxpool_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1,
+          _ptr(_dense(dw_weight, "depthwise.weight")), _ptr(dw_bias), _ptr(w2d), _ptr(wlo), _ptr(scale), _ptr(shift), _ptr(y),
+          Cout * H * W, _ptr(pooled), B, H, W, k, Cout, int(bool(relu)), PW_MODES[mode], _stream())
+    return y, pooled
+
+
 def dsconv(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, mode=None, w_split=None, stats=None, outconv=None):
     """Fused DepthwiseSeparableConv (layers.py:47-50) + affine (+ReLU); returns None when the fused kernel
     does not take this shape/mode (caller then runs dw3x3 + pw1x1).  ``outconv=(weight (1, Cout[,1,1]), bias or None)``
@@ -450,6 +484,37 @@ def dsconv_bf16(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None
           _ptr(dw_bias), _ptr(pack), _ptr(scale), _ptr(shift), _ptr(y), Cout * H * W, _ptr(sc), _ptr(sa), B, H, W, k, Cout,
           int(bool(relu)), _stream())
     return y
+
+
+def dsconv_maxpool_bf16_takes(x, x1, pw_weight, k) -> bool:
+    """True when ``dsconv_maxpool_bf16`` takes bf16 x [, x1] (smaat_dsconv_maxpool_bf16_eligible); set_fused_dsconv(False)
+    declines it too."""
+    if not _fuse_ds:
+        return False
+    x, bs0, x1, C1, bs1 = _concat_operands(x, x1, bf16=True)
+    w2d = _pw_matrix(pw_weight)
+    return bool(_lib.load().smaat_dsconv_maxpool_bf16_eligible(_ptr(x), x.shape[1], bs0, _ptr(x1), C1, bs1, _ptr(w2d), x.shape[2],
+                                                               x.shape[3], k, w2d.shape[0]))
+
+
+def dsconv_maxpool_bf16(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, x1=None, w_split=None, pooled_dtype=torch.bfloat16):
+    """``dsconv_bf16`` that also returns MaxPool2d(2) of its bf16 output (smaat_dsconv_maxpool_bf16_fwd): (y, pooled), pooled in
+    ``pooled_dtype`` (bfloat16 or float32, the dtype of the level it feeds), bit for bit the max-pool of y.  Raises where
+    ``dsconv_maxpool_bf16_takes`` is False."""
+    if pooled_dtype not in (torch.bfloat16, torch.float32):
+        raise ValueError(f"smaat_unet_b200: pooled_dtype must be torch.bfloat16 or torch.float32, got {pooled_dtype}")
+    if not dsconv_maxpool_bf16_takes(x, x1, pw_weight, k):
+        raise RuntimeError("smaat_unet_b200: the bf16 DS conv with the max-pool epilogue does not take this request (k = 1 or 2, W "
+                           "a multiple of 8, the register A form, set_fused_dsconv(True))")
+    x, bs0, x1, C1, bs1, B, C0, H, W, Cin, Cout, pack, dw_w = _ds_bf16_args(x, x1, dw_weight, k, pw_weight, w_split)
+    y = torch.empty((B, Cout, H, W), device=x.device, dtype=torch.bfloat16)
+    pooled = torch.empty((B, Cout, H // 2, W // 2), device=x.device, dtype=pooled_dtype)
+    _call(f"smaat_dsconv_maxpool_bf16_fwd[C{Cin}_N{Cout}_S{H}]",
+          2 * B * H * W * (Cin + Cout) + 2 * k * Cin * Cout + pooled.element_size() * pooled.numel(), 2 * B * H * W * k * Cin * (Cout + 9),
+          _lib.load().smaat_dsconv_maxpool_bf16_fwd, _ptr(x), C0, bs0, _ptr(x1), C1, bs1, _ptr(dw_w), _ptr(dw_bias), _ptr(pack),
+          _ptr(scale), _ptr(shift), _ptr(y), Cout * H * W, _ptr(pooled), int(pooled_dtype == torch.bfloat16), B, H, W, k, Cout,
+          int(bool(relu)), _stream())
+    return y, pooled
 
 
 def dsconv_head_bf16(x, dw_weight, dw_bias, k, pw_weight, scale, shift, relu, oc_weight, oc_bias, head, w_split=None):
