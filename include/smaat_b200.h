@@ -318,6 +318,25 @@ int smaat_mse_metrics_fwd(const float* pred, const float* target, int64_t n, flo
                           int denormalize, double* batch_acc, float* dpred, float grad_scale, void* stream);
 int smaat_metrics_commit(const double* batch_acc, double* totals, int batch_size, int denormalize, void* stream);
 
+/* ---- PrecipitationMetrics for several thresholds at once, every image as a batch of one (test-set evaluation) ------
+ * smaat_precip_sweep_fwd: B images of P pixels.  Image b of pred starts at pred + b * pred_bstride (pred_bstride >= P
+ *   when B > 1: a model's (B, 1, H, W) output has stride P, the last frame x[:, C-1] of a (B, C, H, W) input stride C * P);
+ *   target (B, P) dense.  thresholds: T HOST floats, strictly increasing, 1 <= T <= 32 (else SMAAT_E_BADARG before any
+ *   launch).  A value's bin is #{i : (v * factor) * 12 > thresholds[i]} in fp32 (v * 12 when denormalize == 0), the
+ *   comparison of smaat_mse_metrics_fwd.  Both outputs are overwritten:
+ *   per_image (B, 3) double: sum (p-y)^2, sum (p*f-y*f)^2, number of NaNs in p or y;
+ *   hist (B, T+1, T+1) uint32: hist[b][a][c] = pixels of image b with target bin a and pred bin c.  At threshold i,
+ *   TP = sum_{a>=i, c>=i}, FN = sum_{a>=i, c<i}, FP = sum_{a<i, c>=i}, TN = sum_{a<i, c<i}.
+ *   128-bit loads when pred, target, pred_bstride and P allow (16-byte aligned images), a scalar kernel otherwise.
+ * smaat_precip_sweep_commit folds the B images into totals (double[5 + (T+1)^2]: total_loss, total_loss_denorm,
+ *   total_samples, total_pixels, images skipped, then the summed histogram) as B batches of one: an image with a NaN
+ *   adds nothing but one skipped image (metric/precipitation_metrics.py:46-48 at batch size 1); the others add their
+ *   sums (the denormalised one only when denormalize != 0), 1 sample, P pixels and their histogram. */
+int smaat_precip_sweep_fwd(const float* pred, int64_t pred_bstride, const float* target, int B, int64_t P, float factor,
+                           const float* thresholds, int T, int denormalize, double* per_image, unsigned* hist, void* stream);
+int smaat_precip_sweep_commit(const double* per_image, const unsigned* hist, int B, int64_t P, int T, int denormalize,
+                              double* totals, void* stream);
+
 /* ---- multi-class cross-entropy + confusion matrix of one segmentation step, one pass, no host sync ----------------
  * Replaces nn.CrossEntropyLoss() of train_SmaAtUNet.py:54,182 (log_softmax + nll_loss) and the per-batch host histogram
  * behind metric.iou.IoU.add (metric/iou.py:38-62, metric/confusionmatrix.py:40-69).

@@ -71,6 +71,8 @@ SIGNATURES = {
     "smaat_cbam_mlp_bwd": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p],
     "smaat_mse_metrics_fwd": [_p, _p, _l, _f, _f, _i, _p, _p, _f, _p],
     "smaat_metrics_commit": [_p, _p, _i, _i, _p],
+    "smaat_precip_sweep_fwd": [_p, _l, _p, _i, _l, _f, _p, _i, _i, _p, _p, _p],
+    "smaat_precip_sweep_commit": [_p, _p, _i, _l, _i, _i, _p, _p],
     "smaat_ce_fwd": [_p, _p, _i, _i, _l, _l, _i, _p, _p, _p, _p],
     "smaat_confusion_add": [_p, _p, _l, _i, _p, _p, _p],
     "smaat_cross_entropy_fwd": [_p, _p, _p, _p, _i, _i, _l, _f, _l, _i, _p, _p, _p, _p, _p],

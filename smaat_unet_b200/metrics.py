@@ -6,16 +6,20 @@ Host-side mirror of the reference's interface for this step:
     arguments, ``update(preds, target)``, ``compute()`` keys, ``reset()``, ``total_*`` state names)
   * ``step_loss(y_pred, y_true, metrics)`` -- what training_step/validation_step do (loss_func + metrics.update,
     regression_lightning.py:67-88) fused into ONE pass that also writes the loss gradient.
+  * ``PrecipitationMetricsSweep``        -- PrecipitationMetrics for up to 32 thresholds at once, every sample a batch of
+    one (test-set evaluation, ``evaluate.py``; ``smaat_precip_sweep_fwd`` / ``smaat_precip_sweep_commit``).
 The arithmetic is ``smaat_mse_metrics_fwd`` / ``smaat_metrics_commit`` (include/smaat_b200.h).  The reference's NaN
 guard (`if torch.isnan(...).any()`: a device->host sync every step, precipitation_metrics.py:46) is evaluated on the
 device: a batch containing NaN is not added to the totals, and ``skipped_batches`` counts them.
 """
 from __future__ import annotations
 
+import ctypes as C
+
 import torch
 
 from . import _lib
-from .ops import _call, _dense, _ptr, _stream
+from .ops import _call, _dense, _nchw_bstride, _ptr, _stream
 
 FACTOR = 47.83  # precipitation_metrics.py:23
 
@@ -148,6 +152,122 @@ class PrecipitationMetrics:
 
     def __call__(self, preds, target):
         self.update(preds, target)
+
+
+MAX_SWEEP_THRESHOLDS = 32
+
+
+class PrecipitationMetricsSweep:
+    """``PrecipitationMetrics`` for several thresholds at once, counting every sample as its own batch of one.
+
+    Each ``update`` is one pass over the batch (``smaat_precip_sweep_fwd``): per image, the two squared-error sums, a NaN
+    count and a joint (target bin, prediction bin) histogram over the thresholds, from which every threshold's confusion
+    matrix follows exactly.  ``smaat_precip_sweep_commit`` then adds the images one by one to totals that stay on the
+    device (no host synchronisation per batch).
+
+    Why a batch of one: the reference's ``PrecipitationMetrics.update`` adds ``mse_loss(sum) / batch_size`` to
+    ``total_loss`` and ``batch_size`` to ``total_samples`` (metric/precipitation_metrics.py:62-64), and ``compute()``
+    divides by ``total_samples`` again (:105), so ``mse``, ``mse_denorm`` and ``mse_pixel`` come out B times smaller when
+    it is fed batches of B.  Its NaN guard drops the whole update (:46-48), good samples included.  The published figures
+    use batch size 1 (calc_metrics_test_set.py:95).  Here a batch of B gives exactly what B batch-1 updates of
+    ``PrecipitationMetrics(threshold=t)`` give, for every threshold t: each image adds its sums, 1 sample, its pixels and
+    its counts, and an image containing NaN adds nothing and is counted in ``skipped_images``.
+
+    ``thresholds``: 1 to 32 strictly increasing values in mm/h, compared in fp32 as the reference does.  ``compute()``
+    returns ``{threshold: dict}`` with the reference's ten keys (``compute_from_totals``)."""
+
+    def __init__(self, thresholds, denormalize=True, device="cuda"):
+        th = tuple(float(t) for t in thresholds)
+        th32 = [float(torch.tensor(t, dtype=torch.float32)) for t in th]
+        if not 1 <= len(th) <= MAX_SWEEP_THRESHOLDS or any(not a < b for a, b in zip(th32, th32[1:])) or any(t != t for t in th):
+            raise ValueError(f"PrecipitationMetricsSweep: thresholds must be 1..{MAX_SWEEP_THRESHOLDS} strictly increasing "
+                             f"values (in float32), got {th}")
+        self.thresholds = th
+        self.denormalize = denormalize
+        self.factor = FACTOR
+        self._thr = (C.c_float * len(th))(*th32)
+        cells = (len(th) + 1) ** 2
+        self._totals = torch.zeros(5 + cells, device=device, dtype=torch.float64)
+
+    def to(self, device):
+        self._totals = self._totals.to(device)
+        return self
+
+    def reset(self):
+        self._totals.zero_()
+
+    def totals_snapshot(self):
+        return self._totals.clone()
+
+    def load_totals(self, snap):
+        self._totals.copy_(snap)
+
+    @property
+    def total_samples(self):
+        return self._totals[2].to(torch.int64)
+
+    @property
+    def total_pixels(self):
+        return self._totals[3].to(torch.int64)
+
+    @property
+    def skipped_images(self):
+        return self._totals[4].to(torch.int64)
+
+    def _sweep(self, pred, pred_bstride, target, B, P):
+        T = len(self.thresholds)
+        per_image = torch.empty((B, 3), device=target.device, dtype=torch.float64)
+        hist = torch.empty((B, T + 1, T + 1), device=target.device, dtype=torch.int32)
+        lib = _lib.load()
+        _call("smaat_precip_sweep_fwd", 8 * B * P, 0, lib.smaat_precip_sweep_fwd, pred, int(pred_bstride), _ptr(target), B, P,
+              float(self.factor), self._thr, T, int(bool(self.denormalize)), _ptr(per_image), _ptr(hist), _stream())
+        _call("smaat_precip_sweep_commit", 0, 0, lib.smaat_precip_sweep_commit, _ptr(per_image), _ptr(hist), B, P, T,
+              int(bool(self.denormalize)), _ptr(self._totals), _stream())
+
+    def update(self, preds, target):
+        """Add a batch of model outputs (B, 1, H, W) (or any shape the reference's update reconciles with target) against
+        target (B, H, W), every image as a batch of one."""
+        target = _check(target.detach(), "target")
+        preds = _check(_match_shapes(preds.detach(), target), "preds")
+        B = target.size(0)
+        P = target.numel() // B
+        self._sweep(_ptr(preds), P, target, B, P)
+
+    def update_persistence(self, x, target):
+        """The persistence baseline's update (regression_lightning.py:202-204: the prediction is the input's last frame
+        ``x[:, -1:]``), read in place from x (B, C, H, W) with batch stride C * H * W: no copy of the frame."""
+        target = _check(target.detach(), "target")
+        x, bstride = _nchw_bstride(x.detach(), "x")
+        B, Cc, H, W = x.shape
+        if target.shape != (B, H, W):
+            raise RuntimeError(f"smaat metrics: persistence input {tuple(x.shape)} and target {tuple(target.shape)} do not match")
+        self._sweep(x.data_ptr() + (Cc - 1) * H * W * x.element_size(), bstride, target, B, H * W)
+
+    def sync_across_ranks(self):
+        """dist_reduce_fx="sum" of every state: one all-reduce of the totals."""
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            dist.all_reduce(self._totals, op=dist.ReduceOp.SUM)
+
+    def threshold_totals(self):
+        """``{threshold: totals}`` in ``PrecipitationMetrics``' layout (float64 CPU: total_loss, total_loss_denorm,
+        total_samples, total_pixels, TN, FP, FN, TP, skipped images); one device->host copy."""
+        t = self._totals.cpu()
+        T1 = len(self.thresholds) + 1
+        h = t[5:].to(torch.int64).view(T1, T1)          # [target bin][pred bin], exact integers
+        out = {}
+        for i, thr in enumerate(self.thresholds, start=1):
+            tp = int(h[i:, i:].sum())
+            fn = int(h[i:, :i].sum())
+            fp = int(h[:i, i:].sum())
+            tn = int(h[:i, :i].sum())
+            out[thr] = torch.tensor([float(t[0]), float(t[1]), float(t[2]), float(t[3]), tn, fp, fn, tp, float(t[4])],
+                                    dtype=torch.float64)
+        return out
+
+    def compute(self):
+        """``{threshold: dict}``: for each threshold the reference's ``compute()`` dict (precipitation_metrics.py:97-147)."""
+        return {thr: compute_from_totals(v, self.denormalize) for thr, v in self.threshold_totals().items()}
 
 
 def compute_from_totals(t, denormalize=True):

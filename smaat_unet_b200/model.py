@@ -249,6 +249,21 @@ class UNet(_ServingForward):
         return self.up4(*self._to_up4(x), outconv=self.outc, head=head)
 
 
+class PersistenceModel(_ServingForward):
+    """The persistence baseline of ``models/regression_lightning.py:202-204``: the prediction is the input's last frame,
+    ``x[:, -1:]``; no parameters.  ``metrics.PrecipitationMetricsSweep.update_persistence`` reads that frame in place, so the
+    evaluator never runs this forward.  The serving forward returns a copy of the frame, so an ``InferenceSession``'s output
+    is its own buffer rather than a view of the session's input."""
+
+    def forward(self, x):
+        return x[:, -1:, :, :]
+
+    def _serving(self, x, head):
+        if head == "logits":
+            return self(x).contiguous()
+        return apply_head(self, x, head)
+
+
 class UNetAttention(_ServingForward):
     """``models/unet_precip_regression_lightning.py:41-83``: UNet with a CBAM on every skip (178 state_dict keys with
     ``bilinear=True``).  ``downN`` runs on the un-attended map right after ``cbamN`` did, so the CBAM hands it its 2x2 max-pool.
