@@ -9,6 +9,7 @@
 //
 // One persistent CTA per SM; a tile is a PH x PW = 128-pixel patch of one image and one pass of N_TILE <= 128 output
 // channels (Cout <= 128: one pass, so the depthwise work is done exactly once; Cout in {256, 384, 512}: passes of 128).
+// At Cout <= 64 a tile can instead be two such patches one above the other, sharing each chunk (DsCfg PAIR, dsconv_pair_kernel).
 // K = k*Cin is walked in chunks of 32 depthwise channels (CC = 32/k input channels):
 //   warp 0      TMA: (PH+2) x (PW+8) x CC input halo box per chunk (OOB zero fill = padding=1; box
 //               starts at x0-4, x0-8 for bf16 input: the inner TMA coordinate must be 16-byte aligned) into an IS-deep ring;
@@ -78,41 +79,50 @@ struct DsParams {
 };
 
 constexpr int DS_MAX_CLASSES = 32;   // classes of the fused K-class OutConv + argmax (smaat_dsconv_classify_fwd)
+constexpr int DS_MIN_CLASSES = 21;   // ... that every instance keeps beside its rings (a 21-class model)
 
 // TA: the storage type of the input (x0, x1) and of the output (y or the logits): float, or uint16_t for the bf16 activations
 // of the serving forward's bf16 route (dsconv_bf16act_kernel)
-template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float>
+// PAIR (dsconv_pair_kernel: N_TILE 64, register form, tf32 / 3xTF32, k = 2 and 4): a tile is two vertically adjacent patches
+// (2 PH rows x PW, 256 pixels) that share each chunk's input box, weight chunk and barrier hand-offs; each half keeps the
+// single tile's A layout, accumulator rows and epilogue
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float, bool PAIR = false>
 struct DsCfg {
   static constexpr bool X3 = P == Prec::TF32X3;
   static constexpr int ESZ = (int)sizeof(TA);
   static_assert(ESZ == 4 || (P == Prec::BF16 && KPL != 4), "bf16 activations: the bf16 register-form instances, k = 1, 2");
   static_assert(P != Prec::BF16 || !A_SMEM, "BF16: register A form only");
+  static_assert(!PAIR || (N_TILE == 64 && !A_SMEM && P != Prec::BF16 && ESZ == 4 && KPL != 1),
+                "paired tiles: N_TILE 64, register form, tf32 / 3xTF32, fp32 maps, k = 2, 4");
   static constexpr int PH = TC_BM / PW;
+  static constexpr int NH = PAIR ? 2 : 1;                      // patches (halves) per tile
+  static constexpr int TH = NH * PH;                           // tile rows
   // input boxes start XM columns left of the patch: 16 bytes, the alignment TMA takes for the inner coordinate (4 fp32, 8 bf16)
   static constexpr int XM = 16 / ESZ;
-  static constexpr int BW = PW + 2 * XM, BH = PH + 2;
+  static constexpr int BW = PW + 2 * XM, BH = TH + 2;
   static constexpr int CC = TC_BK / KPL;                       // input channels per chunk
   static constexpr int IN_BYTES = CC * BH * BW * ESZ;          // multiple of 128 for PW in {16,32}
   static constexpr int A_BYTES = TC_BM * TC_BK * 4;            // 16 KB
   static constexpr int B_BYTES = N_TILE * TC_BK * (P == Prec::BF16 ? 2 : 4);   // 128-byte rows (bf16: 64-byte rows)
-  // A ring stage: fp32 (register form: the consumers split hi / lo after loading), or hi [+ lo] (A_SMEM: the tensor core reads
-  // the parts)
-  static constexpr int AST_BYTES = (X3 && A_SMEM ? 2 : 1) * A_BYTES;
+  // A ring stage: fp32 (register form: the consumers split hi / lo after loading; one 16 KB tile per half), or hi [+ lo]
+  // (A_SMEM: the tensor core reads the parts)
+  static constexpr int AST_BYTES = (X3 && A_SMEM ? 2 : 1) * NH * A_BYTES;
   static constexpr int BST_BYTES = (X3 ? 2 : 1) * B_BYTES;     // B ring stage: hi [+ lo]
   static constexpr int OFF_ALO = A_BYTES;
   static constexpr int OFF_BLO = B_BYTES;
   // depthwise producer groups (128 threads each), sized by the register file: the consumers hold N_TILE / 2 accumulators
-  // per thread.  NG <= AS always: the per-stage a_empty barriers are tested by phase parity, which is only unambiguous while
-  // a group can never be two hand-backs of a stage behind
-  static constexpr int NG = N_TILE > 64 ? 1 : 2;
+  // per thread (two sets in a paired tile).  NG <= AS always: the per-stage a_empty barriers are tested by phase parity, which
+  // is only unambiguous while a group can never be two hand-backs of a stage behind
+  static constexpr int NG = N_TILE > 64 || PAIR ? 1 : 2;
   // A ring and weight ring (prefetched by its own warp).  The consumers hold two stages of each (chunk i in flight, chunk i - 1
   // retiring); the producers write NG more, the weight loader runs one ahead.  The input ring gets the rest (it must stay deep
   // enough to cover HBM latency).  TF32X3 in the A_SMEM form (32 KB A stages) keeps two-deep rings at N_TILE 128: deeper ones
   // leave too little for the input ring.  BF16 takes TF32's depths: its A stages are TF32's and the four B stages cover the
   // same two in use, NG producing and one loading; the 16 / 32 KB its half-size B stages free go to the input ring and the
-  // staging buffers (the table in DESIGN §6)
-  static constexpr int AS = X3 ? (A_SMEM ? (N_TILE > 64 ? 2 : 3) : 2 + NG) : 4;
-  static constexpr int BS = X3 ? (A_SMEM && N_TILE > 64 ? 2 : 3) : 4;
+  // staging buffers (the table in DESIGN §6).  A paired tile's 32 KB A stages keep the register form's 2 + NG in both modes;
+  // in 3xTF32 at PW 16 with k = 2 (27 KB boxes of 18 rows) the B ring is 2 deep, so that the input ring keeps 2 stages
+  static constexpr int AS = X3 ? (A_SMEM ? (N_TILE > 64 ? 2 : 3) : 2 + NG) : (PAIR ? 2 + NG : 4);
+  static constexpr int BS = X3 ? (A_SMEM && N_TILE > 64 ? 2 : (PAIR && PW == 16 && KPL == 2 ? 2 : 3)) : 4;
   static constexpr int AFF_N = 512;                            // scale | shift | OutConv weights of up to 512 channels
   static constexpr int BAR_BYTES = 512;
   static constexpr int FREE = 224 * 1024 - 1024 - BAR_BYTES - 3 * AFF_N * 4 - AS * AST_BYTES - BS * BST_BYTES;
@@ -120,9 +130,10 @@ struct DsCfg {
   // input ring.  Two, so that a slice's store overlaps the staging of the next: in 3xTF32 with k = 2 the input ring goes
   // 6 -> 4 at N_TILE 64 and 4 -> 2 at N_TILE 128 (one buffer there, with a 3-deep input ring, measured 1-6 % slower per
   // layer: DESIGN §6).  Where two would leave the input ring under 2 stages one is used, and where even one would (k = 1 at
-  // N_TILE 128 in 3xTF32: 30 KB boxes), the instance keeps the direct-store epilogue (ST_BUFS = 0)
+  // N_TILE 128 in 3xTF32: 30 KB boxes), the instance keeps the direct-store epilogue (ST_BUFS = 0).  Paired tiles take one:
+  // their 25-27 KB boxes would leave the input ring under 2 stages beside two
   static constexpr int ST_BOX = 32 * 64 * ESZ;
-  static constexpr int ST_WANT = 2;
+  static constexpr int ST_WANT = PAIR ? 1 : 2;
   static constexpr int ST_BUFS = (FREE - 2 * ST_WANT * ST_BOX) / IN_BYTES >= 2 ? ST_WANT
                                  : (FREE - 2 * ST_BOX) / IN_BYTES >= 2     ? 1
                                                                            : 0;
@@ -134,7 +145,7 @@ struct DsCfg {
   // Input ring: as deep as shared memory allows, up to 8 stages, with a gate box per stage and, past the ring's end (rounded up
   // to 1 KB: OFF_A), room for the class weights of a 21-class model (MAX_CLASSES, below).  The k <= 2 instances meet both
   // with whole input boxes to spare; the 7 680 B boxes of k = 4 would not
-  static constexpr int CLS_MIN = 21 * (N_TILE + 1) * 4;
+  static constexpr int CLS_MIN = DS_MIN_CLASSES * (N_TILE + 1) * 4;
   static constexpr int RING_CLS = (FREE - ST_BYTES + 3 * 1024 - CLS_MIN) / 1024 * 1024;
   static constexpr int IS_FIT = (RING_CLS < FREE - ST_BYTES ? RING_CLS : FREE - ST_BYTES) / (IN_BYTES + SA_BYTES);
   static constexpr int IS = IS_FIT > 8 ? 8 : IS_FIT;
@@ -154,17 +165,18 @@ struct DsCfg {
   static constexpr int CLS_FIT = (227 * 1024 - TOTAL) / ((N_TILE + 1) * 4);
   static constexpr int MAX_CLASSES = CLS_FIT < DS_MAX_CLASSES ? CLS_FIT : DS_MAX_CLASSES;
   static constexpr int CLS_SMEM = MAX_CLASSES * (N_TILE + 1) * 4;
-  static_assert(MAX_CLASSES >= 21, "the class weights of a 21-class model fit beside the rings");
+  static_assert(MAX_CLASSES >= DS_MIN_CLASSES, "the class weights of a 21-class model fit beside the rings");
   static_assert(TOTAL + CLS_SMEM <= 227 * 1024, "the class weights take no shared memory from the rings");
   static constexpr uint32_t B_TX = BST_BYTES;
   static constexpr int PROD_WARP = 12;                         // first producer warp
   static constexpr int THREADS = 384 + 128 * NG;               // TMA, loader, 2 idle | 2 consumer warpgroups | producers
   // setmaxnreg split of the registers a CTA launches with (__launch_bounds__(THREADS, 1), 128 or 96 per thread): warpgroup 0
   // gives up all but REGS_TMA, the producer group gives some back at N_TILE 128 (its stencil fits in 104 without spills), the
-  // consumers (accumulators + two register-A fragment sets) take the rest: 192 at N_TILE 128, 128 at N_TILE 64
+  // consumers (accumulators + two register-A fragment sets) take the rest: 192 at N_TILE 128 and in paired tiles (two
+  // accumulator sets, two fragment sets per half), 128 at N_TILE 64
   static constexpr int REGS_LAUNCH = (65536 / THREADS) / 8 * 8;
   static constexpr int REGS_TMA = 24;
-  static constexpr int REGS_PROD = N_TILE > 64 ? 104 : REGS_LAUNCH;
+  static constexpr int REGS_PROD = N_TILE > 64 || PAIR ? 104 : REGS_LAUNCH;
   static constexpr int REGS_MMA = ((THREADS / 128 * REGS_LAUNCH - REGS_TMA - NG * REGS_PROD) / 2) / 8 * 8;
   static constexpr int REGS_SUM = REGS_TMA + 2 * REGS_MMA + NG * REGS_PROD;
   static_assert(REGS_SUM <= THREADS / 128 * REGS_LAUNCH && REGS_MMA >= REGS_LAUNCH, "register budget");
@@ -209,14 +221,14 @@ __device__ __forceinline__ void quad_transpose(float (&v)[4], int q) {
 
 // The kernel body, shared by the k = 1 / 2 instances (dsconv_fused_kernel) and the k = 4 ones (dsconv_kpl4_kernel).  The tensor
 // maps are the kernels' __grid_constant__ parameters
-template <int N_TILE, int KPL, int PW, Prec PREC, bool A_SMEM, typename TA = float>
+template <int N_TILE, int KPL, int PW, Prec PREC, bool A_SMEM, typename TA = float, bool PAIR = false>
 __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CUtensorMap& map_in1, const CUtensorMap& map_w,
                                             const CUtensorMap& map_wlo, const CUtensorMap& map_y, const CUtensorMap& map_sa,
                                             const DsParams& p) {
-  using L = DsCfg<N_TILE, KPL, PW, PREC, A_SMEM, TA>;
+  using L = DsCfg<N_TILE, KPL, PW, PREC, A_SMEM, TA, PAIR>;
   constexpr bool X3 = L::X3;
   constexpr bool BA = L::ESZ == 2;   // bf16 activations
-  constexpr int PH = L::PH, BW = L::BW, BH = L::BH, CC = L::CC, IS = L::IS, AS = L::AS, BS = L::BS;
+  constexpr int PH = L::PH, NH = L::NH, TH = L::TH, BW = L::BW, BH = L::BH, CC = L::CC, IS = L::IS, AS = L::AS, BS = L::BS;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   unsigned char* a_base = smem + L::OFF_A;
@@ -293,7 +305,7 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         int b, ty, tx, np;
         decode(tile, b, ty, tx, np);
-        const int x0 = tx * PW, y0 = ty * PH;
+        const int x0 = tx * PW, y0 = ty * TH;
         for (int i = 0; i < nch; ++i, ++gc) {
           const int s = gc % IS;
           mbar_wait(&in_empty[s], ((gc / IS) & 1u) ^ 1u);
@@ -365,9 +377,12 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       int b, ty, tx, np;
       decode(tile, b, ty, tx, np);
-      float acc[N_TILE / 2];
+      // one accumulator set per half of the tile (its 64 rows of that patch)
+      float acc[NH][N_TILE / 2];
 #pragma unroll
-      for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.f;
+      for (int h = 0; h < NH; ++h)
+#pragma unroll
+        for (int i = 0; i < N_TILE / 2; ++i) acc[h][i] = 0.f;
       // Pipelined k loop: chunk i's MMAs are issued as one group, then the wait leaves that group in flight and retires chunk
       // i - 1, whose A and B stages go back to the producers and the weight loader.
       auto release = [&](uint32_t c) {
@@ -395,10 +410,10 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
           wgmma_fence();
 #pragma unroll
           for (int kk = 0; kk < TC_BK / 8; ++kk) {
-            Wgmma<N_TILE>::ss(acc, ad0 + (uint64_t)(2 * kk), bd0 + (uint64_t)(2 * kk), 1u);
+            Wgmma<N_TILE>::ss(acc[0], ad0 + (uint64_t)(2 * kk), bd0 + (uint64_t)(2 * kk), 1u);
             if (X3) {
-              Wgmma<N_TILE>::ss(acc, al0 + (uint64_t)(2 * kk), bd0 + (uint64_t)(2 * kk), 1u);
-              Wgmma<N_TILE>::ss(acc, ad0 + (uint64_t)(2 * kk), bl0 + (uint64_t)(2 * kk), 1u);
+              Wgmma<N_TILE>::ss(acc[0], al0 + (uint64_t)(2 * kk), bd0 + (uint64_t)(2 * kk), 1u);
+              Wgmma<N_TILE>::ss(acc[0], ad0 + (uint64_t)(2 * kk), bl0 + (uint64_t)(2 * kk), 1u);
             }
           }
           wgmma_commit();
@@ -411,21 +426,24 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
         // no control-flow path may load a set whose chunk is still in flight, or ptxas serialises the MMAs: the odd tail is
         // outside the loop)
         // A commit group is KS k-steps: GPC groups per chunk.  Chunk i - 1 has retired once the first group of chunk i is
-        // issued and the wait leaves only that one in flight
+        // issued and the wait leaves only that one in flight.  A paired tile's group loads each half's fragments from that
+        // half's A tile (its own sets, alternating the same way) and issues both halves' MMAs against the same B
         constexpr int KS = L::KS, GPC = (TC_BK / 8) / KS;
         const unsigned char* ast = nullptr;
         uint64_t bd0 = 0, bl0 = 0;
-        auto group = [&](AFrags<PREC, KS>& cur, AFrags<PREC, KS>& prev, int q) {
+        auto group = [&](AFrags<PREC, KS>(&cur)[NH], AFrags<PREC, KS>(&prev)[NH], int q) {
           const int part = q % GPC;
           if (part == 0) wait_stages(ast, bd0, bl0);
-          load_a_frags<PREC, KS>(ast, part * KS, t, m0, m1, cur);
-          mma_a_frags<N_TILE, PREC, KS>(acc, cur, bd0, bl0, part * KS);
+#pragma unroll
+          for (int h = 0; h < NH; ++h) load_a_frags<PREC, KS>(ast + h * L::A_BYTES, part * KS, t, m0, m1, cur[h]);
+          mma_a_frags<N_TILE, PREC, KS, NH>(acc, cur, bd0, bl0, part * KS);
           wgmma_wait<1>();
-          wgmma_keep(prev);
+#pragma unroll
+          for (int h = 0; h < NH; ++h) wgmma_keep(prev[h]);
           if (part == 0 && q > 0) release(gc - 1);
           if (part == GPC - 1) ++gc;
         };
-        AFrags<PREC, KS> fa, fb;
+        AFrags<PREC, KS> fa[NH], fb[NH];
         const int ngrp = nch * GPC;
         int q = 0;
         for (; q + 1 < ngrp; q += 2) {
@@ -434,232 +452,241 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
         }
         if (q < ngrp) group(fa, fb, q);
         wgmma_wait0();
-        wgmma_keep(fa);
-        wgmma_keep(fb);
+#pragma unroll
+        for (int h = 0; h < NH; ++h) {
+          wgmma_keep(fa[h]);
+          wgmma_keep(fb[h]);
+        }
       }
       // the tile's last chunk has retired; its stages are released before the epilogue, so that TMA, the weight loader and
       // the producers run on through it
-      wgmma_keep(acc);
+#pragma unroll
+      for (int h = 0; h < NH; ++h) wgmma_keep(acc[h]);
       release(gc - 1);
 
-      // ----- epilogue: rows g / g + 8 are patch pixels m0 / m1, columns n0 + 8j + 2t + {0, 1}
+      // ----- epilogue, once per half (patch rows y_org ..): rows g / g + 8 are patch pixels m0 / m1, columns n0 + 8j + 2t + {0, 1}
       const int n0 = np * N_TILE;
-      const int gy0 = ty * PH + m0 / PW, gx0 = tx * PW + m0 % PW;
-      const int gy1 = ty * PH + m1 / PW, gx1 = tx * PW + m1 % PW;
-      const bool v0 = gy0 < p.H && gx0 < p.W, v1 = gy1 < p.H && gx1 < p.W;
-      const int64_t o0 = (int64_t)gy0 * p.W + gx0, o1 = (int64_t)gy1 * p.W + gx1;
-      if (p.stats) {
-        // BatchNorm batch statistics from the RAW accumulators (one pass: Cout <= 128); patch pixels outside the image are
-        // masked (their stencil still sees the image edge), channels past Cout are exact zeros (TMA zero fill of the weight
-        // rows); the affine is applied to the sums analytically
-        const double npix = (double)((__popc(__ballot_sync(0xffffffffu, v0)) + __popc(__ballot_sync(0xffffffffu, v1))) / 4);
 #pragma unroll
-        for (int j = 0; j < N_TILE / 8; ++j) {
+      for (int h = 0; h < NH; ++h) {
+        float (&ac)[N_TILE / 2] = acc[h];
+        const int y_org = ty * TH + h * PH;
+        const int gy0 = y_org + m0 / PW, gx0 = tx * PW + m0 % PW;
+        const int gy1 = y_org + m1 / PW, gx1 = tx * PW + m1 % PW;
+        const bool v0 = gy0 < p.H && gx0 < p.W, v1 = gy1 < p.H && gx1 < p.W;
+        const int64_t o0 = (int64_t)gy0 * p.W + gx0, o1 = (int64_t)gy1 * p.W + gx1;
+        if (p.stats) {
+          // BatchNorm batch statistics from the RAW accumulators (one pass: Cout <= 128); patch pixels outside the image are
+          // masked (their stencil still sees the image edge), channels past Cout are exact zeros (TMA zero fill of the weight
+          // rows); the affine is applied to the sums analytically
+          const double npix = (double)((__popc(__ballot_sync(0xffffffffu, v0)) + __popc(__ballot_sync(0xffffffffu, v1))) / 4);
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const float a = v0 ? acc[4 * j + e] : 0.f, bb = v1 ? acc[4 * j + 2 + e] : 0.f;
-            const float s1 = frag_colsum(a + bb), s2 = frag_colsum(fmaf(a, a, bb * bb));
-            const int c = 8 * j + 2 * t + e;
-            if (lane < 4 && c < p.Cout) {
-              const double sc = (double)aff[c], sh = (double)aff[L::AFF_N + c];
-              atomicAdd(p.stats + c, sc * (double)s1 + npix * sh);
-              atomicAdd(p.stats + p.Cout + c, sc * sc * (double)s2 + 2.0 * sc * sh * (double)s1 + npix * sh * sh);
+          for (int j = 0; j < N_TILE / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float a = v0 ? ac[4 * j + e] : 0.f, bb = v1 ? ac[4 * j + 2 + e] : 0.f;
+              const float s1 = frag_colsum(a + bb), s2 = frag_colsum(fmaf(a, a, bb * bb));
+              const int c = 8 * j + 2 * t + e;
+              if (lane < 4 && c < p.Cout) {
+                const double sc = (double)aff[c], sh = (double)aff[L::AFF_N + c];
+                atomicAdd(p.stats + c, sc * (double)s1 + npix * sh);
+                atomicAdd(p.stats + p.Cout + c, sc * sc * (double)s2 + 2.0 * sc * sh * (double)s1 + npix * sh * sh);
+              }
             }
           }
         }
-      }
-      if (p.ncls) {
-        // K-class OutConv + argmax.  The activations replace the accumulators in place (fmaxf(fmaf(acc, sc, sh), act_lo), as
-        // below); then, one class at a time, the one-class dot product below in its order (fmaf over the thread's channels, the
-        // two xor shuffles, + bias), so class j's logit is bit for bit what that epilogue writes with OutConv row j.  After the
-        // butterfly all 4 lanes of a fragment group hold the same logits; each keeps the same running (max, first index) per
-        // pixel -- torch.argmax's rule: a NaN wins and stays -- so the registers hold two logits whatever K is.  A lane's two
-        // channels 2t, 2t + 1 of a fragment column are one 8-byte shared-memory load (the 8 fragment groups read the same
-        // address: a broadcast, conflict-free).  Logit stores rotate over the 4 lanes
+        if (p.ncls) {
+          // K-class OutConv + argmax.  The activations replace the accumulators in place (fmaxf(fmaf(acc, sc, sh), act_lo), as
+          // below); then, one class at a time, the one-class dot product below in its order (fmaf over the thread's channels, the
+          // two xor shuffles, + bias), so class j's logit is bit for bit what that epilogue writes with OutConv row j.  After the
+          // butterfly all 4 lanes of a fragment group hold the same logits; each keeps the same running (max, first index) per
+          // pixel -- torch.argmax's rule: a NaN wins and stays -- so the registers hold two logits whatever K is.  A lane's two
+          // channels 2t, 2t + 1 of a fragment column are one 8-byte shared-memory load (the 8 fragment groups read the same
+          // address: a broadcast, conflict-free).  Logit stores rotate over the 4 lanes
 #pragma unroll
-        for (int j = 0; j < N_TILE / 8; ++j) {
+          for (int j = 0; j < N_TILE / 8; ++j) {
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int c = 8 * j + 2 * t + e;
-            const float sc = aff[c], sh = aff[L::AFF_N + c];
-            acc[4 * j + e] = fmaxf(fmaf(acc[4 * j + e], sc, sh), act_lo);
-            acc[4 * j + 2 + e] = fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo);
+            for (int e = 0; e < 2; ++e) {
+              const int c = 8 * j + 2 * t + e;
+              const float sc = aff[c], sh = aff[L::AFF_N + c];
+              ac[4 * j + e] = fmaxf(fmaf(ac[4 * j + e], sc, sh), act_lo);
+              ac[4 * j + 2 + e] = fmaxf(fmaf(ac[4 * j + 2 + e], sc, sh), act_lo);
+            }
           }
-        }
-        float best0 = -INFINITY, best1 = -INFINITY;
-        int arg0 = 0, arg1 = 0;
+          float best0 = -INFINITY, best1 = -INFINITY;
+          int arg0 = 0, arg1 = 0;
 #pragma unroll 1
-        for (int cl = 0; cl < p.ncls; ++cl) {
-          const float* wr = cls_w + cl * N_TILE + 2 * t;   // zero past Cout, where the activation is 0 too
+          for (int cl = 0; cl < p.ncls; ++cl) {
+            const float* wr = cls_w + cl * N_TILE + 2 * t;   // zero past Cout, where the activation is 0 too
+            float d0 = 0.f, d1 = 0.f;
+#pragma unroll
+            for (int j = 0; j < N_TILE / 8; ++j) {
+              const float2 w = *reinterpret_cast<const float2*>(wr + 8 * j);
+              d0 = fmaf(ac[4 * j], w.x, d0);
+              d1 = fmaf(ac[4 * j + 2], w.x, d1);
+              d0 = fmaf(ac[4 * j + 1], w.y, d0);
+              d1 = fmaf(ac[4 * j + 3], w.y, d1);
+            }
+            d0 += __shfl_xor_sync(0xffffffffu, d0, 1);
+            d0 += __shfl_xor_sync(0xffffffffu, d0, 2);
+            d1 += __shfl_xor_sync(0xffffffffu, d1, 1);
+            d1 += __shfl_xor_sync(0xffffffffu, d1, 2);
+            const float ob = cls_b[cl];
+            const float l0 = d0 + ob, l1 = d1 + ob;
+            if (best0 == best0 && (l0 > best0 || l0 != l0)) { best0 = l0; arg0 = cl; }
+            if (best1 == best1 && (l1 > best1 || l1 != l1)) { best1 = l1; arg1 = cl; }
+            if (p.oc_y && t == (cl & 3)) {
+              TA* yk = reinterpret_cast<TA*>(p.oc_y) + ((int64_t)b * p.ncls + cl) * P;
+              if (v0) st_act(yk + o0, l0);
+              if (v1) st_act(yk + o1, l1);
+            }
+          }
+          if (p.cls) {
+            if (v0 && t == 0) p.cls[(int64_t)b * P + o0] = arg0;
+            if (v1 && t == 1) p.cls[(int64_t)b * P + o1] = arg1;
+          }
+        } else if (p.oc_y) {
+          // fused OutConv: each pixel's dot product over all Cout <= N_TILE activations.  Channels past Cout have zero
+          // accumulators, identity affine and zero OutConv weight: no mask needed
           float d0 = 0.f, d1 = 0.f;
 #pragma unroll
           for (int j = 0; j < N_TILE / 8; ++j) {
-            const float2 w = *reinterpret_cast<const float2*>(wr + 8 * j);
-            d0 = fmaf(acc[4 * j], w.x, d0);
-            d1 = fmaf(acc[4 * j + 2], w.x, d1);
-            d0 = fmaf(acc[4 * j + 1], w.y, d0);
-            d1 = fmaf(acc[4 * j + 3], w.y, d1);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = 8 * j + 2 * t + e;
+              const float sc = aff[c], sh = aff[L::AFF_N + c], w = aff[2 * L::AFF_N + c];
+              d0 = fmaf(fmaxf(fmaf(ac[4 * j + e], sc, sh), act_lo), w, d0);
+              d1 = fmaf(fmaxf(fmaf(ac[4 * j + 2 + e], sc, sh), act_lo), w, d1);
+            }
           }
           d0 += __shfl_xor_sync(0xffffffffu, d0, 1);
           d0 += __shfl_xor_sync(0xffffffffu, d0, 2);
           d1 += __shfl_xor_sync(0xffffffffu, d1, 1);
           d1 += __shfl_xor_sync(0xffffffffu, d1, 2);
-          const float ob = cls_b[cl];
-          const float l0 = d0 + ob, l1 = d1 + ob;
-          if (best0 == best0 && (l0 > best0 || l0 != l0)) { best0 = l0; arg0 = cl; }
-          if (best1 == best1 && (l1 > best1 || l1 != l1)) { best1 = l1; arg1 = cl; }
-          if (p.oc_y && t == (cl & 3)) {
-            TA* yk = reinterpret_cast<TA*>(p.oc_y) + ((int64_t)b * p.ncls + cl) * P;
-            if (v0) st_act(yk + o0, l0);
-            if (v1) st_act(yk + o1, l1);
+          const float ob = p.oc_b ? __ldg(p.oc_b) : 0.f;
+          if (t == 0) {
+            TA* oy = reinterpret_cast<TA*>(p.oc_y) + (int64_t)b * P;
+            if (v0) st_act(oy + o0, d0 + ob);
+            if (v1) st_act(oy + o1, d1 + ob);
           }
-        }
-        if (p.cls) {
-          if (v0 && t == 0) p.cls[(int64_t)b * P + o0] = arg0;
-          if (v1 && t == 1) p.cls[(int64_t)b * P + o1] = arg1;
-        }
-      } else if (p.oc_y) {
-        // fused OutConv: each pixel's dot product over all Cout <= N_TILE activations.  Channels past Cout have zero
-        // accumulators, identity affine and zero OutConv weight: no mask needed
-        float d0 = 0.f, d1 = 0.f;
+        } else if (L::ST_BUFS) {
+          // One 32-channel slice at a time: wait until the buffer's previous store has been read out, stage the slice (the same
+          // fmaxf(fmaf(acc, sc, sh), act_lo) as the direct stores: bit-identical), hand it to the async proxy and store it as
+          // one box.  TMA clips what lies outside W, H or Cout; slices wholly past Cout are skipped
+          const int y_half = y_org + wg * (PH / 2);
 #pragma unroll
-        for (int j = 0; j < N_TILE / 8; ++j) {
+          for (int s = 0; s < N_TILE / 32; ++s) {
+            if (n0 + 32 * s >= p.Cout) break;
+            const uint32_t buf = st_base + (st_n % L::ST_BUFS) * L::ST_BOX;
+            if (st_leader) bulk_wait_read<L::ST_BUFS - 1>();
+            wg_sync(2 + wg);
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int c = 8 * j + 2 * t + e;
-            const float sc = aff[c], sh = aff[L::AFF_N + c], w = aff[2 * L::AFF_N + c];
-            d0 = fmaf(fmaxf(fmaf(acc[4 * j + e], sc, sh), act_lo), w, d0);
-            d1 = fmaf(fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo), w, d1);
-          }
-        }
-        d0 += __shfl_xor_sync(0xffffffffu, d0, 1);
-        d0 += __shfl_xor_sync(0xffffffffu, d0, 2);
-        d1 += __shfl_xor_sync(0xffffffffu, d1, 1);
-        d1 += __shfl_xor_sync(0xffffffffu, d1, 2);
-        const float ob = p.oc_b ? __ldg(p.oc_b) : 0.f;
-        if (t == 0) {
-          TA* oy = reinterpret_cast<TA*>(p.oc_y) + (int64_t)b * P;
-          if (v0) st_act(oy + o0, d0 + ob);
-          if (v1) st_act(oy + o1, d1 + ob);
-        }
-      } else if (L::ST_BUFS) {
-        // One 32-channel slice at a time: wait until the buffer's previous store has been read out, stage the slice (the same
-        // fmaxf(fmaf(acc, sc, sh), act_lo) as the direct stores: bit-identical), hand it to the async proxy and store it as
-        // one box.  TMA clips what lies outside W, H or Cout; slices wholly past Cout are skipped
-        const int y_half = ty * PH + wg * (PH / 2);
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * s + jj;
+              float v[4];
 #pragma unroll
-        for (int s = 0; s < N_TILE / 32; ++s) {
-          if (n0 + 32 * s >= p.Cout) break;
-          const uint32_t buf = st_base + (st_n % L::ST_BUFS) * L::ST_BOX;
-          if (st_leader) bulk_wait_read<L::ST_BUFS - 1>();
-          wg_sync(2 + wg);
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int j = 4 * s + jj;
-            float v[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) v[q] = (t & 2) ? acc[4 * j + (q ^ 2)] : acc[4 * j + q];
-            quad_transpose(v, quad);
-            const int c = n0 + 8 * j + st_ch;
-            const float sc = aff[c], sh = aff[L::AFF_N + c];
-            const float4 o = make_float4(fmaxf(fmaf(v[0], sc, sh), act_lo), fmaxf(fmaf(v[1], sc, sh), act_lo),
-                                         fmaxf(fmaf(v[2], sc, sh), act_lo), fmaxf(fmaf(v[3], sc, sh), act_lo));
-            if constexpr (BA) {
-              asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(buf + st_off + 1024u * jj), "r"(f32x2_bf16x2(o.x, o.y)),
-                           "r"(f32x2_bf16x2(o.z, o.w))
-                           : "memory");
-            } else {
-              asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(buf + st_off + 2048u * jj), "f"(o.x), "f"(o.y),
-                           "f"(o.z), "f"(o.w)
-                           : "memory");
-            }
-          }
-          fence_proxy_async_smem();
-          wg_sync(2 + wg);
-          if (st_leader) {
-            tma_store_4d(&map_y, buf, tx * PW, y_half, n0 + 32 * s, b);
-            bulk_commit();
-          }
-          if (p.pooled) {
-            // The next level's MaxPool2d(2) [and the CBAM channel gate's pools: pool_sum, fp32 maps only], read back from the
-            // staged slice (the stored values bit for bit -- bf16 boxes hold the rounded values, and the max of bf16 values is
-            // one of them; the store reads the buffer too, and nothing writes it before the next wg_sync).  4 threads per
-            // channel, 2 items each: an item is 4 columns of a row pair, i.e. two 2 x 2 windows (the half-patch origin is even
-            // and PH / 2 is even, so no window straddles it).  Pixels outside H or W are masked; an odd last row goes into the
-            // pools but not the max-pool (floor, as MaxPool2d)
-            const bool parts = !BA && p.pool_sum;
-            const int pt = threadIdx.x & 127, pch = pt >> 2, pq = pt & 3;
-            const int c = n0 + 32 * s + pch;
-            float psum = 0.f, pmax = -INFINITY;
-#pragma unroll
-            for (int it = 0; it < 2; ++it) {
-              constexpr int NQ = PW / 4;
-              const int item = pq + 4 * it, rp = item / NQ, qd = item % NQ;   // lanes pq = 0..3: 4 adjacent items, 32 B of max-pool
-              const int px = 2 * rp * PW + 4 * qd;
-              float4 u, v;
-              if constexpr (BA) {
-                // unswizzled [channel][64 pixels] x 2 B: 4 pixels are one 8-byte load
-                const uint32_t a0 = (uint32_t)(pch * 128 + px * 2), a1 = a0 + (uint32_t)(PW * 2);
-                uint2 hu, hv;
-                asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(hu.x), "=r"(hu.y) : "r"(buf + a0));
-                asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(hv.x), "=r"(hv.y) : "r"(buf + a1));
-                u = bf16x4_f32(hu);
-                v = bf16x4_f32(hv);
-              } else {
-                const uint32_t a0 = (uint32_t)(pch * 256 + px * 4), a1 = a0 + (uint32_t)(PW * 4);
-                asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(u.x), "=f"(u.y), "=f"(u.z), "=f"(u.w)
-                             : "r"(buf + (a0 ^ (((a0 >> 7) & SW_MASK) << 4))));
-                asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-                             : "r"(buf + (a1 ^ (((a1 >> 7) & SW_MASK) << 4))));
-              }
-              const int gy = y_half + 2 * rp, gx = tx * PW + 4 * qd;      // W % 4 == 0: a quad is all in or all out
-              const bool in0 = gx < p.W && gy < p.H, in1 = gx < p.W && gy + 1 < p.H;
-              if (parts && in0) {
-                psum += (u.x + u.y) + (u.z + u.w);
-                pmax = fmaxf(pmax, fmaxf(fmaxf(u.x, u.y), fmaxf(u.z, u.w)));
-              }
-              if (in1) {
-                if (parts) {
-                  psum += (v.x + v.y) + (v.z + v.w);
-                  pmax = fmaxf(pmax, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
-                }
-                if (c < p.Cout) {
-                  const int hw = p.W >> 1;
-                  const int64_t o = ((int64_t)b * p.Cout + c) * (int64_t)(p.H >> 1) * hw + (int64_t)(gy >> 1) * hw + (gx >> 1);
-                  const float2 m2 = make_float2(fmaxf(fmaxf(u.x, u.y), fmaxf(v.x, v.y)), fmaxf(fmaxf(u.z, u.w), fmaxf(v.z, v.w)));
-                  if (BA && p.pooled_bf16)   // exact: both maxima are bf16 values
-                    *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.pooled) + o) = f32x2_bf16x2(m2.x, m2.y);
-                  else
-                    *reinterpret_cast<float2*>(p.pooled + o) = m2;
-                }
-              }
-            }
-            if (parts) {   // uniform over the CTA
-              psum += __shfl_xor_sync(0xffffffffu, psum, 1);
-              psum += __shfl_xor_sync(0xffffffffu, psum, 2);
-              pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 1));
-              pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 2));
-              if (pq == 0 && c < p.Cout) {
-                const int64_t o = ((int64_t)b * p.npart + 2 * (ty * p.tiles_x + tx) + wg) * p.Cout + c;
-                p.pool_sum[o] = psum;
-                p.pool_max[o] = pmax;
-              }
-            }
-          }
-          ++st_n;
-        }
-      } else {
-        TA* yb = reinterpret_cast<TA*>(p.y) + (int64_t)b * p.y_bstride;
-#pragma unroll
-        for (int j = 0; j < N_TILE / 8; ++j) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int c = n0 + 8 * j + 2 * t + e;
-            if (c < p.Cout) {
+              for (int q = 0; q < 4; ++q) v[q] = (t & 2) ? ac[4 * j + (q ^ 2)] : ac[4 * j + q];
+              quad_transpose(v, quad);
+              const int c = n0 + 8 * j + st_ch;
               const float sc = aff[c], sh = aff[L::AFF_N + c];
-              TA* yc = yb + (int64_t)c * P;
-              if (v0) st_act(yc + o0, fmaxf(fmaf(acc[4 * j + e], sc, sh), act_lo));
-              if (v1) st_act(yc + o1, fmaxf(fmaf(acc[4 * j + 2 + e], sc, sh), act_lo));
+              const float4 o = make_float4(fmaxf(fmaf(v[0], sc, sh), act_lo), fmaxf(fmaf(v[1], sc, sh), act_lo),
+                                           fmaxf(fmaf(v[2], sc, sh), act_lo), fmaxf(fmaf(v[3], sc, sh), act_lo));
+              if constexpr (BA) {
+                asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(buf + st_off + 1024u * jj), "r"(f32x2_bf16x2(o.x, o.y)),
+                             "r"(f32x2_bf16x2(o.z, o.w))
+                             : "memory");
+              } else {
+                asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(buf + st_off + 2048u * jj), "f"(o.x), "f"(o.y),
+                             "f"(o.z), "f"(o.w)
+                             : "memory");
+              }
+            }
+            fence_proxy_async_smem();
+            wg_sync(2 + wg);
+            if (st_leader) {
+              tma_store_4d(&map_y, buf, tx * PW, y_half, n0 + 32 * s, b);
+              bulk_commit();
+            }
+            if (p.pooled) {
+              // The next level's MaxPool2d(2) [and the CBAM channel gate's pools: pool_sum, fp32 maps only], read back from the
+              // staged slice (the stored values bit for bit -- bf16 boxes hold the rounded values, and the max of bf16 values is
+              // one of them; the store reads the buffer too, and nothing writes it before the next wg_sync).  4 threads per
+              // channel, 2 items each: an item is 4 columns of a row pair, i.e. two 2 x 2 windows (the half-patch origin is even
+              // and PH / 2 is even, so no window straddles it).  Pixels outside H or W are masked; an odd last row goes into the
+              // pools but not the max-pool (floor, as MaxPool2d)
+              const bool parts = !BA && p.pool_sum;
+              const int pt = threadIdx.x & 127, pch = pt >> 2, pq = pt & 3;
+              const int c = n0 + 32 * s + pch;
+              float psum = 0.f, pmax = -INFINITY;
+#pragma unroll
+              for (int it = 0; it < 2; ++it) {
+                constexpr int NQ = PW / 4;
+                const int item = pq + 4 * it, rp = item / NQ, qd = item % NQ;   // lanes pq = 0..3: 4 adjacent items, 32 B of max-pool
+                const int px = 2 * rp * PW + 4 * qd;
+                float4 u, v;
+                if constexpr (BA) {
+                  // unswizzled [channel][64 pixels] x 2 B: 4 pixels are one 8-byte load
+                  const uint32_t a0 = (uint32_t)(pch * 128 + px * 2), a1 = a0 + (uint32_t)(PW * 2);
+                  uint2 hu, hv;
+                  asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(hu.x), "=r"(hu.y) : "r"(buf + a0));
+                  asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(hv.x), "=r"(hv.y) : "r"(buf + a1));
+                  u = bf16x4_f32(hu);
+                  v = bf16x4_f32(hv);
+                } else {
+                  const uint32_t a0 = (uint32_t)(pch * 256 + px * 4), a1 = a0 + (uint32_t)(PW * 4);
+                  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(u.x), "=f"(u.y), "=f"(u.z), "=f"(u.w)
+                               : "r"(buf + (a0 ^ (((a0 >> 7) & SW_MASK) << 4))));
+                  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+                               : "r"(buf + (a1 ^ (((a1 >> 7) & SW_MASK) << 4))));
+                }
+                const int gy = y_half + 2 * rp, gx = tx * PW + 4 * qd;      // W % 4 == 0: a quad is all in or all out
+                const bool in0 = gx < p.W && gy < p.H, in1 = gx < p.W && gy + 1 < p.H;
+                if (parts && in0) {
+                  psum += (u.x + u.y) + (u.z + u.w);
+                  pmax = fmaxf(pmax, fmaxf(fmaxf(u.x, u.y), fmaxf(u.z, u.w)));
+                }
+                if (in1) {
+                  if (parts) {
+                    psum += (v.x + v.y) + (v.z + v.w);
+                    pmax = fmaxf(pmax, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
+                  }
+                  if (c < p.Cout) {
+                    const int hw = p.W >> 1;
+                    const int64_t o = ((int64_t)b * p.Cout + c) * (int64_t)(p.H >> 1) * hw + (int64_t)(gy >> 1) * hw + (gx >> 1);
+                    const float2 m2 = make_float2(fmaxf(fmaxf(u.x, u.y), fmaxf(v.x, v.y)), fmaxf(fmaxf(u.z, u.w), fmaxf(v.z, v.w)));
+                    if (BA && p.pooled_bf16)   // exact: both maxima are bf16 values
+                      *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.pooled) + o) = f32x2_bf16x2(m2.x, m2.y);
+                    else
+                      *reinterpret_cast<float2*>(p.pooled + o) = m2;
+                  }
+                }
+              }
+              if (parts) {   // uniform over the CTA
+                psum += __shfl_xor_sync(0xffffffffu, psum, 1);
+                psum += __shfl_xor_sync(0xffffffffu, psum, 2);
+                pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 1));
+                pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 2));
+                if (pq == 0 && c < p.Cout) {
+                  const int64_t o = ((int64_t)b * p.npart + 2 * ((ty * NH + h) * p.tiles_x + tx) + wg) * p.Cout + c;
+                  p.pool_sum[o] = psum;
+                  p.pool_max[o] = pmax;
+                }
+              }
+            }
+            ++st_n;
+          }
+        } else {
+          TA* yb = reinterpret_cast<TA*>(p.y) + (int64_t)b * p.y_bstride;
+#pragma unroll
+          for (int j = 0; j < N_TILE / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = n0 + 8 * j + 2 * t + e;
+              if (c < p.Cout) {
+                const float sc = aff[c], sh = aff[L::AFF_N + c];
+                TA* yc = yb + (int64_t)c * P;
+                if (v0) st_act(yc + o0, fmaxf(fmaf(ac[4 * j + e], sc, sh), act_lo));
+                if (v1) st_act(yc + o1, fmaxf(fmaf(ac[4 * j + 2 + e], sc, sh), act_lo));
+              }
             }
           }
         }
@@ -772,39 +799,44 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
               }
               wl[0] = left; wl[1] = a.x; wl[2] = a.y; wl[3] = a.z; wl[4] = a.w; wl[5] = right;
             };
+            // a paired tile's halves: rows h PH .. of the box, into that half's A tile (the same task, weights and window)
 #pragma unroll
-            for (int r = 0; r < 2; ++r) load_row(win[r], r);
+            for (int h = 0; h < NH; ++h) {
 #pragma unroll
-            for (int rr = 0; rr < 4; ++rr) {
-              load_row(win[(rr + 2) % 3], rr + 2);
-              const float* w0 = win[rr % 3];
-              const float* w1 = win[(rr + 1) % 3];
-              const float* w2 = win[(rr + 2) % 3];
-              const int m = (r0 + rr) * PW + c0;
+              for (int r = 0; r < 2; ++r) load_row(win[r], h * PH + r);
 #pragma unroll
-              for (int kk = 0; kk < KH; ++kk) {
-                float o4[4];
+              for (int rr = 0; rr < 4; ++rr) {
+                load_row(win[(rr + 2) % 3], h * PH + rr + 2);
+                const float* w0 = win[rr % 3];
+                const float* w1 = win[(rr + 1) % 3];
+                const float* w2 = win[(rr + 2) % 3];
+                const int m = (r0 + rr) * PW + c0;
 #pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  float a = br[kk];
-                  a = fmaf(wr[kk][0], w0[j], a); a = fmaf(wr[kk][1], w0[j + 1], a); a = fmaf(wr[kk][2], w0[j + 2], a);
-                  a = fmaf(wr[kk][3], w1[j], a); a = fmaf(wr[kk][4], w1[j + 1], a); a = fmaf(wr[kk][5], w1[j + 2], a);
-                  a = fmaf(wr[kk][6], w2[j], a); a = fmaf(wr[kk][7], w2[j + 1], a); a = fmaf(wr[kk][8], w2[j + 2], a);
-                  o4[j] = a;
-                }
-                if (A_SMEM) {
-                  const int kr = ci * KPL + kr0 + kk;
+                for (int kk = 0; kk < KH; ++kk) {
+                  float o4[4];
 #pragma unroll
                   for (int j = 0; j < 4; ++j) {
-                    const uint32_t off = kmajor_offset(m + j, kr);
-                    const float h = X3 ? tf32_hi(o4[j]) : o4[j];
-                    *reinterpret_cast<float*>(my_op + off) = h;
-                    if (X3) *reinterpret_cast<float*>(my_op + L::OFF_ALO + off) = o4[j] - h;
+                    float a = br[kk];
+                    a = fmaf(wr[kk][0], w0[j], a); a = fmaf(wr[kk][1], w0[j + 1], a); a = fmaf(wr[kk][2], w0[j + 2], a);
+                    a = fmaf(wr[kk][3], w1[j], a); a = fmaf(wr[kk][4], w1[j + 1], a); a = fmaf(wr[kk][5], w1[j + 2], a);
+                    a = fmaf(wr[kk][6], w2[j], a); a = fmaf(wr[kk][7], w2[j + 1], a); a = fmaf(wr[kk][8], w2[j + 2], a);
+                    o4[j] = a;
                   }
-                  continue;
+                  if (A_SMEM) {
+                    const int kr = ci * KPL + kr0 + kk;
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                      const uint32_t off = kmajor_offset(m + j, kr);
+                      const float hi = X3 ? tf32_hi(o4[j]) : o4[j];
+                      *reinterpret_cast<float*>(my_op + off) = hi;
+                      if (X3) *reinterpret_cast<float*>(my_op + L::OFF_ALO + off) = o4[j] - hi;
+                    }
+                    continue;
+                  }
+                  // fp32 in both modes: the consumers split TF32X3's hi / lo parts after loading (one pass through shared memory)
+                  *reinterpret_cast<float4*>(my_op + h * L::A_BYTES + a_tile_offset(ci * KPL + kr0 + kk, m)) =
+                      make_float4(o4[0], o4[1], o4[2], o4[3]);
                 }
-                // fp32 in both modes: the consumers split TF32X3's hi / lo parts after loading (one pass through shared memory)
-                *reinterpret_cast<float4*>(my_op + a_tile_offset(ci * KPL + kr0 + kk, m)) = make_float4(o4[0], o4[1], o4[2], o4[3]);
               }
             }
           }
@@ -862,20 +894,32 @@ __global__ void __launch_bounds__(DsCfg<N_TILE, KPL, PW, Prec::BF16, false, uint
   dsconv_body<N_TILE, KPL, PW, Prec::BF16, false, uint16_t>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
 }
 
-template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float>
+// Paired tiles (DsCfg PAIR: two patches of PH rows per tile): N_TILE 64, the register form, tf32 / 3xTF32, k = 2 and 4.  A
+// kernel of its own, so that the single-tile kernels above keep their names and instance sets
+template <int KPL, int PW, bool X3>
+__global__ void __launch_bounds__(DsCfg<64, KPL, PW, tf32_prec(X3), false, float, true>::THREADS, 1)
+    dsconv_pair_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
+                       const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
+                       const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_sa,
+                       const DsParams p) {
+  dsconv_body<64, KPL, PW, tf32_prec(X3), false, float, true>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
+}
+
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float, bool PAIR = false>
 static auto ds_kernel() {
   static_assert(KPL == 1 || KPL == 2 || (KPL == 4 && !A_SMEM), "fused DS conv instances: k = 1, 2 (both A forms), 4 (register form)");
-  if constexpr (sizeof(TA) == 2) return dsconv_bf16act_kernel<N_TILE, KPL, PW>;
+  if constexpr (PAIR) return dsconv_pair_kernel<KPL, PW, P == Prec::TF32X3>;
+  else if constexpr (sizeof(TA) == 2) return dsconv_bf16act_kernel<N_TILE, KPL, PW>;
   else if constexpr (P == Prec::BF16) return dsconv_bf16_kernel<N_TILE, KPL, PW>;
   else if constexpr (KPL == 4) return dsconv_kpl4_kernel<N_TILE, PW, P == Prec::TF32X3>;
   else return dsconv_fused_kernel<N_TILE, KPL, PW, P == Prec::TF32X3, A_SMEM>;
 }
 
-template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float>
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float, bool PAIR = false>
 static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl,
                      const CUtensorMap& my, const CUtensorMap& msa, DsParams p, int B, cudaStream_t st) {
-  using L = DsCfg<N_TILE, KPL, PW, P, A_SMEM, TA>;
-  auto kern = ds_kernel<N_TILE, KPL, PW, P, A_SMEM, TA>();
+  using L = DsCfg<N_TILE, KPL, PW, P, A_SMEM, TA, PAIR>;
+  auto kern = ds_kernel<N_TILE, KPL, PW, P, A_SMEM, TA, PAIR>();
   // the pools and the max-pool are read back from the staging buffers: instances with the direct-store epilogue do not take them
   if (p.pooled && !L::ST_BUFS) return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools and the max-pool need the staged epilogue");
   if (p.ncls > L::MAX_CLASSES)
@@ -890,13 +934,13 @@ static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtenso
     if (r) return r;
   }
   p.tiles_x = ceil_div(p.W, PW);
-  p.tiles_y = ceil_div(p.H, L::PH);
+  p.tiles_y = ceil_div(p.H, L::TH);
   p.npass = ceil_div(p.Cout, N_TILE);
   const int64_t total = (int64_t)B * p.tiles_x * p.tiles_y * p.npass;
   SMAAT_REQUIRE(total < (1ll << 31), "dsconv: too many tiles");
   p.total_tiles = (int)total;
   p.nchunks = ceil_div(p.C0 + p.C1, L::CC);
-  p.npart = 2 * p.tiles_x * p.tiles_y;
+  p.npart = 2 * p.tiles_x * p.tiles_y * L::NH;   // per half-patch, as smaat_dsconv_pool_parts counts them
   const int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
   kern<<<grid, L::THREADS, L::TOTAL + (p.ncls ? L::CLS_SMEM : 0), st>>>(m0, m1, mw, mwl, my, msa, p);
   SMAAT_LAUNCH_CHECK("smaat_dsconv_fwd");
@@ -917,6 +961,13 @@ static int pick_pw(int H, int W) {
     }
   }
   return best <= 1.35 ? pw : 0;
+}
+
+// Paired tiles (dsconv_pair_kernel) where they are built (N_TILE 64, k = 2, 4, the register form, tf32 / 3xTF32, fp32 maps) and
+// cover the image with no more rows than single patches: an even number of patch rows.  The pair then runs the same
+// pixels with half the chunks' fixed costs (input box, weight chunk, hand-offs) per pixel
+static bool ds_pair(int n_tile, int k, int pw, int H, int mode, bool a_smem, bool bact) {
+  return n_tile == 64 && (k == 2 || k == 4) && !a_smem && !bact && mode != SMAAT_PW_BF16 && ceil_div(H, TC_BM / pw) % 2 == 0;
 }
 
 // y: the activation output, or null where it is not known yet (smaat_dsconv_eligible*) or not written (the fused OutConv).  The
@@ -1078,6 +1129,10 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   const int cc = TC_BK / k;
   const bool x3 = mode == SMAAT_PW_TF32X3;
   const bool a_smem = ds_impl() == 1;
+  // a paired tile's boxes span both patches.  Its rings leave room for the weights of DS_MIN_CLASSES classes, not always 32: more
+  // classes take the single tile
+  const bool pair = ds_pair(n_tile, k, pw, H, mode, a_smem, bact) && ncls <= DS_MIN_CLASSES;
+  const int th = pair ? 2 * ph : ph;
   const int K = k * (C0 + C1);
   // activation maps: fp32, or bf16 (bact)
   const CUtensorMapDataType adt = bact ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
@@ -1085,7 +1140,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
 
   CUtensorMap m0, m1, mw, mwl;
   const int xm = 16 / (int)esz;   // DsCfg::XM
-  const uint32_t box[4] = {(uint32_t)(pw + 2 * xm), (uint32_t)(ph + 2), (uint32_t)cc, 1u};
+  const uint32_t box[4] = {(uint32_t)(pw + 2 * xm), (uint32_t)(th + 2), (uint32_t)cc, 1u};
   {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)C0, (uint64_t)B};
     const uint64_t str[4] = {0, (uint64_t)W * esz, (uint64_t)H * W * esz, (uint64_t)x0_bstride * esz};
@@ -1129,7 +1184,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   if (gate_sa) {
     const uint64_t dims[3] = {(uint64_t)W, (uint64_t)H, (uint64_t)B};
     const uint64_t str[3] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4};
-    const uint32_t sbox[3] = {(uint32_t)(pw + 2 * xm), (uint32_t)(ph + 2), 1u};
+    const uint32_t sbox[3] = {(uint32_t)(pw + 2 * xm), (uint32_t)(th + 2), 1u};
     int r = make_tmap_f32(&msa, gate_sa, 3, dims, str, sbox, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(gate sa)");
     if (r) return r;
   }
@@ -1152,6 +1207,13 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   if (bf16) return launch_ds<NT, 4, PWv, Prec::BF16, false>(m0, m1, mw, mwl, my, msa, p, B, st);                  \
   return x3 ? launch_ds<NT, 4, PWv, Prec::TF32X3, false>(m0, m1, mw, mwl, my, msa, p, B, st)                  \
             : launch_ds<NT, 4, PWv, Prec::TF32, false>(m0, m1, mw, mwl, my, msa, p, B, st)
+#define DS_DISPATCH_PAIR(KP, PWv)                                                                                      \
+  return x3 ? launch_ds<64, KP, PWv, Prec::TF32X3, false, float, true>(m0, m1, mw, mwl, my, msa, p, B, st)                 \
+            : launch_ds<64, KP, PWv, Prec::TF32, false, float, true>(m0, m1, mw, mwl, my, msa, p, B, st)
+  if (pair) {
+    if (k == 4) { if (pw == 32) { DS_DISPATCH_PAIR(4, 32); } else { DS_DISPATCH_PAIR(4, 16); } }
+    else        { if (pw == 32) { DS_DISPATCH_PAIR(2, 32); } else { DS_DISPATCH_PAIR(2, 16); } }
+  }
   if (n_tile == 64) {
     if (k == 4)      { if (pw == 32) { DS_DISPATCH4(64, 32); } else { DS_DISPATCH4(64, 16); } }
     else if (k == 2) { if (pw == 32) { DS_DISPATCH(64, 2, 32); } else { DS_DISPATCH(64, 2, 16); } }
@@ -1161,6 +1223,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
     else if (k == 2) { if (pw == 32) { DS_DISPATCH(128, 2, 32); } else { DS_DISPATCH(128, 2, 16); } }
     else             { if (pw == 32) { DS_DISPATCH(128, 1, 32); } else { DS_DISPATCH(128, 1, 16); } }
   }
+#undef DS_DISPATCH_PAIR
 #undef DS_DISPATCH4
 #undef DS_DISPATCH
 }

@@ -173,27 +173,44 @@ __device__ __forceinline__ void load_a_frags(const unsigned char* at, int kk0, i
   }
 }
 
-// One fence, the MMAs of k-steps kk0 .. kk0 + KS - 1 (TF32X3: A_hi B_hi + A_lo B_hi + A_hi B_lo per k-step; BF16: one k16 MMA
-// per two k-steps) and one commit.  bd / bl: descriptors of the chunk's B (hi) / lo tiles.  A k8 step of fp32 B and a k16
-// step of bf16 B are both 32 B along the row: + 2 in the descriptor's address field
+// Step s of one commit group's MMAs, without fence or commit: tf32 k-step kk0 + s (TF32X3: A_hi B_hi + A_lo B_hi + A_hi B_lo),
+// or the BF16 k16 step of k-steps kk0 + 2s, kk0 + 2s + 1.  bd / bl: descriptors of the chunk's B (hi) / lo tiles.  A k8 step of
+// fp32 B and a k16 step of bf16 B are both 32 B along the row: + 2 in the descriptor's address field
 template <int N_TILE, Prec P, int KS>
-__device__ __forceinline__ void mma_a_frags(float (&acc)[N_TILE / 2], const AFrags<P, KS>& f, uint64_t bd, uint64_t bl, int kk0) {
+__device__ __forceinline__ void mma_a_step(float (&acc)[N_TILE / 2], const AFrags<P, KS>& f, uint64_t bd, uint64_t bl, int kk0,
+                                           int s) {
   constexpr bool X3 = P == Prec::TF32X3;
-  wgmma_fence();
   if constexpr (P == Prec::BF16) {
-#pragma unroll
-    for (int s = 0; s < KS / 2; ++s) Wgmma<N_TILE>::rs_bf16(acc, f[0][s], bd + (uint64_t)(2 * (kk0 / 2 + s)), 1u);
+    Wgmma<N_TILE>::rs_bf16(acc, f[0][s], bd + (uint64_t)(2 * (kk0 / 2 + s)), 1u);
   } else {
-#pragma unroll
-    for (int kk = 0; kk < KS; ++kk) {
-      const uint64_t k2 = (uint64_t)(2 * (kk0 + kk));
-      Wgmma<N_TILE>::rs(acc, f[0][kk], bd + k2, 1u);
-      if (X3) {
-        Wgmma<N_TILE>::rs(acc, f[X3 ? 1 : 0][kk], bd + k2, 1u);
-        Wgmma<N_TILE>::rs(acc, f[0][kk], bl + k2, 1u);
-      }
+    const uint64_t k2 = (uint64_t)(2 * (kk0 + s));
+    Wgmma<N_TILE>::rs(acc, f[0][s], bd + k2, 1u);
+    if (X3) {
+      Wgmma<N_TILE>::rs(acc, f[X3 ? 1 : 0][s], bd + k2, 1u);
+      Wgmma<N_TILE>::rs(acc, f[0][s], bl + k2, 1u);
     }
   }
+}
+
+// One fence, the MMAs of k-steps kk0 .. kk0 + KS - 1 for NH accumulator sets (the halves of the fused DS conv's paired tile,
+// each with its own fragments) and one commit.  Step by step, each set's MMAs in turn against the same B: every accumulator
+// sees the sequence of a single set
+template <int N_TILE, Prec P, int KS, int NH>
+__device__ __forceinline__ void mma_a_frags(float (&acc)[NH][N_TILE / 2], const AFrags<P, KS> (&f)[NH], uint64_t bd, uint64_t bl,
+                                            int kk0) {
+  wgmma_fence();
+#pragma unroll
+  for (int s = 0; s < (P == Prec::BF16 ? KS / 2 : KS); ++s)
+#pragma unroll
+    for (int h = 0; h < NH; ++h) mma_a_step<N_TILE, P, KS>(acc[h], f[h], bd, bl, kk0, s);
+  wgmma_commit();
+}
+// The same for one accumulator set
+template <int N_TILE, Prec P, int KS>
+__device__ __forceinline__ void mma_a_frags(float (&acc)[N_TILE / 2], const AFrags<P, KS>& f, uint64_t bd, uint64_t bl, int kk0) {
+  wgmma_fence();
+#pragma unroll
+  for (int s = 0; s < (P == Prec::BF16 ? KS / 2 : KS); ++s) mma_a_step<N_TILE, P, KS>(acc, f, bd, bl, kk0, s);
   wgmma_commit();
 }
 
