@@ -55,19 +55,23 @@ def cbam_schema(prefix, c, r=16, ks=7):
     return s
 
 
-def smaat_unet_schema(n_channels, n_classes, k=2, r=16, n_cbams=5):
+def smaat_unet_schema(n_channels, n_classes, k=2, r=16, n_cbams=5, bilinear=True):
     # models/SmaAt_UNet.py:23-39 (bilinear=True -> factor 2); n_cbams = 4 / 0: the Lightning variants
-    # UNetDSAttention4CBAMs / UNetDS (models/unet_precip_regression_lightning.py:167-208, 86-117)
+    # UNetDSAttention4CBAMs / UNetDS (models/unet_precip_regression_lightning.py:167-208, 86-117).  bilinear=False: factor 1
+    # (x5 is 1024 channels wide) and each UpDS upsamples with ConvTranspose2d(in, in // 2, 2, 2) (parts_ds.py:72-73)
+    factor = 2 if bilinear else 1
     s = {}
     s.update(double_conv_ds_schema("inc", n_channels, 64, None, k))
-    chans = [64, 128, 256, 512, 512]
+    chans = [64, 128, 256, 512, 1024 // factor]
     for i in range(n_cbams):
         s.update(cbam_schema(f"cbam{i + 1}", chans[i], r))
     for i in range(1, 5):
         s.update(double_conv_ds_schema(f"down{i}.maxpool_conv.1", chans[i - 1], chans[i], None, k))
-    ups = [(1024, 256), (512, 128), (256, 64), (128, 64)]
+    ups = [(1024, 512 // factor), (512, 256 // factor), (256, 128 // factor), (128, 64)]
     for i, (cin, cout) in enumerate(ups, start=1):
-        s.update(double_conv_ds_schema(f"up{i}.conv", cin, cout, cin // 2, k))
+        if not bilinear:
+            s.update({f"up{i}.up.weight": (cin, cin // 2, 2, 2), f"up{i}.up.bias": (cin // 2,)})
+        s.update(double_conv_ds_schema(f"up{i}.conv", cin, cout, cin // 2 if bilinear else None, k))
     s.update({"outc.conv.weight": (n_classes, 64, 1, 1), "outc.conv.bias": (n_classes,)})
     return s
 
