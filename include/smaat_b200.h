@@ -171,6 +171,12 @@ int smaat_dsconv_maxpool_fwd(const float* x0, int C0, int64_t x0_bstride, const 
  * summation order.  Process-wide; the environment variable SMAAT_DS_IMPL presets it.  For A/B measurements and tests. */
 int smaat_set_dsconv_impl(int impl);
 
+/* How the fused DS conv runs 128 < Cout <= 256 with k = 2 in the register A form, tf32 or 3xTF32, fp32 maps: 1 (default) =
+ * one wide tile per patch, both 128-channel halves fed from one depthwise chunk; 0 = two passes of 128 channels, each
+ * computing the depthwise chunk again (Cout a multiple of 128 only).  Bitwise the same outputs.  Process-wide; the
+ * environment variable SMAAT_DSCONV_WIDE=0 presets 0.  For A/B measurements and tests. */
+int smaat_set_dsconv_wide(int enabled);
+
 /* 1 if this (x, w, K, Cout, P) can take the tensor-core (wgmma) path (P % 4 == 0, K % 4 == 0, 16-byte aligned
  * pointers, Cout >= 8), else 0: the caller then uses SMAAT_PW_FP32_SIMT. */
 int smaat_pw1x1_tc_eligible(const float* x, const float* w, int K, int Cout, int P);

@@ -9,7 +9,8 @@
 //
 // One persistent CTA per SM; a tile is a PH x PW = 128-pixel patch of one image and one pass of N_TILE <= 128 output
 // channels (Cout <= 128: one pass, so the depthwise work is done exactly once; Cout in {256, 384, 512}: passes of 128).
-// At Cout <= 64 a tile can instead be two such patches one above the other, sharing each chunk (DsCfg PAIR, dsconv_pair_kernel).
+// At Cout <= 64 a tile can instead be two such patches one above the other, sharing each chunk (DsCfg PAIR, dsconv_pair_kernel);
+// at 128 < Cout <= 256 one patch and both 128-channel halves, fed by each chunk once (DsCfg WIDE, dsconv_wide_kernel).
 // K = k*Cin is walked in chunks of 32 depthwise channels (CC = 32/k input channels):
 //   warp 0      TMA: (PH+2) x (PW+8) x CC input halo box per chunk (OOB zero fill = padding=1; box
 //               starts at x0-4, x0-8 for bf16 input: the inner TMA coordinate must be 16-byte aligned) into an IS-deep ring;
@@ -86,7 +87,10 @@ constexpr int DS_MIN_CLASSES = 21;   // ... that every instance keeps beside its
 // PAIR (dsconv_pair_kernel: N_TILE 64, register form, tf32 / 3xTF32, k = 2 and 4): a tile is two vertically adjacent patches
 // (2 PH rows x PW, 256 pixels) that share each chunk's input box, weight chunk and barrier hand-offs; each half keeps the
 // single tile's A layout, accumulator rows and epilogue
-template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float, bool PAIR = false>
+// WIDE (dsconv_wide_kernel: 128 < Cout <= 256, N_TILE 128 per channel half, register form, tf32 / 3xTF32, fp32 maps, k = 2): a tile is
+// one patch and both 128-channel halves, so each chunk's input box and depthwise stencil feed 256 channels instead of being
+// computed once per pass; each consumer warpgroup holds one accumulator set per half and feeds both from the same A fragments
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float, bool PAIR = false, bool WIDE = false>
 struct DsCfg {
   static constexpr bool X3 = P == Prec::TF32X3;
   static constexpr int ESZ = (int)sizeof(TA);
@@ -94,8 +98,12 @@ struct DsCfg {
   static_assert(P != Prec::BF16 || !A_SMEM, "BF16: register A form only");
   static_assert(!PAIR || (N_TILE == 64 && !A_SMEM && P != Prec::BF16 && ESZ == 4 && KPL != 1),
                 "paired tiles: N_TILE 64, register form, tf32 / 3xTF32, fp32 maps, k = 2, 4");
+  static_assert(!WIDE || (N_TILE == 128 && !PAIR && !A_SMEM && P != Prec::BF16 && ESZ == 4 && KPL == 2),
+                "wide tiles: two N_TILE 128 halves, register form, tf32 / 3xTF32, fp32 maps, k = 2");
   static constexpr int PH = TC_BM / PW;
   static constexpr int NH = PAIR ? 2 : 1;                      // patches (halves) per tile
+  static constexpr int NW = WIDE ? 2 : 1;                      // N_TILE channel halves per tile
+  static constexpr int NA = NH * NW;                           // accumulator sets per consumer thread
   static constexpr int TH = NH * PH;                           // tile rows
   // input boxes start XM columns left of the patch: 16 bytes, the alignment TMA takes for the inner coordinate (4 fp32, 8 bf16)
   static constexpr int XM = 16 / ESZ;
@@ -107,7 +115,7 @@ struct DsCfg {
   // A ring stage: fp32 (register form: the consumers split hi / lo after loading; one 16 KB tile per half), or hi [+ lo]
   // (A_SMEM: the tensor core reads the parts)
   static constexpr int AST_BYTES = (X3 && A_SMEM ? 2 : 1) * NH * A_BYTES;
-  static constexpr int BST_BYTES = (X3 ? 2 : 1) * B_BYTES;     // B ring stage: hi [+ lo]
+  static constexpr int BST_BYTES = (X3 ? 2 : 1) * B_BYTES;     // B ring stage: hi [+ lo] of N_TILE rows (wide: one channel half)
   static constexpr int OFF_ALO = A_BYTES;
   static constexpr int OFF_BLO = B_BYTES;
   // depthwise producer groups (128 threads each), sized by the register file: the consumers hold N_TILE / 2 accumulators
@@ -121,9 +129,13 @@ struct DsCfg {
   // same two in use, NG producing and one loading; the 16 / 32 KB its half-size B stages free go to the input ring and the
   // staging buffers (the table in DESIGN §6).  A paired tile's 32 KB A stages keep the register form's 2 + NG in both modes;
   // in 3xTF32 at PW 16 with k = 2 (27 KB boxes of 18 rows) the B ring is 2 deep, so that the input ring keeps 2 stages
-  static constexpr int AS = X3 ? (A_SMEM ? (N_TILE > 64 ? 2 : 3) : 2 + NG) : (PAIR ? 2 + NG : 4);
-  static constexpr int BS = X3 ? (A_SMEM && N_TILE > 64 ? 2 : (PAIR && PW == 16 && KPL == 2 ? 2 : 3)) : 4;
-  static constexpr int AFF_N = 512;                            // scale | shift | OutConv weights of up to 512 channels
+  // Wide tiles: the B ring holds half-stages (one per chunk and channel half, 32 KB in 3xTF32), committed and released one by
+  // one, so the consumers hold two of them (the newest MMA group and the one retiring) and the loader fills a third.  Four
+  // would leave no room for the staging buffers beside a 2-deep input ring (the table in DESIGN §6).  Both modes take 2 + NG
+  // A stages and 3 half-stages
+  static constexpr int AS = WIDE ? 2 + NG : X3 ? (A_SMEM ? (N_TILE > 64 ? 2 : 3) : 2 + NG) : (PAIR ? 2 + NG : 4);
+  static constexpr int BS = WIDE ? 3 : X3 ? (A_SMEM && N_TILE > 64 ? 2 : (PAIR && PW == 16 && KPL == 2 ? 2 : 3)) : 4;
+  static constexpr int AFF_N = WIDE ? 256 : 512;               // scale | shift | OutConv weights of up to 512 (wide: 256) channels
   static constexpr int BAR_BYTES = 512;
   static constexpr int FREE = 224 * 1024 - 1024 - BAR_BYTES - 3 * AFF_N * 4 - AS * AST_BYTES - BS * BST_BYTES;
   // Output staging: per consumer warpgroup ST_BUFS buffers of one 32-channel x 64-pixel TMA store box (8 KB), taken from the
@@ -182,11 +194,14 @@ struct DsCfg {
   static_assert(REGS_SUM <= THREADS / 128 * REGS_LAUNCH && REGS_MMA >= REGS_LAUNCH, "register budget");
   // k-steps per MMA commit group in the register form.  A whole chunk (4) holds 2 x 32 fragment registers in TF32X3; at
   // N_TILE 64 the consumers' 128 registers cannot (ptxas would serialise the MMAs), so groups are half chunks there
-  static constexpr int KS = (X3 && N_TILE == 64) ? 2 : TC_BK / 8;
+  // Wide tiles hold 2 x 64 accumulators: with two half-chunk sets (2 x 16 registers in TF32X3, 2 x 8 in tf32)
+  // beside them ptxas serialised the MMAs, so their groups are single k-steps in TF32X3 and half chunks in tf32
+  static constexpr int KS = WIDE ? (X3 ? 1 : 2) : (X3 && N_TILE == 64) ? 2 : TC_BK / 8;
   static_assert(IS >= 2, "input ring");
   static_assert(NG <= AS, "phase-parity barriers");
   static_assert(IN_BYTES % 128 == 0, "TMA destination alignment");
   static_assert(TOTAL <= 227 * 1024, "shared memory budget");
+  static_assert(!WIDE || ST_BUFS > 0, "wide tiles keep the staged epilogue: the max-pool and the CBAM pools are taken as at N_TILE 128");
 };
 
 // ----- staged output epilogue: TMA tensor stores of 32-channel x 64-pixel boxes from shared memory -----
@@ -221,14 +236,14 @@ __device__ __forceinline__ void quad_transpose(float (&v)[4], int q) {
 
 // The kernel body, shared by the k = 1 / 2 instances (dsconv_fused_kernel) and the k = 4 ones (dsconv_kpl4_kernel).  The tensor
 // maps are the kernels' __grid_constant__ parameters
-template <int N_TILE, int KPL, int PW, Prec PREC, bool A_SMEM, typename TA = float, bool PAIR = false>
+template <int N_TILE, int KPL, int PW, Prec PREC, bool A_SMEM, typename TA = float, bool PAIR = false, bool WIDE = false>
 __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CUtensorMap& map_in1, const CUtensorMap& map_w,
                                             const CUtensorMap& map_wlo, const CUtensorMap& map_y, const CUtensorMap& map_sa,
                                             const DsParams& p) {
-  using L = DsCfg<N_TILE, KPL, PW, PREC, A_SMEM, TA, PAIR>;
+  using L = DsCfg<N_TILE, KPL, PW, PREC, A_SMEM, TA, PAIR, WIDE>;
   constexpr bool X3 = L::X3;
   constexpr bool BA = L::ESZ == 2;   // bf16 activations
-  constexpr int PH = L::PH, NH = L::NH, TH = L::TH, BW = L::BW, BH = L::BH, CC = L::CC, IS = L::IS, AS = L::AS, BS = L::BS;
+  constexpr int PH = L::PH, NH = L::NH, NW = L::NW, NA = L::NA, TH = L::TH, BW = L::BW, BH = L::BH, CC = L::CC, IS = L::IS, AS = L::AS, BS = L::BS;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   unsigned char* a_base = smem + L::OFF_A;
@@ -241,7 +256,7 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
   uint64_t* in_empty = in_full + IS * L::NG;      // [IS] producer group finished reading the box (128 arrivals)
   uint64_t* a_full = in_empty + IS;               // [AS] A operand written (128 arrivals)
   uint64_t* a_empty = a_full + AS;                // [AS] the 8 consumer warps' MMAs reading the A stage retired
-  uint64_t* b_full = a_empty + AS;                // [BS] weight chunk landed (TMA tx)
+  uint64_t* b_full = a_empty + AS;                // [BS] weight chunk (wide: half-chunk) landed (TMA tx)
   uint64_t* b_empty = b_full + BS;                // [BS] the 8 consumer warps' MMAs reading the B stage retired
   float* aff = reinterpret_cast<float*>(smem + L::OFF_BAR + L::BAR_BYTES);
 
@@ -325,18 +340,22 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
         }
       }
     }
-    // ===== weight-ring loader: K-major SW128 chunks (hi [+lo]) of this tile's channel pass, decoupled from the input ring =====
+    // ===== weight-ring loader: K-major SW128 chunks (hi [+lo]) of this tile's channel pass, decoupled from the input ring.  Wide
+    // tiles: half-stage hs = NW * chunk + half, each N_TILE rows of the chunk =====
     if (warp == 1 && lane == 0) {
-      uint32_t gc = 0;
+      uint32_t hs = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         int b, ty, tx, np;
         decode(tile, b, ty, tx, np);
-        for (int i = 0; i < nch; ++i, ++gc) {
-          const int sb = gc % BS;
-          mbar_wait(&b_empty[sb], ((gc / BS) & 1u) ^ 1u);
-          mbar_arrive_expect_tx(&b_full[sb], L::B_TX);
-          tma_load_2d(b_base + sb * L::BST_BYTES, &map_w, &b_full[sb], i * TC_BK, np * N_TILE);
-          if (X3) tma_load_2d(b_base + sb * L::BST_BYTES + L::OFF_BLO, &map_wlo, &b_full[sb], i * TC_BK, np * N_TILE);
+        for (int i = 0; i < nch; ++i) {
+#pragma unroll
+          for (int hf = 0; hf < NW; ++hf, ++hs) {
+            const int sb = hs % BS, row = (np * NW + hf) * N_TILE;
+            mbar_wait(&b_empty[sb], ((hs / BS) & 1u) ^ 1u);
+            mbar_arrive_expect_tx(&b_full[sb], L::B_TX);
+            tma_load_2d(b_base + sb * L::BST_BYTES, &map_w, &b_full[sb], i * TC_BK, row);
+            if (X3) tma_load_2d(b_base + sb * L::BST_BYTES + L::OFF_BLO, &map_wlo, &b_full[sb], i * TC_BK, row);
+          }
         }
       }
     }
@@ -377,28 +396,37 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       int b, ty, tx, np;
       decode(tile, b, ty, tx, np);
-      // one accumulator set per half of the tile (its 64 rows of that patch)
-      float acc[NH][N_TILE / 2];
+      // one accumulator set per half of the tile (its 64 rows of that patch, or of that channel half)
+      float acc[NA][N_TILE / 2];
 #pragma unroll
-      for (int h = 0; h < NH; ++h)
+      for (int h = 0; h < NA; ++h)
 #pragma unroll
         for (int i = 0; i < N_TILE / 2; ++i) acc[h][i] = 0.f;
       // Pipelined k loop: chunk i's MMAs are issued as one group, then the wait leaves that group in flight and retires chunk
       // i - 1, whose A and B stages go back to the producers and the weight loader.
+      // release(c): chunk c's A stage and its (last) B stage; wide tiles hand half 0's B stage back on its own (release_b)
       auto release = [&](uint32_t c) {
         __syncwarp();
         if (lane == 0) {
           mbar_arrive(&a_empty[c % AS]);
-          mbar_arrive(&b_empty[c % BS]);
+          mbar_arrive(&b_empty[(NW * c + NW - 1) % BS]);
         }
       };
-      auto wait_stages = [&](const unsigned char*& ast, uint64_t& bd, uint64_t& bl) {
-        const int sa = gc % AS, sb = gc % BS;
-        mbar_wait(&a_full[sa], (gc / AS) & 1u);
-        mbar_wait(&b_full[sb], (gc / BS) & 1u);
-        ast = a_base + sa * L::AST_BYTES;
+      auto release_b = [&](uint32_t hs) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&b_empty[hs % BS]);
+      };
+      auto wait_b = [&](uint32_t hs, uint64_t& bd, uint64_t& bl) {
+        const int sb = hs % BS;
+        mbar_wait(&b_full[sb], (hs / BS) & 1u);
         bd = make_b_desc<PREC>(smem_u32(b_base + sb * L::BST_BYTES));
         bl = make_kmajor_desc(smem_u32(b_base + sb * L::BST_BYTES + L::OFF_BLO));
+      };
+      auto wait_stages = [&](const unsigned char*& ast, uint64_t& bd, uint64_t& bl) {
+        const int sa = gc % AS;
+        mbar_wait(&a_full[sa], (gc / AS) & 1u);
+        ast = a_base + sa * L::AST_BYTES;
+        wait_b(NW * gc, bd, bl);
       };
       if (A_SMEM) {
         for (int i = 0; i < nch; ++i, ++gc) {
@@ -421,6 +449,53 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
           if (i > 0) release(gc - 1);
         }
         wgmma_wait0();
+      } else if constexpr (WIDE) {
+        // A wide tile sweeps each chunk twice, half 0's k-steps and then half 1's, one commit group per KS k-steps, each from
+        // fragments it loads from the chunk's A stage (the A stage is read twice, the input box and the stencil were done once).
+        // The wait after each group retires the one before: at half 0's first group the previous chunk's A stage and half-1 B
+        // stage go back, at half 1's first group this chunk's half-0 B stage.  So the weight loader refills half 0's stage
+        // halfway through the chunk, and each half-stage has about a chunk's MMAs to land in the 3-deep ring.  (With the halves
+        // interleaved per k-step, a chunk's half-0 stage was freed only as its last group retired, two groups before the next
+        // chunk's half 1 needed it.)  Each accumulator set sees the k-steps of a single N_TILE pass in its order, so the sums
+        // are those of the two-pass route.  Two fragment sets alternate over the 2 x GPC groups of a chunk
+        constexpr int KS = L::KS, GPC = (TC_BK / 8) / KS;
+        static_assert(GPC % 2 == 0, "fragment sets alternate within a chunk");
+        const unsigned char* ast = nullptr;
+        uint64_t bd = 0, bl = 0;
+        AFrags<PREC, KS> fa, fb;
+        // group `part` of half hf (both constants once unrolled) of chunk i
+        auto step = [&](int i, int hf, int part, AFrags<PREC, KS>& cur, AFrags<PREC, KS>& prev) {
+          if (part == 0) {
+            if (hf == 0) {
+              const int sa = gc % AS;
+              mbar_wait(&a_full[sa], (gc / AS) & 1u);
+              ast = a_base + sa * L::AST_BYTES;
+            }
+            wait_b(NW * gc + hf, bd, bl);
+          }
+          load_a_frags<PREC, KS>(ast, part * KS, t, m0, m1, cur);
+          if (hf == 0) mma_a_frags<N_TILE, PREC, KS>(acc[0], cur, bd, bl, part * KS);
+          else mma_a_frags<N_TILE, PREC, KS>(acc[NA - 1], cur, bd, bl, part * KS);
+          wgmma_wait<1>();
+          wgmma_keep(prev);
+          if (part == 0) {
+            if (hf == 1) release_b(NW * gc);
+            else if (i > 0) release(gc - 1);
+          }
+        };
+        for (int i = 0; i < nch; ++i, ++gc) {
+#pragma unroll
+          for (int hf = 0; hf < NW; ++hf) {
+#pragma unroll
+            for (int part = 0; part < GPC; part += 2) {
+              step(i, hf, part, fa, fb);
+              step(i, hf, part + 1, fb, fa);
+            }
+          }
+        }
+        wgmma_wait0();
+        wgmma_keep(fa);
+        wgmma_keep(fb);
       } else {
         // Chunk i's fragments must stay untouched until it retires, so two fragment sets alternate (the loop is unrolled by 2;
         // no control-flow path may load a set whose chunk is still in flight, or ptxas serialises the MMAs: the odd tail is
@@ -461,21 +536,23 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
       // the tile's last chunk has retired; its stages are released before the epilogue, so that TMA, the weight loader and
       // the producers run on through it
 #pragma unroll
-      for (int h = 0; h < NH; ++h) wgmma_keep(acc[h]);
+      for (int h = 0; h < NA; ++h) wgmma_keep(acc[h]);
       release(gc - 1);
 
-      // ----- epilogue, once per half (patch rows y_org ..): rows g / g + 8 are patch pixels m0 / m1, columns n0 + 8j + 2t + {0, 1}
-      const int n0 = np * N_TILE;
+      // ----- epilogue, once per half (patch rows y_org .., channels n0 ..): rows g / g + 8 are patch pixels m0 / m1, columns
+      // n0 + 8j + 2t + {0, 1}
 #pragma unroll
-      for (int h = 0; h < NH; ++h) {
+      for (int h = 0; h < NA; ++h) {
         float (&ac)[N_TILE / 2] = acc[h];
-        const int y_org = ty * TH + h * PH;
+        const int hp = WIDE ? 0 : h;                 // the patch half (paired tiles)
+        const int n0 = (np * NW + (WIDE ? h : 0)) * N_TILE;
+        const int y_org = ty * TH + hp * PH;
         const int gy0 = y_org + m0 / PW, gx0 = tx * PW + m0 % PW;
         const int gy1 = y_org + m1 / PW, gx1 = tx * PW + m1 % PW;
         const bool v0 = gy0 < p.H && gx0 < p.W, v1 = gy1 < p.H && gx1 < p.W;
         const int64_t o0 = (int64_t)gy0 * p.W + gx0, o1 = (int64_t)gy1 * p.W + gx1;
-        if (p.stats) {
-          // BatchNorm batch statistics from the RAW accumulators (one pass: Cout <= 128); patch pixels outside the image are
+        if (!WIDE && p.stats) {
+          // BatchNorm batch statistics from the RAW accumulators (one pass: Cout <= 128, not taken by wide tiles); patch pixels outside the image are
           // masked (their stencil still sees the image edge), channels past Cout are exact zeros (TMA zero fill of the weight
           // rows); the affine is applied to the sums analytically
           const double npix = (double)((__popc(__ballot_sync(0xffffffffu, v0)) + __popc(__ballot_sync(0xffffffffu, v1))) / 4);
@@ -494,7 +571,7 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
             }
           }
         }
-        if (p.ncls) {
+        if (!WIDE && p.ncls) {
           // K-class OutConv + argmax.  The activations replace the accumulators in place (fmaxf(fmaf(acc, sc, sh), act_lo), as
           // below); then, one class at a time, the one-class dot product below in its order (fmaf over the thread's channels, the
           // two xor shuffles, + bias), so class j's logit is bit for bit what that epilogue writes with OutConv row j.  After the
@@ -544,7 +621,7 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
             if (v0 && t == 0) p.cls[(int64_t)b * P + o0] = arg0;
             if (v1 && t == 1) p.cls[(int64_t)b * P + o1] = arg1;
           }
-        } else if (p.oc_y) {
+        } else if (!WIDE && p.oc_y) {
           // fused OutConv: each pixel's dot product over all Cout <= N_TILE activations.  Channels past Cout have zero
           // accumulators, identity affine and zero OutConv weight: no mask needed
           float d0 = 0.f, d1 = 0.f;
@@ -666,7 +743,7 @@ __device__ __forceinline__ void dsconv_body(const CUtensorMap& map_in0, const CU
                 pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 1));
                 pmax = fmaxf(pmax, __shfl_xor_sync(0xffffffffu, pmax, 2));
                 if (pq == 0 && c < p.Cout) {
-                  const int64_t o = ((int64_t)b * p.npart + 2 * ((ty * NH + h) * p.tiles_x + tx) + wg) * p.Cout + c;
+                  const int64_t o = ((int64_t)b * p.npart + 2 * ((ty * NH + hp) * p.tiles_x + tx) + wg) * p.Cout + c;
                   p.pool_sum[o] = psum;
                   p.pool_max[o] = pmax;
                 }
@@ -905,21 +982,33 @@ __global__ void __launch_bounds__(DsCfg<64, KPL, PW, tf32_prec(X3), false, float
   dsconv_body<64, KPL, PW, tf32_prec(X3), false, float, true>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
 }
 
-template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float, bool PAIR = false>
+// Wide tiles (DsCfg WIDE: both 128-channel halves of 128 < Cout <= 256 per tile): the register form, tf32 / 3xTF32, k = 2.  A kernel
+// of its own, so that the two-pass kernels keep their names and instance sets
+template <int PW, bool X3>
+__global__ void __launch_bounds__(DsCfg<128, 2, PW, tf32_prec(X3), false, float, false, true>::THREADS, 1)
+    dsconv_wide_kernel(const __grid_constant__ CUtensorMap map_in0, const __grid_constant__ CUtensorMap map_in1,
+                       const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_wlo,
+                       const __grid_constant__ CUtensorMap map_y, const __grid_constant__ CUtensorMap map_sa,
+                       const DsParams p) {
+  dsconv_body<128, 2, PW, tf32_prec(X3), false, float, false, true>(map_in0, map_in1, map_w, map_wlo, map_y, map_sa, p);
+}
+
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float, bool PAIR = false, bool WIDE = false>
 static auto ds_kernel() {
   static_assert(KPL == 1 || KPL == 2 || (KPL == 4 && !A_SMEM), "fused DS conv instances: k = 1, 2 (both A forms), 4 (register form)");
-  if constexpr (PAIR) return dsconv_pair_kernel<KPL, PW, P == Prec::TF32X3>;
+  if constexpr (WIDE) return dsconv_wide_kernel<PW, P == Prec::TF32X3>;
+  else if constexpr (PAIR) return dsconv_pair_kernel<KPL, PW, P == Prec::TF32X3>;
   else if constexpr (sizeof(TA) == 2) return dsconv_bf16act_kernel<N_TILE, KPL, PW>;
   else if constexpr (P == Prec::BF16) return dsconv_bf16_kernel<N_TILE, KPL, PW>;
   else if constexpr (KPL == 4) return dsconv_kpl4_kernel<N_TILE, PW, P == Prec::TF32X3>;
   else return dsconv_fused_kernel<N_TILE, KPL, PW, P == Prec::TF32X3, A_SMEM>;
 }
 
-template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float, bool PAIR = false>
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float, bool PAIR = false, bool WIDE = false>
 static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl,
                      const CUtensorMap& my, const CUtensorMap& msa, DsParams p, int B, cudaStream_t st) {
-  using L = DsCfg<N_TILE, KPL, PW, P, A_SMEM, TA, PAIR>;
-  auto kern = ds_kernel<N_TILE, KPL, PW, P, A_SMEM, TA, PAIR>();
+  using L = DsCfg<N_TILE, KPL, PW, P, A_SMEM, TA, PAIR, WIDE>;
+  auto kern = ds_kernel<N_TILE, KPL, PW, P, A_SMEM, TA, PAIR, WIDE>();
   // the pools and the max-pool are read back from the staging buffers: instances with the direct-store epilogue do not take them
   if (p.pooled && !L::ST_BUFS) return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools and the max-pool need the staged epilogue");
   if (p.ncls > L::MAX_CLASSES)
@@ -935,7 +1024,7 @@ static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtenso
   }
   p.tiles_x = ceil_div(p.W, PW);
   p.tiles_y = ceil_div(p.H, L::TH);
-  p.npass = ceil_div(p.Cout, N_TILE);
+  p.npass = ceil_div(p.Cout, N_TILE * L::NW);
   const int64_t total = (int64_t)B * p.tiles_x * p.tiles_y * p.npass;
   SMAAT_REQUIRE(total < (1ll << 31), "dsconv: too many tiles");
   p.total_tiles = (int)total;
@@ -973,6 +1062,13 @@ static bool ds_pair(int n_tile, int k, int pw, int H, int mode, bool a_smem, boo
 // y: the activation output, or null where it is not known yet (smaat_dsconv_eligible*) or not written (the fused OutConv).  The
 // epilogue stores it by TMA, which needs a 16-byte aligned base and 16-byte multiples as strides
 static int ds_impl();
+static bool ds_wide_on();
+
+// Wide tiles (dsconv_wide_kernel) where they are built (k = 2, the register form, tf32 / 3xTF32, fp32 maps) and switched on
+// (smaat_set_dsconv_wide): 128 < Cout <= 256 in one pass instead of two, with no OutConv (no network ends in such a conv)
+static bool ds_wide(int Cout, int k, bool a_smem, bool bf16, bool bact, bool head) {
+  return ds_wide_on() && Cout > 128 && Cout <= 256 && k == 2 && !a_smem && !bf16 && !bact && !head;
+}
 
 static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* pw_w,
                         const float* pw_w_lo, const float* y, int64_t y_bstride, int H, int W, int k, int Cout, bool stats,
@@ -986,8 +1082,10 @@ static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, i
   if (bact && (!bf16 || k == 4 || stats || W % 8 != 0 || bs0 % 8 != 0 || (C1 > 0 && bs1 % 8 != 0) || (y && y_bstride % 8 != 0)))
     return false;
   if (y && (!aligned16(y) || y_bstride % 4 != 0)) return false;
-  // Cout > 128: whole passes of 128 channels; batch statistics and the fused OutConv need all channels in one pass
-  if (Cout < 8 || Cout > 512 || (Cout > 128 && (Cout % 128 != 0 || stats || outconv))) return false;
+  // Cout > 128: whole passes of 128 channels, or one wide tile for any Cout up to 256; batch statistics and the fused OutConv are
+  // taken up to 128 channels
+  if (Cout < 8 || Cout > 512 || (Cout > 128 && (stats || outconv))) return false;
+  if (Cout > 128 && Cout % 128 != 0 && !ds_wide(Cout, k, ds_impl() == 1, bf16, bact, outconv)) return false;
   if (W % 4 != 0 || !aligned16(x0) || bs0 % 4 != 0) return false;
   if (C1 > 0 && (!aligned16(x1) || bs1 % 4 != 0 || C0 % (TC_BK / k) != 0)) return false;
   const int K = k * (C0 + C1);
@@ -1049,6 +1147,18 @@ static int ds_impl() {
   return v;
 }
 
+// Whether 128 < Cout <= 256 runs as wide tiles (1, the default) or in two 128-channel passes (0).  SMAAT_DSCONV_WIDE presets it
+static std::atomic<int> g_ds_wide{-1};
+static bool ds_wide_on() {
+  int v = g_ds_wide.load(std::memory_order_relaxed);
+  if (v < 0) {
+    const char* e = getenv("SMAAT_DSCONV_WIDE");
+    v = (e && atoi(e) == 0) ? 0 : 1;
+    g_ds_wide.store(v, std::memory_order_relaxed);
+  }
+  return v != 0;
+}
+
 }  // namespace smaat
 
 using namespace smaat;
@@ -1056,6 +1166,12 @@ using namespace smaat;
 extern "C" int smaat_set_dsconv_impl(int impl) {
   SMAAT_REQUIRE(impl >= 0 && impl <= 2, "set_dsconv_impl: 0 = auto, 1 = A operand from shared memory, 2 = A operand from registers");
   g_ds_impl.store(impl, std::memory_order_relaxed);
+  return SMAAT_OK;
+}
+
+extern "C" int smaat_set_dsconv_wide(int enabled) {
+  SMAAT_REQUIRE(enabled == 0 || enabled == 1, "set_dsconv_wide: 1 = wide tiles for 128 < Cout <= 256, 0 = passes of 128 channels");
+  g_ds_wide.store(enabled, std::memory_order_relaxed);
   return SMAAT_OK;
 }
 
@@ -1132,6 +1248,7 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
   // a paired tile's boxes span both patches.  Its rings leave room for the weights of DS_MIN_CLASSES classes, not always 32: more
   // classes take the single tile
   const bool pair = ds_pair(n_tile, k, pw, H, mode, a_smem, bact) && ncls <= DS_MIN_CLASSES;
+  const bool wide = ds_wide(Cout, k, a_smem, bf16, bact, head);
   const int th = pair ? 2 * ph : ph;
   const int K = k * (C0 + C1);
   // activation maps: fp32, or bf16 (bact)
@@ -1210,6 +1327,14 @@ static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* 
 #define DS_DISPATCH_PAIR(KP, PWv)                                                                                      \
   return x3 ? launch_ds<64, KP, PWv, Prec::TF32X3, false, float, true>(m0, m1, mw, mwl, my, msa, p, B, st)                 \
             : launch_ds<64, KP, PWv, Prec::TF32, false, float, true>(m0, m1, mw, mwl, my, msa, p, B, st)
+  if (wide) {
+    if (pw == 32) {
+      return x3 ? launch_ds<128, 2, 32, Prec::TF32X3, false, float, false, true>(m0, m1, mw, mwl, my, msa, p, B, st)
+                : launch_ds<128, 2, 32, Prec::TF32, false, float, false, true>(m0, m1, mw, mwl, my, msa, p, B, st);
+    }
+    return x3 ? launch_ds<128, 2, 16, Prec::TF32X3, false, float, false, true>(m0, m1, mw, mwl, my, msa, p, B, st)
+              : launch_ds<128, 2, 16, Prec::TF32, false, float, false, true>(m0, m1, mw, mwl, my, msa, p, B, st);
+  }
   if (pair) {
     if (k == 4) { if (pw == 32) { DS_DISPATCH_PAIR(4, 32); } else { DS_DISPATCH_PAIR(4, 16); } }
     else        { if (pw == 32) { DS_DISPATCH_PAIR(2, 32); } else { DS_DISPATCH_PAIR(2, 16); } }

@@ -262,6 +262,13 @@ def set_dsconv_impl(impl: str) -> None:
     _lib.check(_lib.load().smaat_set_dsconv_impl({"auto": 0, "smem": 1, "regs": 2}[impl]), "smaat_set_dsconv_impl")
 
 
+def set_dsconv_wide(enabled: bool) -> None:
+    """Run the fused DS conv's 128 < Cout <= 256 layers (k = 2, 'tf32' / 'tf32x3', fp32 maps, the register A form) as wide tiles,
+    both 128-channel halves from one depthwise chunk (default on), or in two 128-channel passes (off; Cout a multiple of 128
+    only).  The outputs are bitwise equal.  SMAAT_DSCONV_WIDE=0 presets off.  For A/B measurements (tools/time_dsconv.py)."""
+    _lib.check(_lib.load().smaat_set_dsconv_wide(int(bool(enabled))), "smaat_set_dsconv_wide")
+
+
 def dsconv_takes(x, x1, pw_weight, k, mode=None, stats=False) -> bool:
     """True when ``dsconv`` would run its fused kernel on these inputs (smaat_dsconv_eligible + the arithmetic mode)."""
     mode = mode or _pw_mode

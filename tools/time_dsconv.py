@@ -11,7 +11,12 @@ With --cbam it times instead the serving forward's CBAM fusions (smaat_dsconv_cb
 tiles: the second DS conv of inc / down1 / down2 with and without the epilogue pools (partial sums / maxima + 2x2 max-pool), and
 the first DS conv of up4 / up3 / up2 with and without the gate applied on load.
 
-  python tools/time_dsconv.py [--tree DIR] [--mode tf32x3|tf32] [--json] [--cbam]
+With --wide it times instead bench.py's three 256-channel layers (down2.0, down2.1, up2.0 at 72^2; up2.0 also with the CBAM
+gate on load) as wide tiles and in two 128-channel passes (ops.set_dsconv_wide), the two alternated --rounds times; medians,
+beside each layer's HBM floor and its tensor floor (the issued tf32 MMA flops, 3 per product in 3xTF32, at the data-sheet
+495 TFLOP/s).
+
+  python tools/time_dsconv.py [--tree DIR] [--mode tf32x3|tf32] [--json] [--cbam | --wide [--rounds N]]
 
 --tree imports smaat_unet_b200 from another checkout (a built one), to compare two builds in one session."""
 import argparse
@@ -24,6 +29,8 @@ ap.add_argument("--tree", default=os.path.dirname(os.path.dirname(os.path.abspat
 ap.add_argument("--mode", default="tf32x3", choices=["tf32", "tf32x3"])
 ap.add_argument("--json", action="store_true", help="one JSON line per shape instead of a table")
 ap.add_argument("--cbam", action="store_true", help="time the CBAM fusions (epilogue pools, gate on load) instead")
+ap.add_argument("--wide", action="store_true", help="time the 256-channel layers as wide tiles and in two passes instead")
+ap.add_argument("--rounds", type=int, default=3, help="--wide: alternated rounds per route")
 args = ap.parse_args()
 sys.path.insert(0, os.path.abspath(args.tree))
 
@@ -105,10 +112,66 @@ def main_cbam():
         print(f"{r['layer']:28s} {r['fusion']:>6s} {r['plain_ms']:9.3f} {r['fused_ms']:9.3f} {r['extra_ms']:9.3f}")
 
 
+# (C0, C1, S, Cout, gated): bench.py's layers with 128 < Cout <= 256
+WIDE_SHAPES = [
+    (128, 0, 72, 256, False),
+    (256, 0, 72, 256, False),
+    (256, 256, 72, 256, False),
+    (256, 256, 72, 256, True),
+]
+TF32_FLOPS = 495e12
+
+
+def main_wide():
+    g = torch.Generator(device="cuda").manual_seed(7)
+    rows = []
+    for C0, C1, S, Cout, gated in WIDE_SHAPES:
+        Cin = C0 + C1
+        K = K_PL * Cin
+        x0 = torch.rand(B, C0, S, S, device="cuda", generator=g)
+        x1 = torch.rand(B, C1, S, S, device="cuda", generator=g) if C1 else None
+        dw_w = torch.randn(K, 1, 3, 3, device="cuda", generator=g) * 0.3
+        dw_b = torch.randn(K, device="cuda", generator=g) * 0.1
+        pw_w = torch.randn(Cout, K, device="cuda", generator=g) * 0.1
+        scale = torch.rand(Cout, device="cuda", generator=g) + 0.5
+        shift = torch.randn(Cout, device="cuda", generator=g) * 0.1
+        split = ops.split_tf32(pw_w) if args.mode == "tf32x3" else None
+        gate = (torch.rand(B, C0, device="cuda", generator=g), torch.rand(B, 1, S, S, device="cuda", generator=g)) if gated else None
+        common = (dw_w, dw_b, K_PL, pw_w, scale, shift, True)
+        fn = lambda: ops.dsconv_cbam(x0, *common, x1=x1, mode=args.mode, w_split=split, gate=gate)
+        times = {True: [], False: []}
+        for _ in range(args.rounds):
+            for wide in (False, True):
+                ops.set_dsconv_wide(wide)
+                times[wide].append(timed(fn))
+        ops.set_dsconv_wide(True)
+        med = {w: sorted(t)[len(t) // 2] for w, t in times.items()}
+        hbm = 4.0 * B * S * S * (Cin + Cout) / HBM_BPS * 1e3
+        mma = (3 if args.mode == "tf32x3" else 1) * 2.0 * B * S * S * K * Cout / TF32_FLOPS * 1e3
+        name = f"C{Cin}->{Cout} {S}^2" + (" (concat)" if C1 else "") + (" gated" if gated else "")
+        rows.append({"layer": name, "two_pass_ms": round(med[False], 4), "wide_ms": round(med[True], 4),
+                     "change": round(med[True] / med[False] - 1, 4), "hbm_ms": round(hbm, 4), "tensor_ms": round(mma, 4),
+                     "two_pass_runs": [round(t, 4) for t in times[False]], "wide_runs": [round(t, 4) for t in times[True]]})
+        del x0, x1
+    dev = torch.cuda.get_device_name()
+    if args.json:
+        for r in rows:
+            print(json.dumps(r))
+        print(json.dumps({"device": dev, "mode": args.mode, "rounds": args.rounds}))
+        return
+    print(f"{dev}, {args.mode}, B = {B}, k = {K_PL}; {args.rounds} alternated rounds of {WARMUP} warm-up + {ITERS} timed launches")
+    print(f"{'layer':32s} {'two-pass ms':>11s} {'wide ms':>8s} {'change':>7s} {'HBM floor':>9s} {'tensor floor':>12s}")
+    for r in rows:
+        print(f"{r['layer']:32s} {r['two_pass_ms']:11.3f} {r['wide_ms']:8.3f} {100 * r['change']:6.1f}% {r['hbm_ms']:9.3f} "
+              f"{r['tensor_ms']:12.3f}")
+
+
 def main():
     assert torch.cuda.is_available(), "time_dsconv.py needs a GPU"
     if args.cbam:
         return main_cbam()
+    if args.wide:
+        return main_wide()
     lib = _lib.load()
     mode = ops.PW_MODES[args.mode]
     g = torch.Generator(device="cuda").manual_seed(7)
