@@ -177,6 +177,12 @@ int smaat_set_dsconv_impl(int impl);
  * environment variable SMAAT_DSCONV_WIDE=0 presets 0.  For A/B measurements and tests. */
 int smaat_set_dsconv_wide(int enabled);
 
+/* How the fused DS conv runs Cout <= 64 with k = 2 or 4 in the register A form, tf32 or 3xTF32, fp32 maps, on an even number
+ * of patch rows: 1 (default) = paired tiles, two vertically adjacent patches sharing each input box and weight chunk; 0 =
+ * one patch per tile.  Bitwise the same outputs.  Process-wide; the environment variable SMAAT_DSCONV_PAIR=0 presets 0.
+ * For A/B measurements and tests. */
+int smaat_set_dsconv_pair(int enabled);
+
 /* 1 if this (x, w, K, Cout, P) can take the tensor-core (wgmma) path (P % 4 == 0, K % 4 == 0, 16-byte aligned
  * pointers, Cout >= 8), else 0: the caller then uses SMAAT_PW_FP32_SIMT. */
 int smaat_pw1x1_tc_eligible(const float* x, const float* w, int K, int Cout, int P);

@@ -26,6 +26,7 @@ SIGNATURES = {
     "smaat_dsconv_eligible2": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i],
     "smaat_set_dsconv_impl": [_i],
     "smaat_set_dsconv_wide": [_i],
+    "smaat_set_dsconv_pair": [_i],
     "smaat_dsconv_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_outconv_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "smaat_dsconv_classify_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _i],

@@ -171,8 +171,9 @@ struct DsCfg {
   static constexpr int TOTAL = OFF_BAR + BAR_BYTES + 3 * AFF_N * 4 + 1024;
   // The K-class OutConv of smaat_dsconv_classify_fwd keeps its weights ([class][N_TILE], zero past Cout) and biases in the shared
   // memory the rings leave under the 227 KB limit (11.5-29.5 KB), appended after the affine block and requested only by class
-  // launches: as many classes as fit, at most DS_MAX_CLASSES (32 at N_TILE 64, 22 at N_TILE 128).  Read through the L1 the
-  // weights were a cache miss per class (the carveout leaves little L1 beside 213 KB of shared memory)
+  // launches: as many classes as fit, at most DS_MAX_CLASSES (22 to 32 by instance, pinned per instance in
+  // tests/test_dsconv_dispatch_abi.py).  Read through the L1 the weights were a cache miss per class (the carveout leaves
+  // little L1 beside 213 KB of shared memory)
   static constexpr int OFF_CLS = OFF_BAR + BAR_BYTES + 3 * AFF_N * 4;
   static constexpr int CLS_FIT = (227 * 1024 - TOTAL) / ((N_TILE + 1) * 4);
   static constexpr int MAX_CLASSES = CLS_FIT < DS_MAX_CLASSES ? CLS_FIT : DS_MAX_CLASSES;
@@ -1055,8 +1056,9 @@ static int pick_pw(int H, int W) {
 // Paired tiles (dsconv_pair_kernel) where they are built (N_TILE 64, k = 2, 4, the register form, tf32 / 3xTF32, fp32 maps) and
 // cover the image with no more rows than single patches: an even number of patch rows.  The pair then runs the same
 // pixels with half the chunks' fixed costs (input box, weight chunk, hand-offs) per pixel
+static bool ds_pair_on();
 static bool ds_pair(int n_tile, int k, int pw, int H, int mode, bool a_smem, bool bact) {
-  return n_tile == 64 && (k == 2 || k == 4) && !a_smem && !bact && mode != SMAAT_PW_BF16 && ceil_div(H, TC_BM / pw) % 2 == 0;
+  return ds_pair_on() && n_tile == 64 && (k == 2 || k == 4) && !a_smem && !bact && mode != SMAAT_PW_BF16 && ceil_div(H, TC_BM / pw) % 2 == 0;
 }
 
 // y: the activation output, or null where it is not known yet (smaat_dsconv_eligible*) or not written (the fused OutConv).  The
@@ -1159,6 +1161,18 @@ static bool ds_wide_on() {
   return v != 0;
 }
 
+// Whether paired tiles run where ds_pair takes them (1, the default) or one patch per tile (0).  SMAAT_DSCONV_PAIR presets it
+static std::atomic<int> g_ds_pair{-1};
+static bool ds_pair_on() {
+  int v = g_ds_pair.load(std::memory_order_relaxed);
+  if (v < 0) {
+    const char* e = getenv("SMAAT_DSCONV_PAIR");
+    v = (e && atoi(e) == 0) ? 0 : 1;
+    g_ds_pair.store(v, std::memory_order_relaxed);
+  }
+  return v != 0;
+}
+
 }  // namespace smaat
 
 using namespace smaat;
@@ -1172,6 +1186,12 @@ extern "C" int smaat_set_dsconv_impl(int impl) {
 extern "C" int smaat_set_dsconv_wide(int enabled) {
   SMAAT_REQUIRE(enabled == 0 || enabled == 1, "set_dsconv_wide: 1 = wide tiles for 128 < Cout <= 256, 0 = passes of 128 channels");
   g_ds_wide.store(enabled, std::memory_order_relaxed);
+  return SMAAT_OK;
+}
+
+extern "C" int smaat_set_dsconv_pair(int enabled) {
+  SMAAT_REQUIRE(enabled == 0 || enabled == 1, "set_dsconv_pair: 1 = paired tiles where they are built, 0 = one patch per tile");
+  g_ds_pair.store(enabled, std::memory_order_relaxed);
   return SMAAT_OK;
 }
 
@@ -1380,7 +1400,7 @@ extern "C" int smaat_dsconv_classify_eligible(const float* x0, int C0, int64_t x
   if (K < 1 || K > DS_MAX_CLASSES) return 0;
   if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, false, true, mode == SMAAT_PW_BF16))
     return 0;
-  // the class weights must fit the shared memory the instance leaves free: 32 classes at Cout <= 64, 22 up to Cout = 128
+  // the class weights must fit the shared memory the instance leaves free: 22 to 32 classes, by instance (DsCfg::MAX_CLASSES)
   return K <= ds_max_classes(Cout > 64 ? 128 : 64, k, pick_pw(H, W), mode, ds_impl() == 1) ? 1 : 0;
 }
 

@@ -269,6 +269,13 @@ def set_dsconv_wide(enabled: bool) -> None:
     _lib.check(_lib.load().smaat_set_dsconv_wide(int(bool(enabled))), "smaat_set_dsconv_wide")
 
 
+def set_dsconv_pair(enabled: bool) -> None:
+    """Run the fused DS conv's Cout <= 64 layers (k = 2 or 4, 'tf32' / 'tf32x3', fp32 maps, the register A form, an even number
+    of patch rows) as paired tiles, two patches sharing each input box and weight chunk (default on), or one patch per tile
+    (off).  The outputs are bitwise equal.  SMAAT_DSCONV_PAIR=0 presets off.  For A/B measurements and tests."""
+    _lib.check(_lib.load().smaat_set_dsconv_pair(int(bool(enabled))), "smaat_set_dsconv_pair")
+
+
 def dsconv_takes(x, x1, pw_weight, k, mode=None, stats=False) -> bool:
     """True when ``dsconv`` would run its fused kernel on these inputs (smaat_dsconv_eligible + the arithmetic mode)."""
     mode = mode or _pw_mode
@@ -408,8 +415,8 @@ def set_fused_classify(enabled: bool) -> None:
 
 def dsconv_classify_takes(x, x1, pw_weight, k, n_classes, mode=None) -> bool:
     """True when ``dsconv_classify`` runs on these inputs: the fused kernel with a ``n_classes``-class OutConv and argmax in its
-    epilogue (smaat_dsconv_classify_eligible: Cout <= 128, 1 <= n_classes <= 32 -- 22 for Cout > 64 -- the fused DS conv's
-    shapes), and neither set_fused_dsconv(False) nor set_fused_classify(False)."""
+    epilogue (smaat_dsconv_classify_eligible: Cout <= 128, 1 <= n_classes <= 32 -- 22 to 32 by instance, at least 22 for Cout > 64 --
+    the fused DS conv's shapes), and neither set_fused_dsconv(False) nor set_fused_classify(False)."""
     mode = mode or _pw_mode
     if not _fuse_ds or not _fuse_classify or PW_MODES[mode] == 0:
         return False
