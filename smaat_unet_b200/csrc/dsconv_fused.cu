@@ -38,7 +38,9 @@
 //                          into registers conflict-free (tc_common.cuh) and feed to wgmma's register-A form.  Storing fp32
 //                          once instead of hi and lo halves the A ring's shared-memory traffic in TF32X3 mode; the split
 //                          in the consumer is the same tf32_hi / v - hi on the same value, so results are unchanged
-// Which one runs is smaat_set_dsconv_impl's choice (csrc/dsconv_fused.cu, below).
+// Which A form a request runs in is smaat_set_dsconv_impl's choice.  ds_select (below) picks the whole instance that runs it
+// (A form, single, paired or wide tile, precision, N_TILE, PW), and the eligibility entry points ask it, so they answer for
+// that instance; ds_visit maps the choice to its DsCfg.
 // BF16 (SMAAT_PW_BF16, dsconv_bf16_kernel): the register form only; the consumers round the fp32 A tiles to bf16 as they load
 // them (two k8 fragments make one k16 fragment, tc_common.cuh bf16_frag), so the producers, the A ring and its layout are
 // those of TF32, and the B stages are half as large.
@@ -203,6 +205,8 @@ struct DsCfg {
   static_assert(IN_BYTES % 128 == 0, "TMA destination alignment");
   static_assert(TOTAL <= 227 * 1024, "shared memory budget");
   static_assert(!WIDE || ST_BUFS > 0, "wide tiles keep the staged epilogue: the max-pool and the CBAM pools are taken as at N_TILE 128");
+  static_assert(!PAIR || ST_BUFS > 0, "paired tiles keep the staged epilogue: the max-pool and the CBAM pools are taken as at N_TILE 64");
+  static_assert(!PAIR || MAX_CLASSES >= DS_MIN_CLASSES, "paired tiles take the class launches of up to DS_MIN_CLASSES classes");
 };
 
 // ----- staged output epilogue: TMA tensor stores of 32-channel x 64-pixel boxes from shared memory -----
@@ -1005,15 +1009,12 @@ static auto ds_kernel() {
   else return dsconv_fused_kernel<N_TILE, KPL, PW, P == Prec::TF32X3, A_SMEM>;
 }
 
-template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA = float, bool PAIR = false, bool WIDE = false>
-static int launch_ds(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mwl,
-                     const CUtensorMap& my, const CUtensorMap& msa, DsParams p, int B, cudaStream_t st) {
+template <int N_TILE, int KPL, int PW, Prec P, bool A_SMEM, typename TA, bool PAIR, bool WIDE>
+static int launch_ds(DsCfg<N_TILE, KPL, PW, P, A_SMEM, TA, PAIR, WIDE>, const CUtensorMap& m0, const CUtensorMap& m1,
+                     const CUtensorMap& mw, const CUtensorMap& mwl, const CUtensorMap& my, const CUtensorMap& msa, DsParams p, int B,
+                     cudaStream_t st) {
   using L = DsCfg<N_TILE, KPL, PW, P, A_SMEM, TA, PAIR, WIDE>;
   auto kern = ds_kernel<N_TILE, KPL, PW, P, A_SMEM, TA, PAIR, WIDE>();
-  // the pools and the max-pool are read back from the staging buffers: instances with the direct-store epilogue do not take them
-  if (p.pooled && !L::ST_BUFS) return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools and the max-pool need the staged epilogue");
-  if (p.ncls > L::MAX_CLASSES)
-    return fail(SMAAT_E_UNSUPPORTED, "dsconv+classify: %d classes, this instance keeps the weights of at most %d", p.ncls, L::MAX_CLASSES);
   static std::atomic<uint64_t> attr_mask{0};   // cudaFuncSetAttribute is per device
   if (first_use_on_device(attr_mask)) {
     // class launches append the class weights (CLS_SMEM); every other launch requests TOTAL, as before
@@ -1053,85 +1054,6 @@ static int pick_pw(int H, int W) {
   return best <= 1.35 ? pw : 0;
 }
 
-// Paired tiles (dsconv_pair_kernel) where they are built (N_TILE 64, k = 2, 4, the register form, tf32 / 3xTF32, fp32 maps) and
-// cover the image with no more rows than single patches: an even number of patch rows.  The pair then runs the same
-// pixels with half the chunks' fixed costs (input box, weight chunk, hand-offs) per pixel
-static bool ds_pair_on();
-static bool ds_pair(int n_tile, int k, int pw, int H, int mode, bool a_smem, bool bact) {
-  return ds_pair_on() && n_tile == 64 && (k == 2 || k == 4) && !a_smem && !bact && mode != SMAAT_PW_BF16 && ceil_div(H, TC_BM / pw) % 2 == 0;
-}
-
-// y: the activation output, or null where it is not known yet (smaat_dsconv_eligible*) or not written (the fused OutConv).  The
-// epilogue stores it by TMA, which needs a 16-byte aligned base and 16-byte multiples as strides
-static int ds_impl();
-static bool ds_wide_on();
-
-// Wide tiles (dsconv_wide_kernel) where they are built (k = 2, the register form, tf32 / 3xTF32, fp32 maps) and switched on
-// (smaat_set_dsconv_wide): 128 < Cout <= 256 in one pass instead of two, with no OutConv (no network ends in such a conv)
-static bool ds_wide(int Cout, int k, bool a_smem, bool bf16, bool bact, bool head) {
-  return ds_wide_on() && Cout > 128 && Cout <= 256 && k == 2 && !a_smem && !bf16 && !bact && !head;
-}
-
-static bool ds_eligible(const float* x0, int C0, int64_t bs0, const float* x1, int C1, int64_t bs1, const float* pw_w,
-                        const float* pw_w_lo, const float* y, int64_t y_bstride, int H, int W, int k, int Cout, bool stats,
-                        bool outconv, bool bf16 = false, bool bact = false) {
-  // k = 4 and BF16 have register-form instances only (dsconv_kpl4_kernel, dsconv_bf16_kernel): with the shared-memory A form
-  // selected they stay unfused
-  if (k != 1 && k != 2 && !(k == 4 && ds_impl() != 1)) return false;
-  if (bf16 && ds_impl() == 1) return false;
-  // bf16 activations (dsconv_bf16act_kernel): bf16 operands, k = 1, 2, no batch statistics; TMA takes 16-byte row and plane
-  // strides, so W and the batch strides are multiples of 8 elements
-  if (bact && (!bf16 || k == 4 || stats || W % 8 != 0 || bs0 % 8 != 0 || (C1 > 0 && bs1 % 8 != 0) || (y && y_bstride % 8 != 0)))
-    return false;
-  if (y && (!aligned16(y) || y_bstride % 4 != 0)) return false;
-  // Cout > 128: whole passes of 128 channels, or one wide tile for any Cout up to 256; batch statistics and the fused OutConv are
-  // taken up to 128 channels
-  if (Cout < 8 || Cout > 512 || (Cout > 128 && (stats || outconv))) return false;
-  if (Cout > 128 && Cout % 128 != 0 && !ds_wide(Cout, k, ds_impl() == 1, bf16, bact, outconv)) return false;
-  if (W % 4 != 0 || !aligned16(x0) || bs0 % 4 != 0) return false;
-  if (C1 > 0 && (!aligned16(x1) || bs1 % 4 != 0 || C0 % (TC_BK / k) != 0)) return false;
-  const int K = k * (C0 + C1);
-  // fp32 weight rows are K * 4 bytes, which TMA takes in multiples of 16; the bf16 pack's rows are padded to 32 k (bact only, so
-  // that the fp32 route keeps its choices)
-  if ((K % 4 != 0 && !bact) || !aligned16(pw_w) || (pw_w_lo && !aligned16(pw_w_lo))) return false;
-  return pick_pw(H, W) != 0;
-}
-
-// The configuration of the instance dsconv_run dispatches to, for a mode (SMAAT_PW_*) and A form (k = 4 and BF16: the register
-// form, the only one they have), handed to `f` as a DsCfg type
-template <int N_TILE, int KPL, int PW, typename F>
-static auto ds_cfg_t(int mode, bool a_smem, F f, bool bact) {
-  if constexpr (KPL != 4) {
-    if (bact) return f(DsCfg<N_TILE, KPL, PW, Prec::BF16, false, uint16_t>{});
-  }
-  if (mode == SMAAT_PW_BF16) return f(DsCfg<N_TILE, KPL, PW, Prec::BF16, false>{});
-  if constexpr (KPL == 4) {
-    return mode == SMAAT_PW_TF32X3 ? f(DsCfg<N_TILE, 4, PW, Prec::TF32X3, false>{}) : f(DsCfg<N_TILE, 4, PW, Prec::TF32, false>{});
-  } else {
-    if (mode == SMAAT_PW_TF32X3) return a_smem ? f(DsCfg<N_TILE, KPL, PW, Prec::TF32X3, true>{}) : f(DsCfg<N_TILE, KPL, PW, Prec::TF32X3, false>{});
-    return a_smem ? f(DsCfg<N_TILE, KPL, PW, Prec::TF32, true>{}) : f(DsCfg<N_TILE, KPL, PW, Prec::TF32, false>{});
-  }
-}
-template <typename F>
-static int ds_cfg(int n_tile, int k, int pw, int mode, bool a_smem, F f, bool bact = false) {
-  if (n_tile == 64) {
-    if (k == 4) return pw == 32 ? ds_cfg_t<64, 4, 32>(mode, a_smem, f, bact) : ds_cfg_t<64, 4, 16>(mode, a_smem, f, bact);
-    if (k == 2) return pw == 32 ? ds_cfg_t<64, 2, 32>(mode, a_smem, f, bact) : ds_cfg_t<64, 2, 16>(mode, a_smem, f, bact);
-    return pw == 32 ? ds_cfg_t<64, 1, 32>(mode, a_smem, f, bact) : ds_cfg_t<64, 1, 16>(mode, a_smem, f, bact);
-  }
-  if (k == 4) return pw == 32 ? ds_cfg_t<128, 4, 32>(mode, a_smem, f, bact) : ds_cfg_t<128, 4, 16>(mode, a_smem, f, bact);
-  if (k == 2) return pw == 32 ? ds_cfg_t<128, 2, 32>(mode, a_smem, f, bact) : ds_cfg_t<128, 2, 16>(mode, a_smem, f, bact);
-  return pw == 32 ? ds_cfg_t<128, 1, 32>(mode, a_smem, f, bact) : ds_cfg_t<128, 1, 16>(mode, a_smem, f, bact);
-}
-// Whether that instance has the staged epilogue (ST_BUFS > 0), which the CBAM pools and the max-pool are read from
-static bool ds_staged(int n_tile, int k, int pw, int mode, bool a_smem, bool bact = false) {
-  return ds_cfg(n_tile, k, pw, mode, a_smem, [](auto c) { return (int)decltype(c)::ST_BUFS; }, bact) > 0;
-}
-// The most classes whose OutConv weights that instance keeps in shared memory (DsCfg::MAX_CLASSES)
-static int ds_max_classes(int n_tile, int k, int pw, int mode, bool a_smem, bool bact = false) {
-  return ds_cfg(n_tile, k, pw, mode, a_smem, [](auto c) { return (int)decltype(c)::MAX_CLASSES; }, bact);
-}
-
 // Where the A operand (the depthwise result) goes to the tensor core: 0 = auto (the register form), 1 = read by wgmma from
 // shared memory through a descriptor, 2 = loaded into registers first.  SMAAT_DS_IMPL presets it.  Auto takes the register
 // form: bench.py's B = 32, 12 x 288 x 288 forward ran at 2 365-2 369 frames/s with it and 2 187-2 194 with the shared-memory
@@ -1161,7 +1083,7 @@ static bool ds_wide_on() {
   return v != 0;
 }
 
-// Whether paired tiles run where ds_pair takes them (1, the default) or one patch per tile (0).  SMAAT_DSCONV_PAIR presets it
+// Whether paired tiles run where ds_select takes them (1, the default) or one patch per tile (0).  SMAAT_DSCONV_PAIR presets it
 static std::atomic<int> g_ds_pair{-1};
 static bool ds_pair_on() {
   int v = g_ds_pair.load(std::memory_order_relaxed);
@@ -1171,6 +1093,223 @@ static bool ds_pair_on() {
     g_ds_pair.store(v, std::memory_order_relaxed);
   }
   return v != 0;
+}
+
+// One fused DS conv request, its operands by name.  x0 / x1, y, the logits (oc_y) and the max-pool are fp32, or bf16 bits where
+// bact (and pooled_bf16) say so; pw_w is fp32, or the smaat_pack_bf16 pack in SMAAT_PW_BF16.  The fields up to Cout are those
+// every entry point takes, initialised in their order there; the eligibility queries then fill the epilogue they ask about,
+// with y null (not known yet)
+struct DsReq {
+  const void* x0; int C0; int64_t x0_bstride;
+  const void* x1; int C1; int64_t x1_bstride;
+  const void* pw_w; int H, W, k, Cout;
+  int B = 0, relu = 0, mode = SMAAT_PW_TF32;
+  bool bact = false;   // bf16 activations
+  const float* dw_w = nullptr; const float* dw_b = nullptr; const float* pw_w_lo = nullptr;
+  const float* scale = nullptr; const float* shift = nullptr;
+  void* y = nullptr; int64_t y_bstride = 0;
+  // the epilogue
+  double* stats = nullptr;                                         // batch statistics
+  const float* oc_w = nullptr; const float* oc_b = nullptr;        // a head, an OutConv in place of y: one class into oc_y,
+  void* oc_y = nullptr; int ncls = 0; int64_t* cls = nullptr;      // or ncls classes into the logits oc_y and / or the map cls
+  const float* gate_sc = nullptr; const float* gate_sa = nullptr;  // the CBAM gate on x0
+  float* pool_sum = nullptr; float* pool_max = nullptr;            // the CBAM partial pools
+  void* pooled = nullptr; int pooled_bf16 = 0;                     // the max-pool
+  bool head() const { return oc_y || ncls > 0; }
+};
+
+// An eligibility query asks about batch statistics or a max-pool it has no address for yet by this one; ds_select only tests
+// those pointers for null
+alignas(16) static char g_ds_asked[16];
+
+// The kernel instance that runs a request, the DsCfg parameters ds_visit maps it to, and why ds_select declines the request if
+// it does
+enum DsDecline { DS_TAKEN, DS_SHAPE, DS_UNSTAGED, DS_CLASSES };
+struct DsInst {
+  int n_tile, k, pw;
+  Prec prec;
+  bool a_smem, bact, pair, wide;
+  DsDecline declined;
+};
+
+// ds_visit: the DsCfg type of an instance, handed to f.  With ds_kernel, the only list of the instances that are built
+template <int N_TILE, int KPL, int PW, Prec P, typename F>
+static int ds_visit_inst(const DsInst& c, F& f) {
+  if constexpr (P != Prec::BF16 && N_TILE == 128 && KPL == 2) {
+    if (c.wide) return f(DsCfg<128, 2, PW, P, false, float, false, true>{});
+  }
+  if constexpr (P != Prec::BF16 && N_TILE == 64 && KPL != 1) {
+    if (c.pair) return f(DsCfg<64, KPL, PW, P, false, float, true>{});
+  }
+  if constexpr (P == Prec::BF16 && KPL != 4) {
+    if (c.bact) return f(DsCfg<N_TILE, KPL, PW, P, false, uint16_t>{});
+  }
+  if constexpr (P != Prec::BF16 && KPL != 4) {
+    if (c.a_smem) return f(DsCfg<N_TILE, KPL, PW, P, true>{});
+  }
+  return f(DsCfg<N_TILE, KPL, PW, P, false>{});
+}
+template <int N_TILE, int KPL, int PW, typename F>
+static int ds_visit_prec(const DsInst& c, F& f) {
+  if (c.prec == Prec::BF16) return ds_visit_inst<N_TILE, KPL, PW, Prec::BF16>(c, f);
+  if (c.prec == Prec::TF32X3) return ds_visit_inst<N_TILE, KPL, PW, Prec::TF32X3>(c, f);
+  return ds_visit_inst<N_TILE, KPL, PW, Prec::TF32>(c, f);
+}
+template <typename F>
+static int ds_visit(const DsInst& c, F f) {
+  if (c.n_tile == 64) {
+    if (c.k == 4) return c.pw == 32 ? ds_visit_prec<64, 4, 32>(c, f) : ds_visit_prec<64, 4, 16>(c, f);
+    if (c.k == 2) return c.pw == 32 ? ds_visit_prec<64, 2, 32>(c, f) : ds_visit_prec<64, 2, 16>(c, f);
+    return c.pw == 32 ? ds_visit_prec<64, 1, 32>(c, f) : ds_visit_prec<64, 1, 16>(c, f);
+  }
+  if (c.k == 4) return c.pw == 32 ? ds_visit_prec<128, 4, 32>(c, f) : ds_visit_prec<128, 4, 16>(c, f);
+  if (c.k == 2) return c.pw == 32 ? ds_visit_prec<128, 2, 32>(c, f) : ds_visit_prec<128, 2, 16>(c, f);
+  return c.pw == 32 ? ds_visit_prec<128, 1, 32>(c, f) : ds_visit_prec<128, 1, 16>(c, f);
+}
+
+// The most classes whose OutConv weights an instance keeps in shared memory
+static int ds_max_classes(const DsInst& c) {
+  return ds_visit(c, [](auto cfg) { return (int)decltype(cfg)::MAX_CLASSES; });
+}
+
+// The instance that runs a request (wide, else paired, else single tiles), or why none does.  The epilogue's limits are those
+// of that instance: the CBAM pools and the max-pool are read back from its staging buffers (ST_BUFS > 0), and the class
+// weights must fit beside its rings (MAX_CLASSES)
+static DsInst ds_select(const DsReq& r) {
+  const bool a_smem = ds_impl() == 1, bf16 = r.mode == SMAAT_PW_BF16, head = r.head(), stats = r.stats;
+  const int k = r.k, Cout = r.Cout;
+  const Prec prec = bf16 ? Prec::BF16 : r.mode == SMAAT_PW_TF32X3 ? Prec::TF32X3 : Prec::TF32;
+  DsInst c{Cout > 64 ? 128 : 64, k, pick_pw(r.H, r.W), prec, a_smem, r.bact, false, false, DS_SHAPE};
+  // k = 4 and BF16 have register-form instances only (dsconv_kpl4_kernel, dsconv_bf16_kernel): with the shared-memory A form
+  // selected they stay unfused
+  if ((k != 1 && k != 2 && k != 4) || (a_smem && (k == 4 || bf16))) return c;
+  // bf16 activations (dsconv_bf16act_kernel): bf16 operands, k = 1, 2, no batch statistics; TMA takes 16-byte row and plane
+  // strides, so W and the batch strides are multiples of 8 elements
+  if (r.bact && (!bf16 || k == 4 || stats || r.W % 8 != 0 || r.x0_bstride % 8 != 0 || (r.C1 > 0 && r.x1_bstride % 8 != 0) ||
+                 (r.y && r.y_bstride % 8 != 0)))
+    return c;
+  // y: the epilogue stores it by TMA, which needs a 16-byte aligned base and 16-byte multiples as strides
+  if (r.y && (!aligned16(r.y) || r.y_bstride % 4 != 0)) return c;
+  // Wide tiles (dsconv_wide_kernel) where they are built (k = 2, the register form, tf32 / 3xTF32, fp32 maps) and switched on
+  // (smaat_set_dsconv_wide): 128 < Cout <= 256 in one pass instead of two, with no OutConv (no network ends in such a conv)
+  c.wide = ds_wide_on() && Cout > 128 && Cout <= 256 && k == 2 && !a_smem && !bf16 && !head;
+  // Cout > 128: whole passes of 128 channels, or one wide tile for any Cout up to 256; batch statistics and the fused OutConv are
+  // taken up to 128 channels
+  if (Cout < 8 || Cout > 512 || (Cout > 128 && (stats || head))) return c;
+  if (Cout > 128 && Cout % 128 != 0 && !c.wide) return c;
+  if (r.W % 4 != 0 || !aligned16(r.x0) || r.x0_bstride % 4 != 0) return c;
+  if (r.C1 > 0 && (!aligned16(r.x1) || r.x1_bstride % 4 != 0 || r.C0 % (TC_BK / k) != 0)) return c;
+  // fp32 weight rows are K * 4 bytes, which TMA takes in multiples of 16; the bf16 pack's rows are padded to 32 k (bact only, so
+  // that the fp32 route keeps its choices)
+  if ((k * (r.C0 + r.C1) % 4 != 0 && !r.bact) || !aligned16(r.pw_w) || (r.pw_w_lo && !aligned16(r.pw_w_lo))) return c;
+  if (!c.pw) return c;
+  // Paired tiles (dsconv_pair_kernel) where they are built (N_TILE 64, k = 2, 4, the register form, tf32 / 3xTF32, fp32 maps)
+  // and they cover the image with no more rows than single patches: an even number of patch rows.  The pair then runs the same
+  // pixels with half the chunks' fixed costs (input box, weight chunk, hand-offs) per pixel.  Its rings leave room for the
+  // weights of DS_MIN_CLASSES classes, not always 32: more classes take the single tile
+  c.pair = ds_pair_on() && c.n_tile == 64 && (k == 2 || k == 4) && !a_smem && !bf16 && ceil_div(r.H, TC_BM / c.pw) % 2 == 0 &&
+           r.ncls <= DS_MIN_CLASSES;
+  const bool staged = ds_visit(c, [](auto cfg) { return (int)decltype(cfg)::ST_BUFS; }) > 0;
+  c.declined = r.pooled && !staged ? DS_UNSTAGED : r.ncls > ds_max_classes(c) ? DS_CLASSES : DS_TAKEN;
+  return c;
+}
+
+// Launches the request on the instance ds_select takes, after the argument checks; a declined request launches nothing
+static int ds_launch(const DsReq& r, void* stream) {
+  const int B = r.B, C0 = r.C0, C1 = r.C1, H = r.H, W = r.W, k = r.k, Cout = r.Cout;
+  const bool head = r.head(), bf16 = r.mode == SMAAT_PW_BF16;
+  SMAAT_REQUIRE(r.x0 && r.dw_w && r.pw_w && (r.y || r.oc_y || r.cls), "dsconv: null pointer");
+  SMAAT_REQUIRE(!r.gate_sc == !r.gate_sa, "dsconv: the CBAM gate needs both sc and sa");
+  SMAAT_REQUIRE(!r.gate_sa || aligned16(r.gate_sa), "dsconv: the CBAM gate map must be 16-byte aligned");
+  SMAAT_REQUIRE(!r.pool_sum || (r.pool_max && r.pooled && r.y && !r.oc_y && !r.stats),
+                "dsconv: the CBAM pools need sum, max and max-pool outputs and y");
+  SMAAT_REQUIRE(!r.pooled || (r.y && !head && !r.stats), "dsconv: the max-pool needs y, and no OutConv or batch statistics");
+  SMAAT_REQUIRE(!r.pooled_bf16 || r.bact, "dsconv: a bf16 max-pool needs bf16 activations");
+  SMAAT_REQUIRE(!r.pooled || (reinterpret_cast<uintptr_t>(r.pooled) & (r.pooled_bf16 ? 3u : 7u)) == 0,
+                "dsconv: the max-pool output must be %d-byte aligned", r.pooled_bf16 ? 4 : 8);
+  SMAAT_REQUIRE(B > 0 && C0 > 0 && C1 >= 0 && H > 0 && W > 0 && Cout > 0, "dsconv: bad shape");
+  SMAAT_REQUIRE(C1 == 0 || r.x1, "dsconv: C1=%d but x1 is null", C1);
+  SMAAT_REQUIRE(r.mode == SMAAT_PW_TF32 || r.mode == SMAAT_PW_TF32X3 || r.mode == SMAAT_PW_BF16,
+                "dsconv: mode must be SMAAT_PW_TF32, SMAAT_PW_TF32X3 or SMAAT_PW_BF16");
+  SMAAT_REQUIRE(r.mode != SMAAT_PW_TF32X3 || r.pw_w_lo, "dsconv: TF32X3 needs pw_w_lo (see smaat_split_tf32)");
+  SMAAT_REQUIRE(head || r.y_bstride >= (int64_t)Cout * H * W, "dsconv: y batch stride too small");
+  SMAAT_REQUIRE(!head || (r.oc_w && !r.stats), "dsconv+outconv: needs the OutConv weight and no batch statistics");
+  SMAAT_REQUIRE(!r.bact || (bf16 && !r.stats && !r.pool_sum), "dsconv: bf16 activations take bf16 operands, no statistics and no pools");
+  const DsInst c = ds_select(r);
+  if (c.declined == DS_SHAPE)
+    return fail(SMAAT_E_UNSUPPORTED,
+                r.bact ? "dsconv_bf16: not taken by the bf16-activation kernel (k=%d Cout=%d H=%d W=%d; needs k = 1 or 2, W and the "
+                         "batch strides multiples of 8, 16-byte aligned tensors, the register A form)"
+                       : "dsconv: shape or output layout not taken by the fused kernel (k=%d Cout=%d H=%d W=%d, y 16-byte aligned "
+                         "with a batch stride that is a multiple of 4); use dw3x3 + pw1x1",
+                k, Cout, H, W);
+  if (c.declined == DS_UNSTAGED)
+    return fail(SMAAT_E_UNSUPPORTED, "dsconv: the CBAM pools and the max-pool need the staged epilogue");
+  if (c.declined == DS_CLASSES)
+    return fail(SMAAT_E_UNSUPPORTED, "dsconv+classify: %d classes, this instance keeps the weights of at most %d", r.ncls,
+                ds_max_classes(c));
+  const int pw = c.pw, ph = TC_BM / pw, cc = TC_BK / k, K = k * (C0 + C1);
+  const int th = c.pair ? 2 * ph : ph;   // a paired tile's boxes span both patches
+  // activation maps: fp32, or bf16 (bact)
+  const CUtensorMapDataType adt = r.bact ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  const uint64_t esz = r.bact ? 2 : 4;
+
+  CUtensorMap m0, m1, mw, mwl;
+  const int xm = 16 / (int)esz;   // DsCfg::XM
+  const uint32_t box[4] = {(uint32_t)(pw + 2 * xm), (uint32_t)(th + 2), (uint32_t)cc, 1u};
+  {
+    const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)C0, (uint64_t)B};
+    const uint64_t str[4] = {0, (uint64_t)W * esz, (uint64_t)H * W * esz, (uint64_t)r.x0_bstride * esz};
+    int e = make_tmap(&m0, adt, r.x0, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(x0)");
+    if (e) return e;
+    m1 = m0;
+  }
+  if (C1 > 0) {
+    const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)C1, (uint64_t)B};
+    const uint64_t str[4] = {0, (uint64_t)W * esz, (uint64_t)H * W * esz, (uint64_t)r.x1_bstride * esz};
+    int e = make_tmap(&m1, adt, r.x1, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(x1)");
+    if (e) return e;
+  }
+  {
+    const uint64_t kw = bf16 ? (uint64_t)(K + TC_BK - 1) / TC_BK * TC_BK : (uint64_t)K;   // the bf16 pack's row length
+    const uint64_t dims[2] = {kw, (uint64_t)Cout};
+    const uint64_t str[2] = {0, kw * (bf16 ? 2 : 4)};
+    const uint32_t wbox[2] = {(uint32_t)TC_BK, (uint32_t)c.n_tile};
+    int e = bf16 ? make_tmap(&mw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, r.pw_w, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_64B, "dsconv(w bf16)")
+                 : make_tmap_f32(&mw, r.pw_w, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "dsconv(w)");
+    if (e) return e;
+    mwl = mw;
+    if (r.mode == SMAAT_PW_TF32X3) {
+      e = make_tmap_f32(&mwl, r.pw_w_lo, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "dsconv(w_lo)");
+      if (e) return e;
+    }
+  }
+  // the staged epilogue's store box: one warpgroup's half-patch (PW x PH / 2 pixels) x 32 channels, swizzled by its row length
+  CUtensorMap my = m0;
+  if (!head) {
+    const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)Cout, (uint64_t)B};
+    const uint64_t str[4] = {0, (uint64_t)W * esz, (uint64_t)H * W * esz, (uint64_t)r.y_bstride * esz};
+    const uint32_t ybox[4] = {(uint32_t)pw, (uint32_t)(ph / 2), 32u, 1u};
+    // bf16 boxes are staged unswizzled (the epilogue's bf16 branch)
+    const CUtensorMapSwizzle ysw = r.bact ? CU_TENSOR_MAP_SWIZZLE_NONE : pw == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    int e = make_tmap(&my, adt, r.y, 4, dims, str, ybox, ysw, "dsconv(y)");
+    if (e) return e;
+  }
+  // the CBAM spatial gate sa (B, 1, H, W): one-channel halo boxes at the input boxes' origin
+  CUtensorMap msa = m0;
+  if (r.gate_sa) {
+    const uint64_t dims[3] = {(uint64_t)W, (uint64_t)H, (uint64_t)B};
+    const uint64_t str[3] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4};
+    const uint32_t sbox[3] = {(uint32_t)(pw + 2 * xm), (uint32_t)(th + 2), 1u};
+    int e = make_tmap_f32(&msa, r.gate_sa, 3, dims, str, sbox, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(gate sa)");
+    if (e) return e;
+  }
+  DsParams p{};
+  p.dw_w = r.dw_w; p.dw_b = r.dw_b; p.scale = r.scale; p.shift = r.shift; p.y = static_cast<float*>(r.y); p.y_bstride = r.y_bstride;
+  p.stats = r.stats; p.oc_w = r.oc_w; p.oc_b = r.oc_b; p.oc_y = static_cast<float*>(r.oc_y); p.ncls = r.ncls; p.cls = r.cls;
+  p.gate_sc = r.gate_sc; p.pool_sum = r.pool_sum; p.pool_max = r.pool_max; p.pooled = static_cast<float*>(r.pooled);
+  p.pooled_bf16 = r.pooled_bf16; p.C0 = C0; p.C1 = C1; p.H = H; p.W = W; p.Cout = Cout; p.relu = r.relu; p.K = K;
+  return ds_visit(c, [&](auto cfg) { return launch_ds(cfg, m0, m1, mw, mwl, my, msa, p, B, (cudaStream_t)stream); });
 }
 
 }  // namespace smaat
@@ -1197,8 +1336,9 @@ extern "C" int smaat_set_dsconv_pair(int enabled) {
 
 extern "C" int smaat_dsconv_eligible2(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                                       const float* pw_w, int H, int W, int k, int Cout, int with_stats) {
-  return ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, with_stats != 0, false) ? 1
-                                                                                                                                : 0;
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.stats = with_stats ? reinterpret_cast<double*>(g_ds_asked) : nullptr;
+  return ds_select(q).declined == DS_TAKEN;
 }
 
 extern "C" int smaat_dsconv_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
@@ -1209,12 +1349,10 @@ extern "C" int smaat_dsconv_eligible(const float* x0, int C0, int64_t x0_bstride
 extern "C" int smaat_dsconv_cbam_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                                           const float* pw_w, int H, int W, int k, int Cout, int mode, int with_gate, int with_pools) {
   if (mode != SMAAT_PW_TF32 && mode != SMAAT_PW_TF32X3 && mode != SMAAT_PW_BF16) return 0;
-  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, false, false,
-                   mode == SMAAT_PW_BF16))
-    return 0;
   (void)with_gate;   // every fused instance takes the gate
-  if (with_pools && !ds_staged(Cout > 64 ? 128 : 64, k, pick_pw(H, W), mode, ds_impl() == 1)) return 0;
-  return 1;
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.mode = mode; q.pooled = with_pools ? g_ds_asked : nullptr;
+  return ds_select(q).declined == DS_TAKEN;
 }
 
 extern "C" int smaat_dsconv_pool_parts(int H, int W) {
@@ -1222,164 +1360,15 @@ extern "C" int smaat_dsconv_pool_parts(int H, int W) {
   return pw ? 2 * ceil_div(W, pw) * ceil_div(H, TC_BM / pw) : 0;
 }
 
-static int dsconv_run(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride, const float* dw_w,
-                      const float* dw_b, const float* pw_w, const float* pw_w_lo, const float* scale, const float* shift, float* y,
-                      int64_t y_bstride, double* stats, const float* oc_w, const float* oc_b, float* oc_y, int ncls, int64_t* cls,
-                      const float* gate_sc, const float* gate_sa, float* pool_sum, float* pool_max, float* pooled, int B, int H, int W,
-                      int k, int Cout, int relu, int mode, void* stream, bool bact = false, int pooled_bf16 = 0) {
-  // head: an OutConv in the epilogue (one class, or ncls classes with the argmax) replaces the activation output
-  const bool head = oc_y || ncls > 0;
-  SMAAT_REQUIRE(x0 && dw_w && pw_w && (y || oc_y || cls), "dsconv: null pointer");
-  SMAAT_REQUIRE(!gate_sc == !gate_sa, "dsconv: the CBAM gate needs both sc and sa");
-  SMAAT_REQUIRE(!gate_sa || aligned16(gate_sa), "dsconv: the CBAM gate map must be 16-byte aligned");
-  SMAAT_REQUIRE(!pool_sum || (pool_max && pooled && y && !oc_y && !stats), "dsconv: the CBAM pools need sum, max and max-pool outputs and y");
-  SMAAT_REQUIRE(!pooled || (y && !head && !stats), "dsconv: the max-pool needs y, and no OutConv or batch statistics");
-  SMAAT_REQUIRE(!pooled_bf16 || bact, "dsconv: a bf16 max-pool needs bf16 activations");
-  SMAAT_REQUIRE(!pooled || (reinterpret_cast<uintptr_t>(pooled) & (pooled_bf16 ? 3u : 7u)) == 0,
-                "dsconv: the max-pool output must be %d-byte aligned", pooled_bf16 ? 4 : 8);
-  SMAAT_REQUIRE(B > 0 && C0 > 0 && C1 >= 0 && H > 0 && W > 0 && Cout > 0, "dsconv: bad shape");
-  SMAAT_REQUIRE(C1 == 0 || x1, "dsconv: C1=%d but x1 is null", C1);
-  SMAAT_REQUIRE(mode == SMAAT_PW_TF32 || mode == SMAAT_PW_TF32X3 || mode == SMAAT_PW_BF16,
-                "dsconv: mode must be SMAAT_PW_TF32, SMAAT_PW_TF32X3 or SMAAT_PW_BF16");
-  SMAAT_REQUIRE(mode != SMAAT_PW_TF32X3 || pw_w_lo, "dsconv: TF32X3 needs pw_w_lo (see smaat_split_tf32)");
-  SMAAT_REQUIRE(head || y_bstride >= (int64_t)Cout * H * W, "dsconv: y batch stride too small");
-  SMAAT_REQUIRE(!head || (oc_w && !stats),"dsconv+outconv: needs the OutConv weight and no batch statistics");
-  const bool bf16 = mode == SMAAT_PW_BF16;
-  SMAAT_REQUIRE(!bact || (bf16 && !stats && !pool_sum), "dsconv: bf16 activations take bf16 operands, no statistics and no pools");
-  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, pw_w_lo, head ? nullptr : y, y_bstride, H, W, k, Cout,
-                   stats != nullptr, head, bf16, bact)) {
-    if (bact)
-      return fail(SMAAT_E_UNSUPPORTED,
-                  "dsconv_bf16: not taken by the bf16-activation kernel (k=%d Cout=%d H=%d W=%d; needs k = 1 or 2, W and the batch "
-                  "strides multiples of 8, 16-byte aligned tensors, the register A form)",
-                  k, Cout, H, W);
-    return fail(SMAAT_E_UNSUPPORTED,
-                "dsconv: shape or output layout not taken by the fused kernel (k=%d Cout=%d H=%d W=%d, y 16-byte aligned with a "
-                "batch stride that is a multiple of 4); use dw3x3 + pw1x1",
-                k, Cout, H, W);
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  const int pw = pick_pw(H, W);
-  const int ph = TC_BM / pw;
-  const int n_tile = Cout > 64 ? 128 : 64;
-  const int cc = TC_BK / k;
-  const bool x3 = mode == SMAAT_PW_TF32X3;
-  const bool a_smem = ds_impl() == 1;
-  // a paired tile's boxes span both patches.  Its rings leave room for the weights of DS_MIN_CLASSES classes, not always 32: more
-  // classes take the single tile
-  const bool pair = ds_pair(n_tile, k, pw, H, mode, a_smem, bact) && ncls <= DS_MIN_CLASSES;
-  const bool wide = ds_wide(Cout, k, a_smem, bf16, bact, head);
-  const int th = pair ? 2 * ph : ph;
-  const int K = k * (C0 + C1);
-  // activation maps: fp32, or bf16 (bact)
-  const CUtensorMapDataType adt = bact ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  const uint64_t esz = bact ? 2 : 4;
-
-  CUtensorMap m0, m1, mw, mwl;
-  const int xm = 16 / (int)esz;   // DsCfg::XM
-  const uint32_t box[4] = {(uint32_t)(pw + 2 * xm), (uint32_t)(th + 2), (uint32_t)cc, 1u};
-  {
-    const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)C0, (uint64_t)B};
-    const uint64_t str[4] = {0, (uint64_t)W * esz, (uint64_t)H * W * esz, (uint64_t)x0_bstride * esz};
-    int r = make_tmap(&m0, adt, x0, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(x0)");
-    if (r) return r;
-    m1 = m0;
-  }
-  if (C1 > 0) {
-    const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)C1, (uint64_t)B};
-    const uint64_t str[4] = {0, (uint64_t)W * esz, (uint64_t)H * W * esz, (uint64_t)x1_bstride * esz};
-    int r = make_tmap(&m1, adt, x1, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(x1)");
-    if (r) return r;
-  }
-  {
-    const uint64_t kw = bf16 ? (uint64_t)(K + TC_BK - 1) / TC_BK * TC_BK : (uint64_t)K;   // the bf16 pack's row length
-    const uint64_t dims[2] = {kw, (uint64_t)Cout};
-    const uint64_t str[2] = {0, kw * (bf16 ? 2 : 4)};
-    const uint32_t wbox[2] = {(uint32_t)TC_BK, (uint32_t)n_tile};
-    int r = bf16 ? make_tmap(&mw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, pw_w, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_64B, "dsconv(w bf16)")
-                 : make_tmap_f32(&mw, pw_w, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "dsconv(w)");
-    if (r) return r;
-    mwl = mw;
-    if (x3) {
-      r = make_tmap_f32(&mwl, pw_w_lo, 2, dims, str, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "dsconv(w_lo)");
-      if (r) return r;
-    }
-  }
-  // the staged epilogue's store box: one warpgroup's half-patch (PW x PH / 2 pixels) x 32 channels, swizzled by its row length
-  CUtensorMap my = m0;
-  if (!head) {
-    const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)Cout, (uint64_t)B};
-    const uint64_t str[4] = {0, (uint64_t)W * esz, (uint64_t)H * W * esz, (uint64_t)y_bstride * esz};
-    const uint32_t ybox[4] = {(uint32_t)pw, (uint32_t)(ph / 2), 32u, 1u};
-    // bf16 boxes are staged unswizzled (the epilogue's bf16 branch)
-    const CUtensorMapSwizzle ysw = bact ? CU_TENSOR_MAP_SWIZZLE_NONE : pw == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-    int r = make_tmap(&my, adt, y, 4, dims, str, ybox, ysw, "dsconv(y)");
-    if (r) return r;
-  }
-  // the CBAM spatial gate sa (B, 1, H, W): one-channel halo boxes at the input boxes' origin
-  CUtensorMap msa = m0;
-  if (gate_sa) {
-    const uint64_t dims[3] = {(uint64_t)W, (uint64_t)H, (uint64_t)B};
-    const uint64_t str[3] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4};
-    const uint32_t sbox[3] = {(uint32_t)(pw + 2 * xm), (uint32_t)(th + 2), 1u};
-    int r = make_tmap_f32(&msa, gate_sa, 3, dims, str, sbox, CU_TENSOR_MAP_SWIZZLE_NONE, "dsconv(gate sa)");
-    if (r) return r;
-  }
-  DsParams p;
-  p.dw_w = dw_w; p.dw_b = dw_b; p.scale = scale; p.shift = shift; p.y = y; p.y_bstride = y_bstride; p.stats = stats;
-  p.oc_w = oc_w; p.oc_b = oc_b; p.oc_y = oc_y; p.ncls = ncls; p.cls = cls;
-  p.gate_sc = gate_sc; p.pool_sum = pool_sum; p.pool_max = pool_max; p.pooled = pooled; p.pooled_bf16 = pooled_bf16; p.npart = 0;
-  p.C0 = C0; p.C1 = C1; p.H = H; p.W = W; p.Cout = Cout; p.relu = relu; p.K = K;
-  p.tiles_x = p.tiles_y = p.npass = p.total_tiles = p.nchunks = 0;
-
-#define DS_DISPATCH(NT, KP, PWv)                                                                           \
-  if (bact) return launch_ds<NT, KP, PWv, Prec::BF16, false, uint16_t>(m0, m1, mw, mwl, my, msa, p, B, st);         \
-  if (bf16) return launch_ds<NT, KP, PWv, Prec::BF16, false>(m0, m1, mw, mwl, my, msa, p, B, st);                    \
-  return x3 ? (a_smem ? launch_ds<NT, KP, PWv, Prec::TF32X3, true>(m0, m1, mw, mwl, my, msa, p, B, st)               \
-                      : launch_ds<NT, KP, PWv, Prec::TF32X3, false>(m0, m1, mw, mwl, my, msa, p, B, st))             \
-            : (a_smem ? launch_ds<NT, KP, PWv, Prec::TF32, true>(m0, m1, mw, mwl, my, msa, p, B, st)                 \
-                      : launch_ds<NT, KP, PWv, Prec::TF32, false>(m0, m1, mw, mwl, my, msa, p, B, st))
-// k = 4: the register form (ds_eligible)
-#define DS_DISPATCH4(NT, PWv)                                                                                  \
-  if (bf16) return launch_ds<NT, 4, PWv, Prec::BF16, false>(m0, m1, mw, mwl, my, msa, p, B, st);                  \
-  return x3 ? launch_ds<NT, 4, PWv, Prec::TF32X3, false>(m0, m1, mw, mwl, my, msa, p, B, st)                  \
-            : launch_ds<NT, 4, PWv, Prec::TF32, false>(m0, m1, mw, mwl, my, msa, p, B, st)
-#define DS_DISPATCH_PAIR(KP, PWv)                                                                                      \
-  return x3 ? launch_ds<64, KP, PWv, Prec::TF32X3, false, float, true>(m0, m1, mw, mwl, my, msa, p, B, st)                 \
-            : launch_ds<64, KP, PWv, Prec::TF32, false, float, true>(m0, m1, mw, mwl, my, msa, p, B, st)
-  if (wide) {
-    if (pw == 32) {
-      return x3 ? launch_ds<128, 2, 32, Prec::TF32X3, false, float, false, true>(m0, m1, mw, mwl, my, msa, p, B, st)
-                : launch_ds<128, 2, 32, Prec::TF32, false, float, false, true>(m0, m1, mw, mwl, my, msa, p, B, st);
-    }
-    return x3 ? launch_ds<128, 2, 16, Prec::TF32X3, false, float, false, true>(m0, m1, mw, mwl, my, msa, p, B, st)
-              : launch_ds<128, 2, 16, Prec::TF32, false, float, false, true>(m0, m1, mw, mwl, my, msa, p, B, st);
-  }
-  if (pair) {
-    if (k == 4) { if (pw == 32) { DS_DISPATCH_PAIR(4, 32); } else { DS_DISPATCH_PAIR(4, 16); } }
-    else        { if (pw == 32) { DS_DISPATCH_PAIR(2, 32); } else { DS_DISPATCH_PAIR(2, 16); } }
-  }
-  if (n_tile == 64) {
-    if (k == 4)      { if (pw == 32) { DS_DISPATCH4(64, 32); } else { DS_DISPATCH4(64, 16); } }
-    else if (k == 2) { if (pw == 32) { DS_DISPATCH(64, 2, 32); } else { DS_DISPATCH(64, 2, 16); } }
-    else             { if (pw == 32) { DS_DISPATCH(64, 1, 32); } else { DS_DISPATCH(64, 1, 16); } }
-  } else {
-    if (k == 4)      { if (pw == 32) { DS_DISPATCH4(128, 32); } else { DS_DISPATCH4(128, 16); } }
-    else if (k == 2) { if (pw == 32) { DS_DISPATCH(128, 2, 32); } else { DS_DISPATCH(128, 2, 16); } }
-    else             { if (pw == 32) { DS_DISPATCH(128, 1, 32); } else { DS_DISPATCH(128, 1, 16); } }
-  }
-#undef DS_DISPATCH_PAIR
-#undef DS_DISPATCH4
-#undef DS_DISPATCH
-}
-
 extern "C" int smaat_dsconv_fwd(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                                 const float* dw_w, const float* dw_b, const float* pw_w, const float* pw_w_lo,
                                 const float* scale, const float* shift, float* y, int64_t y_bstride, double* stats, int B, int H,
                                 int W, int k, int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(y, "dsconv: null output");
-  return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, stats, nullptr,
-                    nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.B = B; q.relu = relu; q.mode = mode; q.dw_w = dw_w; q.dw_b = dw_b; q.pw_w_lo = pw_w_lo; q.scale = scale; q.shift = shift;
+  q.y = y; q.y_bstride = y_bstride; q.stats = stats;
+  return ds_launch(q, stream);
 }
 
 /* The network's last two modules in one kernel: DS conv -> BN/ReLU -> OutConv(Cout -> 1) (reference models/SmaAt_UNet.py:55-56,
@@ -1390,18 +1379,19 @@ extern "C" int smaat_dsconv_outconv_fwd(const float* x0, int C0, int64_t x0_bstr
                                         const float* scale, const float* shift, const float* oc_w, const float* oc_b,
                                         float* logits, int B, int H, int W, int k, int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(oc_w && logits, "dsconv+outconv: null pointer");
-  return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
-                    logits, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.B = B; q.relu = relu; q.mode = mode; q.dw_w = dw_w; q.dw_b = dw_b; q.pw_w_lo = pw_w_lo; q.scale = scale; q.shift = shift;
+  q.oc_w = oc_w; q.oc_b = oc_b; q.oc_y = logits;
+  return ds_launch(q, stream);
 }
 
 extern "C" int smaat_dsconv_classify_eligible(const float* x0, int C0, int64_t x0_bstride, const float* x1, int C1, int64_t x1_bstride,
                                               const float* pw_w, int H, int W, int k, int Cout, int K, int mode) {
   if (mode != SMAAT_PW_TF32 && mode != SMAAT_PW_TF32X3 && mode != SMAAT_PW_BF16) return 0;
   if (K < 1 || K > DS_MAX_CLASSES) return 0;
-  if (!ds_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, nullptr, nullptr, 0, H, W, k, Cout, false, true, mode == SMAAT_PW_BF16))
-    return 0;
-  // the class weights must fit the shared memory the instance leaves free: 22 to 32 classes, by instance (DsCfg::MAX_CLASSES)
-  return K <= ds_max_classes(Cout > 64 ? 128 : 64, k, pick_pw(H, W), mode, ds_impl() == 1) ? 1 : 0;
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.mode = mode; q.ncls = K;
+  return ds_select(q).declined == DS_TAKEN;
 }
 
 /* The network's last two modules for a K-class model, ending in the class map: DS conv -> BN/ReLU -> OutConv(Cout -> K) ->
@@ -1420,8 +1410,10 @@ extern "C" int smaat_dsconv_classify_fwd(const float* x0, int C0, int64_t x0_bst
   SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(oc_w) & 3u) == 0 && (reinterpret_cast<uintptr_t>(logits) & 3u) == 0 &&
                     (reinterpret_cast<uintptr_t>(classes) & 7u) == 0,
                 "dsconv+classify: weights / logits must be 4-byte and classes 8-byte aligned");
-  return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
-                    logits, K, classes, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, mode, stream);
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.B = B; q.relu = relu; q.mode = mode; q.dw_w = dw_w; q.dw_b = dw_b; q.pw_w_lo = pw_w_lo; q.scale = scale; q.shift = shift;
+  q.oc_w = oc_w; q.oc_b = oc_b; q.oc_y = logits; q.ncls = K; q.cls = classes;
+  return ds_launch(q, stream);
 }
 
 /* The fused DS conv of the serving forward with the CBAM fusions around it (models/layers.py:90-141, SmaAt_UNet.py:41-57).
@@ -1435,8 +1427,11 @@ extern "C" int smaat_dsconv_cbam_fwd(const float* x0, int C0, int64_t x0_bstride
                                      const float* gate_sa, float* pool_sum, float* pool_max, float* pooled, int B, int H, int W, int k,
                                      int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(y, "dsconv_cbam: null output");
-  return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, nullptr, nullptr,
-                    nullptr, nullptr, 0, nullptr, gate_sc, gate_sa, pool_sum, pool_max, pooled, B, H, W, k, Cout, relu, mode, stream);
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.B = B; q.relu = relu; q.mode = mode; q.dw_w = dw_w; q.dw_b = dw_b; q.pw_w_lo = pw_w_lo; q.scale = scale; q.shift = shift;
+  q.y = y; q.y_bstride = y_bstride; q.gate_sc = gate_sc; q.gate_sa = gate_sa; q.pool_sum = pool_sum; q.pool_max = pool_max;
+  q.pooled = pooled;
+  return ds_launch(q, stream);
 }
 
 /* The fused DS conv that also writes MaxPool2d(2) of its output, for the DownDS that reads it next (UNetDS's encoder, which has
@@ -1453,8 +1448,10 @@ extern "C" int smaat_dsconv_maxpool_fwd(const float* x0, int C0, int64_t x0_bstr
                                         const float* scale, const float* shift, float* y, int64_t y_bstride, float* pooled, int B,
                                         int H, int W, int k, int Cout, int relu, int mode, void* stream) {
   SMAAT_REQUIRE(y && pooled, "dsconv_maxpool: null output");
-  return dsconv_run(x0, C0, x0_bstride, x1, C1, x1_bstride, dw_w, dw_b, pw_w, pw_w_lo, scale, shift, y, y_bstride, nullptr, nullptr,
-                    nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, pooled, B, H, W, k, Cout, relu, mode, stream);
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.B = B; q.relu = relu; q.mode = mode; q.dw_w = dw_w; q.dw_b = dw_b; q.pw_w_lo = pw_w_lo; q.scale = scale; q.shift = shift;
+  q.y = y; q.y_bstride = y_bstride; q.pooled = pooled;
+  return ds_launch(q, stream);
 }
 
 /* ---- bf16 activations: the serving forward's bf16 route -------------------------------------------------------------------
@@ -1465,10 +1462,9 @@ extern "C" int smaat_dsconv_maxpool_fwd(const float* x0, int C0, int64_t x0_bstr
 extern "C" int smaat_dsconv_bf16_eligible(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
                                           const void* pw_w, int H, int W, int k, int Cout, int ncls) {
   if (ncls < 0 || ncls > DS_MAX_CLASSES) return 0;
-  if (!ds_eligible(static_cast<const float*>(x0), C0, x0_bstride, static_cast<const float*>(x1), C1, x1_bstride,
-                   static_cast<const float*>(pw_w), nullptr, nullptr, 0, H, W, k, Cout, false, ncls > 0, true, true))
-    return 0;
-  return ncls <= ds_max_classes(Cout > 64 ? 128 : 64, k, pick_pw(H, W), SMAAT_PW_BF16, false, true) ? 1 : 0;
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.mode = SMAAT_PW_BF16; q.bact = true; q.ncls = ncls;
+  return ds_select(q).declined == DS_TAKEN;
 }
 
 extern "C" int smaat_dsconv_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
@@ -1476,10 +1472,10 @@ extern "C" int smaat_dsconv_bf16_fwd(const void* x0, int C0, int64_t x0_bstride,
                                      const float* shift, void* y, int64_t y_bstride, const float* gate_sc, const float* gate_sa,
                                      int B, int H, int W, int k, int Cout, int relu, void* stream) {
   SMAAT_REQUIRE(y, "dsconv_bf16: null output");
-  return dsconv_run(static_cast<const float*>(x0), C0, x0_bstride, static_cast<const float*>(x1), C1, x1_bstride, dw_w, dw_b,
-                    reinterpret_cast<const float*>(pw_w), nullptr, scale, shift, static_cast<float*>(y), y_bstride, nullptr, nullptr,
-                    nullptr, nullptr, 0, nullptr, gate_sc, gate_sa, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu, SMAAT_PW_BF16,
-                    stream, true);
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.B = B; q.relu = relu; q.mode = SMAAT_PW_BF16; q.bact = true; q.dw_w = dw_w; q.dw_b = dw_b; q.scale = scale; q.shift = shift;
+  q.y = y; q.y_bstride = y_bstride; q.gate_sc = gate_sc; q.gate_sa = gate_sa;
+  return ds_launch(q, stream);
 }
 
 /* smaat_dsconv_outconv_fwd from bf16 activations: the (B, 1, H, W) logits, accumulated in fp32 and stored as bf16. */
@@ -1489,10 +1485,10 @@ extern "C" int smaat_dsconv_outconv_bf16_fwd(const void* x0, int C0, int64_t x0_
                                              int W, int k, int Cout, int relu, void* stream) {
   SMAAT_REQUIRE(oc_w && logits, "dsconv+outconv bf16: null pointer");
   SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(logits) & 1u) == 0, "dsconv+outconv bf16: logits must be 2-byte aligned");
-  return dsconv_run(static_cast<const float*>(x0), C0, x0_bstride, static_cast<const float*>(x1), C1, x1_bstride, dw_w, dw_b,
-                    reinterpret_cast<const float*>(pw_w), nullptr, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
-                    static_cast<float*>(logits), 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu,
-                    SMAAT_PW_BF16, stream, true);
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.B = B; q.relu = relu; q.mode = SMAAT_PW_BF16; q.bact = true; q.dw_w = dw_w; q.dw_b = dw_b; q.scale = scale; q.shift = shift;
+  q.oc_w = oc_w; q.oc_b = oc_b; q.oc_y = logits;
+  return ds_launch(q, stream);
 }
 
 /* smaat_dsconv_classify_fwd from bf16 activations: the argmax runs on the fp32 logits in registers; the logits, when asked
@@ -1509,18 +1505,19 @@ extern "C" int smaat_dsconv_classify_bf16_fwd(const void* x0, int C0, int64_t x0
   SMAAT_REQUIRE((reinterpret_cast<uintptr_t>(oc_w) & 3u) == 0 && (reinterpret_cast<uintptr_t>(logits) & 1u) == 0 &&
                     (reinterpret_cast<uintptr_t>(classes) & 7u) == 0,
                 "dsconv+classify bf16: weights must be 4-byte, logits 2-byte and classes 8-byte aligned");
-  return dsconv_run(static_cast<const float*>(x0), C0, x0_bstride, static_cast<const float*>(x1), C1, x1_bstride, dw_w, dw_b,
-                    reinterpret_cast<const float*>(pw_w), nullptr, scale, shift, nullptr, 0, nullptr, oc_w, oc_b,
-                    static_cast<float*>(logits), K, classes, nullptr, nullptr, nullptr, nullptr, nullptr, B, H, W, k, Cout, relu,
-                    SMAAT_PW_BF16, stream, true);
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.B = B; q.relu = relu; q.mode = SMAAT_PW_BF16; q.bact = true; q.dw_w = dw_w; q.dw_b = dw_b; q.scale = scale; q.shift = shift;
+  q.oc_w = oc_w; q.oc_b = oc_b; q.oc_y = logits; q.ncls = K; q.cls = classes;
+  return ds_launch(q, stream);
 }
 
 /* smaat_dsconv_maxpool_fwd from bf16 activations: y bf16, the max-pool written as bf16 (pooled_bf16 = 1, 4-byte aligned) or
  * fp32 (8-byte aligned), the dtype of the level it feeds; either way bit for bit MaxPool2d(2) of the stored y. */
 extern "C" int smaat_dsconv_maxpool_bf16_eligible(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1,
                                                   int64_t x1_bstride, const void* pw_w, int H, int W, int k, int Cout) {
-  if (!smaat_dsconv_bf16_eligible(x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout, 0)) return 0;
-  return ds_staged(Cout > 64 ? 128 : 64, k, pick_pw(H, W), SMAAT_PW_BF16, false, true) ? 1 : 0;
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.mode = SMAAT_PW_BF16; q.bact = true; q.pooled = g_ds_asked;
+  return ds_select(q).declined == DS_TAKEN;
 }
 
 extern "C" int smaat_dsconv_maxpool_bf16_fwd(const void* x0, int C0, int64_t x0_bstride, const void* x1, int C1, int64_t x1_bstride,
@@ -1529,8 +1526,8 @@ extern "C" int smaat_dsconv_maxpool_bf16_fwd(const void* x0, int C0, int64_t x0_
                                              int H, int W, int k, int Cout, int relu, void* stream) {
   SMAAT_REQUIRE(y && pooled, "dsconv_maxpool_bf16: null output");
   SMAAT_REQUIRE(pooled_bf16 == 0 || pooled_bf16 == 1, "dsconv_maxpool_bf16: pooled_bf16 must be 0 or 1");
-  return dsconv_run(static_cast<const float*>(x0), C0, x0_bstride, static_cast<const float*>(x1), C1, x1_bstride, dw_w, dw_b,
-                    reinterpret_cast<const float*>(pw_w), nullptr, scale, shift, static_cast<float*>(y), y_bstride, nullptr, nullptr,
-                    nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, static_cast<float*>(pooled), B, H, W, k, Cout,
-                    relu, SMAAT_PW_BF16, stream, true, pooled_bf16);
+  DsReq q{x0, C0, x0_bstride, x1, C1, x1_bstride, pw_w, H, W, k, Cout};
+  q.B = B; q.relu = relu; q.mode = SMAAT_PW_BF16; q.bact = true; q.dw_w = dw_w; q.dw_b = dw_b; q.scale = scale; q.shift = shift;
+  q.y = y; q.y_bstride = y_bstride; q.pooled = pooled; q.pooled_bf16 = pooled_bf16;
+  return ds_launch(q, stream);
 }

@@ -1,11 +1,11 @@
 """The fused DS conv's dispatch table, restated in plain Python and checked against the library's eligibility entry points.
 
 ``expected`` says, for one request, whether the fused DS conv (csrc/dsconv_fused.cu) takes it and, if so, which kernel runs
-it, at which N_TILE and patch width PW, in how many channel passes.  It restates ``ds_eligible``, ``pick_pw``, ``ds_pair``,
-``ds_wide`` and the epilogue rules of the ``smaat_dsconv_*_eligible`` entry points.  Two facts come from compiled shared-memory
-sizes and cannot be restated: whether an instance stages its output (DsCfg::ST_BUFS > 0, which the max-pool and the CBAM pools
-read back) and how many classes' OutConv weights it keeps (DsCfg::MAX_CLASSES).  They are probed per instance and pinned in
-INSTANCES, so that a change to the rings shows up here as a diff.
+it, at which N_TILE and patch width PW, in how many channel passes.  It restates ``ds_select`` (with ``pick_pw``), which both
+launches and the ``smaat_dsconv_*_eligible`` entry points ask.  Two facts come from compiled shared-memory sizes and cannot be
+restated: whether an instance stages its output (DsCfg::ST_BUFS > 0, which the max-pool and the CBAM pools read back) and how
+many classes' OutConv weights it keeps (DsCfg::MAX_CLASSES).  They are probed per instance and pinned in INSTANCES, so that a
+change to the rings shows up here as a diff.
 
 ``SPACE`` is every combination of the axes below; the CPU test asserts that the library agrees with ``expected`` on each
 (host logic only: fake, 16-byte aligned addresses that are never dereferenced).  ``CELLS`` is the subset that
@@ -113,7 +113,7 @@ def expected(C0, C1, bs0, bs1, H, W, k, Cout, mode, impl, wide_on, bact, epilogu
     assert not bact or (mode == "bf16" and epilogue in BACT_EPILOGUES)
     a_smem, bf16 = impl == "smem", mode == "bf16"
     head, stats = epilogue in ("outconv", "classify"), epilogue == "stats"
-    # ds_eligible
+    # ds_select: the shape, stride, alignment, k, mode and A-form rules
     if k not in (1, 2, 4) or (k == 4 and a_smem) or (bf16 and a_smem):
         return DECLINED
     if bact and (k == 4 or W % 8 or bs0 % 8 or (C1 and bs1 % 8)):
@@ -130,14 +130,16 @@ def expected(C0, C1, bs0, bs1, H, W, k, Cout, mode, impl, wide_on, bact, epilogu
     pw = pick_pw(H, W)
     if not pw:
         return DECLINED
-    # the epilogue's own rules, from the single-tile instance of the request (the entry points ask it, not the pair or wide one)
+    # the epilogue's limits: eligibility asks the instance that runs.  The single tile's pinned values stand for a pair or a
+    # wide tile: both keep the staged epilogue (static_asserts), as do the single tiles they replace (INSTANCES); a pair takes
+    # class launches of up to MIN_CLS classes, which every instance keeps; a wide tile takes no head
     n_tile = 128 if Cout > 64 else 64
     staged, max_cls = INSTANCES[(n_tile, k, pw, "bf16maps" if bact else mode, impl)]
     if epilogue in ("maxpool", "pools") and not staged:
         return DECLINED
     if epilogue == "classify" and ncls > min(max_cls, MAX_CLS):
         return DECLINED
-    # dsconv_run
+    # ds_select: which instance runs it, wide, else pair, else the single tile
     if wide:
         return "dsconv_wide_kernel", 128, pw, 1
     pair = (pair_on and n_tile == 64 and k in (2, 4) and not a_smem and not bf16 and math.ceil(H / (128 // pw)) % 2 == 0
