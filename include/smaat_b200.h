@@ -485,6 +485,14 @@ int smaat_adam_step(float* params, const float* grads, float* exp_avg, float* ex
 int smaat_voc_augment_fwd(const uint8_t* x_u8, const uint8_t* y_u8, const int8_t* aug, const float* mean, const float* std,
                           float* x, int64_t x_bstride, int64_t* y, int64_t y_bstride, int B, int H, int W, void* stream);
 
+/* ---- precipitation dataset builder: the rain-pixel count of every frame (reference create_datasets.py:79-82) ----------
+ * counts[f] = #{p < plane : frames[f * plane + p] > 0.0f}, the `np.sum(images[i] > 0)` the reference tests against each rain
+ * threshold, for n_frames dense frames of plane pixels.  IEEE ordered comparison, decided on the bit pattern
+ * (0 < bits <= 0x7f800000 as int32), so no flush-to-zero applies: NaN of either sign, +-0 and negative values are not
+ * counted; positive denormals and +inf are.  Exact integers, deterministic.  16-byte loads when frames is 16-byte aligned
+ * and plane % 4 == 0, 4-byte loads otherwise.  SMAAT_E_BADARG for NULL pointers, n_frames < 1, plane < 1 or plane >= 2^31. */
+int smaat_rain_pixels_fwd(const float* frames, int64_t n_frames, int64_t plane, int32_t* counts, void* stream);
+
 /* ---- bf16 activations: SmaAt-UNet's serving forward from bf16 input ------------------------------------------------------
  * The serving forward's bf16 storage route keeps the input and the level 1-3 feature maps (and the logits / probabilities) as
  * bf16 in HBM: raw uint16_t bits, round to nearest even, passed as void*.  Arithmetic stays fp32 (the GEMMs take bf16 operands

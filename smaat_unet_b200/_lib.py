@@ -91,6 +91,7 @@ SIGNATURES = {
     "smaat_conv3x3_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _l, _p, _i, _i, _i, _i, _i, _i, _p],
     "smaat_conv3x3_bwd_weight": [_p, _p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i, _p],
     "smaat_voc_augment_fwd": [_p, _p, _p, _p, _p, _p, _l, _p, _l, _i, _i, _i, _p],
+    "smaat_rain_pixels_fwd": [_p, _l, _l, _p, _p],
     # ---- bf16 activations (the serving forward's bf16 route)
     "smaat_dsconv_bf16_eligible": [_p, _i, _l, _p, _i, _l, _p, _i, _i, _i, _i, _i],
     "smaat_dsconv_bf16_fwd": [_p, _i, _l, _p, _i, _l, _p, _p, _p, _p, _p, _p, _l, _p, _p, _i, _i, _i, _i, _i, _i, _p],

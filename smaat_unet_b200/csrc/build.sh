@@ -6,7 +6,7 @@ NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 OUT=../libsmaat_b200.so
 FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O2,-Wall
        -Xptxas -v -cudart static)
-SRCS=(runtime.cu dw3x3.cu dw3x3_small.cu pw1x1.cu pw1x1_simt.cu pw1x1_tc.cu pw1x1_wgrad_tc.cu dsconv_fused.cu glue.cu upsample.cu cbam.cu bn.cu backward.cu bn_bwd.cu loss_metrics.cu ce_metrics.cu dw3x3_bwd.cu cbam_bwd.cu optim.cu convt.cu conv3x3_tc.cu conv3x3_wgrad_tc.cu conv3x3_simt.cu voc_augment.cu)
+SRCS=(runtime.cu dw3x3.cu dw3x3_small.cu pw1x1.cu pw1x1_simt.cu pw1x1_tc.cu pw1x1_wgrad_tc.cu dsconv_fused.cu glue.cu upsample.cu cbam.cu bn.cu backward.cu bn_bwd.cu loss_metrics.cu ce_metrics.cu dw3x3_bwd.cu cbam_bwd.cu optim.cu convt.cu conv3x3_tc.cu conv3x3_wgrad_tc.cu conv3x3_simt.cu voc_augment.cu datasets.cu)
 mkdir -p ../../build
 # objects built with other flags (another architecture, say) are rebuilt
 if [[ "$(cat ../../build/.flags 2>/dev/null || true)" != "${FLAGS[*]}" ]]; then rm -f ../../build/*.o; echo "${FLAGS[*]}" > ../../build/.flags; fi

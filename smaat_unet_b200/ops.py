@@ -1031,3 +1031,24 @@ class VOCNormalize:
 
     def __repr__(self):
         return f"VOCNormalize(mean={self.mean}, std={self.std})"
+
+
+# ---- precipitation dataset builder (reference create_datasets.py:79-82) ----
+def rain_pixel_counts(frames, out=None):
+    """The number of rain pixels (``v > 0``, NaN never) of every frame of a CUDA float32 ``(N, H, W)`` tensor, as ``(N,)``
+    int32: ``np.sum(frame > 0)`` per frame, exact (smaat_rain_pixels_fwd).  ``out``: a dense (N,) int32 CUDA tensor to write
+    into (e.g. a slice of a larger count buffer)."""
+    _req(frames, "frames", 3)
+    frames = frames.contiguous()
+    N, H, W = frames.shape
+    if out is None:
+        out = torch.empty((N,), device=frames.device, dtype=torch.int32)
+    elif (not isinstance(out, torch.Tensor) or not out.is_cuda or out.dtype != torch.int32 or tuple(out.shape) != (N,)
+          or not out.is_contiguous()):
+        raise ValueError(f"smaat_unet_b200: out must be a dense ({N},) int32 CUDA tensor, got "
+                         f"{getattr(out, 'dtype', type(out).__name__)} {tuple(getattr(out, 'shape', ()))}")
+    if N == 0:
+        return out
+    _call("smaat_rain_pixels_fwd", 4 * N * H * W + 4 * N, 0, _lib.load().smaat_rain_pixels_fwd, _ptr(frames), N, H * W,
+          _ptr(out), _stream())
+    return out
