@@ -36,6 +36,8 @@ import numpy as np
 import torch
 from torch.utils.data import Dataset
 
+from .parallel import shard_range
+
 
 # ------------------------------------------------------------------------------------------------ shards
 def write_shard(path, images):
@@ -341,13 +343,20 @@ class voc_segmentation_shard(Dataset):
 
 
 # ------------------------------------------------------------------------------------------------ loader
-def shard_indices(indices, rank, world, drop_last=False):
+def shard_indices(indices, rank, world, drop_last=False, disjoint=False):
     """This rank's share of ``indices`` with ``DistributedSampler`` semantics: padded by wrapping around (or truncated
-    with ``drop_last``) to a multiple of ``world``, then strided ``rank::world``."""
+    with ``drop_last``) to a multiple of ``world``, then strided ``rank::world``.  Every rank gets the same count.
+
+    ``disjoint=True`` gives every index to exactly one rank instead (validation and test sets, where a sample counted
+    twice would bias the metrics): rank ``r`` takes the contiguous slice ``parallel.shard_range(n, r, world)``, unpadded,
+    so the ranks' counts may differ by one and a rank may get none."""
     indices = list(indices)
     n = len(indices)
     if world <= 1:
         return indices
+    if disjoint:
+        lo, hi = shard_range(n, rank, world)
+        return indices[lo:hi]
     if drop_last:
         total = (n // world) * world
         indices = indices[:total]
@@ -364,7 +373,8 @@ class PinnedBatchLoader:
 
     ``indices``: explicit sample order (e.g. the reference's train / valid split); default = all samples.
     ``shuffle``: reshuffle every epoch with ``seed + epoch`` (call ``set_epoch`` like a DistributedSampler).
-    ``rank`` / ``world``: shard the (shuffled) index list across data-parallel ranks.
+    ``rank`` / ``world``: shard the (shuffled) index list across data-parallel ranks (``shard_indices``): wrap-padded to
+    equal counts by default, or, with ``disjoint=True``, each sample on exactly one rank (validation and test sets).
     The yielded tensors are views of a ring slot that is handed back to the filler thread when the NEXT batch is
     requested.  If the consumer only *enqueued* an asynchronous host->device copy of the batch (``TrainSession.step``,
     ``InferenceSession.submit``), it must say when that copy is done: ``loader.guard(event)`` attaches a CUDA event to
@@ -385,11 +395,12 @@ class PinnedBatchLoader:
     """
 
     def __init__(self, dataset, batch_size, indices=None, shuffle=False, seed=0, drop_last=True, rank=0, world=1, ring=3,
-                 pin_memory=None):
+                 pin_memory=None, disjoint=False):
         self.dataset, self.batch_size = dataset, int(batch_size)
         self.indices = list(range(len(dataset))) if indices is None else list(indices)
         self.shuffle, self.seed, self.drop_last = bool(shuffle), int(seed), bool(drop_last)
         self.rank, self.world, self.ring = int(rank), int(world), max(2, int(ring))
+        self.disjoint = bool(disjoint)
         self.epoch = 0
         pin = torch.cuda.is_available() if pin_memory is None else bool(pin_memory)
         xs, ys = dataset.sample_shapes()
@@ -416,14 +427,14 @@ class PinnedBatchLoader:
         if self.shuffle:
             rng = np.random.default_rng(self.seed + self.epoch)
             idx = [idx[i] for i in rng.permutation(len(idx))]
-        return shard_indices(idx, self.rank, self.world, drop_last=False)
+        return shard_indices(idx, self.rank, self.world, drop_last=False, disjoint=self.disjoint)
 
     def augmentation_rng(self):
         """The generator this epoch's augmentation choices on this rank are drawn from."""
         return random.Random(f"augment/{self.seed}/{self.epoch}/{self.rank}")
 
     def __len__(self):
-        n = len(shard_indices(self.indices, self.rank, self.world))
+        n = len(shard_indices(self.indices, self.rank, self.world, disjoint=self.disjoint))
         return n // self.batch_size if self.drop_last else -(-n // self.batch_size)
 
     def __iter__(self):

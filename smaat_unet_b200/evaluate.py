@@ -9,7 +9,8 @@ for several thresholds in one pass.
   * ``load_reference_checkpoint(path)`` -- a reference Lightning ``.ckpt`` as a native model, without ``lightning``.
   * ``python -m smaat_unet_b200.evaluate`` -- the reference script's command line and output files
     (calc_metrics_test_set.py:18-72, :209-232), with ``--thresholds`` taking several values and ``--test-shard`` the shard
-    written by ``data.convert_h5``.
+    written by ``data.convert_h5``.  Under ``torchrun --nproc-per-node N`` every rank scores its own contiguous slice of
+    the test set and the totals are summed over the ranks before ``compute()``; rank 0 writes the files.
 """
 from __future__ import annotations
 
@@ -22,6 +23,7 @@ import pickle
 
 import torch
 
+from . import parallel
 from .data import PinnedBatchLoader, precipitation_maps_oversampled_shard
 from .engine import InferenceSession
 from .metrics import PrecipitationMetricsSweep
@@ -37,18 +39,28 @@ def evaluate_precipitation(models, dataset, batch=32, thresholds=(0.5,), denorma
 
     Returns ``{name: {threshold: metrics}}``, in ``models``' order, where ``metrics`` is the reference's ``compute()`` dict
     (``PrecipitationMetricsSweep.compute``).  The batches are ``batch`` samples; the last, partial one runs on a graph
-    captured for its size (``InferenceSession(batch_sizes=(tail,))``), so each sample is counted exactly once."""
+    captured for its size (``InferenceSession(batch_sizes=(tail,))``), so each sample is counted exactly once.
+
+    With a process group, rank r scores the contiguous slice ``parallel.shard_range(len(dataset), r, world)`` at its own
+    batch and tail sizes, and every accumulator's totals are summed over the ranks before ``compute()``: the counts equal
+    a single process's exactly, the squared-error sums up to their summation order."""
     device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
     n = len(dataset)
     if n < 1:
         raise ValueError("evaluate_precipitation: the dataset is empty")
-    batch = min(int(batch), n)
-    tail = n % batch
-    in_shape, _ = dataset.sample_shapes()
-    sessions = {name: InferenceSession(m, batch, in_shape, device=device, batch_sizes=(tail,) if tail else None)
-                for name, m in models.items() if not isinstance(m, PersistenceModel)}
+    rank, world = parallel.rank_world()
+    lo, hi = parallel.shard_range(n, rank, world)
     accs = {name: PrecipitationMetricsSweep(thresholds, denormalize=denormalize, device=device) for name in models}
-    score_batches(PinnedBatchLoader(dataset, batch, drop_last=False), sessions, accs, device)
+    if hi > lo:                                      # a rank of a test set smaller than the world scores nothing
+        batch = min(int(batch), hi - lo)
+        tail = (hi - lo) % batch
+        in_shape, _ = dataset.sample_shapes()
+        sessions = {name: InferenceSession(m, batch, in_shape, device=device, batch_sizes=(tail,) if tail else None)
+                    for name, m in models.items() if not isinstance(m, PersistenceModel)}
+        loader = PinnedBatchLoader(dataset, batch, drop_last=False, rank=rank, world=world, disjoint=True)
+        score_batches(loader, sessions, accs, device)
+    for acc in accs.values():
+        acc.sync_across_ranks()
     return {name: acc.compute() for name, acc in accs.items()}
 
 
@@ -217,23 +229,32 @@ def parse_args(argv=None):
 
 def main(argv=None):
     args = parse_args(argv)
-    thresholds = sorted(set(args.thresholds))
-    tag = "denorm" if args.denormalize else "norm"
-    save_dir = args.save_dir or os.path.join(args.model_folder, f"calc_metrics_test_set_results_{tag}")
-    os.makedirs(save_dir, exist_ok=True)
-    models = {PERSISTENCE: PersistenceModel()}
-    for f in sorted(os.listdir(args.model_folder)):
-        if f.endswith(".ckpt"):
-            name, _ = checkpoint_class(f)
-            print(f"Loading model: {name}")
-            models[name] = load_reference_checkpoint(os.path.join(args.model_folder, f))
-    dataset = precipitation_maps_oversampled_shard(args.test_shard, args.num_input_images, args.num_output_images, train=False)
-    results = evaluate_precipitation(models, dataset, batch=args.batch, thresholds=thresholds, denormalize=args.denormalize)
-    for t in thresholds:
-        per_model = {name: {k: _python(v) for k, v in res[t].items()} for name, res in results.items()}
-        path = os.path.join(save_dir, metrics_file_name(t, args.denormalize, args.file_type))
-        save_metrics(per_model, path, args.file_type)
-        print(f"Metrics saved to {path}")
+    with parallel.process_group_from_env() as (rank, world, _):
+        writer = rank == 0                           # every rank loads the models and scores its slice; rank 0 writes
+        thresholds = sorted(set(args.thresholds))
+        tag = "denorm" if args.denormalize else "norm"
+        save_dir = args.save_dir or os.path.join(args.model_folder, f"calc_metrics_test_set_results_{tag}")
+        if writer:
+            os.makedirs(save_dir, exist_ok=True)
+        models = {PERSISTENCE: PersistenceModel()}
+        for f in sorted(os.listdir(args.model_folder)):
+            if f.endswith(".ckpt"):
+                name, _ = checkpoint_class(f)
+                if writer:
+                    print(f"Loading model: {name}")
+                models[name] = load_reference_checkpoint(os.path.join(args.model_folder, f))
+        dataset = precipitation_maps_oversampled_shard(args.test_shard, args.num_input_images, args.num_output_images,
+                                                       train=False)
+        results = evaluate_precipitation(models, dataset, batch=args.batch, thresholds=thresholds,
+                                         denormalize=args.denormalize)
+        if writer:
+            for t in thresholds:
+                per_model = {name: {k: _python(v) for k, v in res[t].items()} for name, res in results.items()}
+                path = os.path.join(save_dir, metrics_file_name(t, args.denormalize, args.file_type))
+                save_metrics(per_model, path, args.file_type)
+                print(f"Metrics saved to {path}")
+        if world > 1:
+            parallel.barrier(torch.device("cuda", torch.cuda.current_device()))
     return results
 
 

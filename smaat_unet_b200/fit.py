@@ -21,6 +21,19 @@ bumps) or an ``InferenceSession`` re-captured before each validation pass (``val
 the faster of the two as measured by ``tools/bench_fit.py`` (README "Training from start to finish").  Either way the
 model is put back in train mode before the next step.
 
+Data parallelism.  When a process group is initialised (``torchrun --nproc-per-node N python -m smaat_unet_b200.fit ...``
+sets one up through ``parallel.process_group_from_env``), both recipes run data-parallel, as Lightning's DDP does:
+  * ``batch_size`` is per rank; the global batch is ``N x batch_size``, the learning rate is not scaled;
+  * every rank draws the same split and the same per-epoch shuffle, then takes its wrap-padded shard of the train indices
+    (``shard_indices``), so every rank steps the same batch sizes; padded samples are seen twice per epoch, as with torch's
+    ``DistributedSampler``.  Validation indices are split into disjoint slices (``disjoint=True``): each sample counts once;
+  * at the epoch's end rank 0's BatchNorm running statistics replace the others' (DDP's buffer broadcast), then the loss
+    sums and counts and the metric totals are summed over the ranks, and rank 0's early-stopping, plateau and stop
+    decisions are broadcast, so every rank takes the same ones;
+  * rank 0 alone writes checkpoints, ``history.jsonl`` and the printed lines; the others wait at a barrier after each write.
+    Checkpoints of a multi-process run hold ``world_size``, and a resume at another world size is refused.
+Without a process group nothing of this runs.
+
 Deliberate differences from the reference:
   * the train / validation split is drawn from ``np.random.RandomState(seed)`` (the same draw as the reference's
     ``np.random.shuffle`` after ``np.random.seed(seed)``) and the seed is stored in the checkpoint, so a resumed run keeps
@@ -42,7 +55,7 @@ import time
 import numpy as np
 import torch
 
-from . import ops
+from . import ops, parallel
 from .data import PinnedBatchLoader, precipitation_maps_oversampled_shard, precipitation_maps_shard, voc_segmentation_shard
 from .engine import InferenceSession
 from .evaluate import _CTOR_ARGS
@@ -177,10 +190,11 @@ def precip_file_names(class_name, epoch, val_loss):
 
 
 def precip_checkpoint(state_dict, hyper_parameters, epoch, global_step, optimizer_state, scheduler_state, early_stopping,
-                      best_model_score, best_model_path, split):
+                      best_model_score, best_model_path, split, world_size=1):
     """A Lightning-layout checkpoint dict of plain types and CPU tensors only (``evaluate``'s restricted unpickler refuses any
-    other class)."""
-    return {
+    other class).  A data-parallel run's (``world_size`` > 1) also holds ``world_size``; a single process's has no such
+    key."""
+    ckpt = {
         "epoch": int(epoch),
         "global_step": int(global_step),
         "pytorch-lightning_version": LIGHTNING_VERSION,
@@ -196,6 +210,9 @@ def precip_checkpoint(state_dict, hyper_parameters, epoch, global_step, optimize
         "hyper_parameters": dict(hyper_parameters),
         "split": dict(split),
     }
+    if world_size > 1:
+        ckpt["world_size"] = int(world_size)
+    return ckpt
 
 
 def precip_hyper_parameters(model="UNetDSAttention", train_shard=None, batch_size=16, learning_rate=1e-3, epochs=200,
@@ -226,13 +243,18 @@ def build_precip_model(hp):
     return cls(**{k: hp[k] for k in _CTOR_ARGS[cls]})
 
 
-def check_resume(ckpt, hp, num_samples):
-    """Refuse a checkpoint of another network, split or batch size than this run's (``ValueError``)."""
+def check_resume(ckpt, hp, num_samples, world=1):
+    """Refuse a checkpoint of another network, split, batch size or world size than this run's (``ValueError``).  A
+    checkpoint without ``world_size`` was written by a single process."""
     old = ckpt.get("hyper_parameters") or {}
     bad = [f"{k}: checkpoint {old.get(k)!r}, run {hp[k]!r}" for k in _RESUME_KEYS if old.get(k) != hp[k]]
     samples = (ckpt.get("split") or {}).get("samples")
     if samples != num_samples:
         bad.append(f"samples in the train shard: checkpoint {samples!r}, run {num_samples}")
+    ckpt_world = int(ckpt.get("world_size", 1))
+    if ckpt_world != int(world):
+        bad.append(f"world size: checkpoint {ckpt_world}, run {int(world)} (each rank's batches would differ from the "
+                   "interrupted run's)")
     if bad:
         raise ValueError("fit_precipitation: the checkpoint to resume from does not match this run: " + "; ".join(bad))
 
@@ -319,6 +341,11 @@ class _EpochLoop:
                     loss = self.sess.step(*batch[:2], aug=batch[2] if len(batch) > 2 else None)
                     buf[i, 0].copy_(loss)
                     self.train_loader.guard(self.sess.last_h2d_event())
+            if self.sess.world > 1:
+                # each replica's BatchNorm running statistics followed its own batches: validation and the checkpoint take
+                # rank 0's, which is what DDP's buffer broadcast leaves in every replica
+                parallel.broadcast_tensors_(list(self.model.buffers()), self.device)
+                ops.bump_weights_generation()
             fwd = self._forward()
             try:
                 with torch.no_grad(), _sync_check(self.sync_debug):
@@ -335,6 +362,39 @@ class _EpochLoop:
                 self.sess._bnd.clear()
         rows = buf.cpu().numpy()
         return rows[:nt], rows[nt:]
+
+
+def _weighted_sums(values, weights):
+    """[sum of values x weights, sum of weights] in float64: one rank's part of an epoch's weighted mean, which
+    ``parallel.allreduce_sum`` completes over the ranks."""
+    v, w = np.asarray(values, np.float64), np.asarray(weights, np.float64)
+    return [(v * w).sum(), w.sum()]
+
+
+def _agree(stop, value, stopper, plateau, device=None):
+    """Rank 0's epoch decisions on every rank, in one broadcast: its stop decision and monitored value, and its
+    early-stopping and plateau state (and so the next learning rate).  The ranks' values come from the same reductions,
+    but the decisions are made identical by construction, not by floating-point luck: a rank that stopped alone would
+    leave the others waiting in a collective.  Returns (stop, value); without a process group, the arguments."""
+    if parallel.rank_world()[1] == 1:
+        return stop, value
+    d = parallel.broadcast_from_rank0({"stop": bool(stop), "value": value, "early_stopping": stopper.state_dict(),
+                                       "improved": stopper.improved, "plateau": plateau.state_dict(), "lr": plateau.lr},
+                                      device)
+    stopper.load_state_dict(d["early_stopping"])
+    stopper.improved = d["improved"]
+    plateau.load_state_dict(d["plateau"], d["lr"])
+    return d["stop"], d["value"]
+
+
+@contextlib.contextmanager
+def _rank0_writes(device=None):
+    """A block whose files only rank 0 writes: it yields whether this rank is the writer, and at its end every rank waits
+    at a barrier, so that no rank reads (e.g. resumes from) a file rank 0 is still writing."""
+    rank, world = parallel.rank_world()
+    yield rank == 0
+    if world > 1:
+        parallel.barrier(device)
 
 
 def _append_history(out_dir, record):
@@ -382,11 +442,12 @@ def fit_precipitation(model="UNetDSAttention", train_shard=None, out_dir="lightn
     ds_cls = precipitation_maps_oversampled_shard if use_oversampled_dataset else precipitation_maps_shard
     dataset = ds_cls(train_shard, num_input_images, num_output_images, train=True)
     n = len(dataset)
+    rank, world = parallel.rank_world()
     ckpt = None
-    if resume_from_checkpoint is not None:
+    if resume_from_checkpoint is not None:           # every rank loads it; the session's broadcast keeps them identical
         from .evaluate import _RestrictedPickle
         ckpt = torch.load(resume_from_checkpoint, map_location="cpu", pickle_module=_RestrictedPickle, weights_only=False)
-        check_resume(ckpt, hp, n)
+        check_resume(ckpt, hp, n, world)
     train_idx, valid_idx = train_valid_split(n, valid_size, seed)
     if not train_idx or not valid_idx:
         raise ValueError(f"fit_precipitation: {n} samples with valid_size={valid_size} leave an empty train or validation split")
@@ -397,11 +458,16 @@ def fit_precipitation(model="UNetDSAttention", train_shard=None, out_dir="lightn
     net = build_precip_model(hp)
     if ckpt is not None:
         net.load_state_dict(ckpt["state_dict"], strict=True)
-    train_loader = PinnedBatchLoader(dataset, batch_size, indices=train_idx, shuffle=True, seed=seed, drop_last=False)
-    val_loader = PinnedBatchLoader(dataset, batch_size, indices=valid_idx, shuffle=True, seed=seed, drop_last=False)
-    tail = len(train_idx) % batch_size
+    # data-parallel: the same split and per-epoch shuffle on every rank; train shards wrap-padded to equal length (every
+    # rank steps the same sizes), validation slices disjoint (every sample counted once)
+    train_loader = PinnedBatchLoader(dataset, batch_size, indices=train_idx, shuffle=True, seed=seed, drop_last=False,
+                                     rank=rank, world=world)
+    val_loader = PinnedBatchLoader(dataset, batch_size, indices=valid_idx, shuffle=True, seed=seed, drop_last=False,
+                                   rank=rank, world=world, disjoint=True)
+    tail = len(train_loader.epoch_indices()) % batch_size
     sess = TrainSession(net, batch_size, in_shape, lr=learning_rate, device=device, batch_sizes=(tail,) if tail else None,
                         metrics=PrecipitationMetrics(threshold=threshold, device=device))
+    sess.check_partial_rows = False                  # equal step sizes on every rank by construction (shard_indices)
     val_metrics = PrecipitationMetrics(threshold=threshold, device=device)
 
     plateau = PlateauLR(learning_rate, "min", factor=0.1, patience=lr_patience)
@@ -422,7 +488,9 @@ def fit_precipitation(model="UNetDSAttention", train_shard=None, out_dir="lightn
         if not last_name.endswith("_last.ckpt"):
             last_name = None
         del ckpt
-    os.makedirs(ckpt_dir, exist_ok=True)
+    with _rank0_writes(device) as writer:
+        if writer:
+            os.makedirs(ckpt_dir, exist_ok=True)
 
     def val_batch(pred, yd, row):
         acc, _ = mse_metrics(pred.reshape(yd.shape), yd, threshold, True)
@@ -439,45 +507,58 @@ def fit_precipitation(model="UNetDSAttention", train_shard=None, out_dir="lightn
         tsz, vsz = np.asarray(loop.train_sizes, np.float64), np.asarray(loop.val_sizes, np.float64)
         step_losses = train_rows[:, 0].astype(np.float32)                                 # loss_func per step (fp32)
         val_losses = (val_rows[:, 0] / vsz).astype(np.float32)
-        train_loss = float((step_losses * tsz).sum() / tsz.sum())
-        val_loss = float((val_losses * vsz).sum() / vsz.sum())
+        # one reduction over the ranks (none without a process group): the weighted sums, their weights, the batch count
+        t_sum, t_n, v_sum, v_n, v_batches = parallel.allreduce_sum(
+            _weighted_sums(step_losses, tsz) + _weighted_sums(val_losses, vsz) + [len(vsz)], device)
+        train_loss = float(t_sum / t_n)
+        val_loss = float(v_sum / v_n)
         global_step += len(tsz)
+        val_metrics.sync_across_ranks()
+        sess.metrics.sync_across_ranks()
         val_m, train_m = val_metrics.compute(), sess.metrics.compute()
         val_metrics.reset()
         sess.metrics.reset()
         stop = stopper.update(val_loss, epoch)
-        next_lr = plateau.step(val_loss)
+        plateau.step(val_loss)
+        stop, val_loss = _agree(stop, val_loss, stopper, plateau, device)
+        next_lr = plateau.lr
         sess.set_lr(next_lr)
         score = val_loss if math.isfinite(val_loss) else math.inf
         is_best = best_score is None or score < best_score
         best_file, last_file = precip_file_names(hp["model"], epoch, val_loss)
-        payload = precip_checkpoint(_cpu_state_dict(net), hp, epoch, global_step, _cpu_optimizer_state(sess.optimizer_state_dict()),
-                                    plateau.state_dict(), stopper.state_dict(),
-                                    score if is_best else best_score,
-                                    os.path.join(ckpt_dir, best_file if is_best else best_name), split)
-        t_ckpt = time.perf_counter()
-        if is_best:
-            best_score = score
-            payload = _replace_file(ckpt_dir, best_name, best_file, payload)      # the last file is a copy of it
-            best_name = best_file
-        _replace_file(ckpt_dir, last_name, last_file, payload)
-        last_name = last_file
-        t_ckpt = time.perf_counter() - t_ckpt
-        rec = {"recipe": "precip", "model": hp["model"], "epoch": epoch, "global_step": global_step, "train_loss": train_loss,
-               "val_loss": val_loss, "lr": lr, "next_lr": next_lr, "train_samples": int(tsz.sum()),
-               "val_samples": int(vsz.sum()), "train_batches": len(tsz), "val_batches": len(vsz),
-               "train_metrics": _plain_metrics(train_m), "val_metrics": _plain_metrics(val_m), "best": is_best,
-               "es_wait_count": stopper.wait_count, "stop": stop, "epoch_seconds": time.perf_counter() - t0,
-               "checkpoint_seconds": t_ckpt}
-        history.append(rec)
-        _append_history(os.fspath(out_dir), rec)
-        if verbose:
-            print(f"\n\nEpoch {epoch} - Validation Metrics: {make_metrics_str(val_m)}")
-            print(f"\n\nEpoch {epoch} - Train Metrics: {make_metrics_str(train_m)}")
-            print(f"Epoch {epoch}: train_loss={train_loss:.6f}, val_loss={val_loss:.6f}, lr={lr}, "
-                  f"time {(time.perf_counter() - t_start) / 60:.3f} min", flush=True)
+        with _rank0_writes(device) as writer:
+            t_ckpt = 0.0
+            if writer:
+                payload = precip_checkpoint(_cpu_state_dict(net), hp, epoch, global_step,
+                                            _cpu_optimizer_state(sess.optimizer_state_dict()), plateau.state_dict(),
+                                            stopper.state_dict(), score if is_best else best_score,
+                                            os.path.join(ckpt_dir, best_file if is_best else best_name), split, world)
+                t_ckpt = time.perf_counter()
+                if is_best:
+                    payload = _replace_file(ckpt_dir, best_name, best_file, payload)  # the last file is a copy of it
+                _replace_file(ckpt_dir, last_name, last_file, payload)
+                t_ckpt = time.perf_counter() - t_ckpt
+            if is_best:
+                best_score, best_name = score, best_file
+            last_name = last_file
+            rec = {"recipe": "precip", "model": hp["model"], "epoch": epoch, "global_step": global_step,
+                   "train_loss": train_loss, "val_loss": val_loss, "lr": lr, "next_lr": next_lr, "train_samples": int(t_n),
+                   "val_samples": int(v_n), "train_batches": len(tsz), "val_batches": int(v_batches),
+                   "train_metrics": _plain_metrics(train_m), "val_metrics": _plain_metrics(val_m), "best": is_best,
+                   "es_wait_count": stopper.wait_count, "stop": stop, "epoch_seconds": time.perf_counter() - t0,
+                   "checkpoint_seconds": t_ckpt}
+            if world > 1:
+                rec["world_size"] = world
+            history.append(rec)
+            if writer:
+                _append_history(os.fspath(out_dir), rec)
+            if writer and verbose:
+                print(f"\n\nEpoch {epoch} - Validation Metrics: {make_metrics_str(val_m)}")
+                print(f"\n\nEpoch {epoch} - Train Metrics: {make_metrics_str(train_m)}")
+                print(f"Epoch {epoch}: train_loss={train_loss:.6f}, val_loss={val_loss:.6f}, lr={lr}, "
+                      f"time {(time.perf_counter() - t_start) / 60:.3f} min", flush=True)
         if stop:
-            if verbose:
+            if verbose and rank == 0:
                 print(f"Early stopping at epoch {epoch}: val_loss "
                       f"{'is not finite' if not math.isfinite(val_loss) else f'did not improve for {es_patience} epochs'}")
             break
@@ -487,15 +568,19 @@ def fit_precipitation(model="UNetDSAttention", train_shard=None, out_dir="lightn
 
 
 # ------------------------------------------------------------------------------------------------ VOC
-def voc_checkpoint(model, epoch, optimizer_state, val_loss, train_loss, miou):
+def voc_checkpoint(model, epoch, optimizer_state, val_loss, train_loss, miou, world_size=1):
     """train_SmaAtUNet.py:83-96's dict.  ``model`` is a CPU copy of the network (the trained one's parameters live in the
-    session's flat buffers and its CBAMs carry the session's hooks)."""
+    session's flat buffers and its CBAMs carry the session's hooks).  A data-parallel run's (``world_size`` > 1) also
+    holds ``world_size``."""
     copy = SmaAt_UNet(model.n_channels, model.n_classes, kernels_per_layer=model.inc.double_conv[0].kernels_per_layer,
                       bilinear=model.bilinear)
     sd = _cpu_state_dict(model)
     copy.load_state_dict(sd, strict=True)
-    return {"model": copy, "epoch": int(epoch), "state_dict": sd, "optimizer_state_dict": optimizer_state,
+    ckpt = {"model": copy, "epoch": int(epoch), "state_dict": sd, "optimizer_state_dict": optimizer_state,
             "val_loss": float(val_loss), "train_loss": float(train_loss), "mIOU": float(miou)}
+    if world_size > 1:
+        ckpt["world_size"] = int(world_size)
+    return ckpt
 
 
 def voc_file_names(class_name, epoch):
@@ -523,11 +608,14 @@ def fit_voc(train_prefix, val_prefix, out_dir="checkpoints", epochs=200, batch_s
     torch.manual_seed(seed)
     net = SmaAt_UNet(3, 21)
     K = net.n_classes
-    train_loader = PinnedBatchLoader(train_ds, batch_size, shuffle=True, seed=seed, drop_last=False)
-    val_loader = PinnedBatchLoader(val_ds, batch_size, shuffle=False, drop_last=False)
-    tail = len(train_ds) % batch_size
+    rank, world = parallel.rank_world()
+    # the sharding of fit_precipitation: wrap-padded train shards, disjoint validation slices
+    train_loader = PinnedBatchLoader(train_ds, batch_size, shuffle=True, seed=seed, drop_last=False, rank=rank, world=world)
+    val_loader = PinnedBatchLoader(val_ds, batch_size, shuffle=False, drop_last=False, rank=rank, world=world, disjoint=True)
+    tail = len(train_loader.epoch_indices()) % batch_size
     sess = TrainSession(net, batch_size, (3, H, W), lr=learning_rate, device=device, loss="cross_entropy",
                         input_transform=ops.VOCNormalize(), batch_sizes=(tail,) if tail else None, metrics=None)
+    sess.check_partial_rows = False
     iou = IoU(K, normalized=False, device=device)
     norm = ops.VOCNormalize()
 
@@ -538,49 +626,62 @@ def fit_voc(train_prefix, val_prefix, out_dir="checkpoints", epochs=200, batch_s
     loop = _EpochLoop(sess, train_loader, val_loader, lambda x, y: norm(x, y), val_batch, validation, sync_debug)
     plateau = PlateauLR(learning_rate, "max", factor=0.1, patience=lr_patience)
     stopper = EarlyStopping(earlystopping, mode="max", check_finite=False, best=-1.0)
-    os.makedirs(os.fspath(out_dir), exist_ok=True)
+    with _rank0_writes(device) as writer:
+        if writer:
+            os.makedirs(os.fspath(out_dir), exist_ok=True)
     class_name = type(net).__name__
     history, t_start = [], time.perf_counter()
     for epoch in range(epochs):
         t0 = time.perf_counter()
         lr = plateau.lr
         train_rows, val_rows = loop.run(epoch)
-        train_loss = float(train_rows[:, 0].astype(np.float32).astype(np.float64).mean())
+        step_losses = train_rows[:, 0].astype(np.float32)
         with np.errstate(invalid="ignore", divide="ignore"):
             per_batch = np.where(val_rows[:, 2] > 0, np.nan, val_rows[:, 0] / val_rows[:, 1]).astype(np.float32)
-        val_loss = float(per_batch.astype(np.float64).mean())
-        iou.conf_metric._invalid.add_(int(val_rows[:, 2].sum()))
+        # the reference's losses are plain means of the per-batch losses: every batch weighs 1, over all ranks' batches
+        t_sum, t_n, v_sum, v_n, invalid, t_samples, v_samples = parallel.allreduce_sum(
+            _weighted_sums(step_losses, np.ones(len(step_losses))) + _weighted_sums(per_batch, np.ones(len(per_batch)))
+            + [val_rows[:, 2].sum(), sum(loop.train_sizes), sum(loop.val_sizes)], device)
+        train_loss = float(t_sum / t_n)
+        val_loss = float(v_sum / v_n)
+        iou.sync_across_ranks()
+        iou.conf_metric._invalid.add_(int(invalid))
         _, mean_iou = iou.value()
         mean_iou = float(mean_iou)
         iou.reset()
         stop = stopper.update(mean_iou, epoch)
+        if not stop:                              # the reference breaks before its scheduler step
+            plateau.step(mean_iou)
+        stop, mean_iou = _agree(stop, mean_iou, stopper, plateau, device)
+        next_lr = plateau.lr
         best_file, epoch_file = voc_file_names(class_name, epoch)
-        if stopper.improved:
-            torch.save(voc_checkpoint(net, epoch, _cpu_optimizer_state(sess.optimizer_state_dict()), val_loss, train_loss,
-                                      mean_iou), os.path.join(os.fspath(out_dir), best_file))
-        rec = {"recipe": "voc", "model": class_name, "epoch": epoch, "train_loss": train_loss, "val_loss": val_loss,
-               "mIOU": mean_iou, "lr": lr, "best": stopper.improved, "earlystopping_counter": stopper.wait_count,
-               "stop": stop, "train_batches": len(train_rows), "val_batches": len(val_rows),
-               "train_samples": int(sum(loop.train_sizes)), "val_samples": int(sum(loop.val_sizes))}
-        if stop:                                  # the reference breaks before its print, per-epoch file and scheduler step
-            rec.update(next_lr=lr, epoch_seconds=time.perf_counter() - t0)
+        with _rank0_writes(device) as writer:
+            if writer and stopper.improved:
+                torch.save(voc_checkpoint(net, epoch, _cpu_optimizer_state(sess.optimizer_state_dict()), val_loss,
+                                          train_loss, mean_iou, world), os.path.join(os.fspath(out_dir), best_file))
+            rec = {"recipe": "voc", "model": class_name, "epoch": epoch, "train_loss": train_loss, "val_loss": val_loss,
+                   "mIOU": mean_iou, "lr": lr, "best": stopper.improved, "earlystopping_counter": stopper.wait_count,
+                   "stop": stop, "train_batches": len(train_rows), "val_batches": int(v_n),
+                   "train_samples": int(t_samples), "val_samples": int(v_samples)}
+            if world > 1:
+                rec["world_size"] = world
+            if not stop:                          # the reference breaks before its print and per-epoch file
+                if writer and verbose:
+                    print(f"Epoch: {epoch:5d}, Time: {(time.perf_counter() - t_start) / 60:.3f} min,"
+                          f"Train_loss: {train_loss:2.10f}, Val_loss: {val_loss:2.10f},", f"mIOU: {mean_iou:.10f},",
+                          f"lr: {lr},", f"Early stopping counter: {stopper.wait_count}/{earlystopping}", flush=True)
+                if writer and save_every is not None and epoch % save_every == 0:
+                    torch.save(voc_checkpoint(net, epoch, _cpu_optimizer_state(sess.optimizer_state_dict()), val_loss,
+                                              train_loss, mean_iou, world), os.path.join(os.fspath(out_dir), epoch_file))
+                sess.set_lr(next_lr)
+            rec.update(next_lr=next_lr, epoch_seconds=time.perf_counter() - t0)
             history.append(rec)
-            _append_history(os.fspath(out_dir), rec)
-            if verbose:
+            if writer:
+                _append_history(os.fspath(out_dir), rec)
+            if writer and stop and verbose:
                 print(f"Stopping early --> mean IoU has not decreased over {earlystopping} epochs")
+        if stop:
             break
-        if verbose:
-            print(f"Epoch: {epoch:5d}, Time: {(time.perf_counter() - t_start) / 60:.3f} min,"
-                  f"Train_loss: {train_loss:2.10f}, Val_loss: {val_loss:2.10f},", f"mIOU: {mean_iou:.10f},", f"lr: {lr},",
-                  f"Early stopping counter: {stopper.wait_count}/{earlystopping}", flush=True)
-        if save_every is not None and epoch % save_every == 0:
-            torch.save(voc_checkpoint(net, epoch, _cpu_optimizer_state(sess.optimizer_state_dict()), val_loss, train_loss,
-                                      mean_iou), os.path.join(os.fspath(out_dir), epoch_file))
-        next_lr = plateau.step(mean_iou)
-        sess.set_lr(next_lr)
-        rec.update(next_lr=next_lr, epoch_seconds=time.perf_counter() - t0)
-        history.append(rec)
-        _append_history(os.fspath(out_dir), rec)
     return FitResult(history=history, model=net, session=sess, train_loader=train_loader, val_loader=val_loader,
                      best_path=os.path.join(os.fspath(out_dir), voc_file_names(class_name, 0)[0]))
 
@@ -597,8 +698,13 @@ def _bool(v):
     raise argparse.ArgumentTypeError(f"expected a boolean, got {v!r}")
 
 
+_BATCH_HELP = ("samples per step on each GPU: under torchrun --nproc-per-node N the global batch is N x this, as in "
+               "Lightning's DDP; the learning rate is not scaled")
+
+
 def parse_args(argv=None):
-    p = argparse.ArgumentParser(description="Train the reference's models on the GPU path, without Lightning")
+    p = argparse.ArgumentParser(description="Train the reference's models on the GPU path, without Lightning.  Under torchrun "
+                                "(one process per GPU) the run is data-parallel; only rank 0 writes files")
     sub = p.add_subparsers(dest="recipe", required=True)
     pr = sub.add_parser("precip", help="train_precip_lightning.py: a precipitation network on a data.convert_h5 train shard")
     pr.add_argument("--model", default="UNetDSAttention", help=f"one of {', '.join(PRECIP_MODELS)}")
@@ -606,7 +712,7 @@ def parse_args(argv=None):
                     help="(samples, T, H, W) float32 .npy of the train split (data.convert_h5 writes <prefix>_train.npy)")
     pr.add_argument("--out", "--out-dir", dest="out_dir", default="lightning/precip_regression",
                     help="checkpoints go to OUT/<model>/, the per-epoch history to OUT/history.jsonl")
-    pr.add_argument("--batch_size", "--batch-size", type=int, default=16)
+    pr.add_argument("--batch_size", "--batch-size", type=int, default=16, help=_BATCH_HELP)
     pr.add_argument("--learning_rate", "--learning-rate", type=float, default=1e-3)
     pr.add_argument("--epochs", type=int, default=200)
     pr.add_argument("--lr_patience", "--lr-patience", type=int, default=4)
@@ -625,7 +731,7 @@ def parse_args(argv=None):
     vc.add_argument("--train-prefix", required=True, help="data.convert_voc prefix of the train split")
     vc.add_argument("--val-prefix", required=True, help="data.convert_voc prefix of the val split")
     vc.add_argument("--out", "--out-dir", dest="out_dir", default="checkpoints")
-    vc.add_argument("--batch-size", "--batch_size", dest="batch_size", type=int, default=8)
+    vc.add_argument("--batch-size", "--batch_size", dest="batch_size", type=int, default=8, help=_BATCH_HELP)
     vc.add_argument("--learning-rate", "--learning_rate", dest="learning_rate", type=float, default=1e-3)
     vc.add_argument("--epochs", type=int, default=200)
     vc.add_argument("--earlystopping", type=int, default=30)
@@ -642,9 +748,10 @@ def parse_args(argv=None):
 def main(argv=None):
     a = vars(parse_args(argv))
     recipe = a.pop("recipe")
-    if recipe == "precip":
-        return fit_precipitation(**a)
-    return fit_voc(**a)
+    with parallel.process_group_from_env():
+        if recipe == "precip":
+            return fit_precipitation(**a)
+        return fit_voc(**a)
 
 
 if __name__ == "__main__":

@@ -8,8 +8,10 @@ the SmaAt-UNet path -- the training gradient all-reduce -- goes through `allredu
 """
 from __future__ import annotations
 
+import contextlib
 import os
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -27,6 +29,74 @@ def init_from_env(backend=None, device=None):
         kw = {"device_id": device} if (backend == "nccl" and device is not None) else {}
         dist.init_process_group(backend, rank=rank, world_size=world, **kw)
     return rank, world, local
+
+
+@contextlib.contextmanager
+def process_group_from_env():
+    """A command's process group under torchrun: with ``WORLD_SIZE`` > 1, each process takes the GPU of its ``LOCAL_RANK``
+    and joins an NCCL group that is destroyed when the block ends.  Without torchrun's env (or with a group already
+    initialised by the caller) nothing is set up or torn down.  Yields (rank, world, local)."""
+    rank, world, local = env_rank_world()
+    owned = world > 1 and not dist.is_initialized()
+    if owned:
+        torch.cuda.set_device(local)
+        init_from_env("nccl", torch.device("cuda", local))
+    try:
+        yield rank, world, local
+    finally:
+        if owned:
+            dist.destroy_process_group()
+
+
+def rank_world():
+    """(rank, world size) of the default process group; (0, 1) without one."""
+    if dist.is_available() and dist.is_initialized():
+        return dist.get_rank(), dist.get_world_size()
+    return 0, 1
+
+
+def _comm_device(device):
+    """Where a collective's tensor lives: the rank's GPU for NCCL, the host for gloo."""
+    if dist.get_backend() == "nccl":
+        return device if device is not None else torch.device("cuda", torch.cuda.current_device())
+    return torch.device("cpu")
+
+
+def allreduce_sum(values, device=None):
+    """Elementwise sum over the ranks of a vector of host numbers, as float64 (exact for counts below 2**53).  Without a
+    process group the values come back as they are."""
+    v = np.asarray(values, dtype=np.float64)
+    if rank_world()[1] == 1:
+        return v
+    t = torch.from_numpy(v.copy()).to(_comm_device(device))
+    dist.all_reduce(t, op=dist.ReduceOp.SUM)
+    return t.cpu().numpy()
+
+
+def broadcast_from_rank0(obj, device=None):
+    """Rank 0's ``obj`` (any picklable value) on every rank; ``obj`` itself without a process group."""
+    if rank_world()[1] == 1:
+        return obj
+    box = [obj]
+    dist.broadcast_object_list(box, src=0, device=_comm_device(device))
+    return box[0]
+
+
+def broadcast_tensors_(tensors, device=None):
+    """Overwrite ``tensors`` (same device on every rank) with rank 0's values in place: one broadcast per dtype."""
+    if rank_world()[1] == 1:
+        return
+    by_dtype = {}
+    for t in tensors:
+        by_dtype.setdefault(t.dtype, []).append(t)
+    with torch.no_grad():
+        for group in by_dtype.values():
+            flat = torch.cat([t.reshape(-1) for t in group]).to(_comm_device(device))
+            dist.broadcast(flat, src=0)
+            off = 0
+            for t in group:
+                t.copy_(flat[off:off + t.numel()].view_as(t))
+                off += t.numel()
 
 
 def shard_range(n_items: int, rank: int, world: int):

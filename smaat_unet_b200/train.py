@@ -148,6 +148,9 @@ class TrainSession:
         self.allreduce_events = None        # (start, end) pairs of the last step when record_comm_timing is on
         self.record_comm_timing = False
         self.skip_allreduce = False         # measurement only (bench.py: step time without the collective); replicas diverge
+        # a partial step all-gathers its size (_check_rows_agree); a caller whose ranks step equal sizes by construction
+        # (fit's wrap-padded shards) turns it off so that nothing in its batch loop waits for the GPU
+        self.check_partial_rows = True
         self._build(warmup)
 
     def _n_classes(self):
@@ -486,7 +489,7 @@ class TrainSession:
         """Data-parallel ranks must step the same number of samples: a partial step all-gathers n and raises if a rank
         differs.  Full steps are not checked, so that they stay free of host synchronisation; a full step on one rank
         against a partial step on another therefore meets the all-gather with the gradient all-reduce and hangs."""
-        if self.world == 1 or self._rows == self.batch:
+        if self.world == 1 or self._rows == self.batch or not self.check_partial_rows:
             return
         rows = [None] * self.world
         dist.all_gather_object(rows, self._rows)
